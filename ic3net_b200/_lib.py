@@ -125,7 +125,11 @@ SYMBOLS = {
                                        C.POINTER(PolicyPacked), _PTR, _PTR]),
     "ic3_tj_encoder_index": (C.c_int, [C.POINTER(TJCfg), C.POINTER(TJState), C.POINTER(PolicyCfg),
                                        C.POINTER(PolicyPacked), _PTR, _PTR]),
-    "ic3_pp_encoder_table": (C.c_int, [C.POINTER(PPCfg), C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), _PTR, _PTR]),
+    "ic3_pp_obs_encode": (C.c_int, [C.POINTER(PPCfg), C.POINTER(PPState), C.POINTER(PolicyCfg),
+                                    C.POINTER(PolicyPacked), _PTR, _PTR, _PTR]),
+    "ic3_tj_obs_encode": (C.c_int, [C.POINTER(TJCfg), C.POINTER(TJState), C.POINTER(PolicyCfg),
+                                    C.POINTER(PolicyPacked), _PTR, _PTR, _PTR]),
+    "ic3_pp_encoder_table":(C.c_int, [C.POINTER(PPCfg), C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), _PTR, _PTR]),
     "ic3_tj_encoder_table": (C.c_int, [C.POINTER(TJCfg), C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), _PTR, _PTR]),
     "ic3_policy_workspace_bytes": (C.c_uint64, [C.POINTER(PolicyCfg)]),
     "ic3_policy_step": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), C.POINTER(PolicyIO), _PTR]),

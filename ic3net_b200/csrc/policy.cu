@@ -13,6 +13,7 @@
 // contiguous row; h/c/x/h'/c' move through HBM exactly once per step.
 #include <cstring>
 
+#include "encoder_rows.cuh"
 #include "ic3_common.cuh"
 #include "policy_heads.cuh"
 #include "policy_internal.h"
@@ -320,28 +321,8 @@ __global__ void sample_kernel(ic3_policy_cfg cfg, const float* __restrict__ logp
 // ---------------------------------------------------------------------------
 // encoder, dense form (comm.py:119): warp per agent row, obs streamed once with
 // 16-byte evict-first loads; only non-zero features touch the (L2-resident) W^T.
+// (axpy_row / store_x / store_x2: encoder_rows.cuh)
 // ---------------------------------------------------------------------------
-template <int CPT>
-__device__ __forceinline__ void axpy_row(float (&acc)[CPT], float v, const float* __restrict__ wrow, int lane) {
-  if (CPT == 4) {
-    const float4 wv = __ldg(reinterpret_cast<const float4*>(wrow) + lane);
-    acc[0] = fmaf(v, wv.x, acc[0]); acc[1] = fmaf(v, wv.y, acc[1]);
-    acc[2] = fmaf(v, wv.z, acc[2]); acc[3] = fmaf(v, wv.w, acc[3]);
-  } else if (CPT == 2) {
-    const float2 wv = __ldg(reinterpret_cast<const float2*>(wrow) + lane);
-    acc[0] = fmaf(v, wv.x, acc[0]); acc[1] = fmaf(v, wv.y, acc[1]);
-  } else {
-    acc[0] = fmaf(v, __ldg(wrow + lane), acc[0]);
-  }
-}
-
-template <int CPT>
-__device__ __forceinline__ void store_x(const float (&acc)[CPT], float* __restrict__ xrow, int lane) {
-  if (CPT == 4) reinterpret_cast<float4*>(xrow)[lane] = make_float4(acc[0], acc[1], acc[2], acc[3]);
-  else if (CPT == 2) reinterpret_cast<float2*>(xrow)[lane] = make_float2(acc[0], acc[1]);
-  else xrow[lane] = acc[0];
-}
-
 // Observation layout hint of ic3_policy_cfg (obs_off, obs_vocab, obs_ncount): is feature f a one-hot position
 // class (first accumulator, may come from a per-position table) or a count / scalar (second accumulator)?
 struct ObsLayout {
@@ -367,14 +348,6 @@ struct ObsLayout {
     }
   }
 };
-
-template <int CPT>
-__device__ __forceinline__ void store_x2(const float (&a)[CPT], const float (&b)[CPT], float* __restrict__ xrow, int lane) {
-  float r[CPT];
-#pragma unroll
-  for (int c = 0; c < CPT; ++c) r[c] = a[c] + b[c];      // x = (bias + class terms) + (other terms)
-  store_x<CPT>(r, xrow, lane);
-}
 
 template <int H, bool VEC>
 __global__ void __launch_bounds__(256) encoder_dense_kernel(const float* __restrict__ obs, const float* __restrict__ wT,
@@ -457,7 +430,6 @@ __global__ void __launch_bounds__(256) pp_encoder_index_kernel(ic3_pp_cfg env, i
                                                                const float* __restrict__ wT,
                                                                const float* __restrict__ bias, float* __restrict__ x,
                                                                bool split) {
-  constexpr int CPT = H / 32;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row = blockIdx.x * (blockDim.x >> 5) + warp;
   const int N = env.N, D = env.dim, v = env.vision, W = 2 * v + 1, V = D * D + 4;
@@ -471,33 +443,16 @@ __global__ void __launch_bounds__(256) pp_encoder_index_kernel(ic3_pp_cfg env, i
     lc = l[1];
   }
   const int r0 = __shfl_sync(IC3_FULL_MASK, lr, i), c0 = __shfl_sync(IC3_FULL_MASK, lc, i);
-  float acc[CPT], acc2[CPT];
-#pragma unroll
-  for (int c = 0; c < CPT; ++c) {
-    acc[c] = __ldg(bias + lane * CPT + c);
-    acc2[c] = 0.f;
-  }
-  for (int w = 0; w < W * W; ++w) {
+  // the record pp_write_obs builds for window cell w, from the agents' positions held by the lanes
+  auto cell = [&](int w) -> uint32_t {
     const int dy = w / W, dx = w - dy * W;
     const int rr = r0 - v + dy, cc = c0 - v + dx;
-    const float* wcell = wT + (size_t)w * V * H;
     const unsigned here = __ballot_sync(IC3_FULL_MASK, lr == rr && lc == cc);
-    if (rr >= 0 && rr < D && cc >= 0 && cc < D) {
-      const int npred = __popc(here & ((1u << N) - 1u));
-      const int nprey = (here >> N) & 1u;
-      axpy_row<CPT>(acc, 1.f, wcell + (size_t)(rr * D + cc) * H, lane);
-      if (split) {          // counts go to the second sum (ic3_policy_cfg.obs_vocab > 0)
-        if (nprey) axpy_row<CPT>(acc2, (float)nprey, wcell + (size_t)(V - 2) * H, lane);
-        if (npred) axpy_row<CPT>(acc2, (float)npred, wcell + (size_t)(V - 1) * H, lane);
-      } else {
-        if (nprey) axpy_row<CPT>(acc, (float)nprey, wcell + (size_t)(V - 2) * H, lane);
-        if (npred) axpy_row<CPT>(acc, (float)npred, wcell + (size_t)(V - 1) * H, lane);
-      }
-    } else {
-      axpy_row<CPT>(acc, 1.f, wcell + (size_t)(V - 3) * H, lane);
-    }
-  }
-  store_x2<CPT>(acc, acc2, x + (size_t)row * H, lane);
+    if (rr < 0 || rr >= D || cc < 0 || cc >= D) return (uint32_t)(V - 3);      // OUTSIDE, no counts
+    const uint32_t npred = __popc(here & ((1u << N) - 1u)), nprey = (here >> N) & 1u;
+    return (uint32_t)(rr * D + cc) | (npred << 16) | (nprey << 24);
+  };
+  pp_encode_row<H>(cell, W * W, V, wT, bias, split, x + (size_t)row * H, lane);
 }
 
 template <int H>
@@ -505,7 +460,6 @@ __global__ void __launch_bounds__(256) tj_encoder_index_kernel(ic3_tj_cfg env, i
                                                                const float* __restrict__ wT,
                                                                const float* __restrict__ bias, float* __restrict__ x,
                                                                bool split) {
-  constexpr int CPT = H / 32;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int row = blockIdx.x * (blockDim.x >> 5) + warp;
   const int N = env.N, v = env.vision, W = 2 * v + 1, V = env.vocab;
@@ -517,42 +471,19 @@ __global__ void __launch_bounds__(256) tj_encoder_index_kernel(ic3_tj_cfg env, i
     lc = st.loc[((size_t)e * N + lane) * 2 + 1];
   }
   const int r0 = __shfl_sync(IC3_FULL_MASK, lr, i), c0 = __shfl_sync(IC3_FULL_MASK, lc, i);
-  float acc[CPT], acc2s[CPT];
-#pragma unroll
-  for (int c = 0; c < CPT; ++c) {
-    acc[c] = __ldg(bias + lane * CPT + c);
-    acc2s[c] = 0.f;
-  }
-  // split (ic3_policy_cfg.obs_vocab > 0): scalars and car counts form the second sum
-  if (st.alive[(size_t)e * N + i]) {
-    const float la = (float)st.last_act[(size_t)e * N + i];
-    const float ri = (float)st.route_id[(size_t)e * N + i] / (float)(env.npath - 1);
-    if (split) {
-      if (la != 0.f) axpy_row<CPT>(acc2s, la, wT, lane);
-      if (ri != 0.f) axpy_row<CPT>(acc2s, ri, wT + H, lane);
-    } else {
-      if (la != 0.f) axpy_row<CPT>(acc, la, wT, lane);
-      if (ri != 0.f) axpy_row<CPT>(acc, ri, wT + H, lane);
-    }
-    for (int w = 0; w < W * W; ++w) {
-      const int dy = w / W, dx = w - dy * W;
-      const int rr = r0 - v + dy, cc = c0 - v + dx;
-      const float* wcell = wT + (size_t)(2 + w * V) * H;
-      const unsigned here = __ballot_sync(IC3_FULL_MASK, lr == rr && lc == cc);
-      int cls = env.outside_cls, cnt = 0;
-      if (rr >= 0 && rr < env.h && cc >= 0 && cc < env.w) {
-        cls = env.grid[rr * env.w + cc];
-        cnt = __popc(here);
-      }
-      // dense order: class index ascending; cls < car_cls always (BASE+2)
-      axpy_row<CPT>(acc, 1.f, wcell + (size_t)cls * H, lane);
-      if (cnt) {
-        if (split) axpy_row<CPT>(acc2s, (float)cnt, wcell + (size_t)env.car_cls * H, lane);
-        else axpy_row<CPT>(acc, (float)cnt, wcell + (size_t)env.car_cls * H, lane);
-      }
-    }
-  }
-  store_x2<CPT>(acc, acc2s, x + (size_t)row * H, lane);      // acc2s == 0 when not split: x = acc
+  // the record tj_write_obs builds for window cell w (every slot counts, dead ones are parked at (0,0))
+  auto cell = [&](int w) -> uint32_t {
+    const int dy = w / W, dx = w - dy * W;
+    const int rr = r0 - v + dy, cc = c0 - v + dx;
+    const unsigned here = __ballot_sync(IC3_FULL_MASK, lr == rr && lc == cc);
+    if (rr < 0 || rr >= env.h || cc < 0 || cc >= env.w) return (uint32_t)env.outside_cls;
+    return (uint32_t)env.grid[rr * env.w + cc] | ((uint32_t)__popc(here) << 16);
+  };
+  const size_t k = (size_t)e * N + i;
+  const bool alive = st.alive[k] != 0;
+  const float la = alive ? (float)st.last_act[k] : 0.f;
+  const float ri = alive ? (float)st.route_id[k] / (float)(env.npath - 1) : 0.f;
+  tj_encode_row<H>(alive, la, ri, cell, W * W, V, env.car_cls, wT, bias, split, x + (size_t)row * H, lane);
 }
 
 // ---------------------------------------------------------------------------
@@ -705,14 +636,6 @@ int launch_encoder_dense(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, 
 
 }  // namespace
 
-#define IC3_DISPATCH_H(Hval, CALL)          \
-  switch (Hval) {                           \
-    case 32: { constexpr int HH = 32; return CALL; }   \
-    case 64: { constexpr int HH = 64; return CALL; }   \
-    case 128: { constexpr int HH = 128; return CALL; } \
-    default: return IC3_E_UNSUPPORTED;      \
-  }
-
 extern "C" int ic3_policy_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p,
                                const ic3_policy_packed* out, void* stream) {
   int rc = policy_check(cfg);
@@ -740,6 +663,11 @@ extern "C" int ic3_policy_pack(const ic3_policy_cfg* cfg, const ic3_policy_param
 }
 
 extern "C" uint64_t ic3_policy_workspace_bytes(const ic3_policy_cfg* cfg) { return ic3_tc_workspace_bytes(cfg); }
+
+int ic3_encoder_check(const ic3_policy_cfg* cfg, const ic3_policy_packed* w) {
+  const int rc = policy_check(cfg);
+  return rc ? rc : packed_check(w);
+}
 
 // the layout hint, when given, must be the environment's own
 int ic3_pp_layout_check(const ic3_pp_cfg* env, const ic3_policy_cfg* cfg) {

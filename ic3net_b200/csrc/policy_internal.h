@@ -1,4 +1,5 @@
-// Internal (non-ABI) entry points of the tensor-core policy path, called from policy.cu.
+// Internal (non-ABI) entry points of the tensor-core policy path, called from policy.cu, and the policy argument
+// checks shared with the fused observation + encoder entry points (pp_env.cu, tj_env.cu).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -7,6 +8,17 @@
 uint64_t ic3_tc_workspace_bytes(const ic3_policy_cfg* cfg);
 int ic3_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3_policy_packed* out, cudaStream_t s);
 int ic3_tc_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, cudaStream_t s);
+// return CALL with the compile-time hid_size HH = Hval (32 | 64 | 128)
+#define IC3_DISPATCH_H(Hval, CALL)          \
+  switch (Hval) {                           \
+    case 32: { constexpr int HH = 32; return CALL; }   \
+    case 64: { constexpr int HH = 64; return CALL; }   \
+    case 128: { constexpr int HH = 128; return CALL; } \
+    default: return IC3_E_UNSUPPORTED;      \
+  }
+
+// policy configuration and packed weights as every encoder entry point checks them
+int ic3_encoder_check(const ic3_policy_cfg* cfg, const ic3_policy_packed* w);
 // layout hint of ic3_policy_cfg vs the environment (IC3_OK when no hint is given)
 int ic3_pp_layout_check(const ic3_pp_cfg* env, const ic3_policy_cfg* cfg);
 int ic3_tj_layout_check(const ic3_tj_cfg* env, const ic3_policy_cfg* cfg);

@@ -6,7 +6,9 @@
 // [N * W*W cells][V] floats, contiguous, written once with 16-byte evict-first stores.
 #include <cstring>
 
+#include "encoder_rows.cuh"
 #include "ic3_common.cuh"
+#include "policy_internal.h"
 #include "rollout_tail.cuh"
 
 namespace {
@@ -214,6 +216,34 @@ __global__ void pp_step_kernel(PPArgs a, const int32_t* __restrict__ act, int ac
   pp_write_obs<VEC4>(a.cfg, s_r, s_c, s_cell, obs + (size_t)e * NA * W * W * (D * D + 4), keep_l2 != 0);
 }
 
+// _get_obs + _flatten_obs + encoder (comm.py:119) in one pass: the observation block of the env is written exactly
+// as pp_step_kernel writes it, and x = W_e.obs + b of the env's agent rows is summed from the same per-cell records
+// (warp per row, pp_encode_row) -- the block is never read back.  One CTA per env.
+template <int H, bool VEC4>
+__global__ void __launch_bounds__(256) pp_obs_encode_kernel(PPArgs a, float* __restrict__ obs,
+                                                            const float* __restrict__ wT, const float* __restrict__ bias,
+                                                            float* __restrict__ x, bool split, int keep_l2) {
+  ic3_pdl_trigger();
+  ic3_pdl_wait();      // the state comes from the env step launched before; x is read by the policy step after
+  extern __shared__ uint32_t s_cell[];
+  __shared__ int s_r[IC3_MAX_AGENTS + 1], s_c[IC3_MAX_AGENTS + 1];
+  const int N = a.cfg.N, D = a.cfg.dim, W = 2 * a.cfg.vision + 1, WW = W * W, V = D * D + 4;
+  const int NA = ic3_pp_agents(a.cfg);
+  const int e = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x <= N) {
+    const int* l = a.st.loc + ((size_t)e * (N + 1) + threadIdx.x) * 2;
+    s_r[threadIdx.x] = l[0];
+    s_c[threadIdx.x] = l[1];
+  }
+  __syncthreads();
+  pp_write_obs<VEC4>(a.cfg, s_r, s_c, s_cell, obs + (size_t)e * NA * WW * V, keep_l2 != 0);
+  // s_cell: the records of all NA * WW window cells (complete: pp_write_obs synchronised after building them)
+  for (int i = warp; i < NA; i += blockDim.x >> 5) {
+    const uint32_t* rec = s_cell + i * WW;
+    pp_encode_row<H>([rec](int w) { return rec[w]; }, WW, V, wT, bias, split, x + ((size_t)e * NA + i) * H, lane);
+  }
+}
+
 int pp_check(const ic3_pp_cfg* cfg, const ic3_pp_state* st) {
   if (!cfg || !st) return IC3_E_NULL;
   if (!st->loc || !st->reached || !st->done || !st->success || !st->episode || !st->tick) return IC3_E_NULL;
@@ -248,6 +278,27 @@ int pp_launch(const ic3_pp_cfg* cfg, const ic3_pp_state* st, const int32_t* act,
   return IC3_OK;
 }
 
+template <int H>
+int pp_obs_encode_launch(const ic3_pp_cfg* cfg, const ic3_pp_state* st, const ic3_policy_cfg* pcfg,
+                         const ic3_policy_packed* w, float* obs, float* x, cudaStream_t s) {
+  PPArgs a{*cfg, *st};
+  const int W = 2 * cfg->vision + 1, V = cfg->dim * cfg->dim + 4, NA = ic3_pp_agents(*cfg);
+  const size_t smem = (size_t)NA * W * W * sizeof(uint32_t);
+  const bool vec4 = (V % 4 == 0) && ((reinterpret_cast<uintptr_t>(obs) & 15) == 0);
+  const bool split = pcfg->obs_vocab > 0;
+  // same store policy as ic3_pp_obs (IC3_OBS_L2_KEEP_BYTES), so a caller that reads small batches back hits L2
+  const int keep = (size_t)cfg->B * NA * W * W * V * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
+  const float* wT = w->enc_wT;
+  const float* b = w->enc_b;
+  if (vec4)
+    IC3_LAUNCH_RC(ic3_launch_pdl(pp_obs_encode_kernel<H, true>, dim3(cfg->B), dim3(256), smem, s, a, obs, wT, b, x, split,
+                                 keep));
+  else
+    IC3_LAUNCH_RC(ic3_launch_pdl(pp_obs_encode_kernel<H, false>, dim3(cfg->B), dim3(256), smem, s, a, obs, wT, b, x, split,
+                                 keep));
+  return IC3_OK;
+}
+
 }  // namespace
 
 extern "C" int ic3_pp_reset(const ic3_pp_cfg* cfg, const ic3_pp_state* st, const uint8_t* mask,
@@ -279,4 +330,19 @@ extern "C" int ic3_pp_obs(const ic3_pp_cfg* cfg, const ic3_pp_state* st, float* 
   if (rc) return rc;
   if (!obs) return IC3_E_NULL;
   return pp_launch(cfg, st, nullptr, 0, nullptr, obs, nullptr, nullptr, 0, (cudaStream_t)stream);
+}
+
+extern "C" int ic3_pp_obs_encode(const ic3_pp_cfg* env, const ic3_pp_state* st, const ic3_policy_cfg* cfg,
+                                 const ic3_policy_packed* w, float* obs, float* x, void* stream) {
+  int rc = pp_check(env, st);
+  if (rc) return rc;
+  rc = ic3_encoder_check(cfg, w);
+  if (rc) return rc;
+  if (!obs || !x) return IC3_E_NULL;
+  if (env->B != cfg->B || ic3_pp_agents(*env) != cfg->N) return IC3_E_RANGE;
+  const int W = 2 * env->vision + 1;
+  if (cfg->O != W * W * (env->dim * env->dim + 4)) return IC3_E_RANGE;
+  rc = ic3_pp_layout_check(env, cfg);
+  if (rc) return rc;
+  IC3_DISPATCH_H(cfg->H, pp_obs_encode_launch<HH>(env, st, cfg, w, obs, x, (cudaStream_t)stream));
 }

@@ -7,7 +7,9 @@
 // Static tables (road-id grid, routes) are read-only device arrays built once on host.
 #include <cstring>
 
+#include "encoder_rows.cuh"
 #include "ic3_common.cuh"
+#include "policy_internal.h"
 #include "rollout_tail.cuh"
 
 namespace {
@@ -244,6 +246,42 @@ __global__ void tj_step_kernel(TJArgs a, const int32_t* __restrict__ act, int ac
   tj_write_obs(cfg, s_r, s_c, s_alive, s_rid, s_lact, s_cell, obs + (size_t)e * N * (2 + W * W * cfg.vocab), keep_l2 != 0);
 }
 
+// _get_obs + _flatten_obs + encoder (comm.py:119) in one pass: the observation block of the env is written exactly
+// as tj_step_kernel writes it, and x = W_e.obs + b of the env's cars is summed from the same per-cell records and
+// scalars (warp per row, tj_encode_row) -- the block is never read back.  One CTA per env.
+template <int H>
+__global__ void __launch_bounds__(128) tj_obs_encode_kernel(TJArgs a, float* __restrict__ obs,
+                                                            const float* __restrict__ wT, const float* __restrict__ bias,
+                                                            float* __restrict__ x, bool split, int keep_l2) {
+  ic3_pdl_trigger();
+  ic3_pdl_wait();      // the state comes from the env step launched before; x is read by the policy step after
+  extern __shared__ uint32_t s_cell[];
+  __shared__ int s_r[IC3_MAX_AGENTS], s_c[IC3_MAX_AGENTS], s_alive[IC3_MAX_AGENTS], s_rid[IC3_MAX_AGENTS],
+      s_lact[IC3_MAX_AGENTS];
+  const ic3_tj_cfg& cfg = a.cfg;
+  const int N = cfg.N, W = 2 * cfg.vision + 1, WW = W * W, V = cfg.vocab;
+  const int e = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (threadIdx.x < N) {
+    const size_t i = (size_t)e * N + threadIdx.x;
+    s_r[threadIdx.x] = a.st.loc[i * 2];
+    s_c[threadIdx.x] = a.st.loc[i * 2 + 1];
+    s_alive[threadIdx.x] = a.st.alive[i];
+    s_rid[threadIdx.x] = a.st.route_id[i];
+    s_lact[threadIdx.x] = a.st.last_act[i];
+  }
+  __syncthreads();
+  tj_write_obs(cfg, s_r, s_c, s_alive, s_rid, s_lact, s_cell, obs + (size_t)e * N * (2 + WW * V), keep_l2 != 0);
+  // s_cell: the records of all N * WW window cells (complete: tj_write_obs synchronised after building them)
+  for (int i = warp; i < N; i += blockDim.x >> 5) {
+    const uint32_t* rec = s_cell + i * WW;
+    const bool alive = s_alive[i] != 0;
+    const float la = alive ? (float)s_lact[i] : 0.f;
+    const float ri = alive ? (float)s_rid[i] / (float)(cfg.npath - 1) : 0.f;
+    tj_encode_row<H>(alive, la, ri, [rec](int w) { return rec[w]; }, WW, V, cfg.car_cls, wT, bias, split,
+                     x + ((size_t)e * N + i) * H, lane);
+  }
+}
+
 int tj_check(const ic3_tj_cfg* cfg, const ic3_tj_state* st) {
   if (!cfg || !st) return IC3_E_NULL;
   if (!st->loc || !st->alive || !st->wait || !st->route_id || !st->route_pos || !st->last_act ||
@@ -270,6 +308,20 @@ int tj_launch(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const int32_t* act,
   const int keep = obs && (size_t)cfg->B * cfg->N * (2 + W * W * cfg->vocab) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
   IC3_LAUNCH_RC(ic3_launch_pdl(tj_step_kernel, dim3(grid), dim3(threads), smem, s, a, act, act_stride, draws, reward, obs, err,
                                ro, do_step, keep));
+  return IC3_OK;
+}
+
+template <int H>
+int tj_obs_encode_launch(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const ic3_policy_cfg* pcfg,
+                         const ic3_policy_packed* w, float* obs, float* x, cudaStream_t s) {
+  TJArgs a{*cfg, *st};
+  const int W = 2 * cfg->vision + 1;
+  const size_t smem = (size_t)cfg->N * W * W * sizeof(uint32_t);
+  const bool split = pcfg->obs_vocab > 0;
+  // same store policy as ic3_tj_obs: batches that fit in L2 stay there for the record-for-grad copy of the trainer
+  const int keep = (size_t)cfg->B * cfg->N * (2 + W * W * cfg->vocab) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
+  IC3_LAUNCH_RC(ic3_launch_pdl(tj_obs_encode_kernel<H>, dim3(cfg->B), dim3(128), smem, s, a, obs, (const float*)w->enc_wT,
+                               (const float*)w->enc_b, x, split, keep));
   return IC3_OK;
 }
 
@@ -304,4 +356,19 @@ extern "C" int ic3_tj_obs(const ic3_tj_cfg* cfg, const ic3_tj_state* st, float* 
   if (rc) return rc;
   if (!obs) return IC3_E_NULL;
   return tj_launch(cfg, st, nullptr, 0, nullptr, nullptr, obs, nullptr, nullptr, 0, (cudaStream_t)stream);
+}
+
+extern "C" int ic3_tj_obs_encode(const ic3_tj_cfg* env, const ic3_tj_state* st, const ic3_policy_cfg* cfg,
+                                 const ic3_policy_packed* w, float* obs, float* x, void* stream) {
+  int rc = tj_check(env, st);
+  if (rc) return rc;
+  rc = ic3_encoder_check(cfg, w);
+  if (rc) return rc;
+  if (!obs || !x) return IC3_E_NULL;
+  if (env->B != cfg->B || env->N != cfg->N) return IC3_E_RANGE;
+  const int W = 2 * env->vision + 1;
+  if (cfg->O != 2 + W * W * env->vocab) return IC3_E_RANGE;
+  rc = ic3_tj_layout_check(env, cfg);
+  if (rc) return rc;
+  IC3_DISPATCH_H(cfg->H, tj_obs_encode_launch<HH>(env, st, cfg, w, obs, x, (cudaStream_t)stream));
 }

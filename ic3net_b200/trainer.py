@@ -200,9 +200,8 @@ class Trainer(object):
         key = (B, b['obs'].data_ptr(), b['x'].data_ptr(), cfg.obs_vocab, cfg.seed, cfg.env_id0)
         if getattr(self, '_chunks_key', None) == key:
             return self._chunks
-        # default: ONE chunk.  Chunking trades L2 hits of the encoder for the tails of two extra kernels per chunk; on the
-        # PP hard batch (1.19 GB of observations per step) the tails cost more than the L2 hits save.  Batches that fit in L2 anyway (traffic junction) get the
-        # benefit without chunking: the gather kernel keeps them in L2 by itself (IC3_OBS_L2_KEEP_BYTES).
+        # default: ONE chunk.  Each chunk is one fused gather + encoder launch (ic3_*_obs_encode), which never reads the
+        # observations back, so chunking only adds kernel tails; the option remains for bounding a chunk's footprint.
         mb = float(getattr(self.args, 'obs_chunk_mb', 0) or 0)
         per_env = N * O * 4
         nchunk = max(1, -(-B * per_env // int(mb * (1 << 20)))) if mb > 0 else 1
@@ -285,13 +284,12 @@ class Trainer(object):
                     b['ck_h'][t // self.grad_window].copy_(b['h'])
                     b['ck_c'][t // self.grad_window].copy_(b['c'])
             if dense:
-                # gather + encode, optionally in chunks of env slots (args.obs_chunk_mb; default one chunk, see
-                # _dense_chunks); observation batches that fit in L2 are written with plain stores and the encoder
-                # reads them from L2 instead of HBM
-                obs_fn = lib.ic3_tj_obs if self.is_tj else lib.ic3_pp_obs
+                # gather + encode in one kernel per chunk of env slots (args.obs_chunk_mb; default one chunk, see
+                # _dense_chunks): the observation block is written in full and x is summed from the same per-cell
+                # records, so the block is never read back
+                obs_enc = lib.ic3_tj_obs_encode if self.is_tj else lib.ic3_pp_obs_encode
                 for ecfg, est, ccfg, o_ptr, x_ptr in self._dense_chunks(cfg):
-                    _lib.check(obs_fn(C.byref(ecfg), C.byref(est), o_ptr, s))
-                    _lib.check(lib.ic3_encoder_dense(C.byref(ccfg), C.byref(w), o_ptr, x_ptr, s))
+                    _lib.check(obs_enc(C.byref(ecfg), C.byref(est), C.byref(ccfg), C.byref(w), o_ptr, x_ptr, s))
                 if rec and self.is_tj:
                     b['s_obs'][t].copy_(b['obs'])
             elif fused_x:

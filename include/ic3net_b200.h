@@ -306,6 +306,14 @@ int ic3_pp_encoder_index(const ic3_pp_cfg* env, const ic3_pp_state* st, const ic
                          const ic3_policy_packed* w, float* x, void* stream);
 int ic3_tj_encoder_index(const ic3_tj_cfg* env, const ic3_tj_state* st, const ic3_policy_cfg* cfg,
                          const ic3_policy_packed* w, float* x, void* stream);
+/* _get_obs + _flatten_obs + encoder in one kernel (predator_prey_env.py:188-210 / traffic_junction_env.py:321-366,
+ * env_wrappers.py:88-100, comm.py:119): writes obs exactly as ic3_pp_obs / ic3_tj_obs do and x bit-identical to
+ * ic3_encoder_dense(cfg, w, obs), without reading obs back.  obs: [B, N, O], x: [B*N, H]; same argument rules as
+ * ic3_pp_encoder_index / ic3_tj_encoder_index. */
+int ic3_pp_obs_encode(const ic3_pp_cfg* env, const ic3_pp_state* st, const ic3_policy_cfg* cfg,
+                      const ic3_policy_packed* w, float* obs, float* x, void* stream);
+int ic3_tj_obs_encode(const ic3_tj_cfg* env, const ic3_tj_state* st, const ic3_policy_cfg* cfg,
+                      const ic3_policy_packed* w, float* obs, float* x, void* stream);
 /* Class part of the encoder sum per agent position: table[(r*D + c)*H + n] = b[n] + sum over the window cells
  * (row-major) of W_e[n, cell*V + class(cell)] -- the one-hot grid of predator_prey_env.py:176-186 /
  * traffic_junction_env.py:300-319 depends on the position alone.  Rebuild after every weight update.
