@@ -100,7 +100,9 @@ def window_backward(P, G, spec, rec, t0, t1, h0, c0, adv, ret, dh_in=None, dc_in
 
     P: parameters by state_dict name (``heads.m.weight/bias`` for m < nheads);  rec: dict with ``fresh [T,B]``,
     ``comm [T,B,N]``, ``alive [T,B,N]`` (inputs of each policy step), ``t_ep [T,B]``, ``action [T,B,N,nheads]``,
-    ``alive_post [T,B,N]`` and ``obs`` = callable t -> dense [R,O] or (index, value);  adv, ret: [T,B,N];
+    ``alive_post [T,B,N]`` and ``obs`` = callable t -> dense [R,O] or (index, value); optionally ``valid [T,B]`` and
+    the rollout's recorded ``value [T,R]`` / ``logp [T,B,N,sum of head sizes]``, from which the heads' backward then
+    starts instead of re-evaluating the heads on h' (the BPTT kernels read them that way);  adv, ret: [T,B,N];
     (h0, c0): state entering step t0;  (dh_in, dc_in): d loss / d (h', c') of step t1-1 coming from later steps.
     Returns (d loss / d h0, d loss / d c0, stats dict of python floats)."""
     N, H = spec.N, spec.H
@@ -129,8 +131,11 @@ def window_backward(P, G, spec, rec, t0, t1, h0, c0, adv, ret, dh_in=None, dc_in
             alive_post = rec["alive_post"][t].to(dt).reshape(R)
             A, Rt = adv[t].reshape(R).to(dt), ret[t].reshape(R).to(dt)
             act = rec["action"][t].long().reshape(R, -1)
-            # value head
-            value = (h2 @ P["value_head.weight"].t() + P["value_head.bias"])[:, 0]
+            # value head (from the rollout's recorded outputs when given, as the BPTT kernels read them)
+            if "value" in rec:
+                value = rec["value"][t].reshape(R).to(dt)
+            else:
+                value = (h2 @ P["value_head.weight"].t() + P["value_head.bias"])[:, 0]
             dv = 2.0 * spec.value_coeff * alive_post * (value - Rt)
             v_l += (((value - Rt) ** 2) * alive_post).sum()
             G["value_head.weight"] += (dv.unsqueeze(1) * h2).sum(0, keepdim=True)
@@ -140,9 +145,14 @@ def window_backward(P, G, spec, rec, t0, t1, h0, c0, adv, ret, dh_in=None, dc_in
             lp_taken = torch.zeros(R, dtype=dt, device=h.device)
             # slots that already completed their batch (trainer.py:231) contribute nothing, not even entropy
             vrow = rec["valid"][t].to(dt).repeat_interleave(N).unsqueeze(1) if "valid" in rec else 1.0
+            off = 0
             for m in range(spec.nheads):
                 Wm, bm = P["heads.%d.weight" % m], P["heads.%d.bias" % m]
-                logp = torch.log_softmax(h2 @ Wm.t() + bm, dim=-1)
+                if "logp" in rec:
+                    logp = rec["logp"][t].reshape(R, -1)[:, off:off + Wm.shape[0]].to(dt)
+                else:
+                    logp = torch.log_softmax(h2 @ Wm.t() + bm, dim=-1)
+                off += Wm.shape[0]
                 pm = logp.exp()
                 am = act[:, m:m + 1]
                 lp_taken += logp.gather(-1, am).squeeze(-1)

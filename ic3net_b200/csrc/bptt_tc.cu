@@ -789,61 +789,75 @@ __global__ void bptt_finish_lstm_kernel(FinishArgs f) {
   if (idx < TC_H * TC_H) f.g_c_w[idx] += (float)f.dC[idx];     // [k][m]
 }
 
-// encoder / comm-bias / heads gradients
+// encoder window-cell features per update: W^2 cells x V classes (+ the two TJ scalars)
+__host__ __device__ inline int finish_enc_items(const FinishArgs& f) {
+  const int W = f.is_tj ? 2 * f.tj.vision + 1 : 2 * f.pp.vision + 1;
+  return W * W * (f.is_tj ? f.tj.vocab : f.pp.dim * f.pp.dim + 4) + (f.is_tj ? 2 : 0);
+}
+
+// encoder / comm-bias gradients.  Thread = (encoder feature, hidden unit k).  Each feature column of the encoder
+// weight [H][O] is written by exactly one thread, which adds up the P columns that feed it (position one-hot columns
+// whose window cell holds that class, count and scalar columns) in a fixed order: no atomics, so the gradient is
+// bit-identical from run to run.
 __global__ void bptt_finish_misc_kernel(FinishArgs f) {
-  const int ones_col = f.ones_col;
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const int k = idx & 127;
+  const double* Yk = f.Y + (size_t)k * f.np;
   if (idx < TC_H) {
-    const double y1 = f.Y[(size_t)k * f.np + ones_col];
+    const double y1 = Yk[f.ones_col];
     f.g_c_b[k] += (float)y1;                   // W_ih^T g1
     f.g_enc_b[k] += (float)y1;
   }
-  // encoder weight [H][O]: position one-hot columns -> every window cell's class feature of that position
   const int W = f.is_tj ? 2 * f.tj.vision + 1 : 2 * f.pp.vision + 1;
   const int WW = W * W;
+  const int V = f.is_tj ? f.tj.vocab : f.pp.dim * f.pp.dim + 4;
   const int item = idx >> 7;
-  if (item < f.npos * WW) {
-    const int pos = item / WW, w = item - pos * WW;
-    const int dy = w / W, dx = w - dy * W;
-    int feat;
-    if (!f.is_tj) {
-      const int D = f.pp.dim, v = f.pp.vision, V = D * D + 4;
-      const int rr = pos / D - v + dy, cc = pos % D - v + dx;
-      feat = (rr >= 0 && rr < D && cc >= 0 && cc < D) ? w * V + rr * D + cc : w * V + V - 3;
-    } else {
-      const int v = f.tj.vision, V = f.tj.vocab;
+  if (item >= finish_enc_items(f)) return;
+  if (item >= WW * V) {                        // TJ scalars: last_act; route id ratio (hi + lo columns)
+    if (item == WW * V) f.g_enc_w[(size_t)k * f.O] += (float)Yk[f.npos + WW];
+    else f.g_enc_w[(size_t)k * f.O + 1] += (float)(Yk[f.npos + WW + 1] + Yk[f.npos + WW + 2]);
+    return;
+  }
+  const int w = item / V, c = item - w * V;    // window cell w, class c
+  const int dy = w / W, dx = w - dy * W;
+  double y = 0.0;
+  bool fed = false;
+  if (!f.is_tj) {
+    const int D = f.pp.dim, v = f.pp.vision;
+    if (c < D * D) {                           // a grid cell: the one position whose window cell w it is
+      const int pr = c / D + v - dy, pc = c % D + v - dx;
+      if (pr >= 0 && pr < D && pc >= 0 && pc < D) {
+        y = Yk[pr * D + pc];
+        fed = true;
+      }
+    } else if (c == V - 3) {                   // outside the grid: every position whose window cell w leaves it
+      for (int pos = 0; pos < f.npos; ++pos) {
+        const int rr = pos / D - v + dy, cc = pos % D - v + dx;
+        if (rr < 0 || rr >= D || cc < 0 || cc >= D) {
+          y += Yk[pos];
+          fed = true;
+        }
+      }
+    } else if (c >= V - 2) {                   // prey (V - 2) / predator (V - 1) count of window cell w
+      y = Yk[f.npos + 2 * w + (c == V - 1 ? 1 : 0)];
+      fed = true;
+    }
+  } else {
+    const int v = f.tj.vision;
+    for (int pos = 0; pos < f.npos; ++pos) {   // every position whose window cell w holds class c
       const int rr = pos / f.tj.w - v + dy, cc = pos % f.tj.w - v + dx;
-      int cls = f.tj.outside_cls;
-      if (rr >= 0 && rr < f.tj.h && cc >= 0 && cc < f.tj.w) cls = f.tj.grid[rr * f.tj.w + cc];
-      feat = 2 + w * V + cls;
+      const int cls = (rr >= 0 && rr < f.tj.h && cc >= 0 && cc < f.tj.w) ? f.tj.grid[rr * f.tj.w + cc] : f.tj.outside_cls;
+      if (cls == c) {
+        y += Yk[pos];
+        fed = true;
+      }
     }
-    atomicAdd(&f.g_enc_w[(size_t)k * f.O + feat], (float)f.Y[(size_t)k * f.np + pos]);
-  }
-  // count / scalar feature columns
-  const int nextra = f.is_tj ? WW + 3 : 2 * WW;
-  if (item < nextra) {
-    int feat;
-    double y;
-    if (!f.is_tj) {
-      const int V = f.pp.dim * f.pp.dim + 4;
-      const int w = item >> 1;
-      feat = w * V + ((item & 1) ? V - 1 : V - 2);          // predator : prey count
-      y = f.Y[(size_t)k * f.np + f.npos + item];
-    } else if (item < WW) {
-      feat = 2 + item * f.tj.vocab + f.tj.car_cls;
-      y = f.Y[(size_t)k * f.np + f.npos + item];
-    } else if (item == WW) {
-      feat = 0;                                               // last_act
-      y = f.Y[(size_t)k * f.np + f.npos + WW];
-    } else if (item == WW + 1) {
-      feat = 1;                                               // route id ratio: hi + lo columns
-      y = f.Y[(size_t)k * f.np + f.npos + WW + 1] + f.Y[(size_t)k * f.np + f.npos + WW + 2];
-    } else {
-      return;
+    if (c == f.tj.car_cls) {                   // car count of window cell w
+      y += Yk[f.npos + w];
+      fed = true;
     }
-    atomicAdd(&f.g_enc_w[(size_t)k * f.O + feat], (float)y);
   }
+  if (fed) f.g_enc_w[(size_t)k * f.O + (f.is_tj ? 2 : 0) + w * V + c] += (float)y;
 }
 
 __global__ void bptt_finish_heads_kernel(FinishArgs f) {
@@ -1466,8 +1480,7 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
   f.ones_col = npos + (is_tj ? WW + 3 : 2 * WW);     // the constant column of P is its last used column
   bptt_finish_lstm_kernel<<<(512 * TC_H + 255) / 256, 256, 0, s>>>(f);
   IC3_LAUNCH_CHECK();
-  const int items = npos * WW > (is_tj ? WW + 3 : 2 * WW) ? npos * WW : (is_tj ? WW + 3 : 2 * WW);
-  bptt_finish_misc_kernel<<<(items * 128 + 255) / 256, 256, 0, s>>>(f);
+  bptt_finish_misc_kernel<<<(finish_enc_items(f) * 128 + 255) / 256, 256, 0, s>>>(f);
   IC3_LAUNCH_CHECK();
   bptt_finish_heads_kernel<<<(BP_HEADS * TC_H + 255) / 256, 256, 0, s>>>(f);
   IC3_LAUNCH_CHECK();

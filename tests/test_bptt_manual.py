@@ -113,6 +113,39 @@ def test_manual_backward_matches_autograd_oracle(name):
                 assert np.allclose(G[key].numpy(), v, rtol=1e-8, atol=1e-10), (key, W)
 
 
+@pytest.mark.parametrize("name", golden_names("grad_"))
+def test_one_step_windows_from_recorded_states_equal_one_window(name):
+    """The float64 reference of the BPTT kernel tests (tests/bptt_ref.py) runs one-step windows, each started from the
+    recorded state entering its step, with (dh, dc) chained from the step after.  Given the exact per-step states
+    this is the same backward as one window over the whole batch (detach cuts, episode starts, chained gradients)."""
+    from bptt_ref import chain_one_step
+    meta, _ = load_golden(name)
+    T = 2 * meta["args"]["max_steps"] + 7
+    meta, args, p, rec, adv, ret, want, wstat = _lockstep_records(name, B=3, T=T)
+    G1, tot1 = _run_manual(args, meta, p, rec, adv, ret, T)
+    N, H = args.nagents, args.hid_size
+    B = rec["fresh"].shape[1]
+    P = {k: torch.tensor(v, dtype=torch.float64) for k, v in p.items()}
+    G = {k: torch.zeros_like(v) for k, v in P.items()}
+    spec = bptt.Spec(N, H, len(meta["heads"]), bool(args.hard_attn) and bool(args.commnet),
+                     getattr(args, "comm_mode", "avg") == "avg", bool(args.comm_mask_zero), args.value_coeff, args.entr,
+                     args.detach_gap, args.max_steps)
+    tobs = torch.tensor(rec["obs"]).reshape(T, B * N, -1)
+    R = dict(fresh=torch.tensor(rec["fresh"]), comm=torch.tensor(rec["comm"]), alive=torch.tensor(rec["alive"]),
+             t_ep=torch.tensor(rec["t_ep"]), action=torch.tensor(rec["action"]),
+             alive_post=torch.tensor(rec["alive_post"]), obs=lambda t: tobs[t])
+    states = [(torch.zeros(B * N, H, dtype=torch.float64), torch.zeros(B * N, H, dtype=torch.float64))]
+    for t in range(T - 1):              # the state entering every step, as the kernel trainer records it (rec_h, rec_c)
+        h, c, _ = bptt._forward(P, spec, R, t, *states[-1])
+        states.append((h, c))
+    tot = chain_one_step(P, G, spec, R, lambda t: states[t], torch.tensor(adv), torch.tensor(ret))
+    for q in tot:
+        assert np.isclose(tot[q], tot1[q], rtol=1e-12, atol=1e-12), (q, tot[q], tot1[q])
+    for key in G:
+        scale = max(float(G1[key].abs().max()), 1e-300)
+        assert float((G[key] - G1[key]).abs().max()) <= 1e-12 * scale, key
+
+
 def test_sparse_observation_path_equals_dense():
     meta, args, p, rec, adv, ret, want, _ = _lockstep_records("grad_pp_easy_ic3net", B=2, T=25)
     Gd, _ = _run_manual(args, meta, p, rec, adv, ret, 10)

@@ -6,11 +6,11 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import finish_args, golden_names, load_golden, make_oracle_env, ns, tj_tables
+from bptt_ref import oracle_grad_sum
+from helpers import finish_args, golden_names, load_golden, ns
 from oracle import grad as ograd
 from oracle import policy as opolicy
 from oracle.gen_golden import make_weights
-from oracle.rollout import run_episode
 
 pytestmark = pytest.mark.gpu
 
@@ -61,27 +61,9 @@ def test_compute_grad_matches_oracle(name, impl, grad_impl):
     assert quota == args.batch_size
     tr.optimizer.zero_grad(set_to_none=False)
     s = tr.compute_grad(batch)
-    act = cpu(batch.action)
-    valid = cpu(batch.valid)
     # ---- oracle: every slot is one reference process ----
     p = opolicy.params_to_f64(sd)
-    is_tj = args.env_name == "traffic_junction"
-    want, wstat = None, dict(action_loss=0.0, value_loss=0.0, entropy=0.0)
-    nsteps_total = 0
-    for b in range(B):
-        orc = make_oracle_env(args, tj_tables(z) if is_tj else None)
-        eps, t0, k = [], 0, 0
-        while t0 < quota:                    # trainer.py:231: whole episodes until the slot holds >= batch_size steps
-            ep = run_episode(orc, p, args, seed, id0 + b, epoch=0, tick0=t0, episode=k, forced_actions=act[t0:, b])
-            eps.append(ep)
-            t0 += ep["num_steps"]
-            k += 1
-        assert t0 <= T and valid[:t0, b].all() and not valid[t0:, b].any(), (b, t0)
-        nsteps_total += t0
-        g, st, _ = ograd.compute_grad(p, eps, args)
-        want = g if want is None else {q: (want[q] + g[q] if g[q] is not None else None) for q in g}
-        for q in wstat:
-            wstat[q] += st[q]
+    want, wstat, nsteps_total = oracle_grad_sum(args, z, p, cpu(batch.action), cpu(batch.valid), seed, id0, quota, T)
     for q in wstat:
         assert np.isclose(s[q], wstat[q], rtol=2e-4, atol=1e-3), (q, s[q], wstat[q])
     assert stat["num_steps"] == nsteps_total
