@@ -115,10 +115,12 @@ SYMBOLS = {
     "ic3_pp_step": (C.c_int, [C.POINTER(PPCfg), C.POINTER(PPState), _PTR, C.c_int32, _PTR, _PTR, _PTR,
                               C.POINTER(RolloutIO), _PTR]),
     "ic3_pp_obs": (C.c_int, [C.POINTER(PPCfg), C.POINTER(PPState), _PTR, _PTR]),
+    "ic3_pp_obs_bounded": (C.c_int, [C.POINTER(PPCfg), C.POINTER(PPState), _PTR, _PTR]),
     "ic3_tj_reset": (C.c_int, [C.POINTER(TJCfg), C.POINTER(TJState), _PTR, _PTR, _PTR]),
     "ic3_tj_step": (C.c_int, [C.POINTER(TJCfg), C.POINTER(TJState), _PTR, C.c_int32, _PTR, _PTR, _PTR, _PTR,
                               C.POINTER(RolloutIO), _PTR]),
     "ic3_tj_obs": (C.c_int, [C.POINTER(TJCfg), C.POINTER(TJState), _PTR, _PTR]),
+    "ic3_tj_obs_bounded": (C.c_int, [C.POINTER(TJCfg), C.POINTER(TJState), _PTR, _PTR]),
     "ic3_policy_pack": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyParams), C.POINTER(PolicyPacked), _PTR]),
     "ic3_encoder_dense": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), _PTR, _PTR, _PTR]),
     "ic3_pp_encoder_index": (C.c_int, [C.POINTER(PPCfg), C.POINTER(PPState), C.POINTER(PolicyCfg),

@@ -7,6 +7,11 @@
 
 #define IC3_FULL_MASK 0xffffffffu
 #define IC3_ENV_WARPS 8      // envs per CTA of an env step launched without an observation block (warp = env)
+// persistent observation writers (ic3_pp_obs_bounded / ic3_tj_obs_bounded): one 256-thread CTA per SM at <= 64
+// registers writes the predator-prey hard block at 3.0 TB/s on its own (H100 SXM, 700 W); CTAs of 2 or 3 warps fit beside
+// a resident LSTM CTA but slow it several-fold, which costs more than the overlap gains
+#define IC3_OBS_WRITER_THREADS 256
+#define IC3_OBS_WRITER_MIN_CTAS (65536 / (IC3_OBS_WRITER_THREADS * 64))
 
 // predator-prey: agent rows per environment (the prey is row N with --enemy_comm, predator_prey_env.py:203-207)
 __host__ __device__ __forceinline__ int ic3_pp_agents(const ic3_pp_cfg& c) { return c.N + (c.enemy_comm != 0 ? 1 : 0); }

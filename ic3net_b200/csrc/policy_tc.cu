@@ -20,10 +20,66 @@
 //                 producer, warps 0-7 = two warpgroups of 64 rows each issuing wgmma 64 x 256 x 16 into
 //                 registers, then the LSTM cell -> c', h' and the partial head logits.
 //   heads kernel  value / action heads + sampling from h' (thread per row, from the partial logits).
+#include <algorithm>
+
 #include "policy_tc_kernels.cuh"
 
 
 constexpr int TC_TILE_PAD = 8;   // tiles are padded to a multiple of 8 (operand image and workspace layout)
+// dynamic shared memory of lstm_tc_kernel: the ring, its barriers, head weights, bias
+constexpr size_t LSTM_SMEM_BYTES = NSTAGE_P * STAGE_BYTES + 256 + TC_H * HEAD_PAD * sizeof(float) + 4 * TC_H * sizeof(float);
+
+// CTAs of kern per SM that fit beside one lstm_tc_kernel CTA, counting registers, shared memory, threads and CTA slots
+// of the SM (at least 1).  The register file is split into four quadrants, which this count does not model: on an
+// H100, an LSTM CTA (9 warps x 168 registers, three of them in one quadrant) was measured to start on an SM only once
+// a resident 8-warp writer CTA there has retired.  The writer therefore overlaps the operand preparation, heads and env
+// step of the policy step more than the LSTM kernel itself.
+static int ctas_beside_lstm(const void* kern, int threads, size_t smem, int* per_sm, int* nsm) {
+  cudaFuncAttributes la, ka;
+  cudaError_t e = cudaFuncGetAttributes(&la, lstm_tc_kernel);
+  if (e == cudaSuccess) e = cudaFuncGetAttributes(&ka, kern);
+  int dev = 0, regs = 0, smem_sm = 0, reserved = 0, thr_sm = 0, blk_sm = 0;
+  if (e == cudaSuccess) e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(nsm, cudaDevAttrMultiProcessorCount, dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&regs, cudaDevAttrMaxRegistersPerMultiprocessor, dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&thr_sm, cudaDevAttrMaxThreadsPerMultiProcessor, dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&blk_sm, cudaDevAttrMaxBlocksPerMultiprocessor, dev);
+  if (e != cudaSuccess) return (int)e;
+  // registers are allocated per warp in units of 256
+  auto cta_regs = [](const cudaFuncAttributes& a, int nthr) { return ((a.numRegs * 32 + 255) / 256 * 256) * ((nthr + 31) / 32); };
+  const long free_regs = (long)regs - cta_regs(la, TC_P_THREADS);
+  const long free_smem = (long)smem_sm - (long)(LSTM_SMEM_BYTES + la.sharedSizeBytes + reserved);
+  long n = free_regs / cta_regs(ka, threads);
+  n = std::min(n, free_smem / (long)(smem + ka.sharedSizeBytes + reserved));
+  n = std::min(n, (long)(thr_sm - TC_P_THREADS) / threads);
+  n = std::min(n, (long)blk_sm - 1);
+  *per_sm = n > 1 ? (int)n : 1;
+  return IC3_OK;
+}
+
+int ic3_grid_beside_lstm(const void* kern, int threads, size_t smem, int nwork, int* grid) {
+  struct Entry { const void* kern; int threads; size_t smem; int ctas; };
+  static Entry cache[8];
+  static int ncache = 0;
+  int ctas = 0;
+  for (int i = 0; i < ncache; ++i)
+    if (cache[i].kern == kern && cache[i].threads == threads && cache[i].smem == smem) ctas = cache[i].ctas;
+  if (ctas == 0) {
+    // an SM configured for a kernel that needs little shared memory keeps that L1 / shared split while any of its
+    // CTAs is resident, and the LSTM kernel's 198 KB CTA cannot start there: ask for the largest shared carveout
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+    if (e != cudaSuccess) return (int)e;
+    int per_sm = 0, nsm = 0;
+    const int rc = ctas_beside_lstm(kern, threads, smem, &per_sm, &nsm);
+    if (rc) return rc;
+    ctas = per_sm * nsm;
+    if (ncache < 8) cache[ncache++] = Entry{kern, threads, smem, ctas};
+  }
+  *grid = nwork < ctas ? nwork : ctas;
+  return IC3_OK;
+}
 
 static int launch_lstm(const ic3_policy_cfg* cfg, const ic3_policy_io* io, const ic3_policy_packed* w, const __half* a_img,
                        int ntiles_pad, size_t smem, int nout, float* partial, cudaStream_t s) {
@@ -219,7 +275,7 @@ static int tc_pass(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const 
     return IC3_E_NULL;
   }
   prof_mark(1, s);
-  const size_t smem = NSTAGE_P * STAGE_BYTES + 256 + TC_H * HEAD_PAD * sizeof(float) + 4 * TC_H * sizeof(float);
+  const size_t smem = LSTM_SMEM_BYTES;
   int nout = 1;
   for (int k = 0; k < cfg->nheads; ++k) nout += cfg->head_dim[k];
   const bool fused_heads = nout <= HEAD_PAD;

@@ -244,6 +244,42 @@ __global__ void __launch_bounds__(256) pp_obs_encode_kernel(PPArgs a, float* __r
   }
 }
 
+// The observation block of every env exactly as pp_step_kernel writes it (pp_write_obs, same store policy), no x, from
+// a persistent grid that strides over the envs (ic3_pp_obs_bounded), so the dense rollout can write the observation
+// while the policy step runs (ic3_grid_beside_lstm).  The positions of the next env are loaded while the current block
+// is written.
+template <bool VEC4>
+__global__ void __launch_bounds__(IC3_OBS_WRITER_THREADS, IC3_OBS_WRITER_MIN_CTAS)
+    pp_obs_writer_kernel(PPArgs a, float* __restrict__ obs, int keep_l2) {
+  ic3_pdl_trigger();
+  ic3_pdl_wait();
+  extern __shared__ uint32_t s_cell[];
+  __shared__ int s_r[IC3_MAX_AGENTS + 1], s_c[IC3_MAX_AGENTS + 1];
+  const int N = a.cfg.N, W = 2 * a.cfg.vision + 1, B = a.cfg.B;
+  const size_t per_env = (size_t)ic3_pp_agents(a.cfg) * W * W * (a.cfg.dim * a.cfg.dim + 4);
+  const int k = threadIdx.x;
+  int r = 0, c = 0;
+  if (k <= N && (int)blockIdx.x < B) {
+    const int* l = a.st.loc + ((size_t)blockIdx.x * (N + 1) + k) * 2;
+    r = l[0];
+    c = l[1];
+  }
+  for (int e = blockIdx.x; e < B; e += gridDim.x) {
+    if (k <= N) {
+      s_r[k] = r;
+      s_c[k] = c;
+      if (e + (int)gridDim.x < B) {
+        const int* l = a.st.loc + ((size_t)(e + gridDim.x) * (N + 1) + k) * 2;
+        r = l[0];
+        c = l[1];
+      }
+    }
+    __syncthreads();
+    pp_write_obs<VEC4>(a.cfg, s_r, s_c, s_cell, obs + (size_t)e * per_env, keep_l2 != 0);
+    __syncthreads();      // s_r, s_c and s_cell are rebuilt for the next env
+  }
+}
+
 int pp_check(const ic3_pp_cfg* cfg, const ic3_pp_state* st) {
   if (!cfg || !st) return IC3_E_NULL;
   if (!st->loc || !st->reached || !st->done || !st->success || !st->episode || !st->tick) return IC3_E_NULL;
@@ -299,7 +335,30 @@ int pp_obs_encode_launch(const ic3_pp_cfg* cfg, const ic3_pp_state* st, const ic
   return IC3_OK;
 }
 
+template <bool VEC4>
+int pp_obs_bounded_launch(const ic3_pp_cfg* cfg, const ic3_pp_state* st, float* obs, cudaStream_t s) {
+  PPArgs a{*cfg, *st};
+  const int W = 2 * cfg->vision + 1, V = cfg->dim * cfg->dim + 4, NA = ic3_pp_agents(*cfg);
+  const size_t smem = (size_t)NA * W * W * sizeof(uint32_t);
+  const int keep = (size_t)cfg->B * NA * W * W * V * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;   // as ic3_pp_obs
+  auto kern = pp_obs_writer_kernel<VEC4>;
+  int grid = 0;
+  const int rc = ic3_grid_beside_lstm((const void*)kern, IC3_OBS_WRITER_THREADS, smem, cfg->B, &grid);
+  if (rc) return rc;
+  IC3_LAUNCH_RC(ic3_launch_pdl(kern, dim3(grid), dim3(IC3_OBS_WRITER_THREADS), smem, s, a, obs, keep));
+  return IC3_OK;
+}
+
 }  // namespace
+
+extern "C" int ic3_pp_obs_bounded(const ic3_pp_cfg* cfg, const ic3_pp_state* st, float* obs, void* stream) {
+  int rc = pp_check(cfg, st);
+  if (rc) return rc;
+  if (!obs) return IC3_E_NULL;
+  const bool vec4 = ((cfg->dim * cfg->dim + 4) % 4 == 0) && ((reinterpret_cast<uintptr_t>(obs) & 15) == 0);
+  return vec4 ? pp_obs_bounded_launch<true>(cfg, st, obs, (cudaStream_t)stream)
+              : pp_obs_bounded_launch<false>(cfg, st, obs, (cudaStream_t)stream);
+}
 
 extern "C" int ic3_pp_reset(const ic3_pp_cfg* cfg, const ic3_pp_state* st, const uint8_t* mask,
                             float* obs, void* stream) {

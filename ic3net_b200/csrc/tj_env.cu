@@ -282,6 +282,44 @@ __global__ void __launch_bounds__(128) tj_obs_encode_kernel(TJArgs a, float* __r
   }
 }
 
+// The observation block of every env exactly as tj_step_kernel writes it (tj_write_obs, same store policy), no x, from
+// a persistent grid that strides over the envs (ic3_tj_obs_bounded); see pp_obs_writer_kernel.
+__global__ void __launch_bounds__(IC3_OBS_WRITER_THREADS, IC3_OBS_WRITER_MIN_CTAS)
+    tj_obs_writer_kernel(TJArgs a, float* __restrict__ obs, int keep_l2) {
+  ic3_pdl_trigger();
+  ic3_pdl_wait();
+  extern __shared__ uint32_t s_cell[];
+  __shared__ int s_r[IC3_MAX_AGENTS], s_c[IC3_MAX_AGENTS], s_alive[IC3_MAX_AGENTS], s_rid[IC3_MAX_AGENTS],
+      s_lact[IC3_MAX_AGENTS];
+  const ic3_tj_cfg& cfg = a.cfg;
+  const int N = cfg.N, W = 2 * cfg.vision + 1, B = cfg.B;
+  const size_t per_env = (size_t)N * (2 + W * W * cfg.vocab);
+  const int k = threadIdx.x;
+  int r = 0, c = 0, alive = 0, rid = 0, lact = 0;
+  auto load = [&](int e) {
+    const size_t i = (size_t)e * N + k;
+    r = a.st.loc[i * 2];
+    c = a.st.loc[i * 2 + 1];
+    alive = a.st.alive[i];
+    rid = a.st.route_id[i];
+    lact = a.st.last_act[i];
+  };
+  if (k < N && (int)blockIdx.x < B) load(blockIdx.x);
+  for (int e = blockIdx.x; e < B; e += gridDim.x) {
+    if (k < N) {
+      s_r[k] = r;
+      s_c[k] = c;
+      s_alive[k] = alive;
+      s_rid[k] = rid;
+      s_lact[k] = lact;
+      if (e + (int)gridDim.x < B) load(e + gridDim.x);
+    }
+    __syncthreads();
+    tj_write_obs(cfg, s_r, s_c, s_alive, s_rid, s_lact, s_cell, obs + (size_t)e * per_env, keep_l2 != 0);
+    __syncthreads();      // the per-car arrays and s_cell are rebuilt for the next env
+  }
+}
+
 int tj_check(const ic3_tj_cfg* cfg, const ic3_tj_state* st) {
   if (!cfg || !st) return IC3_E_NULL;
   if (!st->loc || !st->alive || !st->wait || !st->route_id || !st->route_pos || !st->last_act ||
@@ -326,6 +364,22 @@ int tj_obs_encode_launch(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const ic
 }
 
 }  // namespace
+
+extern "C" int ic3_tj_obs_bounded(const ic3_tj_cfg* cfg, const ic3_tj_state* st, float* obs, void* stream) {
+  int rc = tj_check(cfg, st);
+  if (rc) return rc;
+  if (!obs) return IC3_E_NULL;
+  TJArgs a{*cfg, *st};
+  const int W = 2 * cfg->vision + 1;
+  const size_t smem = (size_t)cfg->N * W * W * sizeof(uint32_t);
+  const int keep = (size_t)cfg->B * cfg->N * (2 + W * W * cfg->vocab) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;  // as ic3_tj_obs
+  int grid = 0;
+  rc = ic3_grid_beside_lstm((const void*)tj_obs_writer_kernel, IC3_OBS_WRITER_THREADS, smem, cfg->B, &grid);
+  if (rc) return rc;
+  IC3_LAUNCH_RC(ic3_launch_pdl(tj_obs_writer_kernel, dim3(grid), dim3(IC3_OBS_WRITER_THREADS), smem,
+                               (cudaStream_t)stream, a, obs, keep));
+  return IC3_OK;
+}
 
 extern "C" int ic3_tj_reset(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const uint8_t* mask,
                             float* obs, void* stream) {

@@ -16,6 +16,9 @@ synchronisation:
   encoder (index form from the env state, or obs-gather + dense encoder)
   -> policy step (comm mean, C, LSTM, heads, sampling; wgmma tensor-core or fp32 SIMT kernels)
   -> env step + Trainer.get_episode bookkeeping + auto-reset (ic3_rollout_io).
+Dense observations on the tensor-core path (``_overlap_obs``): the policy step takes x from the env state, and a side
+stream writes the [B, N, O] observation block of the same state concurrently (ic3_*_obs_bounded); the env step waits
+for that write.
 The whole T-step sequence can be captured once into a CUDA graph (``use_graph``).
 
 Gradient (``compute_grad``, trainer.py:128-225; scope row 8(f)-1): returns by a CUDA scan kernel,
@@ -104,6 +107,7 @@ class Trainer(object):
         self._buf = None
         self._graph = None
         self._graph_key = None
+        self._side = None                    # stream of the dense observation writer (_overlap_obs)
         # encoder layout of this environment (class terms / counts summed separately, comm.py set_obs_layout) and
         # the per-position table of the class terms for the fused index encoder, rebuilt when the weights change
         policy_net.set_obs_layout(*getattr(env.env, 'obs_layout', (0, 0, 0)))
@@ -200,8 +204,9 @@ class Trainer(object):
         key = (B, b['obs'].data_ptr(), b['x'].data_ptr(), cfg.obs_vocab, cfg.seed, cfg.env_id0)
         if getattr(self, '_chunks_key', None) == key:
             return self._chunks
-        # default: ONE chunk.  Each chunk is one fused gather + encoder launch (ic3_*_obs_encode), which never reads the
-        # observations back, so chunking only adds kernel tails; the option remains for bounding a chunk's footprint.
+        # default: ONE chunk.  Each chunk is one launch of the fused gather + encoder (ic3_*_obs_encode), which never reads
+        # the observations back, or of the observation writer (_overlap_obs), so chunking only adds kernel tails; the
+        # option remains for bounding a chunk's footprint.
         mb = float(getattr(self.args, 'obs_chunk_mb', 0) or 0)
         per_env = N * O * 4
         nchunk = max(1, -(-B * per_env // int(mb * (1 << 20)))) if mb > 0 else 1
@@ -222,6 +227,25 @@ class Trainer(object):
         W = 2 * self.env.env.vision + 1
         return (not dense) and self.policy_net.policy_impl == 'tc' and W * W <= 25
 
+    # Smaller observation blocks per step keep the fused gather + encoder: their write is short and latency-bound in the
+    # persistent writer (measured on an H100: predator-prey easy, 2.9 MB, 3 % slower with the overlap; traffic-junction
+    # medium, 20 MB, 1 % faster; predator-prey hard, 1.19 GB, 9 % faster).
+    OVERLAP_MIN_OBS_BYTES = 8 << 20
+
+    def _overlap_obs(self):
+        """Dense observations on the tensor-core policy path: the policy step computes x from the env state (the fused
+        index encoder; without the per-position table, which measured no faster beside the writer, so dense mode never
+        builds it) and the observation block is written concurrently on a side stream.  Not when the traffic-junction
+        records copy every step's observation (record_for_grad without the BPTT kernels), nor for blocks smaller than
+        OVERLAP_MIN_OBS_BYTES."""
+        if self.obs_mode != 'dense' or (self.record_for_grad and self.is_tj and not self.grad_kernels):
+            return False
+        e = self.env.env
+        if e.nenvs * self.args.nagents * self.env.observation_dim * 4 < self.OVERLAP_MIN_OBS_BYTES:
+            return False
+        W = 2 * e.vision + 1
+        return self.policy_net.policy_impl == 'tc' and W * W <= 25
+
     def _enqueue(self, T, quota=0):
         """Enqueue T lock-step iterations on the current stream (no host sync).  quota > 0: reference batch
         boundary -- a slot halts at the first episode end with >= quota steps (ic3_rollout_io.batch_size);
@@ -239,13 +263,21 @@ class Trainer(object):
         rec = self.record_for_grad
         gk = rec and self.grad_kernels
         dense = self.obs_mode == 'dense' or (rec and self.is_tj and not gk)
+        # dense observations written on a side stream while the policy step runs (see _overlap_obs)
+        overlap = self._overlap_obs()
         # tensor-core path: the index encoder is fused into the policy step (x never leaves the operand image)
-        fused_x = self._fused_x()
+        fused_x = self._fused_x() or overlap
         src = {}
         if fused_x:
             src = dict(tj_env=C.addressof(e.cfg), tj_state=C.addressof(e.state)) if self.is_tj else \
                 dict(pp_env=C.addressof(e.cfg), pp_state=C.addressof(e.state))
-            src['x_table'] = _lib.ptr(self._encoder_table(cfg, w))
+            src['x_table'] = None if overlap else _lib.ptr(self._encoder_table(cfg, w))
+        if overlap:
+            main = torch.cuda.current_stream()
+            if self._side is None or self._side.device != main.device:
+                self._side = torch.cuda.Stream(device=main.device)
+            side = self._side
+            obs_write = lib.ic3_tj_obs_bounded if self.is_tj else lib.ic3_pp_obs_bounded
         # Option (args.fuse_heads, default off): on the tensor-core path with <= 7 action logits the env step kernel can
         # finish the policy heads (value, log-softmax, sampling) from the LSTM epilogue's partial logits -- one launch
         # less per lock-step iteration, but one 32-thread CTA per env hides the 64 partial-logit loads of a row worse than the
@@ -283,7 +315,13 @@ class Trainer(object):
                 if not gk and t % self.grad_window == 0:
                     b['ck_h'][t // self.grad_window].copy_(b['h'])
                     b['ck_c'][t // self.grad_window].copy_(b['c'])
-            if dense:
+            if overlap:
+                # the writer reads the state the previous env step left and must finish before this step's env step
+                # moves the agents (the join below); one launch per chunk of env slots, as in the branch below
+                side.wait_stream(main)
+                for ecfg, est, _, o_ptr, _ in self._dense_chunks(cfg):
+                    _lib.check(obs_write(C.byref(ecfg), C.byref(est), o_ptr, side.cuda_stream))
+            elif dense:
                 # gather + encode in one kernel per chunk of env slots (args.obs_chunk_mb; default one chunk, see
                 # _dense_chunks): the observation block is written in full and x is summed from the same per-cell
                 # records, so the block is never read back
@@ -311,6 +349,8 @@ class Trainer(object):
             _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
             if fuse_heads:
                 heads_kw.update(head_value=b['value'][t].data_ptr(), head_logp=b['logp'][t].data_ptr())
+            if overlap:
+                main.wait_stream(side)
             r = _lib.RolloutIO(t=t, max_steps=args.max_steps, nheads=nh, hard_attn=hard,
                                comm_action_one=int(bool(args.comm_action_one)),
                                last=int(t == T - 1 and quota <= 0), batch_size=int(quota),

@@ -162,6 +162,9 @@ int ic3_pp_step(const ic3_pp_cfg* cfg, const ic3_pp_state* st, const int32_t* ac
 /* _get_obs + env_wrappers._flatten_obs: predator_prey_env.py:188-210, env_wrappers.py:88-100.
  * obs: [B, N, W*W*V] float32, window-major then class. */
 int ic3_pp_obs(const ic3_pp_cfg* cfg, const ic3_pp_state* st, float* obs, void* stream);
+/* The same obs as ic3_pp_obs, written by a persistent grid small enough to share every SM with the tensor-core policy
+ * step (one CTA of its LSTM kernel per SM), so the two can run concurrently on different streams. */
+int ic3_pp_obs_bounded(const ic3_pp_cfg* cfg, const ic3_pp_state* st, float* obs, void* stream);
 
 /* ------------------------------------------------------------------------
  * Traffic junction  (ic3net_envs/traffic_junction_env.py, traffic_helper.py)
@@ -208,6 +211,8 @@ int ic3_tj_step(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const int32_t* ac
 /* _get_obs + _flatten_obs: traffic_junction_env.py:321-366, env_wrappers.py:88-100.
  * obs: [B, N, 2 + W*W*V] float32. */
 int ic3_tj_obs(const ic3_tj_cfg* cfg, const ic3_tj_state* st, float* obs, void* stream);
+/* The same obs as ic3_tj_obs from a grid that shares every SM with the policy step (see ic3_pp_obs_bounded). */
+int ic3_tj_obs_bounded(const ic3_tj_cfg* cfg, const ic3_tj_state* st, float* obs, void* stream);
 
 /* ------------------------------------------------------------------------
  * CommNet / IC3Net policy step  (comm.py:134-244, action_utils.py:27-36)
