@@ -27,6 +27,14 @@ in windows of ``grad_window`` steps processed last-to-first; (h, c) at every win
 checkpointed during the rollout and the gradient w.r.t. them is handed to the previous window,
 so back-propagation through time is exact (truncated only where the reference truncates it:
 ``detach_gap``, trainer.py:56-60, and episode starts).
+
+With the hand-written BPTT kernels (``grad_impl = 'kernels'``, the default where supported) the backward needs every
+step's (h, c).  ``record_mode == 'full'``: the policy step writes them into ``rec_h / rec_c [T+1, B*N, H]``, 2 (T+1) B N H
+4 bytes (48.7 GB at predator-prey hard, 8192 slots, batch 500).  When those do not fit in the device memory left after
+the other buffers (``RECORD_BYTES_LIMIT``, ``RECORD_MARGIN_BYTES``), ``record_mode == 'window'``: the rollout keeps (h, c)
+only at every ``grad_window``-th step plus max |c| per step, and the backward re-runs the tensor-core policy step over
+one window at a time from its checkpoint into one of two window buffers, just ahead of the BPTT kernels of that window
+(``_recompute_window``).  The recompute is bit-exact, so the gradient equals the full records' bit for bit.
 """
 import ctypes as C
 import math
@@ -105,6 +113,7 @@ class Trainer(object):
         self.grad_kernels = False
         self._bptt = None
         self._buf = None
+        self._record_mode = None             # 'full' | 'window' per allocation (record_mode)
         self._graph = None
         self._graph_key = None
         self._side = None                    # stream of the dense observation writer (_overlap_obs)
@@ -152,6 +161,7 @@ class Trainer(object):
 
     # ------------------------------------------------------------------ buffers
     def _alloc(self, T):
+        self._buf = self._graph = None       # the previous buffers go back to the allocator before the records are sized
         e = self.env.env
         B, N, H = e.nenvs, self.args.nagents, self.args.hid_size
         dev = e.device
@@ -171,16 +181,30 @@ class Trainer(object):
         if self.obs_mode == 'dense' or (self.record_for_grad and self.is_tj and not self.grad_kernels):
             b['obs'] = torch.empty(B, N, self.env.observation_dim, dtype=torch.float32, device=dev)
         if self.record_for_grad and self.grad_kernels:
-            # hand-written BPTT (csrc/bptt_tc.cu): every step's (h, c) -- the policy step writes them straight into
-            # the record, rec_h[t] -> rec_h[t + 1] -- and the inputs / env state each observation was taken from
+            # hand-written BPTT (csrc/bptt_tc.cu): the inputs / env state each observation was taken from, and the
+            # (h, c) of every step in one of two forms (_record_bytes):
+            #   'full'   rec_h, rec_c [T+1, B*N, H] -- the policy step writes them straight into the record,
+            #            rec_h[t] -> rec_h[t + 1];
+            #   'window' (h, c) checkpoints at the starts of grad_window-step windows plus max |c| of every step; the
+            #            backward re-runs the policy step over one window at a time (_recompute_window)
             b.update(s_fresh=z(T, B, dtype=torch.uint8), s_comm=z(T, B, N, dtype=torch.uint8),
-                     s_alive=z(T, B, N, dtype=torch.uint8), s_tep=z(T, B, dtype=torch.int32),
-                     rec_h=torch.empty(T + 1, B * N, H, device=dev), rec_c=torch.empty(T + 1, B * N, H, device=dev))
+                     s_alive=z(T, B, N, dtype=torch.uint8), s_tep=z(T, B, dtype=torch.int32))
             if self.is_tj:
                 b.update(s_tjloc=z(T, B, N, 2, dtype=torch.int32), s_tjalive=z(T, B, N, dtype=torch.uint8),
                          s_tjlast=z(T, B, N, dtype=torch.uint8), s_tjroute=z(T, B, N, dtype=torch.int32))
             else:
                 b['s_loc'] = z(T, B, e.npredator + 1, 2, dtype=torch.int32)    # predators + the prey
+            self._record_mode = self._pick_record_mode(T)
+            if self._record_mode == 'full':
+                b.update(rec_h=torch.empty(T + 1, B * N, H, device=dev), rec_c=torch.empty(T + 1, B * N, H, device=dev))
+            else:
+                W = self.grad_window
+                nw = (T + W - 1) // W
+                nb, L = min(nw, self._window_buffers()), min(W, T)      # window k lives in buffer k % _window_buffers()
+                e_ = lambda *s: torch.empty(*s, device=dev)
+                b.update(ck_h=z(nw, B * N, H), ck_c=z(nw, B * N, H), c_abs=z(T),
+                         win_h=[e_(L, B * N, H) for _ in range(nb)], win_c=[e_(L, B * N, H) for _ in range(nb)],
+                         win_value=e_(B * N), win_logp=e_(B * N, A))
         elif self.record_for_grad:
             # inputs of every policy step + (h, c) checkpoints at the window starts
             W = self.grad_window
@@ -195,6 +219,54 @@ class Trainer(object):
         self._buf = b
         self._graph = None
         return b
+
+    # The BPTT kernels' (h, c) records.  What the device has for them is measured when the rollout buffers have been
+    # allocated: free memory plus the caching allocator's unused reserve, minus RECORD_MARGIN_BYTES and the compute_grad
+    # temporaries (RECORD_TEMP_FACTOR float32 [T, B, N] tensors: returns, advantages and their intermediates).  Full
+    # records are kept while they take at most RECORD_BYTES_LIMIT bytes (None: what the device has); beyond that the
+    # records switch to windows of grad_window steps, which must fit in what the device has.
+    RECORD_BYTES_LIMIT = None
+    RECORD_MARGIN_BYTES = 2 << 30            # BPTT workspace (~0.9 GB at 81 920 rows) and allocator slack
+    RECORD_TEMP_FACTOR = 6
+
+    @property
+    def record_mode(self):
+        """How the BPTT kernels get every step's (h, c): 'full' records or 'window' recompute (None without the BPTT
+        kernels).  Chosen per rollout length when the buffers are allocated; before the first rollout, the choice
+        run_batch would make now."""
+        if not (self.record_for_grad and self.grad_kernels):
+            return None
+        if self._buf is None:
+            return self._pick_record_mode(self.batch_plan()[0])
+        return self._record_mode
+
+    def _window_buffers(self):
+        # windows are re-run two ahead of the backward (_compute_grad_kernels); one-step windows need a third buffer
+        return 2 if self.grad_window >= 2 else 3
+
+    def _record_bytes(self, T):
+        """{'full': bytes of rec_h + rec_c, 'window': bytes of the checkpoints + window buffers} for T steps."""
+        R, H, W = self.env.env.nenvs * self.args.nagents, self.args.hid_size, self.grad_window
+        row = R * H * 4
+        nw = (T + W - 1) // W
+        nb = min(nw, self._window_buffers())
+        return dict(full=2 * (T + 1) * row, window=2 * nw * row + 2 * nb * min(W, T) * row + T * 4)
+
+    def _pick_record_mode(self, T):
+        need = self._record_bytes(T)
+        dev = self.env.env.device
+        free, _ = torch.cuda.mem_get_info(dev)
+        free += torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
+        avail = free - self.RECORD_MARGIN_BYTES - self.RECORD_TEMP_FACTOR * T * self.env.env.nenvs * self.args.nagents * 4
+        limit = avail if self.RECORD_BYTES_LIMIT is None else min(avail, self.RECORD_BYTES_LIMIT)
+        if need['full'] <= limit:
+            return 'full'
+        if need['window'] <= avail:
+            return 'window'
+        raise RuntimeError("the BPTT kernels need %.3g GB for the (h, c) records of %d steps in windows of %d steps "
+                           "(%.3g GB as full records) but the device has %.3g GB for them; reduce --nenvs or "
+                           "--batch_size" % (need['window'] / 1e9, T, self.grad_window, need['full'] / 1e9,
+                                             max(avail, 0) / 1e9))
 
     # ------------------------------------------------------------------ rollout
     def _dense_chunks(self, cfg):
@@ -262,6 +334,8 @@ class Trainer(object):
         ws, _ = net.workspace(B)          # tensor-core path scratch (None for the fp32 SIMT kernel)
         rec = self.record_for_grad
         gk = rec and self.grad_kernels
+        full = gk and self._record_mode == 'full'     # the policy step writes (h, c) straight into the records
+        window = gk and not full                      # (h, c) checkpoints + max |c| per step (_alloc)
         dense = self.obs_mode == 'dense' or (rec and self.is_tj and not gk)
         # dense observations written on a side stream while the policy step runs (see _overlap_obs)
         overlap = self._overlap_obs()
@@ -312,7 +386,7 @@ class Trainer(object):
                         b['s_tjalive'][0].copy_(e.alive_mask)
                         b['s_tjlast'][0].copy_(e.car_last_act)
                         b['s_tjroute'][0].copy_(e.route_id)
-                if not gk and t % self.grad_window == 0:
+                if not full and t % self.grad_window == 0:
                     b['ck_h'][t // self.grad_window].copy_(b['h'])
                     b['ck_c'][t // self.grad_window].copy_(b['c'])
             if overlap:
@@ -328,7 +402,7 @@ class Trainer(object):
                 obs_enc = lib.ic3_tj_obs_encode if self.is_tj else lib.ic3_pp_obs_encode
                 for ecfg, est, ccfg, o_ptr, x_ptr in self._dense_chunks(cfg):
                     _lib.check(obs_enc(C.byref(ecfg), C.byref(est), C.byref(ccfg), C.byref(w), o_ptr, x_ptr, s))
-                if rec and self.is_tj:
+                if rec and self.is_tj and not gk:       # the BPTT kernels take x from the recorded env state
                     b['s_obs'][t].copy_(b['obs'])
             elif fused_x:
                 pass
@@ -338,8 +412,8 @@ class Trainer(object):
             else:
                 _lib.check(lib.ic3_pp_encoder_index(C.byref(e.cfg), C.byref(e.state), C.byref(cfg), C.byref(w),
                                                     b['x'].data_ptr(), s))
-            hin, cin = (b['rec_h'][t], b['rec_c'][t]) if gk else (b['h'], b['c'])
-            hout, cout = (b['rec_h'][t + 1], b['rec_c'][t + 1]) if gk else (b['h'], b['c'])
+            hin, cin = (b['rec_h'][t], b['rec_c'][t]) if full else (b['h'], b['c'])
+            hout, cout = (b['rec_h'][t + 1], b['rec_c'][t + 1]) if full else (b['h'], b['c'])
             io = _lib.PolicyIO(x=None if fused_x else b['x'].data_ptr(), h=hin.data_ptr(), c=cin.data_ptr(),
                                comm_action=b['comm'].data_ptr() if hard else None, alive=b['alive'].data_ptr(),
                                fresh=b['fresh'].data_ptr(), tick=e.tick.data_ptr(), draws=None,
@@ -347,6 +421,10 @@ class Trainer(object):
                                logp=b['logp'][t].data_ptr(), action=b['action'][t].data_ptr(),
                                workspace=_lib.ptr(ws), err=b['err'].data_ptr(), defer_heads=int(fuse_heads), **src)
             _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
+            if window:
+                # max |c'| of this step: the backward's operand scale needs the bound over every step's c before it
+                # re-runs any window, the same value a full record gives (_compute_grad_kernels)
+                torch.linalg.vector_norm(b['c'], math.inf, out=b['c_abs'][t])
             if fuse_heads:
                 heads_kw.update(head_value=b['value'][t].data_ptr(), head_logp=b['logp'][t].data_ptr())
             if overlap:
@@ -620,8 +698,9 @@ class Trainer(object):
 
     def _compute_grad_kernels(self, adv, ret):
         """Hand-written BPTT (csrc/bptt_tc.cu): one ic3_bptt_step per lock-step iteration, last to first (one host read
-        up front: max |c| of the record, the bound behind the operand scale).  Returns the device float64 vector of the
-        three loss sums."""
+        up front: max |c| of the record, the bound behind the operand scale).  In window mode (record_mode) the policy
+        step re-runs each window from its checkpoint just ahead of the backward (_recompute_window); the gradient is
+        bit-identical to full records'.  Returns the device float64 vector of the three loss sums."""
         b, net, args, e = self._buf, self.policy_net, self.args, self.env.env
         lib = _lib.load()
         T, B, N, H = b['T'], e.nenvs, args.nagents, args.hid_size
@@ -650,16 +729,43 @@ class Trainer(object):
         cut = None
         if args.detach_gap <= args.max_steps:                                  # trainer.py:56-60
             cut = (((b['s_tep'] + 1) % args.detach_gap) == 0).to(torch.uint8).contiguous()
-        lo, hi = torch.aminmax(b['rec_c'][1:])                                  # bound of |c| for the operand scale
-        cmax = max(abs(float(lo.item())), abs(float(hi.item())))
+        window = self._record_mode == 'window'
+        W = self.grad_window
+        if window:
+            cmax = float(b['c_abs'].max().item())                              # tracked per step by the rollout
+            nb = self._window_buffers()
+
+            def state(t):                      # (h, c) entering step t and h' leaving it, in the window buffers
+                k, j = divmod(t, W)
+                wh, wc = b['win_h'][k % nb], b['win_c'][k % nb]
+                hp, cp = (b['ck_h'][k], b['ck_c'][k]) if j == 0 else (wh[j - 1], wc[j - 1])
+                return hp, cp, wh[j]
+        else:
+            lo, hi = torch.aminmax(b['rec_c'][1:])                              # bound of |c| for the operand scale
+            cmax = max(abs(float(lo.item())), abs(float(hi.item())))
+
+            def state(t):
+                return b['rec_h'][t], b['rec_c'][t], b['rec_h'][t + 1]
+        # window mode: window k, steps [t0, t1), is re-run on this stream right before ic3_bptt_step(t1 + 1) is issued
+        # (before ic3_bptt_begin when there is no such step).  The look-ahead ic3_bptt_prepare(t) on the library's side
+        # stream waits for this stream's work up to ic3_bptt_step(t + 2), so it sees every window it reads; and the
+        # buffer window k overwrites (that of window k + nb, all of whose steps are >= t1 + 2) has no reader left.
+        todo = list(reversed(range((T + W - 1) // W))) if window else []
+
+        def recompute_due(t):
+            while todo and min(T, (todo[0] + 1) * W) + 1 >= t:
+                self._recompute_window(todo.pop(0))
+
+        recompute_due(T)
         st['dh'].zero_()
         st['dc'].zero_()
         _lib.check(lib.ic3_bptt_begin(C.byref(plan), cmax, s))
         value = b['value']
 
         def step_io(t):
-            return _lib.BpttStepIO(t=t, h_prev=b['rec_h'][t].data_ptr(), c_prev=b['rec_c'][t].data_ptr(),
-                                   h_new=b['rec_h'][t + 1].data_ptr(), fresh=b['s_fresh'][t].data_ptr(),
+            hp, cp, hn = state(t)
+            return _lib.BpttStepIO(t=t, h_prev=hp.data_ptr(), c_prev=cp.data_ptr(),
+                                   h_new=hn.data_ptr(), fresh=b['s_fresh'][t].data_ptr(),
                                    comm=b['s_comm'][t].data_ptr() if hard else None, alive=b['s_alive'][t].data_ptr(),
                                    cut=cut[t].data_ptr() if cut is not None else None,
                                    pp_loc=None if self.is_tj else b['s_loc'][t].data_ptr(),
@@ -677,6 +783,7 @@ class Trainer(object):
         if nxt is not None:
             _lib.check(lib.ic3_bptt_prepare(C.byref(plan), C.byref(nxt), s))
         for t in reversed(range(T)):
+            recompute_due(t)
             io = nxt
             if t > 0:
                 nxt = step_io(t - 1)
@@ -686,6 +793,47 @@ class Trainer(object):
         params, grads = self._param_structs()
         _lib.check(lib.ic3_bptt_finish(C.byref(plan), C.byref(params), C.byref(grads), st['losses'].data_ptr(), s))
         return st['losses']
+
+    def _recompute_window(self, k):
+        """Window mode: re-run the policy step over steps [k W, min(T, (k+1) W)) from checkpoint k into the window
+        buffer k % nb on the current stream; returns its (h, c) views [steps, B*N, H], row j = (h', c') of step k W + j.
+        Inputs come from the per-step records (fresh / comm / alive, and x from the recorded env state through the
+        fused index encoder with the per-position table); nothing is sampled and value / log-probs go to scratch.  The
+        tensor-core policy step is deterministic and every encoder form gives the same x, so each row equals the
+        rollout's (h', c') bit for bit -- except for slots that had already completed their batch (valid = 0), whose
+        inputs the env step no longer records; those rows carry no loss and no gradient."""
+        b, e, net, args = self._buf, self.env.env, self.policy_net, self.args
+        lib = _lib.load()
+        B, W = e.nenvs, self.grad_window
+        t0, t1 = k * W, min(b['T'], (k + 1) * W)
+        cfg = net.policy_cfg(B)
+        cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
+        w = net.packed()
+        table = self._encoder_table(cfg, w)
+        ws, _ = net.workspace(B)
+        hard = bool(args.hard_attn) and bool(args.commnet)
+        nb = self._window_buffers()
+        wh, wc = b['win_h'][k % nb], b['win_c'][k % nb]
+        s = _lib.stream()
+        for t in range(t0, t1):
+            j = t - t0
+            hin, cin = (b['ck_h'][k], b['ck_c'][k]) if j == 0 else (wh[j - 1], wc[j - 1])
+            if self.is_tj:
+                est = _lib.TJState(loc=b['s_tjloc'][t].data_ptr(), alive=b['s_tjalive'][t].data_ptr(),
+                                   last_act=b['s_tjlast'][t].data_ptr(), route_id=b['s_tjroute'][t].data_ptr())
+                src = dict(tj_env=C.addressof(e.cfg), tj_state=C.addressof(est))
+            else:
+                est = _lib.PPState(loc=b['s_loc'][t].data_ptr())
+                src = dict(pp_env=C.addressof(e.cfg), pp_state=C.addressof(est))
+            io = _lib.PolicyIO(x=None, h=hin.data_ptr(), c=cin.data_ptr(),
+                               comm_action=b['s_comm'][t].data_ptr() if hard else None,
+                               alive=b['s_alive'][t].data_ptr(), fresh=b['s_fresh'][t].data_ptr(), tick=None,
+                               draws=None, h_out=wh[j].data_ptr(), c_out=wc[j].data_ptr(),
+                               value=b['win_value'].data_ptr(), logp=b['win_logp'].data_ptr(), action=None,
+                               workspace=_lib.ptr(ws), err=b['err'].data_ptr(), defer_heads=0, x_table=table.data_ptr(),
+                               **src)
+            _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
+        return wh[:t1 - t0], wc[:t1 - t0]
 
     def _param_structs(self):
         """ic3_policy_params of the parameters and of their gradient buffers (reference layouts), by kernel role."""
