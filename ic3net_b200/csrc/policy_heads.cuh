@@ -69,7 +69,7 @@ __device__ __forceinline__ void heads_for_row(const ic3_policy_cfg& cfg, const f
 // ---------------------------------------------------------------------------------------------------------------
 // Finishing the heads from the per-slot partial logits of the tensor-core LSTM epilogue (fixed summation order ->
 // deterministic): value, log-softmax per head, inverse-CDF sampling of ONE agent row by ONE thread.  Used by
-// heads_finish_kernel (policy_tc) and, fused, by the env step kernels (ic3_rollout_io.head_partial).
+// heads_finish_kernel (policy_tc).
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int IC3_HEAD_PAD = 8;    // outputs (value + action logits) the fused epilogue supports
 constexpr int IC3_HEAD_NSLOT = 8;  // partial-logit slots per row
@@ -88,8 +88,7 @@ struct HeadsFinish {
   int32_t* action;        // [R, nheads] or NULL (no sampling)
 };
 
-// returns the sampled action of the LAST head in *last_act / of head 0 in *first_act (env kernels consume head 0)
-__device__ __forceinline__ void heads_finish_row(const HeadsFinish& f, long row, int e, int i, int* first_act) {
+__device__ __forceinline__ void heads_finish_row(const HeadsFinish& f, long row, int e, int i) {
   float logit[IC3_HEAD_PAD];
   const float4* p4 = reinterpret_cast<const float4*>(f.partial + (size_t)row * IC3_HEAD_NSLOT * IC3_HEAD_PAD);
   {
@@ -143,7 +142,6 @@ __device__ __forceinline__ void heads_finish_row(const HeadsFinish& f, long row,
       }
     }
     if (do_sample) f.action[(size_t)row * f.nheads + k] = act;
-    if (k == 0 && first_act) *first_act = act;
     off += na;
   }
 }

@@ -124,18 +124,6 @@ uint64_t ic3_tc_workspace_bytes(const ic3_policy_cfg* cfg) {
   return (uint64_t)ntiles_pad * TC_NCHUNK * A_CHUNK_BYTES + (uint64_t)R * NSLOT * HEAD_PAD * sizeof(float) + carry;
 }
 
-extern "C" const float* ic3_policy_partial_ptr(const ic3_policy_cfg* cfg, const void* workspace) {
-  if (!cfg || !workspace || cfg->H != TC_H) return nullptr;
-  int nout = 1;
-  for (int k = 0; k < cfg->nheads; ++k) nout += cfg->head_dim[k];
-  if (nout > HEAD_PAD) return nullptr;
-  const long R = (long)cfg->B * cfg->N;
-  const long ntiles = (R + TC_M - 1) / TC_M;
-  const long ntiles_pad = (ntiles + TC_TILE_PAD - 1) / TC_TILE_PAD * TC_TILE_PAD;
-  return reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(workspace) +
-                                        (size_t)ntiles_pad * TC_NCHUNK * A_CHUNK_BYTES);
-}
-
 int ic3_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3_policy_packed* out, cudaStream_t s) {
   if (cfg->H != TC_H) return IC3_E_UNSUPPORTED;
   const int total = 4 * TC_H * TC_K;
@@ -286,10 +274,6 @@ static int tc_pass(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const 
   if (rc) return rc;
   prof_mark(2, s);
   if (!last) return IC3_OK;                  // heads after the last comm pass only
-  if (fused_heads && io->defer_heads) {      // the env step kernel finishes the heads (ic3_rollout_io.head_partial)
-    prof_mark(3, s);
-    return IC3_OK;
-  }
   if (fused_heads) {
     IC3_LAUNCH_RC(ic3_launch_pdl(heads_finish_kernel, dim3((unsigned)((R + 127) / 128)), dim3(128), 0, s, *cfg, *w, *io,
                                  (const float*)partial));

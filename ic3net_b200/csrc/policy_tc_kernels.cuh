@@ -789,7 +789,7 @@ __global__ void __launch_bounds__(128) heads_finish_kernel(ic3_policy_cfg cfg, i
   f.seed = cfg.seed; f.env_id0 = cfg.env_id0; f.tick = io.tick; f.draws = io.draws;
   f.value = io.value; f.logp = io.logp; f.action = io.action;
   const int e = (int)(row / cfg.N), i = (int)(row - (long)e * cfg.N);
-  heads_finish_row(f, row, e, i, nullptr);
+  heads_finish_row(f, row, e, i);
 }
 
 }  // namespace

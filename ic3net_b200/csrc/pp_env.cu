@@ -142,10 +142,7 @@ __global__ void pp_step_kernel(PPArgs a, const int32_t* __restrict__ act, int ac
       if (a.st.done[e]) {  // :129-130 RuntimeError("Episode is done")
         if (lane == 0) atomicOr(err, IC3_ERR_EPISODE_DONE);
       } else {
-        int av = 4;
-        if (r.has && r.io.head_partial) av = ic3_rollout_heads(r.io, a.cfg.seed, a.cfg.env_id0, a.st.tick, e, NA, lane);
-        else if (lane < NA) av = act[((size_t)e * NA + lane) * act_stride];
-        if (lane >= NA) av = 4;
+        const int av = lane < NA ? act[((size_t)e * NA + lane) * act_stride] : 4;
         if (lane < NA && (av < 0 || av > a.cfg.naction)) atomicOr(err, IC3_ERR_BAD_ACTION);  // :137 (sic, <=)
         if (lane < N && !rch) {  // _take_action :212-252: every move is a clamped move
           if (av == 0) rr = max(0, rr - 1);

@@ -119,10 +119,7 @@ __global__ void tj_step_kernel(TJArgs a, const int32_t* __restrict__ act, int ac
     } else if (do_step) {
       // ---- _take_action :540-581 ----
       int completed = 0;
-      int av = 1;
-      if (r.has && r.io.head_partial) av = ic3_rollout_heads(r.io, cfg.seed, cfg.env_id0, a.st.tick, e, N, lane);
-      else if (lane < N) av = act[i * act_stride];
-      if (lane >= N) av = 1;
+      const int av = lane < N ? act[i * act_stride] : 1;
       if (lane < N && (av < 0 || av > 2)) atomicOr(err, IC3_ERR_BAD_ACTION);  // :228 (sic, <=)
       if (lane < N && alive) {
         wait += 1;                       // :546
@@ -356,7 +353,7 @@ int tj_obs_encode_launch(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const ic
   const int W = 2 * cfg->vision + 1;
   const size_t smem = (size_t)cfg->N * W * W * sizeof(uint32_t);
   const bool split = pcfg->obs_vocab > 0;
-  // same store policy as ic3_tj_obs: batches that fit in L2 stay there for the record-for-grad copy of the trainer
+  // same store policy as ic3_tj_obs: batches that fit in L2 stay there for a reader that follows
   const int keep = (size_t)cfg->B * cfg->N * (2 + W * W * cfg->vocab) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
   IC3_LAUNCH_RC(ic3_launch_pdl(tj_obs_encode_kernel<H>, dim3(cfg->B), dim3(128), smem, s, a, obs, (const float*)w->enc_wT,
                                (const float*)w->enc_b, x, split, keep));

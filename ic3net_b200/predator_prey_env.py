@@ -97,8 +97,7 @@ class PredatorPreyEnv(object):
         return
 
     def chunk_view(self, k0, k1):
-        """(cfg, state) of the env slots [k0, k1): the same device memory, for kernels run on a slice of the batch
-        (the trainer gathers + encodes observations in L2-sized chunks)."""
+        """(cfg, state) of the env slots [k0, k1): the same device memory, for kernels run on a slice of the batch."""
         cfg = _lib.PPCfg.from_buffer_copy(self.cfg)
         cfg.B, cfg.env_id0 = k1 - k0, self.cfg.env_id0 + k0
         st = _lib.PPState(loc=self.loc[k0:k1].data_ptr(), reached=self.reached_prey[k0:k1].data_ptr(),

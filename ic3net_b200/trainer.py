@@ -21,7 +21,10 @@ stream writes the [B, N, O] observation block of the same state concurrently (ic
 for that write.
 The whole T-step sequence can be captured once into a CUDA graph (``use_graph``).
 
-Gradient (``compute_grad``, trainer.py:128-225; scope row 8(f)-1): returns by a CUDA scan kernel,
+Gradient (``compute_grad``, trainer.py:128-225; scope row 8(f)-1): with ``record_for_grad`` the env step kernels record
+the inputs of every policy step and the env state its observation is taken from (predator-prey: positions; traffic
+junction: positions, alive, last action, route), the same records for every ``grad_impl``; an observation is rebuilt
+from them when the backward needs it (``_record_state``).  Returns by a CUDA scan kernel,
 then the policy forward is RECOMPUTED with differentiable torch ops (fp32, batched over all slots)
 in windows of ``grad_window`` steps processed last-to-first; (h, c) at every window start are
 checkpointed during the rollout and the gradient w.r.t. them is handed to the previous window,
@@ -178,15 +181,17 @@ class Trainer(object):
                  stat_episodes=z(B, dtype=torch.int32), stat_steps=z(B, dtype=torch.int32),
                  err=z(1, dtype=torch.int32), halted=z(B, dtype=torch.uint8), valid=z(T, B, dtype=torch.uint8),
                  statvec=z(4 + 2 * N, dtype=torch.float64))
-        if self.obs_mode == 'dense' or (self.record_for_grad and self.is_tj and not self.grad_kernels):
+        if self.obs_mode == 'dense':
             b['obs'] = torch.empty(B, N, self.env.observation_dim, dtype=torch.float32, device=dev)
-        if self.record_for_grad and self.grad_kernels:
-            # hand-written BPTT (csrc/bptt_tc.cu): the inputs / env state each observation was taken from, and the
-            # (h, c) of every step in one of two forms (_record_bytes):
-            #   'full'   rec_h, rec_c [T+1, B*N, H] -- the policy step writes them straight into the record,
-            #            rec_h[t] -> rec_h[t + 1];
-            #   'window' (h, c) checkpoints at the starts of grad_window-step windows plus max |c| of every step; the
-            #            backward re-runs the policy step over one window at a time (_recompute_window)
+        if self.record_for_grad:
+            # the inputs of every policy step and the env state its observation is taken from (_record_state), then
+            # (h, c) in one of three forms:
+            #   torch paths  (h, c) checkpoints at the starts of grad_window-step windows (_forward_window re-runs them)
+            #   BPTT kernels (_record_bytes):
+            #     'full'   rec_h, rec_c [T+1, B*N, H] -- the policy step writes them straight into the record,
+            #              rec_h[t] -> rec_h[t + 1];
+            #     'window' the checkpoints plus max |c| of every step; the backward re-runs the policy step over one
+            #              window at a time (_recompute_window)
             b.update(s_fresh=z(T, B, dtype=torch.uint8), s_comm=z(T, B, N, dtype=torch.uint8),
                      s_alive=z(T, B, N, dtype=torch.uint8), s_tep=z(T, B, dtype=torch.int32))
             if self.is_tj:
@@ -194,28 +199,18 @@ class Trainer(object):
                          s_tjlast=z(T, B, N, dtype=torch.uint8), s_tjroute=z(T, B, N, dtype=torch.int32))
             else:
                 b['s_loc'] = z(T, B, e.npredator + 1, 2, dtype=torch.int32)    # predators + the prey
-            self._record_mode = self._pick_record_mode(T)
+            W = self.grad_window
+            nw = (T + W - 1) // W
+            self._record_mode = self._pick_record_mode(T) if self.grad_kernels else None
             if self._record_mode == 'full':
                 b.update(rec_h=torch.empty(T + 1, B * N, H, device=dev), rec_c=torch.empty(T + 1, B * N, H, device=dev))
             else:
-                W = self.grad_window
-                nw = (T + W - 1) // W
+                b.update(ck_h=z(nw, B * N, H), ck_c=z(nw, B * N, H))
+            if self._record_mode == 'window':
                 nb, L = min(nw, self._window_buffers()), min(W, T)      # window k lives in buffer k % _window_buffers()
                 e_ = lambda *s: torch.empty(*s, device=dev)
-                b.update(ck_h=z(nw, B * N, H), ck_c=z(nw, B * N, H), c_abs=z(T),
-                         win_h=[e_(L, B * N, H) for _ in range(nb)], win_c=[e_(L, B * N, H) for _ in range(nb)],
-                         win_value=e_(B * N), win_logp=e_(B * N, A))
-        elif self.record_for_grad:
-            # inputs of every policy step + (h, c) checkpoints at the window starts
-            W = self.grad_window
-            nw = (T + W - 1) // W
-            b.update(s_fresh=z(T, B, dtype=torch.uint8), s_comm=z(T, B, N, dtype=torch.uint8),
-                     s_alive=z(T, B, N, dtype=torch.uint8), s_tep=z(T, B, dtype=torch.int32),
-                     ck_h=z(nw, B * N, H), ck_c=z(nw, B * N, H))
-            if self.is_tj:
-                b['s_obs'] = z(T, B, N, self.env.observation_dim)
-            else:
-                b['s_loc'] = z(T, B, e.npredator + 1, 2, dtype=torch.int32)    # predators + the prey
+                b.update(c_abs=z(T), win_h=[e_(L, B * N, H) for _ in range(nb)],
+                         win_c=[e_(L, B * N, H) for _ in range(nb)], win_value=e_(B * N), win_logp=e_(B * N, A))
         self._buf = b
         self._graph = None
         return b
@@ -269,35 +264,10 @@ class Trainer(object):
                                              max(avail, 0) / 1e9))
 
     # ------------------------------------------------------------------ rollout
-    def _dense_chunks(self, cfg):
-        """[(env cfg, env state, policy cfg, obs ptr, x ptr)] per chunk of env slots; chunk bytes <= obs_chunk_mb."""
-        e, b = self.env.env, self._buf
-        B, N, O, H = e.nenvs, self.args.nagents, self.env.observation_dim, self.args.hid_size
-        key = (B, b['obs'].data_ptr(), b['x'].data_ptr(), cfg.obs_vocab, cfg.seed, cfg.env_id0)
-        if getattr(self, '_chunks_key', None) == key:
-            return self._chunks
-        # default: ONE chunk.  Each chunk is one launch of the fused gather + encoder (ic3_*_obs_encode), which never reads
-        # the observations back, or of the observation writer (_overlap_obs), so chunking only adds kernel tails; the
-        # option remains for bounding a chunk's footprint.
-        mb = float(getattr(self.args, 'obs_chunk_mb', 0) or 0)
-        per_env = N * O * 4
-        nchunk = max(1, -(-B * per_env // int(mb * (1 << 20)))) if mb > 0 else 1
-        step = -(-B // nchunk)
-        out = []
-        for k0 in range(0, B, step):
-            k1 = min(B, k0 + step)
-            ecfg, est = e.chunk_view(k0, k1)
-            ccfg = _lib.PolicyCfg.from_buffer_copy(cfg)
-            ccfg.B, ccfg.env_id0 = k1 - k0, cfg.env_id0 + k0
-            out.append((ecfg, est, ccfg, b['obs'].data_ptr() + k0 * per_env, b['x'].data_ptr() + k0 * N * H * 4))
-        self._chunks, self._chunks_key = out, key
-        return out
-
     def _fused_x(self):
         """Index-form observations on the tensor-core policy path: the encoder runs inside the policy step."""
-        dense = self.obs_mode == 'dense' or (self.record_for_grad and self.is_tj and not self.grad_kernels)
         W = 2 * self.env.env.vision + 1
-        return (not dense) and self.policy_net.policy_impl == 'tc' and W * W <= 25
+        return self.obs_mode != 'dense' and self.policy_net.policy_impl == 'tc' and W * W <= 25
 
     # Smaller observation blocks per step keep the fused gather + encoder: their write is short and latency-bound in the
     # persistent writer (measured on an H100: predator-prey easy, 2.9 MB, 3 % slower with the overlap; traffic-junction
@@ -307,10 +277,9 @@ class Trainer(object):
     def _overlap_obs(self):
         """Dense observations on the tensor-core policy path: the policy step computes x from the env state (the fused
         index encoder; without the per-position table, which measured no faster beside the writer, so dense mode never
-        builds it) and the observation block is written concurrently on a side stream.  Not when the traffic-junction
-        records copy every step's observation (record_for_grad without the BPTT kernels), nor for blocks smaller than
+        builds it) and the observation block is written concurrently on a side stream.  Not for blocks smaller than
         OVERLAP_MIN_OBS_BYTES."""
-        if self.obs_mode != 'dense' or (self.record_for_grad and self.is_tj and not self.grad_kernels):
+        if self.obs_mode != 'dense':
             return False
         e = self.env.env
         if e.nenvs * self.args.nagents * self.env.observation_dim * 4 < self.OVERLAP_MIN_OBS_BYTES:
@@ -333,10 +302,9 @@ class Trainer(object):
         s = _lib.stream()
         ws, _ = net.workspace(B)          # tensor-core path scratch (None for the fp32 SIMT kernel)
         rec = self.record_for_grad
-        gk = rec and self.grad_kernels
-        full = gk and self._record_mode == 'full'     # the policy step writes (h, c) straight into the records
-        window = gk and not full                      # (h, c) checkpoints + max |c| per step (_alloc)
-        dense = self.obs_mode == 'dense' or (rec and self.is_tj and not gk)
+        full = rec and self._record_mode == 'full'    # the policy step writes (h, c) straight into the records
+        window = rec and self._record_mode == 'window'    # (h, c) checkpoints + max |c| per step (_alloc)
+        dense = self.obs_mode == 'dense'
         # dense observations written on a side stream while the policy step runs (see _overlap_obs)
         overlap = self._overlap_obs()
         # tensor-core path: the index encoder is fused into the policy step (x never leaves the operand image)
@@ -352,26 +320,15 @@ class Trainer(object):
                 self._side = torch.cuda.Stream(device=main.device)
             side = self._side
             obs_write = lib.ic3_tj_obs_bounded if self.is_tj else lib.ic3_pp_obs_bounded
-        # Option (args.fuse_heads, default off): on the tensor-core path with <= 7 action logits the env step kernel can
-        # finish the policy heads (value, log-softmax, sampling) from the LSTM epilogue's partial logits -- one launch
-        # less per lock-step iteration, but one 32-thread CTA per env hides the 64 partial-logit loads of a row worse than the
-        # thread-per-row heads_finish kernel at full occupancy, so the separate kernel stays the default.
-        fuse_heads = (net.policy_impl == 'tc' and 1 + sum(args.naction_heads) <= 8 and ws is not None
-                      and bool(getattr(args, 'fuse_heads', False)))
-        heads_kw = {}
-        if fuse_heads:
-            hd = (C.c_int32 * _lib.MAX_HEADS)(*(list(args.naction_heads) + [0] * (_lib.MAX_HEADS - nh)))
-            heads_kw = dict(head_partial=lib.ic3_policy_partial_ptr(C.byref(cfg), ws.data_ptr()),
-                            head_b=net._bufs['head_b'].data_ptr(), head_dim=hd)
         snap = {}
         if rec:
             snap = dict(snap_T=T, snap_fresh=b['s_fresh'].data_ptr(), snap_comm=b['s_comm'].data_ptr(),
                         snap_alive=b['s_alive'].data_ptr(), snap_tep=b['s_tep'].data_ptr())
-            if not self.is_tj:
-                snap['snap_pp_loc'] = b['s_loc'].data_ptr()
-            elif gk:
+            if self.is_tj:
                 snap.update(snap_tj_loc=b['s_tjloc'].data_ptr(), snap_tj_alive=b['s_tjalive'].data_ptr(),
                             snap_tj_last_act=b['s_tjlast'].data_ptr(), snap_tj_route_id=b['s_tjroute'].data_ptr())
+            else:
+                snap['snap_pp_loc'] = b['s_loc'].data_ptr()
         for t in range(T):
             if rec:
                 if t == 0:          # inputs of the first step; the env step kernels record those of every later step
@@ -379,31 +336,27 @@ class Trainer(object):
                     b['s_comm'][0].copy_(b['comm'])
                     b['s_alive'][0].copy_(b['alive'])
                     b['s_tep'][0].copy_(b['t_ep'])
-                    if not self.is_tj:
-                        b['s_loc'][0].copy_(e.loc)
-                    elif gk:
+                    if self.is_tj:
                         b['s_tjloc'][0].copy_(e.car_loc)
                         b['s_tjalive'][0].copy_(e.alive_mask)
                         b['s_tjlast'][0].copy_(e.car_last_act)
                         b['s_tjroute'][0].copy_(e.route_id)
+                    else:
+                        b['s_loc'][0].copy_(e.loc)
                 if not full and t % self.grad_window == 0:
                     b['ck_h'][t // self.grad_window].copy_(b['h'])
                     b['ck_c'][t // self.grad_window].copy_(b['c'])
             if overlap:
                 # the writer reads the state the previous env step left and must finish before this step's env step
-                # moves the agents (the join below); one launch per chunk of env slots, as in the branch below
+                # moves the agents (the join below)
                 side.wait_stream(main)
-                for ecfg, est, _, o_ptr, _ in self._dense_chunks(cfg):
-                    _lib.check(obs_write(C.byref(ecfg), C.byref(est), o_ptr, side.cuda_stream))
+                _lib.check(obs_write(C.byref(e.cfg), C.byref(e.state), b['obs'].data_ptr(), side.cuda_stream))
             elif dense:
-                # gather + encode in one kernel per chunk of env slots (args.obs_chunk_mb; default one chunk, see
-                # _dense_chunks): the observation block is written in full and x is summed from the same per-cell
-                # records, so the block is never read back
+                # gather + encode in one kernel: the observation block is written in full and x is summed from the
+                # same per-cell records, so the block is never read back
                 obs_enc = lib.ic3_tj_obs_encode if self.is_tj else lib.ic3_pp_obs_encode
-                for ecfg, est, ccfg, o_ptr, x_ptr in self._dense_chunks(cfg):
-                    _lib.check(obs_enc(C.byref(ecfg), C.byref(est), C.byref(ccfg), C.byref(w), o_ptr, x_ptr, s))
-                if rec and self.is_tj and not gk:       # the BPTT kernels take x from the recorded env state
-                    b['s_obs'][t].copy_(b['obs'])
+                _lib.check(obs_enc(C.byref(e.cfg), C.byref(e.state), C.byref(cfg), C.byref(w), b['obs'].data_ptr(),
+                                   b['x'].data_ptr(), s))
             elif fused_x:
                 pass
             elif self.is_tj:
@@ -419,20 +372,18 @@ class Trainer(object):
                                fresh=b['fresh'].data_ptr(), tick=e.tick.data_ptr(), draws=None,
                                h_out=hout.data_ptr(), c_out=cout.data_ptr(), value=b['value'][t].data_ptr(),
                                logp=b['logp'][t].data_ptr(), action=b['action'][t].data_ptr(),
-                               workspace=_lib.ptr(ws), err=b['err'].data_ptr(), defer_heads=int(fuse_heads), **src)
+                               workspace=_lib.ptr(ws), err=b['err'].data_ptr(), **src)
             _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
             if window:
                 # max |c'| of this step: the backward's operand scale needs the bound over every step's c before it
                 # re-runs any window, the same value a full record gives (_compute_grad_kernels)
                 torch.linalg.vector_norm(b['c'], math.inf, out=b['c_abs'][t])
-            if fuse_heads:
-                heads_kw.update(head_value=b['value'][t].data_ptr(), head_logp=b['logp'][t].data_ptr())
             if overlap:
                 main.wait_stream(side)
             r = _lib.RolloutIO(t=t, max_steps=args.max_steps, nheads=nh, hard_attn=hard,
                                comm_action_one=int(bool(args.comm_action_one)),
                                last=int(t == T - 1 and quota <= 0), batch_size=int(quota),
-                               halted=b['halted'].data_ptr(), rec_valid=b['valid'].data_ptr(), **snap, **heads_kw,
+                               halted=b['halted'].data_ptr(), rec_valid=b['valid'].data_ptr(), **snap,
                                action=b['action'][t].data_ptr(), t_ep=b['t_ep'].data_ptr(),
                                fresh=b['fresh'].data_ptr(), comm_next=b['comm'].data_ptr(),
                                alive_next=b['alive'].data_ptr(), rec_reward=b['reward'].data_ptr(),
@@ -573,6 +524,28 @@ class Trainer(object):
         return batch, self.stats
 
     # ------------------------------------------------------------------ gradient (trainer.py:128-225)
+    def _record_state(self, t, k0=0, k1=None):
+        """(env cfg, env state) of env slots [k0, k1) as the records hold them entering step t: the live state view with
+        the recorded fields substituted (predator-prey: loc; traffic junction: loc, alive, last_act, route_id), which
+        are all the encoders and observation writers read."""
+        e, b = self.env.env, self._buf
+        k1 = e.nenvs if k1 is None else k1
+        cfg, st = e.chunk_view(k0, k1)
+        rec = lambda key: b[key][t, k0:k1].data_ptr()
+        if self.is_tj:
+            st.loc, st.alive, st.last_act, st.route_id = rec('s_tjloc'), rec('s_tjalive'), rec('s_tjlast'), rec('s_tjroute')
+        else:
+            st.loc = rec('s_loc')
+        return cfg, st
+
+    def _tj_record_obs(self, t, k0=0, k1=None):
+        """[k1 - k0, N, O] traffic-junction observation of step t for env slots [k0, k1), written by ic3_tj_obs from the
+        recorded env state into a new tensor (the torch backward keeps each step's observation until it has run)."""
+        cfg, st = self._record_state(t, k0, k1)
+        obs = torch.empty(cfg.B, self.args.nagents, self.env.observation_dim, device=self.env.env.device)
+        _lib.check(_lib.load().ic3_tj_obs(C.byref(cfg), C.byref(st), obs.data_ptr(), _lib.stream()))
+        return obs
+
     def _pp_sparse_obs(self, loc):
         """Non-zeros of the PP observation (predator_prey_env.py:188-210) as (index, value) pairs
         [R, 3*W*W] from a state snapshot loc [B, N+1, 2]."""
@@ -610,7 +583,7 @@ class Trainer(object):
             keep = (1 - b['s_fresh'][t].float()).repeat_interleave(N).unsqueeze(1)        # trainer.py:50-51
             h, c = h * keep, c * keep
             if self.is_tj:
-                x = F.linear(b['s_obs'][t].reshape(B * N, -1), w_e, b_e)                  # comm.py:119
+                x = F.linear(self._tj_record_obs(t).reshape(B * N, -1), w_e, b_e)         # comm.py:119
             else:
                 idx, val = self._pp_sparse_obs(b['s_loc'][t])
                 x = F.embedding_bag(idx, w_eT, per_sample_weights=val, mode='sum') + b_e
@@ -818,20 +791,15 @@ class Trainer(object):
         for t in range(t0, t1):
             j = t - t0
             hin, cin = (b['ck_h'][k], b['ck_c'][k]) if j == 0 else (wh[j - 1], wc[j - 1])
-            if self.is_tj:
-                est = _lib.TJState(loc=b['s_tjloc'][t].data_ptr(), alive=b['s_tjalive'][t].data_ptr(),
-                                   last_act=b['s_tjlast'][t].data_ptr(), route_id=b['s_tjroute'][t].data_ptr())
-                src = dict(tj_env=C.addressof(e.cfg), tj_state=C.addressof(est))
-            else:
-                est = _lib.PPState(loc=b['s_loc'][t].data_ptr())
-                src = dict(pp_env=C.addressof(e.cfg), pp_state=C.addressof(est))
+            ecfg, est = self._record_state(t)
+            src = dict(tj_env=C.addressof(ecfg), tj_state=C.addressof(est)) if self.is_tj else \
+                dict(pp_env=C.addressof(ecfg), pp_state=C.addressof(est))
             io = _lib.PolicyIO(x=None, h=hin.data_ptr(), c=cin.data_ptr(),
                                comm_action=b['s_comm'][t].data_ptr() if hard else None,
                                alive=b['s_alive'][t].data_ptr(), fresh=b['s_fresh'][t].data_ptr(), tick=None,
                                draws=None, h_out=wh[j].data_ptr(), c_out=wc[j].data_ptr(),
                                value=b['win_value'].data_ptr(), logp=b['win_logp'].data_ptr(), action=None,
-                               workspace=_lib.ptr(ws), err=b['err'].data_ptr(), defer_heads=0, x_table=table.data_ptr(),
-                               **src)
+                               workspace=_lib.ptr(ws), err=b['err'].data_ptr(), x_table=table.data_ptr(), **src)
             _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
         return wh[:t1 - t0], wc[:t1 - t0]
 
@@ -878,7 +846,7 @@ class Trainer(object):
                          getattr(args, 'comm_mode', 'avg') == 'avg', bool(args.comm_mask_zero), args.value_coeff,
                          args.entr, args.detach_gap, args.max_steps)
         if self.is_tj:
-            obs_fn = lambda t: b['s_obs'][t].reshape(B * N, -1)
+            obs_fn = lambda t: self._tj_record_obs(t).reshape(B * N, -1)
         else:
             obs_fn = lambda t: self._pp_sparse_obs(b['s_loc'][t])
         rec = dict(fresh=b['s_fresh'], comm=b['s_comm'], alive=b['s_alive'], t_ep=b['s_tep'], action=b['action'],

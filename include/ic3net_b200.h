@@ -101,7 +101,8 @@ typedef struct {
   int32_t hard_attn;       /* args.hard_attn && args.commnet (trainer.py:70) */
   int32_t comm_action_one; /* args.comm_action_one (trainer.py:71) */
   int32_t last;            /* 1 on the final lock-step of the batch: open episodes are cut (treated like max_steps) */
-  const int32_t* action;   /* [B, N, nheads] sampled this step; env consumes head 0 (env_wrappers.py:76-77) */
+  const int32_t* action;   /* [B, N, nheads] in: the actions the policy step sampled (read for comm_next; the env
+                            * step takes head 0 from its `act` argument, env_wrappers.py:76-77) */
   int32_t* t_ep;           /* [B] step index inside the current episode */
   uint8_t* fresh;          /* [B] out: next policy step starts an episode (h=c=0, nobody talks, all alive; trainer.py:45-51) */
   uint8_t* comm_next;      /* [B, N] out: info['comm_action'] for the next policy step (trainer.py:70-71) */
@@ -137,15 +138,6 @@ typedef struct {
   uint8_t* snap_tj_alive;  /* [T, B, N] */
   uint8_t* snap_tj_last_act; /* [T, B, N] */
   int32_t* snap_tj_route_id; /* [T, B, N] */
-  /* Fused policy heads (tensor-core path, ic3_policy_io.defer_heads): when head_partial != NULL the env step kernel first
-   * finishes the heads of this step from the LSTM epilogue's partial logits -- value, log-softmax, inverse-CDF sampling
-   * on the action stream of (cfg.seed, cfg.env_id0 + env, tick) -- writing head_value / head_logp and the `action`
-   * tensor (which is then an OUTPUT of the step, not an input), and consumes head 0 itself.  One launch less per step. */
-  const float* head_partial; /* ic3_policy_partial_ptr(...) */
-  const float* head_b;       /* ic3_policy_packed.head_b */
-  float* head_value;         /* [B*N] */
-  float* head_logp;          /* [B*N, sum(na)] */
-  int32_t head_dim[IC3_MAX_HEADS];
 } ic3_rollout_io;
 
 /* reset(): predator_prey_env.py:146-168.  Draws N+1 distinct cells per env from
@@ -353,16 +345,10 @@ typedef struct {
   /* optional, fused index encoder only: [positions, H] table of ic3_pp_encoder_table / ic3_tj_encoder_table
    * for the CURRENT weights (device pointer); needs cfg->obs_vocab > 0. */
   const float* x_table;
-  /* tensor-core path with at most 7 action logits: 1 = stop after the LSTM kernel and leave the heads' partial logits in
-   * the workspace (ic3_policy_partial_ptr); the env step kernel finishes them (ic3_rollout_io.head_partial). */
-  int32_t defer_heads;
   int32_t pass_index;         /* callers pass 0.  comm_passes > 1 on the tensor-core path: the library runs the step once per
                                  pass on a private copy of this struct and numbers the copies here (a fresh episode's
                                  zero state applies to pass 0 only; its masks to every pass, comm.py:179-218) */
 } ic3_policy_io;
-
-/* Partial-logit block inside a tensor-core workspace (NULL when the configuration does not use it). */
-const float* ic3_policy_partial_ptr(const ic3_policy_cfg* cfg, const void* workspace);
 
 /* Scratch the tensor-core policy path needs for a batch of cfg->B environments (0 when unsupported). */
 uint64_t ic3_policy_workspace_bytes(const ic3_policy_cfg* cfg);

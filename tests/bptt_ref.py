@@ -9,8 +9,6 @@ sparse pattern of ``s_loc[t]``, the traffic-junction block that ``ic3_tj_obs`` w
 
 ``oracle_grad_sum`` is the other yardstick: the float64 oracle replaying every env slot of a ``run_batch`` as one
 reference process (teacher-forced with the GPU's actions) and summing the gradients over slots."""
-import ctypes as C
-
 import numpy as np
 import torch
 
@@ -54,18 +52,8 @@ def returns_and_advantages(tr):
 
 def tj_record_obs(tr, t, k0, k1):
     """[k1 - k0, N, O] float32 traffic-junction observation of step t for env slots [k0, k1), written by ic3_tj_obs
-    from the recorded state (loc, alive, last_act, route_id); the rest of the state view is the live env's, which
-    the observation does not read."""
-    from ic3net_b200 import _lib
-    e, b = tr.env.env, tr._buf
-    cfg, st = e.chunk_view(k0, k1)
-    st.loc = b["s_tjloc"][t, k0:k1].data_ptr()
-    st.alive = b["s_tjalive"][t, k0:k1].data_ptr()
-    st.last_act = b["s_tjlast"][t, k0:k1].data_ptr()
-    st.route_id = b["s_tjroute"][t, k0:k1].data_ptr()
-    obs = torch.empty(k1 - k0, tr.args.nagents, tr.env.observation_dim, device=e.device)
-    _lib.check(_lib.load().ic3_tj_obs(C.byref(cfg), C.byref(st), obs.data_ptr(), _lib.stream()))
-    return obs
+    from the recorded state (Trainer._record_state)."""
+    return tr._tj_record_obs(t, k0, k1)
 
 
 def trainer_reference(tr, slots=None, heads_from_records=True):

@@ -12,6 +12,7 @@ also per input column (1e-4 of that column's largest entry plus 1e-6 of the tens
 observation-pattern columns cannot hide behind a large neighbour; the action heads' entries also get 2^-20 of their
 sum of |terms| (the comm head's two-logit gradient cancels to a small fraction of that sum, and its fp32 per-row
 terms are exact to a few ulps of the sum; a lost row or tile still breaks the bar); loss sums rtol 2e-4, atol 1e-3."""
+import ctypes as C
 import os
 import subprocess
 import sys
@@ -147,26 +148,32 @@ def test_reference_matches_oracle_and_kernels(name):
     assert_within_bar(tr, got, gloss, ref, rloss, name)
 
 
-def test_tj_record_obs_equals_dense_rollout_obs():
-    """The traffic-junction observation the reference rebuilds from the recorded state (loc, alive, last_act,
-    route_id of step t) equals the observation a dense-mode rollout with the same seeds recorded at step t, on
-    every slot whose trajectory the two rollouts share up to that step."""
-    name = "grad_tj_hard_ic3net_h128"
-    tk, _, _ = make_trainer(name, 16)
-    td, _, _ = make_trainer(name, 16, grad_impl="autograd")
-    tk.run_batch(0)
-    td.run_batch(0)
-    assert tk.grad_kernels and not td.grad_kernels and "s_obs" in td._buf
-    T = tk._buf["T"]
-    same = torch.ones(16, dtype=torch.bool, device="cuda")
-    compared = 0
+def test_tj_record_obs_equals_the_live_obs_of_the_same_rollout():
+    """The traffic-junction observation rebuilt from the recorded state of step t (loc, alive, last_act, route_id;
+    Trainer._record_state) equals what ic3_tj_obs writes from the live env state before step t of the same rollout
+    (the dense rollout's observation), on every slot and step and across episode resets, for the whole batch and for
+    a range of slots.  Every gradient path records the same state, so a trainer without the BPTT kernels is used."""
+    from ic3net_b200 import _lib
+    name, B, quota = "grad_tj_hard_ic3net_h128", 16, 1 << 30       # no slot halts: every step is recorded
+    tr, _, _ = make_trainer(name, B, grad_impl="autograd")
+    live, _, _ = make_trainer(name, B, grad_impl="autograd")
+    assert not tr.grad_kernels
+    T = tr.batch_plan()[0]
+    assert T > tr.args.max_steps                                     # the records cross an episode reset
+    tr.rollout(T, 0, quota=quota)
+    e = live.env.env
+    live._alloc(T)
+    live._episode_boundary(0)
+    live._buf["err"].zero_()
+    want = torch.empty(T, B, tr.args.nagents, tr.env.observation_dim, device="cuda")
+    for t in range(T):                       # the same rollout one lock-step at a time, observed before each step
+        _lib.check(_lib.load().ic3_tj_obs(C.byref(e.cfg), C.byref(e.state), want[t].data_ptr(), _lib.stream()))
+        live._enqueue(1, quota=quota)
+        assert torch.equal(live._buf["action"][0], tr._buf["action"][t]), t
     for t in range(T):
-        got = tj_record_obs(tk, t, 0, 16)
-        want = td._buf["s_obs"][t]
-        assert torch.equal(got[same], want[same]), t
-        compared += int(same.sum())
-        same &= (tk._buf["action"][t] == td._buf["action"][t]).flatten(1).all(1)
-    assert compared >= T * 16 // 2, compared
+        assert torch.equal(tj_record_obs(tr, t, 0, B), want[t]), t
+        assert torch.equal(tj_record_obs(tr, t, 5, 13), want[t, 5:13]), t
+    assert int(tr._buf["err"].item()) == 0 and int(live._buf["err"].item()) == 0
 
 
 # ---------------------------------------------------------------------------------------------------- full size

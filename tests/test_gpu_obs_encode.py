@@ -83,33 +83,3 @@ def test_fused_obs_encoder_equals_gather_then_dense_encoder(env_name, B, H, hint
         del of
     env.err.zero_()
 
-
-def test_trainer_dense_rollout_chunks_are_identical():
-    """The dense rollout calls the fused kernel once per chunk of env slots (args.obs_chunk_mb): any chunking gives
-    the same rollout as one chunk."""
-    from ic3net_b200 import data
-    from ic3net_b200.action_utils import parse_action_args
-    from ic3net_b200.comm import CommNetMLP
-    from ic3net_b200.trainer import Trainer
-    outs = []
-    for mb in (0.0, 0.05):
-        a = argparse.Namespace(env_name="predator_prey", nagents=4, nfriendly=4, dim=6, vision=1, mode="mixed",
-                               nenemies=1, no_stay=False, moving_prey=False, enemy_comm=False, nenvs=37, seed=11,
-                               env_id0=0, hid_size=128, recurrent=True, rnn_type="LSTM", commnet=True, hard_attn=True,
-                               comm_action_one=False, comm_mode="avg", comm_passes=1, comm_mask_zero=False,
-                               comm_init="uniform", share_weights=False, max_steps=20, batch_size=40, lrate=1e-3,
-                               obs_mode="dense", use_graph=False, obs_chunk_mb=mb)
-        env = data.init(a.env_name, a)
-        a.num_inputs = env.observation_dim
-        a.num_actions, a.dim_actions = [env.num_actions, 2], 2
-        parse_action_args(a)
-        net = CommNetMLP(a, a.num_inputs)
-        sd = make_weights(1, a.num_inputs, a.hid_size, a.naction_heads)
-        net.load_state_dict({k: torch.from_numpy(v).float() for k, v in sd.items()})
-        tr = Trainer(a, net, env)
-        batch = tr.rollout(30, 0)
-        if mb > 0:
-            assert len(tr._dense_chunks(net.policy_cfg(a.nenvs))) > 1      # the chunked path really ran
-        outs.append({k: getattr(batch, k).cpu() for k in ("action", "reward", "value")})
-    for k in outs[0]:
-        assert torch.equal(outs[0][k], outs[1][k]), k

@@ -189,7 +189,7 @@ def trainer_rows(tr, T, label, sensitivity=False):
 
     def obs(t):
         if tr.is_tj:
-            return (tj_record_obs(tr, t, 0, B) if gk else b["s_obs"][t]).reshape(R, -1).double()
+            return tj_record_obs(tr, t, 0, B).reshape(R, -1).double()
         idx, val = tr._pp_sparse_obs(b["s_loc"][t])
         return idx, val.double()
 
