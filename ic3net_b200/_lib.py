@@ -91,6 +91,15 @@ class PolicyIO(C.Structure):
                 ("x_table", _p), ("pass_index", C.c_int32)]
 
 
+def env_source(cfg, state):
+    """The PolicyIO fields through which the fused index encoder reads an environment state: pp_env / pp_state for a
+    PPCfg, tj_env / tj_state for a TJCfg.  They are bare addresses: the caller keeps cfg and state alive while they
+    are in use."""
+    if isinstance(cfg, TJCfg):
+        return dict(tj_env=C.addressof(cfg), tj_state=C.addressof(state))
+    return dict(pp_env=C.addressof(cfg), pp_state=C.addressof(state))
+
+
 class BpttPlan(C.Structure):
     _fields_ = [("cfg", C.POINTER(PolicyCfg)), ("w", C.POINTER(PolicyPacked)), ("pp_env", C.POINTER(PPCfg)),
                 ("tj_env", C.POINTER(TJCfg)), ("x_table", _p), ("value_coeff", C.c_float), ("entr", C.c_float),

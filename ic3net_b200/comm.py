@@ -13,6 +13,7 @@ fp32 SIMT kernel.  The rollout forward is inference-only (the reference detaches
 from, action_utils.py:35); gradients are taken by the trainer.
 """
 import ctypes as C
+import weakref
 
 import numpy as np
 import torch
@@ -130,13 +131,37 @@ class CommNetMLP(nn.Module):
             raise NotImplementedError("the tensor-core policy path implements the recurrent LSTM policy; the tanh-cell "
                                       "variants run on policy_impl='simt'")
         self._ws = {}
-        self._xtab, self._xtab_key = None, None     # per-position encoder table of forward() on observation handles
+        self._enc_tables = weakref.WeakKeyDictionary()     # env -> (packed-weights key, encoder_table(env))
 
     def set_obs_layout(self, off, vocab, ncount):
         """Observation layout hint (include/ic3net_b200.h, ic3_policy_cfg.obs_vocab): lets the encoder sum the
         one-hot class terms separately from the counts, so the class part can come from a per-position table and
         the dense / index / fused encoders stay bit-identical.  (0, 0, 0) = plain single sum."""
         self._cfg_proto.update(obs_off=int(off), obs_vocab=int(vocab), obs_ncount=int(ncount))
+
+    def fuses_encoder(self, env):
+        """Whether the policy step can form x from the env state itself (the fused index encoder): the tensor-core
+        path, with a vision window of at most 5x5."""
+        W = 2 * env.vision + 1
+        return self.policy_impl == 'tc' and W * W <= 25
+
+    def encoder_table(self, env):
+        """[positions, H] class part of x per agent position of env (ic3_*_encoder_table) for the current packed
+        weights, rebuilt when they change; one table per environment.  None where the fused index encoder takes no
+        table: no fused encoder (fuses_encoder), or a layout without separate class terms (obs_vocab = 0)."""
+        if not self.fuses_encoder(env) or self._cfg_proto['obs_vocab'] == 0:
+            return None
+        w = self.packed()
+        key, table = self._enc_tables.get(env, (None, None))
+        if table is None:
+            table = torch.empty(env.obs_positions, self.hid_size, device=self._dev)
+        if key != self._packed_key:
+            lib = _lib.load()
+            fn = lib.ic3_tj_encoder_table if isinstance(env.cfg, _lib.TJCfg) else lib.ic3_pp_encoder_table
+            cfg = self.policy_cfg(env.nenvs)
+            _lib.check(fn(C.byref(env.cfg), C.byref(cfg), C.byref(w), table.data_ptr(), _lib.stream()))
+            self._enc_tables[env] = (self._packed_key, table)
+        return table
 
     # ---- kernel-side weights ---------------------------------------------------
     def policy_cfg(self, B):
@@ -282,31 +307,21 @@ class CommNetMLP(nn.Module):
 
     def _index_encoder(self, obs, B):
         """Encoder input for an observation HANDLE: returns (cfg, packed weights, PolicyIO source fields, x tensor or
-        None).  Tensor-core path with a small vision window: the encoder is fused into the policy step (x is formed from
-        the env state and the per-position table inside the operand-preparation kernel); otherwise the index-form
-        encoder kernel writes x.  Either way the same sums in the same order as ic3_encoder_dense."""
+        None).  Where the policy has an encoder table for the env (encoder_table): the encoder is fused into the policy
+        step (x is formed from the env state and the table inside the operand-preparation kernel); otherwise the
+        index-form encoder kernel writes x.  Either way the same sums in the same order as ic3_encoder_dense."""
         e = obs.check_current()
         lib = _lib.load()
-        is_tj = type(e).__name__ == 'TrafficJunctionEnv'
         if self._cfg_proto['obs_vocab'] == 0 and getattr(e, 'obs_layout', (0, 0, 0))[1]:
             self.set_obs_layout(*e.obs_layout)
         cfg = self.policy_cfg(B)
         cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
         w = self.packed()
-        W = 2 * e.vision + 1
-        if self.policy_impl == 'tc' and W * W <= 25 and cfg.obs_vocab > 0:
-            if self._xtab is None:
-                self._xtab = torch.empty(e.obs_positions, self.hid_size, device=self._dev)
-            if self._xtab_key != self._packed_key:
-                fn = lib.ic3_tj_encoder_table if is_tj else lib.ic3_pp_encoder_table
-                _lib.check(fn(C.byref(e.cfg), C.byref(cfg), C.byref(w), self._xtab.data_ptr(), _lib.stream()))
-                self._xtab_key = self._packed_key
-            src = dict(tj_env=C.addressof(e.cfg), tj_state=C.addressof(e.state)) if is_tj else \
-                dict(pp_env=C.addressof(e.cfg), pp_state=C.addressof(e.state))
-            src['x_table'] = self._xtab.data_ptr()
-            return cfg, w, src, None
+        table = self.encoder_table(e)
+        if table is not None:
+            return cfg, w, dict(_lib.env_source(e.cfg, e.state), x_table=table.data_ptr()), None
         xenc = torch.empty(B * self.nagents, self.hid_size, device=self._dev)
-        fn = lib.ic3_tj_encoder_index if is_tj else lib.ic3_pp_encoder_index
+        fn = lib.ic3_tj_encoder_index if isinstance(e.cfg, _lib.TJCfg) else lib.ic3_pp_encoder_index
         _lib.check(fn(C.byref(e.cfg), C.byref(e.state), C.byref(cfg), C.byref(w), xenc.data_ptr(), _lib.stream()))
         return cfg, w, {}, xenc
 

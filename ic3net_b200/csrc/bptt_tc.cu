@@ -1005,39 +1005,6 @@ cudaError_t prefer_max_smem(K kern) {
   return cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
 }
 
-// Development aid (IC3_BPTT_TRACE=1): CUDA events after every kernel of the first steps of a compute_grad, on whatever
-// stream the kernel ran, dumped by ic3_debug_bptt_trace() as end times on one clock -- shows what overlaps what.
-constexpr int TR_STEPS = 16, TR_KERNELS = 7;     // heads, prep, scale, gates, dgrad, comm, wgrad
-struct BpttTrace {
-  bool on;
-  cudaEvent_t base, ev[TR_STEPS][TR_KERNELS];
-  bool used[TR_STEPS][TR_KERNELS];
-  int t_first;
-};
-BpttTrace* bptt_trace() {
-  static BpttTrace tr;
-  static int state = 0;
-  if (state == 0) {
-    const char* e = getenv("IC3_BPTT_TRACE");
-    tr.on = e && atoi(e) != 0;
-    if (tr.on) {
-      cudaEventCreate(&tr.base);
-      for (int i = 0; i < TR_STEPS; ++i)
-        for (int k = 0; k < TR_KERNELS; ++k) cudaEventCreate(&tr.ev[i][k]);
-    }
-    state = 1;
-  }
-  return &tr;
-}
-inline void trace_mark(int kernel, int t, cudaStream_t s) {
-  BpttTrace* tr = bptt_trace();
-  if (!tr->on) return;
-  const int i = tr->t_first - t;
-  if (i < 0 || i >= TR_STEPS) return;
-  cudaEventRecord(tr->ev[i][kernel], s);
-  tr->used[i][kernel] = true;
-}
-
 struct Layout {         // of the workspace, in bytes
   size_t a_img, p_img, dg_img, img_stride, w2_img, dout, dSs, dh_direct, gs, gr, partial, gw_part, gs_part, sc, G, Y, GSC, dC, wj, cw, losses,
       total;
@@ -1147,11 +1114,6 @@ extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) 
   BpttStreams* ss = bptt_streams();
   if (!ss) return IC3_E_UNSUPPORTED;
   ss->prepared_t[0] = ss->prepared_t[1] = -1;
-  if (BpttTrace* tr = bptt_trace(); tr->on) {
-    memset(tr->used, 0, sizeof(tr->used));
-    tr->t_first = -1;
-    cudaEventRecord(tr->base, s);
-  }
   BpttScalars init;
   memset(&init, 0, sizeof(init));
   init.cmax = cmax;
@@ -1205,8 +1167,8 @@ static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, c
     src.pp = *p->pp_env;
     memset(&src.pps, 0, sizeof(src.pps));
     src.pps.loc = const_cast<int32_t*>(io->pp_loc);
-    IC3_LAUNCH_RC(ic3_launch_pdl(prep_kernel<XSRC_PP, true, true>, dim3(2 * ntiles), dim3(PREP_THREADS), prep_T_bytes(cfg->N), s, *cfg, pio, a_img, src, bw));
-    trace_mark(1, io->t, s);
+    prep_kernel<XSRC_PP, true, true><<<2 * ntiles, PREP_THREADS, prep_T_bytes(cfg->N), s>>>(*cfg, pio, a_img, src, bw);
+    IC3_LAUNCH_CHECK();
   } else {
     if (!io->tj_loc || !io->tj_alive || !io->tj_last_act || !io->tj_route_id) return IC3_E_NULL;
     src.tj = *p->tj_env;
@@ -1215,7 +1177,8 @@ static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, c
     src.tjs.alive = const_cast<uint8_t*>(io->tj_alive);
     src.tjs.last_act = const_cast<uint8_t*>(io->tj_last_act);
     src.tjs.route_id = const_cast<int32_t*>(io->tj_route_id);
-    IC3_LAUNCH_RC(ic3_launch_pdl(prep_kernel<XSRC_TJ, true, true>, dim3(2 * ntiles), dim3(PREP_THREADS), prep_T_bytes(cfg->N), s, *cfg, pio, a_img, src, bw));
+    prep_kernel<XSRC_TJ, true, true><<<2 * ntiles, PREP_THREADS, prep_T_bytes(cfg->N), s>>>(*cfg, pio, a_img, src, bw);
+    IC3_LAUNCH_CHECK();
   }
   // ---- heads ----
   HeadsArgs ha;
@@ -1232,7 +1195,6 @@ static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, c
   ha.q = q;
   bptt_heads_kernel<<<L.nhb, 256, 0, s>>>(ha);
   IC3_LAUNCH_CHECK();
-  trace_mark(0, io->t, s);
   return IC3_OK;
 }
 
@@ -1263,7 +1225,6 @@ extern "C" int ic3_bptt_prepare(const ic3_bptt_plan* p, const ic3_bptt_step_io* 
   if (rc) return rc;
   BpttStreams* ss = bptt_streams();
   if (!ss) return IC3_E_UNSUPPORTED;
-  if (BpttTrace* tr = bptt_trace(); tr->on && tr->t_first < 0) tr->t_first = io->t;
   if (!ss->overlap) return IC3_OK;                  // ic3_bptt_step will do it inline
   const int q = io->t & 1;
   // buffer set q was last used by step t + 2: its main-stream kernels (gates / dgrad / comm read A, dout, gs, gr) and
@@ -1297,7 +1258,6 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
   __half* dg_img = reinterpret_cast<__half*>(ws + L.dg_img + (size_t)q * L.img_stride);
   BpttStreams* ss = bptt_streams();
   if (!ss) return IC3_E_UNSUPPORTED;
-  if (BpttTrace* tr = bptt_trace(); tr->on && tr->t_first < 0) tr->t_first = io->t;
   // buffer set q (images, scale) was last read by the weight-gradient kernel of step t + 2 (side stream)
   cudaError_t se = cudaStreamWaitEvent(s, ss->wgrad_done[q], 0);
   if (se != cudaSuccess) return (int)se;
@@ -1311,7 +1271,6 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
   }
   bptt_scale_kernel<<<1, 1, 0, s>>>(sc, q);
   IC3_LAUNCH_CHECK();
-  trace_mark(2, io->t, s);
 
   // ---- gates ----
   {
@@ -1333,7 +1292,6 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
     bptt_gates_kernel<<<grid, TC_P_THREADS, smem, s>>>(ga, a_img, reinterpret_cast<const __half*>(p->w->lstm_img),
                                                       (const float*)p->w->bias_cat, nitems, (const float*)p->w->head_w, nout);
     IC3_LAUNCH_CHECK();
-    trace_mark(3, io->t, s);
     se = cudaEventRecord(ss->gates_done[q], s);
     if (se != cudaSuccess) return (int)se;
   }
@@ -1353,7 +1311,6 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
     const int grid = ntiles < sm_count() ? ntiles : sm_count();
     bptt_dgrad_kernel<<<grid, TC_P_THREADS, smem, s>>>(da, dg_img, reinterpret_cast<const __half*>(ws + L.w2_img), ntiles);
     IC3_LAUNCH_CHECK();
-    trace_mark(4, io->t, s);
   }
   // ---- comm backward -> dh_{t-1} ----
   {
@@ -1363,7 +1320,6 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
     ca.fresh = io->fresh; ca.no_comm = cfg->comm_mask_zero || cfg->N < 2; ca.dh = io->dh; ca.sc = sc;
     bptt_comm_kernel<<<(cfg->B + 7) / 8, 256, 0, s>>>(ca);
     IC3_LAUNCH_CHECK();
-    trace_mark(5, io->t, s);
     se = cudaEventRecord(ss->main_done[q], s);          // buffer set q may be refilled for step t - 2 once wgrad(t) is done too
     if (se != cudaSuccess) return (int)se;
   }
@@ -1407,7 +1363,6 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
     }
     bptt_wgrad_kernel<<<2 * L.ncta_wg, WG_THREADS, smem, ws_stream>>>(wa, map_dg[q], map_a[q], map_p[q]);
     IC3_LAUNCH_CHECK();
-    trace_mark(6, io->t, ws_stream);
     se = cudaEventRecord(ss->wgrad_done[q], ws_stream);
     if (se != cudaSuccess) return (int)se;
   }
@@ -1484,20 +1439,5 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
   IC3_LAUNCH_CHECK();
   bptt_finish_heads_kernel<<<(BP_HEADS * TC_H + 255) / 256, 256, 0, s>>>(f);
   IC3_LAUNCH_CHECK();
-  return IC3_OK;
-}
-
-// Development aid: end time (us after ic3_bptt_begin) of every traced kernel, [TR_STEPS][TR_KERNELS], -1 = not recorded.
-// Not part of the C ABI; only meaningful with IC3_BPTT_TRACE=1.
-extern "C" int ic3_debug_bptt_trace(float* out) {
-  BpttTrace* tr = bptt_trace();
-  if (!tr->on) return IC3_E_UNSUPPORTED;
-  cudaDeviceSynchronize();
-  for (int i = 0; i < TR_STEPS; ++i)
-    for (int k = 0; k < TR_KERNELS; ++k) {
-      float ms = -1.f;
-      if (tr->used[i][k] && cudaEventElapsedTime(&ms, tr->base, tr->ev[i][k]) != cudaSuccess) ms = -1.f;
-      out[i * TR_KERNELS + k] = ms < 0.f ? -1.f : ms * 1000.f;
-    }
   return IC3_OK;
 }

@@ -1,21 +1,7 @@
 // Library-level entry points of the C ABI (include/ic3net_b200.h).
 #include "ic3_common.cuh"
 
-#include <cstdlib>
-
 unsigned long long g_ic3_launches = 0;
-
-// Programmatic dependent launch of the rollout kernels (ic3_common.cuh).  The early-resident dependent grids can cost
-// more than the ~1 us launch gaps they hide (they occupy SM resources the running grid wants), so it is OFF unless
-// IC3_PDL=1.
-bool ic3_pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("IC3_PDL");
-    v = (e && atoi(e) != 0) ? 1 : 0;
-  }
-  return v == 1;
-}
 
 extern "C" const char* ic3_version(void) { return "ic3net_b200 0.1 (sm_90a)"; }
 

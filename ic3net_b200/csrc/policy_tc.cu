@@ -96,21 +96,11 @@ static int launch_lstm(const ic3_policy_cfg* cfg, const ic3_policy_io* io, const
     max_ctas = per_sm * nsm;                                        // persistent grid: every CTA resident
   }
   const int nitems = 2 * ntiles_pad;                                // (tile, column half)
-  cudaLaunchConfig_t lc{};
-  lc.gridDim = dim3(nitems < max_ctas ? nitems : max_ctas);
-  lc.blockDim = dim3(TC_P_THREADS);
-  lc.dynamicSmemBytes = smem;
-  lc.stream = s;
-  cudaLaunchAttribute la[1];
-  la[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  la[0].val.programmaticStreamSerializationAllowed = 1;
-  lc.attrs = la; lc.numAttrs = ic3_pdl_enabled() ? 1 : 0;
   const __half* b_img = reinterpret_cast<const __half*>(w->lstm_img) + (size_t)io->pass_index * B_IMG_HALFS;
-  cudaError_t e = cudaLaunchKernelEx(&lc, kern, *cfg, *io, a_img, b_img,
-                                     (const float*)w->bias_cat + (size_t)io->pass_index * 4 * TC_H, nitems,
-                                     (const float*)w->head_w, nout, partial);
-  ++g_ic3_launches;
-  return e == cudaSuccess ? IC3_OK : (int)e;
+  kern<<<nitems < max_ctas ? nitems : max_ctas, TC_P_THREADS, smem, s>>>(
+      *cfg, *io, a_img, b_img, w->bias_cat + (size_t)io->pass_index * 4 * TC_H, nitems, w->head_w, nout, partial);
+  IC3_LAUNCH_CHECK();
+  return IC3_OK;
 }
 
 uint64_t ic3_tc_workspace_bytes(const ic3_policy_cfg* cfg) {
@@ -222,7 +212,8 @@ static int tc_pass(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const 
   if (src.table && !src.split) return IC3_E_RANGE;      // the table IS the first of the two sums
   prof_mark(0, s);
   if (io->x) {
-    IC3_LAUNCH_RC(ic3_launch_pdl(prep_kernel<XSRC_TENSOR, false>, dim3(2 * ntiles_pad), dim3(PREP_THREADS), prep_T_bytes(cfg->N), s, *cfg, *io, img, src, PrepBwd{}));
+    prep_kernel<XSRC_TENSOR, false><<<2 * ntiles_pad, PREP_THREADS, prep_T_bytes(cfg->N), s>>>(*cfg, *io, img, src, PrepBwd{});
+    IC3_LAUNCH_CHECK();
   } else if (io->pp_env && io->pp_state) {       // fused index encoder, predator-prey
     const int W = 2 * io->pp_env->vision + 1;
     if (W * W > PREP_MAX_WW || io->pp_env->B != cfg->B || ic3_pp_agents(*io->pp_env) != cfg->N) return IC3_E_RANGE;
@@ -231,7 +222,8 @@ static int tc_pass(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const 
     src.pps = *io->pp_state;
     if (int lrc = ic3_pp_layout_check(io->pp_env, cfg)) return lrc;
     if (src.table) {
-      IC3_LAUNCH_RC(ic3_launch_pdl(prep_kernel<XSRC_PP, true>, dim3(2 * ntiles_pad), dim3(PREP_THREADS), prep_T_bytes(cfg->N), s, *cfg, *io, img, src, PrepBwd{}));
+      prep_kernel<XSRC_PP, true><<<2 * ntiles_pad, PREP_THREADS, prep_T_bytes(cfg->N), s>>>(*cfg, *io, img, src, PrepBwd{});
+      IC3_LAUNCH_CHECK();
     } else {
       static bool cfgd = false;
       if (!cfgd) {
@@ -239,7 +231,8 @@ static int tc_pass(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const 
         if (e != cudaSuccess) return (int)e;
         cfgd = true;
       }
-      IC3_LAUNCH_RC(ic3_launch_pdl(prep_kernel<XSRC_PP, false>, dim3(2 * ntiles_pad), dim3(256), PREP_X_BYTES + prep_T_bytes(cfg->N), s, *cfg, *io, img, src, PrepBwd{}));
+      prep_kernel<XSRC_PP, false><<<2 * ntiles_pad, 256, PREP_X_BYTES + prep_T_bytes(cfg->N), s>>>(*cfg, *io, img, src, PrepBwd{});
+      IC3_LAUNCH_CHECK();
     }
   } else if (io->tj_env && io->tj_state) {       // fused index encoder, traffic junction
     const int W = 2 * io->tj_env->vision + 1;
@@ -249,7 +242,8 @@ static int tc_pass(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const 
     src.tjs = *io->tj_state;
     if (int lrc = ic3_tj_layout_check(io->tj_env, cfg)) return lrc;
     if (src.table) {
-      IC3_LAUNCH_RC(ic3_launch_pdl(prep_kernel<XSRC_TJ, true>, dim3(2 * ntiles_pad), dim3(PREP_THREADS), prep_T_bytes(cfg->N), s, *cfg, *io, img, src, PrepBwd{}));
+      prep_kernel<XSRC_TJ, true><<<2 * ntiles_pad, PREP_THREADS, prep_T_bytes(cfg->N), s>>>(*cfg, *io, img, src, PrepBwd{});
+      IC3_LAUNCH_CHECK();
     } else {
       static bool cfgd = false;
       if (!cfgd) {
@@ -257,7 +251,8 @@ static int tc_pass(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const 
         if (e != cudaSuccess) return (int)e;
         cfgd = true;
       }
-      IC3_LAUNCH_RC(ic3_launch_pdl(prep_kernel<XSRC_TJ, false>, dim3(2 * ntiles_pad), dim3(256), PREP_X_BYTES + prep_T_bytes(cfg->N), s, *cfg, *io, img, src, PrepBwd{}));
+      prep_kernel<XSRC_TJ, false><<<2 * ntiles_pad, 256, PREP_X_BYTES + prep_T_bytes(cfg->N), s>>>(*cfg, *io, img, src, PrepBwd{});
+      IC3_LAUNCH_CHECK();
     }
   } else {
     return IC3_E_NULL;
@@ -275,8 +270,8 @@ static int tc_pass(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const 
   prof_mark(2, s);
   if (!last) return IC3_OK;                  // heads after the last comm pass only
   if (fused_heads) {
-    IC3_LAUNCH_RC(ic3_launch_pdl(heads_finish_kernel, dim3((unsigned)((R + 127) / 128)), dim3(128), 0, s, *cfg, *w, *io,
-                                 (const float*)partial));
+    heads_finish_kernel<<<(unsigned)((R + 127) / 128), 128, 0, s>>>(*cfg, *w, *io, partial);
+    IC3_LAUNCH_CHECK();
     prof_mark(3, s);
     return IC3_OK;
   }

@@ -151,12 +151,10 @@ __global__ void __launch_bounds__(256) prep_kernel(ic3_policy_cfg cfg, ic3_polic
   const int R = cfg.B * N;
   const int tile = blockIdx.x >> 1, hb = blockIdx.x & 1;
   const int row0 = tile * TC_M + hb * PREP_ROWS;
-  ic3_pdl_trigger();
   if (TAB) {
     if (threadIdx.x < PREP_ROWS) s_mask[threadIdx.x] = 0u;
     __syncthreads();
   }
-  ic3_pdl_wait();      // h, masks, env state: written by the previous kernels of the step
   if (blockIdx.x == 0 && threadIdx.x == 0 && src.wflags && io.err && *src.wflags) atomicOr(io.err, *src.wflags);
   for (int w = threadIdx.x; w < PREP_ROWS + 64; w += blockDim.x) {
     const int row = row0 - 32 + w;
@@ -648,7 +646,6 @@ __global__ void __launch_bounds__(TC_P_THREADS, 1) lstm_tc_kernel(ic3_policy_cfg
   // of its hidden units into per-slot partial logits (partial != nullptr  <=>  nout <= 8)
   float* s_hw = reinterpret_cast<float*>(smem + NSTAGE_P * STAGE_BYTES + 256);
   float* s_bias = s_hw + TC_H * HEAD_PAD;
-  ic3_pdl_trigger();
   const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + NSTAGE_P);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -658,9 +655,6 @@ __global__ void __launch_bounds__(TC_P_THREADS, 1) lstm_tc_kernel(ic3_policy_cfg
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  // barriers are set up while the previous kernel (prep) drains; weights (they may have been re-packed by an earlier
-  // kernel of the stream) and the operand image are only touched from here on
-  ic3_pdl_wait();
   load_scaled_bias(s_bias, bias_cat);
   if (partial) {
     for (int idx = threadIdx.x; idx < TC_H * HEAD_PAD; idx += blockDim.x) {
@@ -778,8 +772,6 @@ __global__ void __launch_bounds__(256) heads_kernel(ic3_policy_cfg cfg, ic3_poli
 // value, log-softmax per head, inverse-CDF sampling.  One thread per agent row.
 __global__ void __launch_bounds__(128) heads_finish_kernel(ic3_policy_cfg cfg, ic3_policy_packed w, ic3_policy_io io,
                                                             const float* __restrict__ partial) {
-  ic3_pdl_trigger();
-  ic3_pdl_wait();      // the partial logits come from the LSTM kernel
   const long row = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (row >= (long)cfg.B * cfg.N) return;
   HeadsFinish f;

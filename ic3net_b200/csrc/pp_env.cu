@@ -118,8 +118,6 @@ template <bool VEC4>
 __global__ void pp_step_kernel(PPArgs a, const int32_t* __restrict__ act, int act_stride,
                                float* __restrict__ reward, float* __restrict__ obs, int32_t* err,
                                RolloutOpt r, int do_step, int keep_l2) {
-  ic3_pdl_trigger();
-  ic3_pdl_wait();      // everything below reads state / actions written by the previous kernel of the step
   extern __shared__ uint32_t s_cell[];
   __shared__ int s_r[IC3_MAX_AGENTS + 1], s_c[IC3_MAX_AGENTS + 1];
   const int N = a.cfg.N, D = a.cfg.dim;
@@ -220,8 +218,6 @@ template <int H, bool VEC4>
 __global__ void __launch_bounds__(256) pp_obs_encode_kernel(PPArgs a, float* __restrict__ obs,
                                                             const float* __restrict__ wT, const float* __restrict__ bias,
                                                             float* __restrict__ x, bool split, int keep_l2) {
-  ic3_pdl_trigger();
-  ic3_pdl_wait();      // the state comes from the env step launched before; x is read by the policy step after
   extern __shared__ uint32_t s_cell[];
   __shared__ int s_r[IC3_MAX_AGENTS + 1], s_c[IC3_MAX_AGENTS + 1];
   const int N = a.cfg.N, D = a.cfg.dim, W = 2 * a.cfg.vision + 1, WW = W * W, V = D * D + 4;
@@ -248,8 +244,6 @@ __global__ void __launch_bounds__(256) pp_obs_encode_kernel(PPArgs a, float* __r
 template <bool VEC4>
 __global__ void __launch_bounds__(IC3_OBS_WRITER_THREADS, IC3_OBS_WRITER_MIN_CTAS)
     pp_obs_writer_kernel(PPArgs a, float* __restrict__ obs, int keep_l2) {
-  ic3_pdl_trigger();
-  ic3_pdl_wait();
   extern __shared__ uint32_t s_cell[];
   __shared__ int s_r[IC3_MAX_AGENTS + 1], s_c[IC3_MAX_AGENTS + 1];
   const int N = a.cfg.N, W = 2 * a.cfg.vision + 1, B = a.cfg.B;
@@ -303,11 +297,10 @@ int pp_launch(const ic3_pp_cfg* cfg, const ic3_pp_state* st, const int32_t* act,
   // small observation batches stay in L2 for the encoder that follows (see IC3_OBS_L2_KEEP_BYTES)
   const int keep = obs && (size_t)cfg->B * NA * W * W * V * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
   if (vec4)
-    IC3_LAUNCH_RC(ic3_launch_pdl(pp_step_kernel<true>, dim3(grid), dim3(threads), smem, s, a, act, act_stride, reward, obs,
-                                 err, ro, do_step, keep));
+    pp_step_kernel<true><<<grid, threads, smem, s>>>(a, act, act_stride, reward, obs, err, ro, do_step, keep);
   else
-    IC3_LAUNCH_RC(ic3_launch_pdl(pp_step_kernel<false>, dim3(grid), dim3(threads), smem, s, a, act, act_stride, reward, obs,
-                                 err, ro, do_step, keep));
+    pp_step_kernel<false><<<grid, threads, smem, s>>>(a, act, act_stride, reward, obs, err, ro, do_step, keep);
+  IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
 
@@ -324,11 +317,10 @@ int pp_obs_encode_launch(const ic3_pp_cfg* cfg, const ic3_pp_state* st, const ic
   const float* wT = w->enc_wT;
   const float* b = w->enc_b;
   if (vec4)
-    IC3_LAUNCH_RC(ic3_launch_pdl(pp_obs_encode_kernel<H, true>, dim3(cfg->B), dim3(256), smem, s, a, obs, wT, b, x, split,
-                                 keep));
+    pp_obs_encode_kernel<H, true><<<cfg->B, 256, smem, s>>>(a, obs, wT, b, x, split, keep);
   else
-    IC3_LAUNCH_RC(ic3_launch_pdl(pp_obs_encode_kernel<H, false>, dim3(cfg->B), dim3(256), smem, s, a, obs, wT, b, x, split,
-                                 keep));
+    pp_obs_encode_kernel<H, false><<<cfg->B, 256, smem, s>>>(a, obs, wT, b, x, split, keep);
+  IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
 
@@ -342,7 +334,8 @@ int pp_obs_bounded_launch(const ic3_pp_cfg* cfg, const ic3_pp_state* st, float* 
   int grid = 0;
   const int rc = ic3_grid_beside_lstm((const void*)kern, IC3_OBS_WRITER_THREADS, smem, cfg->B, &grid);
   if (rc) return rc;
-  IC3_LAUNCH_RC(ic3_launch_pdl(kern, dim3(grid), dim3(IC3_OBS_WRITER_THREADS), smem, s, a, obs, keep));
+  kern<<<grid, IC3_OBS_WRITER_THREADS, smem, s>>>(a, obs, keep);
+  IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
 

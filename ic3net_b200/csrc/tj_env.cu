@@ -92,8 +92,6 @@ __device__ __forceinline__ void tj_write_obs(const ic3_tj_cfg& cfg, const int* s
 __global__ void tj_step_kernel(TJArgs a, const int32_t* __restrict__ act, int act_stride,
                                const uint32_t* __restrict__ draws, float* __restrict__ reward,
                                float* __restrict__ obs, int32_t* err, RolloutOpt r, int do_step, int keep_l2) {
-  ic3_pdl_trigger();
-  ic3_pdl_wait();      // everything below reads state / actions written by the previous kernel of the step
   extern __shared__ uint32_t s_cell[];
   __shared__ int s_r[IC3_MAX_AGENTS], s_c[IC3_MAX_AGENTS], s_alive[IC3_MAX_AGENTS], s_rid[IC3_MAX_AGENTS],
       s_lact[IC3_MAX_AGENTS];
@@ -250,8 +248,6 @@ template <int H>
 __global__ void __launch_bounds__(128) tj_obs_encode_kernel(TJArgs a, float* __restrict__ obs,
                                                             const float* __restrict__ wT, const float* __restrict__ bias,
                                                             float* __restrict__ x, bool split, int keep_l2) {
-  ic3_pdl_trigger();
-  ic3_pdl_wait();      // the state comes from the env step launched before; x is read by the policy step after
   extern __shared__ uint32_t s_cell[];
   __shared__ int s_r[IC3_MAX_AGENTS], s_c[IC3_MAX_AGENTS], s_alive[IC3_MAX_AGENTS], s_rid[IC3_MAX_AGENTS],
       s_lact[IC3_MAX_AGENTS];
@@ -283,8 +279,6 @@ __global__ void __launch_bounds__(128) tj_obs_encode_kernel(TJArgs a, float* __r
 // a persistent grid that strides over the envs (ic3_tj_obs_bounded); see pp_obs_writer_kernel.
 __global__ void __launch_bounds__(IC3_OBS_WRITER_THREADS, IC3_OBS_WRITER_MIN_CTAS)
     tj_obs_writer_kernel(TJArgs a, float* __restrict__ obs, int keep_l2) {
-  ic3_pdl_trigger();
-  ic3_pdl_wait();
   extern __shared__ uint32_t s_cell[];
   __shared__ int s_r[IC3_MAX_AGENTS], s_c[IC3_MAX_AGENTS], s_alive[IC3_MAX_AGENTS], s_rid[IC3_MAX_AGENTS],
       s_lact[IC3_MAX_AGENTS];
@@ -341,8 +335,8 @@ int tj_launch(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const int32_t* act,
   const int grid = obs ? cfg->B : (cfg->B + IC3_ENV_WARPS - 1) / IC3_ENV_WARPS;
   RolloutOpt ro = make_rollout_opt(r);
   const int keep = obs && (size_t)cfg->B * cfg->N * (2 + W * W * cfg->vocab) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
-  IC3_LAUNCH_RC(ic3_launch_pdl(tj_step_kernel, dim3(grid), dim3(threads), smem, s, a, act, act_stride, draws, reward, obs, err,
-                               ro, do_step, keep));
+  tj_step_kernel<<<grid, threads, smem, s>>>(a, act, act_stride, draws, reward, obs, err, ro, do_step, keep);
+  IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
 
@@ -355,8 +349,8 @@ int tj_obs_encode_launch(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const ic
   const bool split = pcfg->obs_vocab > 0;
   // same store policy as ic3_tj_obs: batches that fit in L2 stay there for a reader that follows
   const int keep = (size_t)cfg->B * cfg->N * (2 + W * W * cfg->vocab) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
-  IC3_LAUNCH_RC(ic3_launch_pdl(tj_obs_encode_kernel<H>, dim3(cfg->B), dim3(128), smem, s, a, obs, (const float*)w->enc_wT,
-                               (const float*)w->enc_b, x, split, keep));
+  tj_obs_encode_kernel<H><<<cfg->B, 128, smem, s>>>(a, obs, w->enc_wT, w->enc_b, x, split, keep);
+  IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
 
@@ -373,8 +367,8 @@ extern "C" int ic3_tj_obs_bounded(const ic3_tj_cfg* cfg, const ic3_tj_state* st,
   int grid = 0;
   rc = ic3_grid_beside_lstm((const void*)tj_obs_writer_kernel, IC3_OBS_WRITER_THREADS, smem, cfg->B, &grid);
   if (rc) return rc;
-  IC3_LAUNCH_RC(ic3_launch_pdl(tj_obs_writer_kernel, dim3(grid), dim3(IC3_OBS_WRITER_THREADS), smem,
-                               (cudaStream_t)stream, a, obs, keep));
+  tj_obs_writer_kernel<<<grid, IC3_OBS_WRITER_THREADS, smem, (cudaStream_t)stream>>>(a, obs, keep);
+  IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
 

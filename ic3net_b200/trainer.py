@@ -120,12 +120,9 @@ class Trainer(object):
         self._graph = None
         self._graph_key = None
         self._side = None                    # stream of the dense observation writer (_overlap_obs)
-        # encoder layout of this environment (class terms / counts summed separately, comm.py set_obs_layout) and
-        # the per-position table of the class terms for the fused index encoder, rebuilt when the weights change
+        # encoder layout of this environment (class terms / counts summed separately, comm.py set_obs_layout); the
+        # fused index encoder's per-position table of the class terms belongs to the policy (encoder_table)
         policy_net.set_obs_layout(*getattr(env.env, 'obs_layout', (0, 0, 0)))
-        self.use_xtable = bool(getattr(args, 'encoder_table', True))
-        self._xtable = None
-        self._xtable_key = None
         if self.record_for_grad and self.grad_impl in ('auto', 'kernels'):
             ok = self._bptt_supported()
             if self.grad_impl == 'kernels' and not ok:
@@ -138,7 +135,7 @@ class Trainer(object):
     def _bptt_supported(self):
         e, net = self.env.env, self.policy_net
         W = 2 * e.vision + 1
-        if net.policy_impl != 'tc' or not self.use_xtable or W * W > 25 or 1 + sum(self.args.naction_heads) > 8:
+        if not net.fuses_encoder(e) or 1 + sum(self.args.naction_heads) > 8:
             return False
         if getattr(net, 'is_variant', False):          # the BPTT kernels differentiate ONE comm pass
             return False
@@ -148,19 +145,10 @@ class Trainer(object):
         used = npos + ((W * W + 4) if self.is_tj else (2 * W * W + 1))
         return (used + 15) // 16 * 16 <= 512
 
-    def _encoder_table(self, cfg, w):
-        """[positions, H] class part of x per agent position for the CURRENT weights (None when not applicable)."""
-        e, net = self.env.env, self.policy_net
-        if not self.use_xtable or cfg.obs_vocab == 0:
-            return None
-        key = net._packed_key
-        if self._xtable is None:
-            self._xtable = torch.empty(e.obs_positions, net.hid_size, device=e.device)
-        if key != self._xtable_key:
-            fn = _lib.load().ic3_tj_encoder_table if self.is_tj else _lib.load().ic3_pp_encoder_table
-            _lib.check(fn(C.byref(e.cfg), C.byref(cfg), C.byref(w), self._xtable.data_ptr(), _lib.stream()))
-            self._xtable_key = key
-        return self._xtable
+    def _encoder_table(self, cfg=None, w=None):
+        """The policy's per-position encoder table for this environment (CommNetMLP.encoder_table), built from its
+        current packed weights; cfg and w are accepted for callers that hold them and are not needed."""
+        return self.policy_net.encoder_table(self.env.env)
 
     # ------------------------------------------------------------------ buffers
     def _alloc(self, T):
@@ -266,8 +254,7 @@ class Trainer(object):
     # ------------------------------------------------------------------ rollout
     def _fused_x(self):
         """Index-form observations on the tensor-core policy path: the encoder runs inside the policy step."""
-        W = 2 * self.env.env.vision + 1
-        return self.obs_mode != 'dense' and self.policy_net.policy_impl == 'tc' and W * W <= 25
+        return self.obs_mode != 'dense' and self.policy_net.fuses_encoder(self.env.env)
 
     # Smaller observation blocks per step keep the fused gather + encoder: their write is short and latency-bound in the
     # persistent writer (measured on an H100: predator-prey easy, 2.9 MB, 3 % slower with the overlap; traffic-junction
@@ -284,8 +271,7 @@ class Trainer(object):
         e = self.env.env
         if e.nenvs * self.args.nagents * self.env.observation_dim * 4 < self.OVERLAP_MIN_OBS_BYTES:
             return False
-        W = 2 * e.vision + 1
-        return self.policy_net.policy_impl == 'tc' and W * W <= 25
+        return self.policy_net.fuses_encoder(e)
 
     def _enqueue(self, T, quota=0):
         """Enqueue T lock-step iterations on the current stream (no host sync).  quota > 0: reference batch
@@ -311,9 +297,7 @@ class Trainer(object):
         fused_x = self._fused_x() or overlap
         src = {}
         if fused_x:
-            src = dict(tj_env=C.addressof(e.cfg), tj_state=C.addressof(e.state)) if self.is_tj else \
-                dict(pp_env=C.addressof(e.cfg), pp_state=C.addressof(e.state))
-            src['x_table'] = None if overlap else _lib.ptr(self._encoder_table(cfg, w))
+            src = dict(_lib.env_source(e.cfg, e.state), x_table=None if overlap else _lib.ptr(self._encoder_table()))
         if overlap:
             main = torch.cuda.current_stream()
             if self._side is None or self._side.device != main.device:
@@ -419,7 +403,7 @@ class Trainer(object):
         b['err'].zero_()
         w = self.policy_net.packed()              # (re)pack weights outside any graph capture
         if self._fused_x():
-            self._encoder_table(self.policy_net.policy_cfg(e.nenvs), w)  # ... and the encoder table with them
+            self._encoder_table()                 # ... and the encoder table with them
         if self.use_graph:
             # kernel arguments passed BY VALUE are frozen into a captured graph: everything of that kind that can
             # change between rollouts is part of the key (the TJ curriculum moves cfg.spawn_thr, traffic_junction_env.py:
@@ -681,7 +665,7 @@ class Trainer(object):
         cfg = net.policy_cfg(B)
         cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
         w = net.packed()
-        table = self._encoder_table(cfg, w)
+        table = self._encoder_table()
         if self._bptt is None or self._bptt['B'] != B:
             plan = _lib.BpttPlan(cfg=C.pointer(cfg), w=C.pointer(w),
                                  pp_env=None if self.is_tj else C.pointer(e.cfg),
@@ -782,7 +766,7 @@ class Trainer(object):
         cfg = net.policy_cfg(B)
         cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
         w = net.packed()
-        table = self._encoder_table(cfg, w)
+        table = self._encoder_table()
         ws, _ = net.workspace(B)
         hard = bool(args.hard_attn) and bool(args.commnet)
         nb = self._window_buffers()
@@ -791,9 +775,8 @@ class Trainer(object):
         for t in range(t0, t1):
             j = t - t0
             hin, cin = (b['ck_h'][k], b['ck_c'][k]) if j == 0 else (wh[j - 1], wc[j - 1])
-            ecfg, est = self._record_state(t)
-            src = dict(tj_env=C.addressof(ecfg), tj_state=C.addressof(est)) if self.is_tj else \
-                dict(pp_env=C.addressof(ecfg), pp_state=C.addressof(est))
+            ecfg, est = self._record_state(t)          # held until the policy step below has read them
+            src = _lib.env_source(ecfg, est)
             io = _lib.PolicyIO(x=None, h=hin.data_ptr(), c=cin.data_ptr(),
                                comm_action=b['s_comm'][t].data_ptr() if hard else None,
                                alive=b['s_alive'][t].data_ptr(), fresh=b['s_fresh'][t].data_ptr(), tick=None,

@@ -145,19 +145,24 @@ def test_graph_replay_equals_eager():
         assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1]) and np.array_equal(a[2], b[2])
 
 
-@pytest.mark.parametrize("name", ["ep_pp_hard_ic3net", "ep_tj_medium_ic3net", "ep_tj_medium_v1_commnet"])
-def test_dense_and_index_rollouts_are_identical(name):
-    """Dense obs + dense encoder, fused index encoder from the per-position table, fused index encoder without
-    the table: bit-identical rollouts (same additions in the same order, include/ic3net_b200.h obs_vocab)."""
+@pytest.mark.parametrize("name", ["ep_pp_hard_ic3net", "ep_tj_medium_ic3net", "ep_tj_medium_v1_commnet",
+                                  "ep_tj_hard_ic3net", "ep_pp_enemy_ic3net"])
+def test_encoder_forms_give_identical_rollouts(name):
+    """Fused index encoder from the per-position table (index mode), fused index encoder without the table (dense mode
+    with the observation block written on a side stream) and obs gather + dense encoder (dense mode, one stream):
+    bit-identical rollouts (same additions in the same order, include/ic3net_b200.h obs_vocab)."""
     meta, z = load_golden(name)
     if meta["args"]["hid_size"] != 128:
         pytest.skip("fused encoder is part of the tensor-core path (hid_size 128)")
     res = []
-    for mode, table in (("index", True), ("index", False), ("dense", True)):
-        args, env, net, tr, p = build(meta, 24, mode, seed=77, encoder_table=table)
+    for mode, overlap in (("index", False), ("dense", True), ("dense", False)):
+        args, env, net, tr, p = build(meta, 24, mode, seed=77)
+        if overlap:
+            tr.OVERLAP_MIN_OBS_BYTES = 0             # the small fixtures take the two-stream path too
+        assert tr._overlap_obs() == overlap
         b = tr.rollout(30, 0)
         torch.cuda.synchronize()
-        assert (tr._xtable is not None) == (mode == "index" and table)
+        assert (env.env in net._enc_tables) == (mode == "index")
         res.append((cpu(b.action).copy(), cpu(b.value).copy(), cpu(b.reward).copy()))
     for k in (1, 2):
         assert np.array_equal(res[0][0], res[k][0]) and np.array_equal(res[0][1], res[k][1])
