@@ -107,7 +107,7 @@ class BpttPlan(C.Structure):
 
 
 class BpttStepIO(C.Structure):
-    _fields_ = [("t", C.c_int32), ("reserved0", C.c_int32), ("h_prev", _p), ("c_prev", _p), ("h_new", _p), ("fresh", _p), ("comm", _p), ("alive", _p), ("cut", _p),
+    _fields_ = [("t", C.c_int32), ("pass_index", C.c_int32), ("h_prev", _p), ("c_prev", _p), ("h_new", _p), ("fresh", _p), ("comm", _p), ("alive", _p), ("cut", _p),
                 ("pp_loc", _p), ("tj_loc", _p), ("tj_alive", _p), ("tj_last_act", _p), ("tj_route_id", _p),
                 ("logp", _p), ("action", _p), ("value", _p), ("ret", _p), ("adv", _p), ("alive_post", _p),
                 ("valid", _p), ("dh", _p), ("dc", _p), ("err", _p)]
@@ -145,6 +145,8 @@ SYMBOLS = {
     "ic3_policy_step": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), C.POINTER(PolicyIO), _PTR]),
     "ic3_policy_step_profile": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), C.POINTER(PolicyIO), _PTR,
                                           C.POINTER(C.c_float)]),
+    "ic3_policy_pass_states": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), C.POINTER(PolicyIO), C.c_int32,
+                                         _PTR, _PTR, _PTR]),
     "ic3_sample_actions": (C.c_int, [C.POINTER(PolicyCfg), _PTR, _PTR, _PTR, _PTR, _PTR]),
     "ic3_returns_scan": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, _PTR, _PTR, _PTR, _PTR,
                                    _PTR]),

@@ -1,6 +1,8 @@
 // Back-propagation through time of the rollout loss (Trainer.compute_grad, reference trainer.py:128-225) as
 // hand-written sm_90a kernels (H = 128).  One call of ic3_bptt_step differentiates ONE lock-step iteration t of
-// the recorded rollout for all env slots; the host walks t = T-1 .. 0.  Per step:
+// the recorded rollout for all env slots; the host walks t = T-1 .. 0.  With comm_passes P > 1 a step is P backward
+// units (t, P-1) .. (t, 0), each the chain below on its pass's weight image (heads on the last pass only), after the
+// states entering passes 1 .. P-1 have been re-run from the record (ic3_tc_pass_states).  Per unit:
 //
 //   heads      d(loss)/d(value, logits) from the records (advantages, log-probs, actions, masks), the value /
 //              action-head weight gradients, the three loss sums                               [bptt_heads_kernel]
@@ -1006,12 +1008,16 @@ cudaError_t prefer_max_smem(K kern) {
 }
 
 struct Layout {         // of the workspace, in bytes
-  size_t a_img, p_img, dg_img, img_stride, w2_img, dout, dSs, dh_direct, gs, gr, partial, gw_part, gs_part, sc, G, Y, GSC, dC, wj, cw, losses,
-      total;
+  size_t a_img, p_img, dg_img, img_stride, w2_img, hc_pass, tc_ws, dout, dSs, dh_direct, gs, gr, partial, part_stride, dout0,
+      gw_part, gs_part, sc, G, Y, GSC, dC, wj, cw, losses, total;
   int ntiles, np, npos, WW, j0, j1, ncta_wg, nhb;
+  int P;                // comm passes: backward units per lock-step
 };
 
 int plan_layout(const ic3_policy_cfg* cfg, int npos, int WW, int is_tj, Layout* L) {
+  // the LSTM-cell policies of the tensor-core path, 1 .. IC3_MAX_PASSES comm passes
+  if (cfg->cell != IC3_CELL_LSTM || cfg->x_tanh || cfg->h_from_x || cfg->passes > IC3_MAX_PASSES) return IC3_E_UNSUPPORTED;
+  L->P = cfg->passes > 1 ? cfg->passes : 1;
   const long R = (long)cfg->B * cfg->N;
   L->ntiles = (int)((R + TC_M - 1) / TC_M);
   L->npos = npos;
@@ -1039,13 +1045,22 @@ int plan_layout(const ic3_policy_cfg* cfg, int npos, int WW, int is_tj, Layout* 
   L->dg_img = take((size_t)L->ntiles * DG_TILE_HALFS * 2);
   L->img_stride = off;
   take(off);                                   // second set: same sizes, same order
-  L->w2_img = take(W2_IMG_HALFS * 2);
+  L->w2_img = take((size_t)L->P * W2_IMG_HALFS * 2);                    // one dgrad weight image per pass
+  // comm_passes > 1: (h, c) after passes 0 .. P-2 of the step being differentiated (re-run from the record by
+  // ic3_tc_pass_states), and the scratch of that re-run (operand image, head partials)
+  ic3_policy_cfg one_pass = *cfg;
+  one_pass.passes = 1;
+  L->hc_pass = take(L->P > 1 ? (size_t)(L->P - 1) * 2 * R * TC_H * 4 : 0);
+  L->tc_ws = take(L->P > 1 ? (size_t)ic3_tc_workspace_bytes(&one_pass) : 0);
   L->dout = take((size_t)2 * L->ntiles * TC_M * BP_HEADS * 4);         // [2]: heads of step t - 1 run while step t reads
   L->dSs = take((size_t)L->ntiles * TC_M * TC_H * 4);
   L->dh_direct = take((size_t)L->ntiles * TC_M * TC_H * 4);
   L->gs = take((size_t)2 * L->ntiles * TC_M * 4);                       // [2] by step parity, like the images
   L->gr = take((size_t)2 * L->ntiles * TC_M * 4);
-  L->partial = take((size_t)L->ncta_wg * 512 * 128 * 4);
+  // weight-gradient partials per pass: the S block and the constant column of G belong to pass p's C_modules[p]
+  L->part_stride = (size_t)L->ncta_wg * 512 * 128 * 4;
+  L->partial = take((size_t)L->P * L->part_stride);
+  L->dout0 = take(L->P > 1 ? (size_t)L->ntiles * TC_M * BP_HEADS * 4 : 0);   // zeros: no heads after passes < P-1
   L->gw_part = take((size_t)L->nhb * BP_HEADS * TC_H * 4);
   L->gs_part = take((size_t)L->nhb * (BP_HEADS + 3) * 8);
   L->sc = take(sizeof(BpttScalars));
@@ -1108,15 +1123,20 @@ extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) 
   if (e != cudaSuccess) return (int)e;
   e = cudaMemsetAsync(ws + L.a_img, 0, L.w2_img - L.a_img, s);                  // both image sets
   if (e != cudaSuccess) return (int)e;
-  bptt_pack_w2_kernel<<<(256 * 512 + 255) / 256, 256, 0, s>>>(reinterpret_cast<const __half*>(p->w->lstm_img),
-                                                              reinterpret_cast<__half*>(ws + L.w2_img));
-  IC3_LAUNCH_CHECK();
+  for (int ps = 0; ps < L.P; ++ps) {           // w->lstm_img holds the forward image of every pass, back to back
+    bptt_pack_w2_kernel<<<(256 * 512 + 255) / 256, 256, 0, s>>>(
+        reinterpret_cast<const __half*>(p->w->lstm_img) + (size_t)ps * B_IMG_HALFS,
+        reinterpret_cast<__half*>(ws + L.w2_img) + (size_t)ps * W2_IMG_HALFS);
+    IC3_LAUNCH_CHECK();
+  }
   BpttStreams* ss = bptt_streams();
   if (!ss) return IC3_E_UNSUPPORTED;
   ss->prepared_t[0] = ss->prepared_t[1] = -1;
   BpttScalars init;
   memset(&init, 0, sizeof(init));
-  init.cmax = cmax;
+  // the cell states entering passes 1 .. P-1 are not in the record: each pass changes |c| by at most 1
+  // (|f c + i g| <= |c| + 1), so |c^p| <= |c_{t-1}| + p bounds them
+  init.cmax = L.P > 1 ? cmax + (float)(L.P - 1) : cmax;
   init.scale[0] = init.scale[1] = 1.f;
   init.inv_scale[0] = init.inv_scale[1] = 1.f;
   e = cudaMemcpyAsync(ws + L.sc, &init, sizeof(init), cudaMemcpyHostToDevice, s);
@@ -1130,25 +1150,26 @@ extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) 
   return IC3_OK;
 }
 
-// Recursion-independent part of a step: d loss / d outputs from the records (heads) and the operand images of the
-// step (prep).  Runs on `s` into buffer set q = t & 1.
+// Recursion-independent part of a backward unit (step t, comm pass ps): the operand images of the pass (prep) from
+// the state h_in entering it, and -- for the last pass only -- d loss / d outputs from the records (heads).  Runs on
+// `s` into buffer set q (parity of the unit counter t * P + ps).
 static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const Layout& L, int npos, int is_tj,
-                           cudaStream_t s) {
+                           cudaStream_t s, int q, int ps, const float* h_in) {
   const ic3_policy_cfg* cfg = p->cfg;
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
   const int R = cfg->B * cfg->N;
   int atot = 0;
   for (int k = 0; k < cfg->nheads; ++k) atot += cfg->head_dim[k];
   BpttScalars* sc = reinterpret_cast<BpttScalars*>(ws + L.sc);
-  const int q = io->t & 1;
   const size_t rows_pad = (size_t)L.ntiles * TC_M;
   __half* a_img = reinterpret_cast<__half*>(ws + L.a_img + (size_t)q * L.img_stride);
   __half* p_img = reinterpret_cast<__half*>(ws + L.p_img + (size_t)q * L.img_stride);
-  // ---- operand images of step t from the records ----
+  // ---- operand images of pass ps of step t from the records ----
   ic3_policy_io pio;
   memset(&pio, 0, sizeof(pio));
-  pio.h = io->h_prev; pio.c = io->c_prev; pio.comm_action = io->comm; pio.alive = io->alive; pio.fresh = io->fresh;
+  pio.h = h_in; pio.c = io->c_prev; pio.comm_action = io->comm; pio.alive = io->alive; pio.fresh = io->fresh;
   pio.err = io->err;
+  pio.pass_index = ps;                 // a fresh slot's zero state and silent first pass apply to pass 0 only
   if (cfg->hard_attn && !io->comm) return IC3_E_NULL;
   PrepSrc src;
   memset(&src, 0, sizeof(src));
@@ -1180,6 +1201,7 @@ static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, c
     prep_kernel<XSRC_TJ, true, true><<<2 * ntiles, PREP_THREADS, prep_T_bytes(cfg->N), s>>>(*cfg, pio, a_img, src, bw);
     IC3_LAUNCH_CHECK();
   }
+  if (ps != L.P - 1) return IC3_OK;    // heads and loss act on the last pass's h'
   // ---- heads ----
   HeadsArgs ha;
   memset(&ha, 0, sizeof(ha));
@@ -1218,6 +1240,9 @@ static int bptt_common(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, Layou
 // on the library's side stream, so that they overlap the tensor-core kernels of step t + 1 (which leave one CTA slot
 // per SM free).  `stream` is the stream ic3_bptt_step will be called on.  Without this call (or with
 // IC3_BPTT_OVERLAP=0) ic3_bptt_step runs them itself.
+// comm_passes > 1: a no-op.  The units (t, p) of a step alternate the two buffer sets, so the set the look-ahead of
+// step t - 1 would fill is the one unit (t, 1) uses, and the operand images of passes >= 1 need the re-run pass
+// states; ic3_bptt_step then prepares every unit inline (the weight-gradient kernels still run on the side stream).
 extern "C" int ic3_bptt_prepare(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, void* stream) {
   Layout L;
   int npos, is_tj;
@@ -1225,13 +1250,13 @@ extern "C" int ic3_bptt_prepare(const ic3_bptt_plan* p, const ic3_bptt_step_io* 
   if (rc) return rc;
   BpttStreams* ss = bptt_streams();
   if (!ss) return IC3_E_UNSUPPORTED;
-  if (!ss->overlap) return IC3_OK;                  // ic3_bptt_step will do it inline
+  if (!ss->overlap || L.P > 1) return IC3_OK;       // ic3_bptt_step will do it inline
   const int q = io->t & 1;
   // buffer set q was last used by step t + 2: its main-stream kernels (gates / dgrad / comm read A, dout, gs, gr) and
   // its weight-gradient kernel (side stream, already ordered before this call)
   cudaError_t e = cudaStreamWaitEvent(ss->side, ss->main_done[q], 0);
   if (e != cudaSuccess) return (int)e;
-  rc = bptt_prepare_on(p, io, L, npos, is_tj, ss->side);
+  rc = bptt_prepare_on(p, io, L, npos, is_tj, ss->side, q, 0, io->h_prev);
   if (rc) return rc;
   e = cudaEventRecord(ss->prep_done[q], ss->side);
   if (e != cudaSuccess) return (int)e;
@@ -1239,34 +1264,33 @@ extern "C" int ic3_bptt_prepare(const ic3_bptt_plan* p, const ic3_bptt_step_io* 
   return IC3_OK;
 }
 
-extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, void* stream) {
-  Layout L;
-  int npos, is_tj;
-  int rc = bptt_common(p, io, &L, &npos, &is_tj);
-  if (rc) return rc;
+// One backward unit: comm pass ps of step io->t, entered with state (h_in, c_in), on buffer set q.  The incoming
+// io->dh / io->dc are d loss / d (h, c) leaving the pass; they are replaced by d loss / d (h_in, c_in).
+static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const Layout& L, int npos, int is_tj,
+                     cudaStream_t s, int q, int ps, const float* h_in, const float* c_in) {
+  int rc;
   const ic3_policy_cfg* cfg = p->cfg;
-  cudaStream_t s = (cudaStream_t)stream;
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
   const int R = cfg->B * cfg->N;
   int nout = 1;
   for (int k = 0; k < cfg->nheads; ++k) nout += cfg->head_dim[k];
   BpttScalars* sc = reinterpret_cast<BpttScalars*>(ws + L.sc);
-  const int q = io->t & 1;
   const size_t rows_pad = (size_t)L.ntiles * TC_M;
   const int ntiles = L.ntiles;
+  const bool first = ps == 0, last = ps == L.P - 1;
   __half* a_img = reinterpret_cast<__half*>(ws + L.a_img + (size_t)q * L.img_stride);
   __half* dg_img = reinterpret_cast<__half*>(ws + L.dg_img + (size_t)q * L.img_stride);
   BpttStreams* ss = bptt_streams();
   if (!ss) return IC3_E_UNSUPPORTED;
-  // buffer set q (images, scale) was last read by the weight-gradient kernel of step t + 2 (side stream)
+  // buffer set q (images, scale) was last read by the weight-gradient kernel of unit u + 2 (side stream)
   cudaError_t se = cudaStreamWaitEvent(s, ss->wgrad_done[q], 0);
   if (se != cudaSuccess) return (int)se;
-  if (ss->prepared_t[q] == io->t) {                 // heads + images were launched ahead (ic3_bptt_prepare)
+  if (L.P == 1 && ss->prepared_t[q] == io->t) {    // heads + images were launched ahead (ic3_bptt_prepare)
     se = cudaStreamWaitEvent(s, ss->prep_done[q], 0);
     if (se != cudaSuccess) return (int)se;
     ss->prepared_t[q] = -1;
   } else {
-    rc = bptt_prepare_on(p, io, L, npos, is_tj, s);
+    rc = bptt_prepare_on(p, io, L, npos, is_tj, s, q, ps, h_in);
     if (rc) return rc;
   }
   bptt_scale_kernel<<<1, 1, 0, s>>>(sc, q);
@@ -1282,15 +1306,20 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
       prefer_max_smem(bptt_gates_kernel);
       cfgd = true;
     }
+    // the episode start zeroes the state entering pass 0; the detach cut drops what reaches the step's output (the
+    // last pass) from later steps; heads act on the last pass only (passes before it read a zero d outputs block)
     GatesArgs ga;
-    ga.R = R; ga.N = cfg->N; ga.c_prev = io->c_prev; ga.fresh = io->fresh; ga.cut = io->cut;
-    ga.dout = reinterpret_cast<const float*>(ws + L.dout) + (size_t)q * rows_pad * BP_HEADS; ga.dh = io->dh; ga.dc = io->dc; ga.dg_img = dg_img; ga.sc = sc;
+    ga.R = R; ga.N = cfg->N; ga.c_prev = c_in; ga.fresh = first ? io->fresh : nullptr; ga.cut = last ? io->cut : nullptr;
+    ga.dout = last ? reinterpret_cast<const float*>(ws + L.dout) + (size_t)q * rows_pad * BP_HEADS
+                   : reinterpret_cast<const float*>(ws + L.dout0);
+    ga.dh = io->dh; ga.dc = io->dc; ga.dg_img = dg_img; ga.sc = sc;
     ga.q = q;
     ga.err = io->err;
     const int nitems = 2 * ntiles;
     const int grid = nitems < sm_count() ? nitems : sm_count();
-    bptt_gates_kernel<<<grid, TC_P_THREADS, smem, s>>>(ga, a_img, reinterpret_cast<const __half*>(p->w->lstm_img),
-                                                      (const float*)p->w->bias_cat, nitems, (const float*)p->w->head_w, nout);
+    bptt_gates_kernel<<<grid, TC_P_THREADS, smem, s>>>(
+        ga, a_img, reinterpret_cast<const __half*>(p->w->lstm_img) + (size_t)ps * B_IMG_HALFS,
+        (const float*)p->w->bias_cat + (size_t)ps * 4 * TC_H, nitems, (const float*)p->w->head_w, nout);
     IC3_LAUNCH_CHECK();
     se = cudaEventRecord(ss->gates_done[q], s);
     if (se != cudaSuccess) return (int)se;
@@ -1309,7 +1338,8 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
     da.R = R; da.gs = reinterpret_cast<const float*>(ws + L.gs) + (size_t)q * rows_pad; da.dSs = reinterpret_cast<float*>(ws + L.dSs);
     da.dh_direct = reinterpret_cast<float*>(ws + L.dh_direct); da.sc = sc; da.q = q; da.err = io->err;
     const int grid = ntiles < sm_count() ? ntiles : sm_count();
-    bptt_dgrad_kernel<<<grid, TC_P_THREADS, smem, s>>>(da, dg_img, reinterpret_cast<const __half*>(ws + L.w2_img), ntiles);
+    bptt_dgrad_kernel<<<grid, TC_P_THREADS, smem, s>>>(
+        da, dg_img, reinterpret_cast<const __half*>(ws + L.w2_img) + (size_t)ps * W2_IMG_HALFS, ntiles);
     IC3_LAUNCH_CHECK();
   }
   // ---- comm backward -> dh_{t-1} ----
@@ -1317,10 +1347,10 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
     CommArgs ca;
     ca.B = cfg->B; ca.N = cfg->N; ca.dSs = reinterpret_cast<const float*>(ws + L.dSs);
     ca.dh_direct = reinterpret_cast<const float*>(ws + L.dh_direct); ca.gr = reinterpret_cast<const float*>(ws + L.gr) + (size_t)q * rows_pad;
-    ca.fresh = io->fresh; ca.no_comm = cfg->comm_mask_zero || cfg->N < 2; ca.dh = io->dh; ca.sc = sc;
+    ca.fresh = first ? io->fresh : nullptr; ca.no_comm = cfg->comm_mask_zero || cfg->N < 2; ca.dh = io->dh; ca.sc = sc;
     bptt_comm_kernel<<<(cfg->B + 7) / 8, 256, 0, s>>>(ca);
     IC3_LAUNCH_CHECK();
-    se = cudaEventRecord(ss->main_done[q], s);          // buffer set q may be refilled for step t - 2 once wgrad(t) is done too
+    se = cudaEventRecord(ss->main_done[q], s);          // buffer set q may be refilled for unit u - 2 once wgrad(u) is done too
     if (se != cudaSuccess) return (int)se;
   }
   // ---- weight gradients: on the side stream, overlapping the small kernels of this and the next step ----
@@ -1355,7 +1385,7 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
     }
     WgradArgs wa;
     wa.ntiles = ntiles; wa.np = L.np; wa.j0 = L.j0; wa.j1 = L.j1;
-    wa.partial = reinterpret_cast<float*>(ws + L.partial); wa.sc = sc; wa.q = q; wa.err = io->err;
+    wa.partial = reinterpret_cast<float*>(ws + L.partial + (size_t)ps * L.part_stride); wa.sc = sc; wa.q = q; wa.err = io->err;
     cudaStream_t ws_stream = ss->overlap ? ss->side : s;
     if (ss->overlap) {
       se = cudaStreamWaitEvent(ws_stream, ss->gates_done[q], 0);
@@ -1365,6 +1395,55 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
     IC3_LAUNCH_CHECK();
     se = cudaEventRecord(ss->wgrad_done[q], ws_stream);
     if (se != cudaSuccess) return (int)se;
+  }
+  return IC3_OK;
+}
+
+// Step t = the units (t, P-1) .. (t, 0).  With P > 1 comm passes the states entering passes 1 .. P-1 are re-run first
+// from the record (h_{t-1}, c_{t-1}) with the rollout's own kernels (ic3_tc_pass_states).
+extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, void* stream) {
+  Layout L;
+  int npos, is_tj;
+  int rc = bptt_common(p, io, &L, &npos, &is_tj);
+  if (rc) return rc;
+  if (io->pass_index != 0) return IC3_E_RANGE;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (L.P == 1) return bptt_unit(p, io, L, npos, is_tj, s, io->t & 1, 0, io->h_prev, io->c_prev);
+  const ic3_policy_cfg* cfg = p->cfg;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
+  const size_t RH = (size_t)cfg->B * cfg->N * TC_H;
+  float* h_pass = reinterpret_cast<float*>(ws + L.hc_pass);     // [P-1][R][H]: state after pass 0 .. P-2
+  float* c_pass = h_pass + (size_t)(L.P - 1) * RH;
+  ic3_policy_io pio;
+  memset(&pio, 0, sizeof(pio));
+  pio.h = io->h_prev; pio.c = io->c_prev; pio.comm_action = io->comm; pio.alive = io->alive; pio.fresh = io->fresh;
+  pio.err = io->err; pio.x_table = p->x_table;
+  pio.workspace = ws + L.tc_ws;
+  ic3_pp_state pps;
+  ic3_tj_state tjs;
+  memset(&pps, 0, sizeof(pps));
+  memset(&tjs, 0, sizeof(tjs));
+  if (!is_tj) {
+    if (!io->pp_loc) return IC3_E_NULL;
+    pps.loc = const_cast<int32_t*>(io->pp_loc);
+    pio.pp_env = p->pp_env; pio.pp_state = &pps;
+  } else {
+    if (!io->tj_loc || !io->tj_alive || !io->tj_last_act || !io->tj_route_id) return IC3_E_NULL;
+    tjs.loc = const_cast<int32_t*>(io->tj_loc);
+    tjs.alive = const_cast<uint8_t*>(io->tj_alive);
+    tjs.last_act = const_cast<uint8_t*>(io->tj_last_act);
+    tjs.route_id = const_cast<int32_t*>(io->tj_route_id);
+    pio.tj_env = p->tj_env; pio.tj_state = &tjs;
+  }
+  if (cfg->hard_attn && !io->comm) return IC3_E_NULL;
+  rc = ic3_tc_pass_states(cfg, p->w, &pio, L.P - 1, h_pass, c_pass, s);
+  if (rc) return rc;
+  for (int ps = L.P - 1; ps >= 0; --ps) {
+    const int q = (io->t * L.P + ps) & 1;                 // unit counter parity: consecutive units alternate sets
+    const float* h_in = ps == 0 ? io->h_prev : h_pass + (size_t)(ps - 1) * RH;
+    const float* c_in = ps == 0 ? io->c_prev : c_pass + (size_t)(ps - 1) * RH;
+    rc = bptt_unit(p, io, L, npos, is_tj, s, q, ps, h_in, c_in);
+    if (rc) return rc;
   }
   return IC3_OK;
 }
@@ -1396,29 +1475,15 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
   double* dC = reinterpret_cast<double*>(ws + L.dC);
   double* wj = reinterpret_cast<double*>(ws + L.wj);
   double* cw = reinterpret_cast<double*>(ws + L.cw);
-  bptt_reduce_partials_kernel<<<(512 * NC + 255) / 256, 256, 0, s>>>(reinterpret_cast<const float*>(ws + L.partial), L.j0, L.j1,
-                                                                     L.np, G, NC);
-  IC3_LAUNCH_CHECK();
-  bptt_weights_f64_kernel<<<(512 * TC_H + 255) / 256, 256, 0, s>>>(params->w_ih, params->c_w, wj, cw);
-  IC3_LAUNCH_CHECK();
-  // Y[k][n] = sum_j W_ih[j][k] Q[j][n],  Q = G[:, 384:]
-  small_gemm_tn_kernel<<<(TC_H * L.np + 255) / 256, 256, 0, s>>>(TC_H, L.np, 512, wj, TC_H, G + 384, NC, Y, L.np, 0);
-  IC3_LAUNCH_CHECK();
-  // dC[k][m] = sum_j W_ih[j][k] G_S[j][m]
-  small_gemm_tn_kernel<<<(TC_H * TC_H + 255) / 256, 256, 0, s>>>(TC_H, TC_H, 512, wj, TC_H, G + 128, NC, dC, TC_H, 0);
-  IC3_LAUNCH_CHECK();
-  bptt_gsc_kernel<<<(512 * TC_H + 255) / 256, 256, 0, s>>>(G, NC, cw, GSC);
-  IC3_LAUNCH_CHECK();
   FinishArgs f;
   memset(&f, 0, sizeof(f));
   int atot = 0;
   for (int k = 0; k < cfg->nheads; ++k) atot += cfg->head_dim[k];
   f.O = cfg->O; f.nheads = cfg->nheads; f.atot = atot; f.npos = npos; f.np = L.np; f.WW = WW;
   for (int k = 0; k < IC3_MAX_HEADS; ++k) f.head_dim[k] = cfg->head_dim[k];
-  f.G = G; f.NC = NC; f.Y = Y; f.GSC = GSC; f.dC = dC; f.c_b = params->c_b;
+  f.G = G; f.NC = NC; f.Y = Y; f.GSC = GSC; f.dC = dC;
   f.g_w_ih = const_cast<float*>(grads->w_ih); f.g_w_hh = const_cast<float*>(grads->w_hh);
   f.g_b_ih = const_cast<float*>(grads->b_ih); f.g_b_hh = const_cast<float*>(grads->b_hh);
-  f.g_c_w = const_cast<float*>(grads->c_w); f.g_c_b = const_cast<float*>(grads->c_b);
   f.g_enc_w = const_cast<float*>(grads->encoder_w); f.g_enc_b = const_cast<float*>(grads->encoder_b);
   f.g_value_w = const_cast<float*>(grads->value_w); f.g_value_b = const_cast<float*>(grads->value_b);
   for (int k = 0; k < IC3_MAX_HEADS; ++k) {
@@ -1433,10 +1498,36 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
   if (is_tj) f.tj = *p->tj_env;
   else f.pp = *p->pp_env;
   f.ones_col = npos + (is_tj ? WW + 3 : 2 * WW);     // the constant column of P is its last used column
-  bptt_finish_lstm_kernel<<<(512 * TC_H + 255) / 256, 256, 0, s>>>(f);
-  IC3_LAUNCH_CHECK();
-  bptt_finish_misc_kernel<<<(finish_enc_items(f) * 128 + 255) / 256, 256, 0, s>>>(f);
-  IC3_LAUNCH_CHECK();
+  // One fold per comm pass, in pass order, each ADDING its share: pass p's partials hold G_x, G_h and the P columns of
+  // its units (summed over the passes by the additions) and its own S block / constant column, which go with
+  // C_modules[p] (share_weights: every pass adds into the one module's gradient buffers).
+  for (int ps = 0; ps < L.P; ++ps) {
+    const bool own = ps > 0;                           // pass 0 is c_w / c_b, as in ic3_policy_pack
+    const float* c_w = own && params->c_w_pass[ps] ? params->c_w_pass[ps] : params->c_w;
+    const float* c_b = own && params->c_b_pass[ps] ? params->c_b_pass[ps] : params->c_b;
+    const float* g_c_w = own && grads->c_w_pass[ps] ? grads->c_w_pass[ps] : grads->c_w;
+    const float* g_c_b = own && grads->c_b_pass[ps] ? grads->c_b_pass[ps] : grads->c_b;
+    if (!c_w || !c_b || !g_c_w || !g_c_b) return IC3_E_NULL;
+    bptt_reduce_partials_kernel<<<(512 * NC + 255) / 256, 256, 0, s>>>(
+        reinterpret_cast<const float*>(ws + L.partial + (size_t)ps * L.part_stride), L.j0, L.j1, L.np, G, NC);
+    IC3_LAUNCH_CHECK();
+    bptt_weights_f64_kernel<<<(512 * TC_H + 255) / 256, 256, 0, s>>>(params->w_ih, c_w, wj, cw);
+    IC3_LAUNCH_CHECK();
+    // Y[k][n] = sum_j W_ih[j][k] Q[j][n],  Q = G[:, 384:]
+    small_gemm_tn_kernel<<<(TC_H * L.np + 255) / 256, 256, 0, s>>>(TC_H, L.np, 512, wj, TC_H, G + 384, NC, Y, L.np, 0);
+    IC3_LAUNCH_CHECK();
+    // dC[k][m] = sum_j W_ih[j][k] G_S[j][m]
+    small_gemm_tn_kernel<<<(TC_H * TC_H + 255) / 256, 256, 0, s>>>(TC_H, TC_H, 512, wj, TC_H, G + 128, NC, dC, TC_H, 0);
+    IC3_LAUNCH_CHECK();
+    bptt_gsc_kernel<<<(512 * TC_H + 255) / 256, 256, 0, s>>>(G, NC, cw, GSC);
+    IC3_LAUNCH_CHECK();
+    f.c_b = c_b;
+    f.g_c_w = const_cast<float*>(g_c_w); f.g_c_b = const_cast<float*>(g_c_b);
+    bptt_finish_lstm_kernel<<<(512 * TC_H + 255) / 256, 256, 0, s>>>(f);
+    IC3_LAUNCH_CHECK();
+    bptt_finish_misc_kernel<<<(finish_enc_items(f) * 128 + 255) / 256, 256, 0, s>>>(f);
+    IC3_LAUNCH_CHECK();
+  }
   bptt_finish_heads_kernel<<<(BP_HEADS * TC_H + 255) / 256, 256, 0, s>>>(f);
   IC3_LAUNCH_CHECK();
   return IC3_OK;

@@ -791,6 +791,19 @@ extern "C" int ic3_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packe
   IC3_DISPATCH_H(cfg->H, launch_policy<HH>(a, (cudaStream_t)stream));
 }
 
+extern "C" int ic3_policy_pass_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,
+                                      int32_t npasses, float* h_pass, float* c_pass, void* stream) {
+  int rc = policy_check(cfg);
+  if (rc) return rc;
+  rc = packed_check(w);
+  if (rc) return rc;
+  if (!io || !io->h || !io->c || !h_pass || !c_pass || !io->workspace || !w->lstm_img) return IC3_E_NULL;
+  if (cfg->hard_attn && !io->comm_action) return IC3_E_NULL;
+  if (cfg->N > ROWS) return IC3_E_RANGE;
+  if (!policy_tc_capable(cfg)) return IC3_E_UNSUPPORTED;
+  return ic3_tc_pass_states(cfg, w, io, npasses, h_pass, c_pass, (cudaStream_t)stream);
+}
+
 extern "C" int ic3_sample_actions(const ic3_policy_cfg* cfg, const float* logp, const uint32_t* tick,
                                   const uint32_t* draws, int32_t* action, void* stream) {
   int rc = policy_check(cfg);

@@ -8,6 +8,8 @@
 uint64_t ic3_tc_workspace_bytes(const ic3_policy_cfg* cfg);
 int ic3_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3_policy_packed* out, cudaStream_t s);
 int ic3_tc_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, cudaStream_t s);
+int ic3_tc_pass_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, int npasses,
+                       float* h_pass, float* c_pass, cudaStream_t s);
 // grid of a persistent kernel `kern` (threads per CTA, dynamic shared memory smem) over nwork items that runs beside the
 // tensor-core LSTM kernel: min(nwork, SMs x the CTAs of kern that fit on one SM next to a resident lstm_tc_kernel CTA --
 // registers, shared memory, threads, CTA slots -- at least one per SM)

@@ -197,6 +197,31 @@ int ic3_tc_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, co
   return IC3_OK;
 }
 
+// Passes 0 .. npasses-1 of ic3_tc_policy_step on the same inputs, pass p writing its (h, c) to row block p of h_pass /
+// c_pass ([npasses][R][H]) and reading pass p - 1's block: the kernels and operands of the step itself, so every
+// block equals the state the step carries between its passes (and block P - 1 its h_out / c_out) bit for bit.
+int ic3_tc_pass_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, int npasses,
+                       float* h_pass, float* c_pass, cudaStream_t s) {
+  if (cfg->H != TC_H) return IC3_E_UNSUPPORTED;
+  if (!io->workspace || !w->lstm_img || !w->bias_cat || !h_pass || !c_pass) return IC3_E_NULL;
+  const int P = cfg->passes > 1 ? cfg->passes : 1;
+  if (npasses < 1 || npasses > P) return IC3_E_RANGE;
+  const size_t RH = (size_t)cfg->B * cfg->N * TC_H;
+  for (int ps = 0; ps < npasses; ++ps) {
+    ic3_policy_io q = *io;
+    q.pass_index = ps;
+    if (ps > 0) {
+      q.h = h_pass + (size_t)(ps - 1) * RH;
+      q.c = c_pass + (size_t)(ps - 1) * RH;
+    }
+    q.h_out = h_pass + (size_t)ps * RH;
+    q.c_out = c_pass + (size_t)ps * RH;
+    const int rc = tc_pass(cfg, w, &q, s, false);
+    if (rc) return rc;
+  }
+  return IC3_OK;
+}
+
 static int tc_pass(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, cudaStream_t s, bool last) {
   const long R = (long)cfg->B * cfg->N;
   const int ntiles = (int)((R + TC_M - 1) / TC_M);

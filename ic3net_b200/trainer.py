@@ -109,8 +109,8 @@ class Trainer(object):
         self.is_tj = args.env_name == 'traffic_junction'
         self.record_for_grad = bool(getattr(args, 'record_for_grad', False))
         self.grad_window = int(getattr(args, 'grad_window', 40))
-        # compute_grad implementation: 'kernels' = hand-written BPTT (csrc/bptt_tc.cu; tensor-core policy path, at most
-        # 7 action logits, observation pattern of <= 512 columns), 'autograd' = windowed recompute under torch autograd,
+        # compute_grad implementation: 'kernels' = hand-written BPTT (csrc/bptt_tc.cu; tensor-core policy path with the
+        # LSTM cell and 1..4 comm passes, at most 7 action logits, observation pattern of <= 512 columns), 'autograd' = windowed recompute under torch autograd,
         # 'manual' = explicit formulas with torch GEMMs (bptt.py).  Default: kernels when the configuration allows.
         self.grad_impl = getattr(args, 'grad_impl', None) or 'auto'
         self.grad_kernels = False
@@ -126,8 +126,9 @@ class Trainer(object):
         if self.record_for_grad and self.grad_impl in ('auto', 'kernels'):
             ok = self._bptt_supported()
             if self.grad_impl == 'kernels' and not ok:
-                raise NotImplementedError("grad_impl='kernels' needs the tensor-core policy path (hid_size 128), the "
-                                          "per-position encoder table, <= 7 action logits and a small vision window")
+                raise NotImplementedError("grad_impl='kernels' needs the tensor-core policy path (hid_size 128, LSTM "
+                                          "cell), the per-position encoder table, <= 7 action logits and a small "
+                                          "vision window")
             self.grad_kernels = ok
         if self.grad_impl == 'auto':
             self.grad_impl = 'kernels' if self.grad_kernels else 'autograd'
@@ -137,7 +138,8 @@ class Trainer(object):
         W = 2 * e.vision + 1
         if not net.fuses_encoder(e) or 1 + sum(self.args.naction_heads) > 8:
             return False
-        if getattr(net, 'is_variant', False):          # the BPTT kernels differentiate ONE comm pass
+        # the recurrent LSTM policies, any number of comm passes (share_weights included); not the tanh cells
+        if not net.tc_capable or net.comm_passes > _lib.MAX_PASSES:
             return False
         if getattr(e, 'obs_layout', (0, 0, 0))[1] == 0:
             return False
@@ -209,7 +211,8 @@ class Trainer(object):
     # records are kept while they take at most RECORD_BYTES_LIMIT bytes (None: what the device has); beyond that the
     # records switch to windows of grad_window steps, which must fit in what the device has.
     RECORD_BYTES_LIMIT = None
-    RECORD_MARGIN_BYTES = 2 << 30            # BPTT workspace (~0.9 GB at 81 920 rows) and allocator slack
+    RECORD_MARGIN_BYTES = 2 << 30            # one-pass BPTT workspace (~0.9 GB at 81 920 rows) and allocator slack;
+    #                                          what comm_passes > 1 adds to the workspace is counted on top (_pick_record_mode)
     RECORD_TEMP_FACTOR = 6
 
     @property
@@ -235,12 +238,31 @@ class Trainer(object):
         nb = min(nw, self._window_buffers())
         return dict(full=2 * (T + 1) * row, window=2 * nw * row + 2 * nb * min(W, T) * row + T * 4)
 
+    def _bptt_extra_bytes(self):
+        """Bytes the BPTT workspace of this policy needs beyond the one-pass workspace RECORD_MARGIN_BYTES covers: the
+        per-pass states, weight images and partials of comm_passes > 1 (0 with one pass)."""
+        if int(self.args.comm_passes) <= 1:
+            return 0
+        e = self.env.env
+        lib = _lib.load()
+
+        def nbytes(cfg):
+            plan = _lib.BpttPlan(cfg=C.pointer(cfg), w=None, pp_env=None if self.is_tj else C.pointer(e.cfg),
+                                 tj_env=C.pointer(e.cfg) if self.is_tj else None, x_table=None,
+                                 value_coeff=float(self.args.value_coeff), entr=float(self.args.entr), workspace=None)
+            return int(lib.ic3_bptt_workspace_bytes(C.byref(plan)))
+        cfg = self.policy_net.policy_cfg(e.nenvs)
+        one = self.policy_net.policy_cfg(e.nenvs)
+        one.passes = 1
+        return max(0, nbytes(cfg) - nbytes(one))
+
     def _pick_record_mode(self, T):
         need = self._record_bytes(T)
         dev = self.env.env.device
         free, _ = torch.cuda.mem_get_info(dev)
         free += torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
-        avail = free - self.RECORD_MARGIN_BYTES - self.RECORD_TEMP_FACTOR * T * self.env.env.nenvs * self.args.nagents * 4
+        avail = (free - self.RECORD_MARGIN_BYTES - self._bptt_extra_bytes()
+                 - self.RECORD_TEMP_FACTOR * T * self.env.env.nenvs * self.args.nagents * 4)
         limit = avail if self.RECORD_BYTES_LIMIT is None else min(avail, self.RECORD_BYTES_LIMIT)
         if need['full'] <= limit:
             return 'full'
@@ -804,10 +826,13 @@ class Trainer(object):
 
         def mk(get):
             arr = lambda lst: (C.c_void_p * _lib.MAX_HEADS)(*([get(t) for t in lst] + [None] * (_lib.MAX_HEADS - len(lst))))
+            # C_modules[p] per comm pass (share_weights: the same module, so the gradient pointers alias)
+            parr = lambda lst: (C.c_void_p * _lib.MAX_PASSES)(*([get(t) for t in lst] + [None] * (_lib.MAX_PASSES - len(lst))))
             return _lib.PolicyParams(encoder_w=get(w['enc_w']), encoder_b=get(w['enc_b']), c_w=get(w['c_w'][0]),
                                      c_b=get(w['c_b'][0]), w_ih=get(w['w_ih']), w_hh=get(w['w_hh']), b_ih=get(w['b_ih']),
                                      b_hh=get(w['b_hh']), value_w=get(w['value_w']), value_b=get(w['value_b']),
-                                     head_w=arr(w['head_w']), head_b=arr(w['head_b']))
+                                     head_w=arr(w['head_w']), head_b=arr(w['head_b']),
+                                     c_w_pass=parr(w['c_w']), c_b_pass=parr(w['c_b']))
         return mk(lambda p: p.data_ptr()), mk(grad_ptr)
 
     def _compute_grad_manual(self, adv, ret, W, nw):

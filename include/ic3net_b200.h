@@ -361,6 +361,13 @@ int ic3_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const
  * LSTM/comm tensor-core kernel, heads + sampling}.  Not for the production loop. */
 int ic3_policy_step_profile(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,
                             void* stream, float* ms);
+/* The recurrent state after each of the first `npasses` comm passes (1 <= npasses <= cfg->passes) of ic3_policy_step on
+ * the tensor-core path, for the same io inputs (h, c, masks, x or the fused encoder source, workspace): pass p writes
+ * h_pass / c_pass rows [p * B*N, (p + 1) * B*N) of [npasses, B*N, H] float32.  Same kernels and operands as the step, so
+ * the block of pass cfg->passes - 1 equals the step's h_out / c_out bit for bit.  Nothing is sampled and no head runs.
+ * The BPTT kernels re-run the intermediate passes this way. */
+int ic3_policy_pass_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,
+                           int32_t npasses, float* h_pass, float* c_pass, void* stream);
 /* select_action alone (action_utils.py:32-36) on given log-probabilities. */
 int ic3_sample_actions(const ic3_policy_cfg* cfg, const float* logp, const uint32_t* tick,
                        const uint32_t* draws, int32_t* action, void* stream);
@@ -384,14 +391,20 @@ int ic3_stat_reduce(int32_t B, int32_t N, const int32_t* stat_episodes, const in
 /* ------------------------------------------------------------------------
  * Back-propagation through time of the rollout loss (Trainer.compute_grad, trainer.py:128-225;
  * utils.multinomials_log_density utils.py:42-46) over the records of a lock-step rollout, hid_size 128,
- * at most 7 action logits.  The host walks the lock-step iterations t = T-1 .. 0:
+ * at most 7 action logits, the recurrent LSTM CommNet / IC3Net with 1 .. IC3_MAX_PASSES comm passes (share_weights
+ * included; cfg->cell == IC3_CELL_LSTM, no x_tanh / h_from_x).  The host walks the lock-step iterations t = T-1 .. 0:
  *     ic3_bptt_begin(plan, max |c| of the record, stream)
  *     for t in reversed(range(T)): ic3_bptt_step(plan, &io_t, stream)
  *     ic3_bptt_finish(plan, params, grads, losses, stream)
- * Per step: d loss / d (value, logits) from the recorded log-probs / actions / advantages / masks, LSTM cell and
- * comm backward, and the three GEMMs (gate re-computation, d gates . W, (d gates)^T . features) on the tensor cores
- * with the forward's fp16 hi/lo operand split.  Parameter gradients are ADDED to the `grads` buffers (the caller
- * zeroes them, trainer.py:248) and are not divided by num_steps (trainer.py:251-253 does that).
+ * The backward unit is one (step t, comm pass p); ic3_bptt_step runs the units (t, P-1) .. (t, 0), after re-running
+ * passes 0 .. P-2 of step t from the record (h_{t-1}, c_{t-1}) for the states entering passes 1 .. P-1
+ * (ic3_policy_pass_states).  Per unit: d loss / d (value, logits) from the recorded log-probs / actions / advantages /
+ * masks (last pass only), LSTM cell and comm backward, and the three GEMMs (gate re-computation, d gates . W,
+ * (d gates)^T . features) on the tensor cores with the forward's fp16 hi/lo operand split, on pass p's weight image.
+ * A fresh slot's zero state applies at pass 0, the detach cut at the step's output (pass P-1).  Parameter gradients
+ * are ADDED to the `grads` buffers (the caller zeroes them, trainer.py:248) and are not divided by num_steps
+ * (trainer.py:251-253 does that); with comm_passes > 1 ic3_bptt_finish reads c_w_pass / c_b_pass of params and
+ * grads (NULL or index 0: c_w / c_b), adding pass by pass, so share_weights may alias them.
  * ---------------------------------------------------------------------- */
 typedef struct {
   const ic3_policy_cfg* cfg;    /* HOST pointers: same structs the rollout used */
@@ -405,8 +418,9 @@ typedef struct {
 } ic3_bptt_plan;
 
 typedef struct {
-  int32_t t;                    /* lock-step index (its parity selects the operand-image set of the step) */
-  int32_t reserved0;
+  int32_t t;                    /* lock-step index (the parity of the unit counter t * passes + p selects the
+                                   operand-image set of unit (t, p)) */
+  int32_t pass_index;           /* callers pass 0: the library walks the passes of step t itself */
   /* state entering / leaving policy step t */
   const float* h_prev;          /* [B*N, H] h_{t-1} as fed to the step (ignored for fresh slots) */
   const float* c_prev;          /* [B*N, H] */
@@ -442,7 +456,8 @@ int ic3_bptt_step(const ic3_bptt_plan* plan, const ic3_bptt_step_io* io, void* s
 /* Optional look-ahead: launches the recursion-independent kernels of step io->t (heads gradient, operand images) on the
  * library's side stream so that they overlap the tensor-core kernels of step t + 1; call it for step t - 1 right before
  * ic3_bptt_step(t) (and once for t = T - 1 after ic3_bptt_begin).  The step's records must not change until
- * ic3_bptt_step(io->t) has been issued. */
+ * ic3_bptt_step(io->t) has been issued.  comm_passes > 1: does nothing (every unit is prepared inline on the caller's
+ * stream; the weight-gradient kernels still overlap on the side stream). */
 int ic3_bptt_prepare(const ic3_bptt_plan* plan, const ic3_bptt_step_io* io, void* stream);
 /* params: the CURRENT parameters; grads: same struct holding the gradient buffers (reference layouts);
  * losses: device double[3] = action_loss, value_loss, entropy sums (trainer.py:198-216). */
