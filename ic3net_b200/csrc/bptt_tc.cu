@@ -21,6 +21,15 @@
 //   d encoder = W_ih^T (d gates)^T P scattered back through the observation layout (one-hot class per window cell
 //   of the agent position, count / scalar features), with g1 = column of ones of P.
 //
+// The tanh recurrence without communication (models.RNN with rnn_type 'MLP': the IC / IRIC baselines, run by the SIMT
+// policy kernel), h' = tanh(z), z = affine1(obs) + affine2(h), is the same chain with one 128-column "gate" block:
+//   tanh       dz = (dh + W_heads^T dout) (1 - h'^2), h' from the record -> dz image (no GEMM)     [bptt_tanh_kernel]
+//   dgrad      dh_{t-1} = dz . W_f (K = 128)                                                      [bptt_dgrad_kernel<4>]
+//   comm       the episode-start cut only (no_comm)                                               [bptt_comm_kernel]
+//   wgrad      G += dz^T . [h | P]  (slice 0 narrowed to the h block of the operand image)          [bptt_wgrad_kernel]
+// and ic3_bptt_finish folds  d affine2.weight = G_h,  d affine2.bias = d affine1.bias = g1,  d affine1.weight = dz^T P
+// scattered through the observation layout (the fold above with W_ih^T replaced by the identity).
+//
 // Arithmetic of the three GEMMs: the forward's fp16 hi/lo split (3 MMAs, fp32 accumulate).  d gates of a step are
 // scaled by a power of two s_t chosen from an upper bound of their magnitude (so hi stays below 2^14 and lo keeps
 // 2^-35 of the step's largest element); products are unscaled when they leave the accumulator registers.
@@ -396,9 +405,86 @@ __global__ void __launch_bounds__(TC_P_THREADS, 1) bptt_gates_kernel(GatesArgs g
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+// tanh cell backward: dz = (dh + W_heads^T dout) (1 - h'^2), elementwise.  h' is the record the forward wrote (its own
+// tanhf value), so nothing is re-computed and no GEMM is needed.  The dz image has the d gates image's layout with 128
+// columns (column = hidden unit): [tile][hi, lo][cg 16][rg 16][8][8].  Thread = (row, 8 consecutive units = one column
+// group); rows past R (up to whole tiles) write zeros, the GEMMs read whole tiles.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int DZ_TILE_HALFS = 2 * 16 * 16 * 64;
+constexpr int DZ_PART_HALFS = 16 * 16 * 64;
+constexpr int TZ_ROWS = 16;                        // rows per 256-thread block
+
+struct TanhArgs {
+  int R, N, nrows;          // nrows: R rounded up to whole tiles
+  const uint8_t* cut;       // [B] or NULL: h' of step t was detached (trainer.py:56-60): the incoming dh is dropped
+  const float* dout;        // [R, 8]
+  const float* h_new;       // [R, H] h'_t
+  const float* dh;          // [R, H] d loss / d h'_t from later steps
+  const float* head_w;      // packed [nout, H]
+  int nout;
+  __half* dz_img;
+  const BpttScalars* sc;
+  int q;                    // t & 1
+};
+
+__global__ void __launch_bounds__(256) bptt_tanh_kernel(TanhArgs a) {
+  __shared__ __align__(16) float s_hw[HEAD_PAD][TC_H];
+  for (int idx = threadIdx.x; idx < HEAD_PAD * TC_H; idx += blockDim.x) {
+    const int o = idx / TC_H, u = idx - o * TC_H;
+    s_hw[o][u] = o < a.nout ? __ldg(a.head_w + (size_t)o * TC_H + u) : 0.f;
+  }
+  __syncthreads();
+  const int cg = threadIdx.x & 15;
+  const int row = blockIdx.x * TZ_ROWS + (threadIdx.x >> 4);
+  if (row >= a.nrows) return;
+  float dz[8];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) dz[k] = 0.f;
+  if (row < a.R) {
+    const bool ct = a.cut && a.cut[row / a.N] != 0;
+    const float4 d0 = *reinterpret_cast<const float4*>(a.dout + (size_t)row * BP_HEADS);
+    const float4 d1 = *reinterpret_cast<const float4*>(a.dout + (size_t)row * BP_HEADS + 4);
+    const float dsum[HEAD_PAD] = {d0.x, d0.y, d0.z, d0.w, d1.x, d1.y, d1.z, d1.w};
+    const size_t base = (size_t)row * TC_H + 8 * cg;
+    const float4 h0 = *reinterpret_cast<const float4*>(a.h_new + base);
+    const float4 h1 = *reinterpret_cast<const float4*>(a.h_new + base + 4);
+    float4 g0 = make_float4(0.f, 0.f, 0.f, 0.f), g1 = g0;
+    if (!ct) {
+      g0 = *reinterpret_cast<const float4*>(a.dh + base);
+      g1 = *reinterpret_cast<const float4*>(a.dh + base + 4);
+    }
+    const float hv[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
+    float dh[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+    // heads: dh += sum_o dout_o W_o[u], in output order (as bptt_gates_kernel)
+#pragma unroll
+    for (int o = 0; o < HEAD_PAD; ++o) {
+      const float4 w0 = *reinterpret_cast<const float4*>(&s_hw[o][8 * cg]);
+      const float4 w1 = *reinterpret_cast<const float4*>(&s_hw[o][8 * cg + 4]);
+      dh[0] = fmaf(dsum[o], w0.x, dh[0]); dh[1] = fmaf(dsum[o], w0.y, dh[1]);
+      dh[2] = fmaf(dsum[o], w0.z, dh[2]); dh[3] = fmaf(dsum[o], w0.w, dh[3]);
+      dh[4] = fmaf(dsum[o], w1.x, dh[4]); dh[5] = fmaf(dsum[o], w1.y, dh[5]);
+      dh[6] = fmaf(dsum[o], w1.z, dh[6]); dh[7] = fmaf(dsum[o], w1.w, dh[7]);
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) dz[k] = dh[k] * (1.f - hv[k] * hv[k]);
+  }
+  const float scale = a.sc->scale[a.q];
+  const float v4[2][4] = {{dz[0], dz[1], dz[2], dz[3]}, {dz[4], dz[5], dz[6], dz[7]}};
+  uint2 lo0, lo1;
+  const uint2 hi0 = pack4_hi_lo(v4[0], scale, lo0);
+  const uint2 hi1 = pack4_hi_lo(v4[1], scale, lo1);
+  const int tile = row / TC_M, rt = row - tile * TC_M;
+  __half* p = a.dz_img + (size_t)tile * DZ_TILE_HALFS + (size_t)(cg * 16 + (rt >> 3)) * 64 + (rt & 7) * 8;
+  *reinterpret_cast<uint4*>(p) = make_uint4(hi0.x, hi0.y, hi1.x, hi1.y);
+  *reinterpret_cast<uint4*>(p + DZ_PART_HALFS) = make_uint4(lo0.x, lo0.y, lo1.x, lo1.y);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
 // dgrad: [dS | dh_direct] = d gates . [W_ih C | W_hh]        (M = rows, K = 512 gate columns, N = 256)
+// tanh cell: [0 | dh_direct] = dz . [0 | W_f]                 (K = 128 units, the S half of the weight image is zero)
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int DGR_NCHUNK = 16;                       // 512 gate columns / 32
+constexpr int DGR_NCHUNK_TANH = 4;                   // 128 units / 32
 constexpr int DGR_STAGE = A_CHUNK_BYTES + B_CHUNK_BYTES;   // 16 KB (hi + lo of 32 columns x 128 rows) + 32 KB
 
 // weight image of the dgrad GEMM: element (n = S / h feature, k = gate column j) = scaled forward weight
@@ -418,19 +504,36 @@ __global__ void bptt_pack_w2_kernel(const __half* __restrict__ b_img, __half* __
   for (int part = 0; part < 2; ++part) w2[w2_img_off(j, n, part)] = b_img[b_img_off(nh, 128 + n, col, part)];
 }
 
+// the tanh cell's image, from the packed f_wT (f_wT[k][n] = f.weight[n][k]): element (n, k = unit u) = SCALE_B *
+// f.weight[u][n - 128] for n >= 128, zero for the S half n < 128; same hi/lo split as the forward's weight images
+constexpr size_t W2_IMG_HALFS_TANH = (size_t)DGR_NCHUNK_TANH * 2 * 4 * 32 * 64;
+
+__global__ void bptt_pack_w2_tanh_kernel(const float* __restrict__ f_wT, __half* __restrict__ w2) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;      // (n, k)
+  if (idx >= 256 * TC_H) return;
+  const int n = idx >> 7, k = idx & 127;
+  __half hi, lo;
+  split_f16(n < TC_H ? 0.f : f_wT[(size_t)(n - TC_H) * TC_H + k], SCALE_B, hi, lo);
+  w2[w2_img_off(k, n, 0)] = hi;
+  w2[w2_img_off(k, n, 1)] = lo;
+}
+
 struct DgradArgs {
   int R;
   const float* gs;       // [R] g / den
-  float* dSs;            // [R, H]  out: gs * dS
+  float* dSs;            // [R, H]  out: gs * dS  (NULL: not stored, the tanh cell)
   float* dh_direct;      // [R, H]  out
   const BpttScalars* sc;
   int q;
   int32_t* err;
 };
 
+// NCHUNK = K / 32: the d gates image of a tile is [hi, lo][K / 8 column groups][rg 16][8][8]
+template <int NCHUNK>
 __global__ void __launch_bounds__(TC_P_THREADS, 1) bptt_dgrad_kernel(DgradArgs g, const __half* __restrict__ dg_img,
                                                                     const __half* __restrict__ w2_img, int ntiles) {
   static_assert(DGR_STAGE == STAGE_BYTES, "dgrad shares the stage layout of the gate GEMM");
+  constexpr size_t PART_BYTES = (size_t)NCHUNK * 32 * TC_M * 2, TILE_BYTES = 2 * PART_BYTES;
   extern __shared__ __align__(1024) unsigned char smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NSTAGE_P * DGR_STAGE);
   const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + NSTAGE_P);
@@ -450,9 +553,9 @@ __global__ void __launch_bounds__(TC_P_THREADS, 1) bptt_dgrad_kernel(DgradArgs g
       // 32 gate columns = 4 column groups = 8 KB per part, contiguous in the d gates image
       const unsigned char* a = reinterpret_cast<const unsigned char*>(dg_img);
       const unsigned char* b = reinterpret_cast<const unsigned char*>(w2_img);
-      ring_producer<DGR_NCHUNK>(
-          smem_base, bar_full, bar_empty, blockIdx.x, ntiles, gridDim.x, (size_t)DG_PART_HALFS * 2,
-          [=](int tile, int c) { return a + (size_t)tile * DG_TILE_HALFS * 2 + (size_t)c * 8192; },
+      ring_producer<NCHUNK>(
+          smem_base, bar_full, bar_empty, blockIdx.x, ntiles, gridDim.x, PART_BYTES,
+          [=](int tile, int c) { return a + (size_t)tile * TILE_BYTES + (size_t)c * 8192; },
           [=](int, int c) { return b + (size_t)c * B_CHUNK_BYTES; }, g.err);
     }
     return;
@@ -465,16 +568,17 @@ __global__ void __launch_bounds__(TC_P_THREADS, 1) bptt_dgrad_kernel(DgradArgs g
   uint32_t li = 0;
   bool ok = true;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++li) {
-    wg_gemm_item<DGR_NCHUNK>(d, smem_base, wg * 1024, bar_full, bar_empty, li, lane, ok, g.err);
+    wg_gemm_item<NCHUNK>(d, smem_base, wg * 1024, bar_full, bar_empty, li, lane, ok, g.err);
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int row = tile * TC_M + wg * 64 + w4 * 16 + (lane >> 2) + 8 * i;
       if (!ok || row >= g.R) continue;
-      const float fs = unscale * g.gs[row];
+      const float fs = g.dSs ? unscale * g.gs[row] : 0.f;
       // columns 0..127 -> gs * dS, 128..255 -> dh_direct
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
         const int col = 8 * j + 2 * (lane & 3);
+        if (j < 16 && !g.dSs) continue;
         const float f = j < 16 ? fs : unscale;
         float* dst = (j < 16 ? g.dSs + (size_t)row * TC_H + col : g.dh_direct + (size_t)row * TC_H + col - 128);
         *reinterpret_cast<float2*>(dst) = make_float2(d[4 * j + 2 * i] * f, d[4 * j + 2 * i + 1] * f);
@@ -555,7 +659,8 @@ constexpr int WG_NSTAGE1 = 4;
 struct WgradArgs {
   int ntiles;
   int np;                // columns of P (multiple of 16, <= WG_MAX_NP)
-  int j0, j1;            // row-tile subsets of slice 0 / slice 1 (4 * (j0 + j1) roles)
+  int j0, j1;            // row-tile subsets of slice 0 / slice 1 ((gate blocks) * (j0 + j1) roles)
+  int h_only;            // slice 0 = the h block of the operand image alone (tanh cell: G_h is all it needs)
   float* partial;        // [nroles][512 columns max][128] fp32, role-private
   const BpttScalars* sc;
   int q;
@@ -596,7 +701,7 @@ __device__ __forceinline__ unsigned char* wgrad_smem() {
 }
 
 struct WgradRole {
-  int role, mh, sl, nstage, stage_bytes, nchunks, n0;
+  int role, mh, sl, nstage, stage_bytes, a_bytes, nchunks, n0;   // a_bytes: one part of the slice-0 features
   uint32_t bar_full, bar_empty;
 };
 
@@ -627,7 +732,7 @@ __device__ __forceinline__ void wgrad_consumer(const WgradArgs g, const WgradRol
       const uint32_t f = st + 2 * WG_DG_BYTES + (r.n0 / 8) * 512 + ks * 256;
       wgmma_mn<NW>(d, dg_hi, make_desc(f, 128, 512), accum);
       wgmma_mn<NW>(d, dg_lo, make_desc(f, 128, 512), 1);
-      if (SPLIT) wgmma_mn<NW>(d, dg_hi, make_desc(f + WG_A_BYTES, 128, 512), 1);
+      if (SPLIT) wgmma_mn<NW>(d, dg_hi, make_desc(f + r.a_bytes, 128, 512), 1);
     }
     wgmma_commit();
     wgmma_wait<1>();                               // the MMAs of slab ch - 1 have read their stage
@@ -667,10 +772,11 @@ __global__ void __launch_bounds__(WG_THREADS, 1) bptt_wgrad_kernel(WgradArgs g, 
   const int mb = role / per_mb, rj = role - mb * per_mb;
   const int sl = rj < g.j0 ? 0 : 1;
   const int jj = sl == 0 ? rj : rj - g.j0, jn = sl == 0 ? g.j0 : g.j1;
-  const int nstage = sl == 0 ? WG_NSTAGE0 : WG_NSTAGE1;
+  const int nstage = sl == 0 && !g.h_only ? WG_NSTAGE0 : WG_NSTAGE1;
   const int p_bytes = g.np * 64;                    // np/8 groups x 4 row groups x 128 B
-  const int stage_bytes = sl == 0 ? WG_STAGE0 : 2 * WG_DG_BYTES + p_bytes;
-  const int ncols = sl == 0 ? 384 : g.np;
+  const int a_bytes = g.h_only ? WG_A_BYTES / 3 : WG_A_BYTES;
+  const int stage_bytes = sl == 0 ? 2 * WG_DG_BYTES + 2 * a_bytes : 2 * WG_DG_BYTES + p_bytes;
+  const int ncols = sl == 0 ? (g.h_only ? 128 : 384) : g.np;
   const int nact = (ncols + 127) / 128;             // consumer warpgroups with columns
   const uint32_t bar_full = smem_u32(bars), bar_empty = smem_u32(bars + WG_NSTAGE1);
   if (threadIdx.x == 0) {
@@ -697,9 +803,10 @@ __global__ void __launch_bounds__(WG_THREADS, 1) bptt_wgrad_kernel(WgradArgs g, 
       mbar_expect_tx(bar_full + 8 * s, stage_bytes);
       tma_load_5d(dst, &map_dg, 0, 4 * rc, 16 * mb, 0, tile, bar_full + 8 * s);
       tma_load_5d(dst + WG_DG_BYTES, &map_dg, 0, 4 * rc, 16 * mb, 1, tile, bar_full + 8 * s);
-      if (sl == 0) {
-        tma_load_5d(dst + 2 * WG_DG_BYTES, &map_a, 0, 4 * rc, 0, 0, tile, bar_full + 8 * s);
-        tma_load_5d(dst + 2 * WG_DG_BYTES + WG_A_BYTES, &map_a, 0, 4 * rc, 0, 1, tile, bar_full + 8 * s);
+      if (sl == 0) {                                // h_only: the box is the 16 groups of h, from feature group 32
+        const int g0 = g.h_only ? 32 : 0;
+        tma_load_5d(dst + 2 * WG_DG_BYTES, &map_a, 0, 4 * rc, g0, 0, tile, bar_full + 8 * s);
+        tma_load_5d(dst + 2 * WG_DG_BYTES + a_bytes, &map_a, 0, 4 * rc, g0, 1, tile, bar_full + 8 * s);
       } else {
         tma_load_4d(dst + 2 * WG_DG_BYTES, &map_p, 0, 4 * rc, 0, tile, bar_full + 8 * s);
       }
@@ -708,7 +815,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) bptt_wgrad_kernel(WgradArgs g, 
   }
   const int w = warp >> 2, w4 = warp & 3;
   if (w >= nact || nchunks == 0) return;
-  const WgradRole r{role, mh, sl, nstage, stage_bytes, nchunks, 128 * w, bar_full, bar_empty};
+  const WgradRole r{role, mh, sl, nstage, stage_bytes, a_bytes, nchunks, 128 * w, bar_full, bar_empty};
   if (sl == 0) {
     wgrad_consumer<128, true>(g, r, w4, lane);
     return;
@@ -729,13 +836,14 @@ __global__ void __launch_bounds__(WG_THREADS, 1) bptt_wgrad_kernel(WgradArgs g, 
 // finish
 // ------------------------------------------------------------------------------------------------------------------
 // G[j][n] = sum over the CTAs of (mb = j / 128, slice(n)) of partial[cta][n_local][j % 128]   (float64)
-__global__ void bptt_reduce_partials_kernel(const float* __restrict__ partial, int j0, int j1, int np, double* __restrict__ G,
-                                            int ncols_total) {
+// ng gate columns (512; tanh cell 128), nc0 slice-0 feature columns (x | S | h = 384; tanh cell h = 128)
+__global__ void bptt_reduce_partials_kernel(const float* __restrict__ partial, int ng, int nc0, int j0, int j1,
+                                            double* __restrict__ G, int ncols_total) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;     // (n, j): j fastest -> coalesced partial reads
-  if (idx >= 512 * ncols_total) return;
-  const int n = idx >> 9, j = idx & 511;
+  if (idx >= ng * ncols_total) return;
+  const int n = idx / ng, j = idx - n * ng;
   const int mb = j >> 7, m = j & 127;
-  const int sl = n < 384 ? 0 : 1, nl = sl == 0 ? n : n - 384;
+  const int sl = n < nc0 ? 0 : 1, nl = sl == 0 ? n : n - nc0;
   const int per_mb = j0 + j1;
   const int first = mb * per_mb + (sl == 0 ? 0 : j0), cnt = sl == 0 ? j0 : j1;
   double acc = 0.0;
@@ -760,13 +868,15 @@ struct FinishArgs {
   int head_dim[IC3_MAX_HEADS];
   const double* G;          // [512][NC] rows = gate column j = 4u + gate
   int NC;
-  const double* Y;          // [128][np]  W_ih^T Q
+  const double* Y;          // [128][ldy]  W_ih^T Q  (tanh cell: Q itself, the P block of G)
+  int ldy;
   const double* GSC;        // [512][128] G_S C^T
   const double* dC;         // [128][128] W_ih^T G_S
   const float* c_b;
   float* g_w_ih; float* g_w_hh; float* g_b_ih; float* g_b_hh; float* g_c_w; float* g_c_b;
   float* g_enc_w; float* g_enc_b; float* g_value_w; float* g_value_b;
   float* g_head_w[IC3_MAX_HEADS]; float* g_head_b[IC3_MAX_HEADS];
+  float* g_f_w; float* g_f_b;                               // tanh cell: affine2
   const float* gw_part; const double* gs_part; int nhb;     // heads partials
   double* losses;            // [3] out
   ic3_pp_cfg pp; ic3_tj_cfg tj; int is_tj;
@@ -791,6 +901,16 @@ __global__ void bptt_finish_lstm_kernel(FinishArgs f) {
   if (idx < TC_H * TC_H) f.g_c_w[idx] += (float)f.dC[idx];     // [k][m]
 }
 
+// tanh cell: d affine2.weight[u][k] = G_h[u][k], d affine2.bias[u] = g1[u]  (G = [h | P], rows = unit u)
+__global__ void bptt_finish_tanh_kernel(FinishArgs f) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= TC_H * TC_H) return;
+  const int u = idx >> 7, k = idx & 127;
+  const double* Gu = f.G + (size_t)u * f.NC;
+  f.g_f_w[idx] += (float)Gu[k];
+  if (k == 0) f.g_f_b[u] += (float)Gu[TC_H + f.ones_col];
+}
+
 // encoder window-cell features per update: W^2 cells x V classes (+ the two TJ scalars)
 __host__ __device__ inline int finish_enc_items(const FinishArgs& f) {
   const int W = f.is_tj ? 2 * f.tj.vision + 1 : 2 * f.pp.vision + 1;
@@ -804,10 +924,10 @@ __host__ __device__ inline int finish_enc_items(const FinishArgs& f) {
 __global__ void bptt_finish_misc_kernel(FinishArgs f) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const int k = idx & 127;
-  const double* Yk = f.Y + (size_t)k * f.np;
+  const double* Yk = f.Y + (size_t)k * f.ldy;
   if (idx < TC_H) {
     const double y1 = Yk[f.ones_col];
-    f.g_c_b[k] += (float)y1;                   // W_ih^T g1
+    if (f.g_c_b) f.g_c_b[k] += (float)y1;      // W_ih^T g1 (NULL: the tanh RNN's frozen zero C bias gets nothing)
     f.g_enc_b[k] += (float)y1;
   }
   const int W = f.is_tj ? 2 * f.tj.vision + 1 : 2 * f.pp.vision + 1;
@@ -1012,11 +1132,19 @@ struct Layout {         // of the workspace, in bytes
       gw_part, gs_part, sc, G, Y, GSC, dC, wj, cw, losses, total;
   int ntiles, np, npos, WW, j0, j1, ncta_wg, nhb;
   int P;                // comm passes: backward units per lock-step
+  int tanh;             // the tanh recurrence without communication (models.RNN, rnn_type 'MLP')
+  int ng, nc0;          // gate columns (512; tanh 128) and slice-0 feature columns of G (x | S | h = 384; tanh h = 128)
 };
 
 int plan_layout(const ic3_policy_cfg* cfg, int npos, int WW, int is_tj, Layout* L) {
-  // the LSTM-cell policies of the tensor-core path, 1 .. IC3_MAX_PASSES comm passes
-  if (cfg->cell != IC3_CELL_LSTM || cfg->x_tanh || cfg->h_from_x || cfg->passes > IC3_MAX_PASSES) return IC3_E_UNSUPPORTED;
+  // the LSTM-cell policies of the tensor-core path, 1 .. IC3_MAX_PASSES comm passes; the tanh recurrence with one pass
+  // and no communication (comm_mask_zero, no hard attention: the IC / IRIC baselines of the SIMT path)
+  if (cfg->x_tanh || cfg->h_from_x || cfg->passes > IC3_MAX_PASSES) return IC3_E_UNSUPPORTED;
+  const bool tanh_cell = cfg->cell == IC3_CELL_TANH && cfg->passes <= 1 && cfg->comm_mask_zero && !cfg->hard_attn;
+  if (cfg->cell != IC3_CELL_LSTM && !tanh_cell) return IC3_E_UNSUPPORTED;
+  L->tanh = tanh_cell;
+  L->ng = tanh_cell ? TC_H : 4 * TC_H;
+  L->nc0 = tanh_cell ? TC_H : 3 * TC_H;
   L->P = cfg->passes > 1 ? cfg->passes : 1;
   const long R = (long)cfg->B * cfg->N;
   L->ntiles = (int)((R + TC_M - 1) / TC_M);
@@ -1025,16 +1153,19 @@ int plan_layout(const ic3_policy_cfg* cfg, int npos, int WW, int is_tj, Layout* 
   const int used = npos + (is_tj ? WW + 4 : 2 * WW + 1);
   L->np = (used + 15) / 16 * 16;
   if (L->np > WG_MAX_NP) return IC3_E_UNSUPPORTED;
-  const int per_mb = sm_count() / 8;       // 4 gate-column blocks x per_mb roles x 2 CTAs: one CTA per SM
+  const int nmb = L->ng / 128;             // gate-column blocks
+  const int per_mb = sm_count() / (2 * nmb);   // nmb gate-column blocks x per_mb roles x 2 CTAs: one CTA per SM
   if (per_mb < 2) return IC3_E_UNSUPPORTED;
-  // MMA cycles per 16 rows: slice 0 = 3 * (128 + 86), slice 1 = 2 * (n0 + n1 shapes) -> split the CTAs accordingly
-  const double c0 = 3.0 * (128 + 86), c1 = 2.0 * (L->np > 256 ? 128 + 0.5 * (L->np - 256) + 22 : 0.5 * L->np + 22);
+  // MMA cycles per 16 rows: slice 0 = 3 * (128 + 86) for x | S | h (a third of it for the h block alone), slice 1 =
+  // 2 * (n0 + n1 shapes) -> split the CTAs accordingly
+  const double c0 = 3.0 * (128 + 86) * L->nc0 / 384.0;
+  const double c1 = 2.0 * (L->np > 256 ? 128 + 0.5 * (L->np - 256) + 22 : 0.5 * L->np + 22);
   int j0 = (int)(per_mb * c0 / (c0 + c1) + 0.5);
   if (j0 < 1) j0 = 1;
   if (j0 > per_mb - 1) j0 = per_mb - 1;
   L->j0 = j0;
   L->j1 = per_mb - j0;
-  L->ncta_wg = 4 * per_mb;                 // roles (weight-gradient partials); the kernel runs two CTAs per role
+  L->ncta_wg = nmb * per_mb;               // roles (weight-gradient partials); the kernel runs two CTAs per role
   L->nhb = (int)((R + HB_ROWS - 1) / HB_ROWS);
   size_t off = 0;
   auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 1023) / 1024 * 1024; return o; };
@@ -1042,10 +1173,10 @@ int plan_layout(const ic3_policy_cfg* cfg, int npos, int WW, int is_tj, Layout* 
   // while the main stream fills the other set for step t - 1
   L->a_img = take((size_t)L->ntiles * A_TILE_HALFS * 2);
   L->p_img = take((size_t)L->ntiles * (L->np / 8) * 16 * 128);
-  L->dg_img = take((size_t)L->ntiles * DG_TILE_HALFS * 2);
+  L->dg_img = take((size_t)L->ntiles * (tanh_cell ? DZ_TILE_HALFS : DG_TILE_HALFS) * 2);
   L->img_stride = off;
   take(off);                                   // second set: same sizes, same order
-  L->w2_img = take((size_t)L->P * W2_IMG_HALFS * 2);                    // one dgrad weight image per pass
+  L->w2_img = take((size_t)L->P * (tanh_cell ? W2_IMG_HALFS_TANH : W2_IMG_HALFS) * 2);   // one dgrad weight image per pass
   // comm_passes > 1: (h, c) after passes 0 .. P-2 of the step being differentiated (re-run from the record by
   // ic3_tc_pass_states), and the scratch of that re-run (operand image, head partials)
   ic3_policy_cfg one_pass = *cfg;
@@ -1053,7 +1184,7 @@ int plan_layout(const ic3_policy_cfg* cfg, int npos, int WW, int is_tj, Layout* 
   L->hc_pass = take(L->P > 1 ? (size_t)(L->P - 1) * 2 * R * TC_H * 4 : 0);
   L->tc_ws = take(L->P > 1 ? (size_t)ic3_tc_workspace_bytes(&one_pass) : 0);
   L->dout = take((size_t)2 * L->ntiles * TC_M * BP_HEADS * 4);         // [2]: heads of step t - 1 run while step t reads
-  L->dSs = take((size_t)L->ntiles * TC_M * TC_H * 4);
+  L->dSs = take(tanh_cell ? 0 : (size_t)L->ntiles * TC_M * TC_H * 4);
   L->dh_direct = take((size_t)L->ntiles * TC_M * TC_H * 4);
   L->gs = take((size_t)2 * L->ntiles * TC_M * 4);                       // [2] by step parity, like the images
   L->gr = take((size_t)2 * L->ntiles * TC_M * 4);
@@ -1064,13 +1195,15 @@ int plan_layout(const ic3_policy_cfg* cfg, int npos, int WW, int is_tj, Layout* 
   L->gw_part = take((size_t)L->nhb * BP_HEADS * TC_H * 4);
   L->gs_part = take((size_t)L->nhb * (BP_HEADS + 3) * 8);
   L->sc = take(sizeof(BpttScalars));
-  const int NC = 384 + L->np;
-  L->G = take((size_t)512 * NC * 8);
-  L->Y = take((size_t)TC_H * L->np * 8);
-  L->GSC = take((size_t)512 * TC_H * 8);
-  L->dC = take((size_t)TC_H * TC_H * 8);
-  L->wj = take((size_t)512 * TC_H * 8);
-  L->cw = take((size_t)TC_H * TC_H * 8);
+  const int NC = L->nc0 + L->np;
+  L->G = take((size_t)L->ng * NC * 8);
+  // the LSTM cell's folds through W_ih and C (the tanh cell reads its G directly)
+  const int lstm = tanh_cell ? 0 : 1;
+  L->Y = take(lstm * (size_t)TC_H * L->np * 8);
+  L->GSC = take(lstm * (size_t)512 * TC_H * 8);
+  L->dC = take(lstm * (size_t)TC_H * TC_H * 8);
+  L->wj = take(lstm * (size_t)512 * TC_H * 8);
+  L->cw = take(lstm * (size_t)TC_H * TC_H * 8);
   L->losses = take(3 * 8);
   L->total = off;
   return IC3_OK;
@@ -1123,7 +1256,12 @@ extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) 
   if (e != cudaSuccess) return (int)e;
   e = cudaMemsetAsync(ws + L.a_img, 0, L.w2_img - L.a_img, s);                  // both image sets
   if (e != cudaSuccess) return (int)e;
-  for (int ps = 0; ps < L.P; ++ps) {           // w->lstm_img holds the forward image of every pass, back to back
+  if (L.tanh) {                                // SIMT-packed weights: no forward image, the dgrad image comes from f_wT
+    if (!p->w->f_wT) return IC3_E_NULL;
+    bptt_pack_w2_tanh_kernel<<<(256 * TC_H + 255) / 256, 256, 0, s>>>(p->w->f_wT, reinterpret_cast<__half*>(ws + L.w2_img));
+    IC3_LAUNCH_CHECK();
+  }
+  for (int ps = 0; ps < L.P && !L.tanh; ++ps) {   // w->lstm_img holds the forward image of every pass, back to back
     bptt_pack_w2_kernel<<<(256 * 512 + 255) / 256, 256, 0, s>>>(
         reinterpret_cast<const __half*>(p->w->lstm_img) + (size_t)ps * B_IMG_HALFS,
         reinterpret_cast<__half*>(ws + L.w2_img) + (size_t)ps * W2_IMG_HALFS);
@@ -1173,9 +1311,10 @@ static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, c
   if (cfg->hard_attn && !io->comm) return IC3_E_NULL;
   PrepSrc src;
   memset(&src, 0, sizeof(src));
-  src.wT = p->w->enc_wT; src.bias = p->w->enc_b; src.split = cfg->obs_vocab > 0; src.table = p->x_table;
+  // tanh cell: x is no operand of its GEMMs (the x block of the image stays zero), so it needs no table
+  src.wT = p->w->enc_wT; src.bias = p->w->enc_b; src.split = cfg->obs_vocab > 0; src.table = L.tanh ? nullptr : p->x_table;
   src.wflags = p->w->flags;
-  if (!src.table || !src.split) return IC3_E_NULL;
+  if ((!src.table && !L.tanh) || !src.split) return IC3_E_NULL;
   PrepBwd bw;
   bw.p_img = p_img;
   bw.gs = reinterpret_cast<float*>(ws + L.gs) + (size_t)q * rows_pad;
@@ -1222,8 +1361,8 @@ static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, c
 
 static int bptt_common(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, Layout* L, int* npos, int* is_tj) {
   if (!p || !io || !p->cfg || !p->w || !p->workspace) return IC3_E_NULL;
-  if (!io->h_prev || !io->c_prev || !io->h_new || !io->logp || !io->action || !io->value || !io->ret || !io->adv ||
-      !io->alive_post || !io->dh || !io->dc)
+  if (!io->h_prev || !io->h_new || !io->logp || !io->action || !io->value || !io->ret || !io->adv || !io->alive_post ||
+      !io->dh)
     return IC3_E_NULL;
   if (p->cfg->H != TC_H) return IC3_E_UNSUPPORTED;
   int WW;
@@ -1231,6 +1370,7 @@ static int bptt_common(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, Layou
   if (rc) return rc;
   rc = plan_layout(p->cfg, *npos, WW, *is_tj, L);
   if (rc) return rc;
+  if (!L->tanh && (!io->c_prev || !io->dc)) return IC3_E_NULL;     // the tanh cell has no c
   int nout = 1;
   for (int k = 0; k < p->cfg->nheads; ++k) nout += p->cfg->head_dim[k];
   return nout > BP_HEADS ? IC3_E_UNSUPPORTED : IC3_OK;
@@ -1296,8 +1436,20 @@ static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const L
   bptt_scale_kernel<<<1, 1, 0, s>>>(sc, q);
   IC3_LAUNCH_CHECK();
 
+  // ---- tanh cell: dz image (takes the place of the gate GEMM) ----
+  if (L.tanh) {
+    TanhArgs ta;
+    ta.R = R; ta.N = cfg->N; ta.nrows = ntiles * TC_M; ta.cut = io->cut;
+    ta.dout = reinterpret_cast<const float*>(ws + L.dout) + (size_t)q * rows_pad * BP_HEADS;
+    ta.h_new = io->h_new; ta.dh = io->dh; ta.head_w = (const float*)p->w->head_w; ta.nout = nout;
+    ta.dz_img = dg_img; ta.sc = sc; ta.q = q;
+    bptt_tanh_kernel<<<ntiles * (TC_M / TZ_ROWS), 256, 0, s>>>(ta);
+    IC3_LAUNCH_CHECK();
+    se = cudaEventRecord(ss->gates_done[q], s);
+    if (se != cudaSuccess) return (int)se;
+  }
   // ---- gates ----
-  {
+  if (!L.tanh) {
     static bool cfgd = false;
     const size_t smem = NSTAGE_P * STAGE_BYTES + 256 + TC_H * HEAD_PAD * sizeof(float) + 4 * TC_H * sizeof(float);
     if (!cfgd) {
@@ -1329,17 +1481,23 @@ static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const L
     static bool cfgd = false;
     const size_t smem = NSTAGE_P * DGR_STAGE + 256;
     if (!cfgd) {
-      cudaError_t e = cudaFuncSetAttribute(bptt_dgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return (int)e;
-      prefer_max_smem(bptt_dgrad_kernel);
+      for (auto kern : {bptt_dgrad_kernel<DGR_NCHUNK>, bptt_dgrad_kernel<DGR_NCHUNK_TANH>}) {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return (int)e;
+        prefer_max_smem(kern);
+      }
       cfgd = true;
     }
     DgradArgs da;
-    da.R = R; da.gs = reinterpret_cast<const float*>(ws + L.gs) + (size_t)q * rows_pad; da.dSs = reinterpret_cast<float*>(ws + L.dSs);
+    da.R = R; da.gs = reinterpret_cast<const float*>(ws + L.gs) + (size_t)q * rows_pad;
+    da.dSs = L.tanh ? nullptr : reinterpret_cast<float*>(ws + L.dSs);
     da.dh_direct = reinterpret_cast<float*>(ws + L.dh_direct); da.sc = sc; da.q = q; da.err = io->err;
     const int grid = ntiles < sm_count() ? ntiles : sm_count();
-    bptt_dgrad_kernel<<<grid, TC_P_THREADS, smem, s>>>(
-        da, dg_img, reinterpret_cast<const __half*>(ws + L.w2_img) + (size_t)ps * W2_IMG_HALFS, ntiles);
+    const __half* w2 = reinterpret_cast<const __half*>(ws + L.w2_img);
+    if (L.tanh)
+      bptt_dgrad_kernel<DGR_NCHUNK_TANH><<<grid, TC_P_THREADS, smem, s>>>(da, dg_img, w2, ntiles);
+    else
+      bptt_dgrad_kernel<DGR_NCHUNK><<<grid, TC_P_THREADS, smem, s>>>(da, dg_img, w2 + (size_t)ps * W2_IMG_HALFS, ntiles);
     IC3_LAUNCH_CHECK();
   }
   // ---- comm backward -> dh_{t-1} ----
@@ -1358,7 +1516,7 @@ static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const L
     static bool cfgd = false;
     static CUtensorMap map_dg[2], map_a[2], map_p[2];
     static void* key_ws = nullptr;
-    static int key_tiles = 0, key_np = 0;
+    static int key_tiles = 0, key_np = 0, key_tanh = 0;
     const size_t smem1 = (size_t)WG_NSTAGE1 * (2 * WG_DG_BYTES + (size_t)L.np * 64);
     const size_t smem = (size_t)WG_NSTAGE0 * WG_STAGE0 > smem1 ? (size_t)WG_NSTAGE0 * WG_STAGE0 : smem1;
     if (!cfgd) {
@@ -1372,19 +1530,20 @@ static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const L
       cfgd = true;
     }
     if (smem > 200 * 1024) return IC3_E_UNSUPPORTED;
-    if (key_ws != p->workspace || key_tiles != ntiles || key_np != L.np) {
+    if (key_ws != p->workspace || key_tiles != ntiles || key_np != L.np || key_tanh != L.tanh) {
       for (int k = 0; k < 2; ++k) {
-        rc = make_image_map(&map_dg[k], ws + L.dg_img + (size_t)k * L.img_stride, ntiles, 2, 64, 16);
+        rc = make_image_map(&map_dg[k], ws + L.dg_img + (size_t)k * L.img_stride, ntiles, 2, L.ng / 8, 16);
         if (rc) return rc;
-        rc = make_image_map(&map_a[k], ws + L.a_img + (size_t)k * L.img_stride, ntiles, 2, 48, 48);
+        // tanh cell: the box is the h block alone (16 of the 48 feature groups)
+        rc = make_image_map(&map_a[k], ws + L.a_img + (size_t)k * L.img_stride, ntiles, 2, 48, L.tanh ? 16 : 48);
         if (rc) return rc;
         rc = make_image_map(&map_p[k], ws + L.p_img + (size_t)k * L.img_stride, ntiles, 0, L.np / 8, L.np / 8);
         if (rc) return rc;
       }
-      key_ws = p->workspace; key_tiles = ntiles; key_np = L.np;
+      key_ws = p->workspace; key_tiles = ntiles; key_np = L.np; key_tanh = L.tanh;
     }
     WgradArgs wa;
-    wa.ntiles = ntiles; wa.np = L.np; wa.j0 = L.j0; wa.j1 = L.j1;
+    wa.ntiles = ntiles; wa.np = L.np; wa.j0 = L.j0; wa.j1 = L.j1; wa.h_only = L.tanh;
     wa.partial = reinterpret_cast<float*>(ws + L.partial + (size_t)ps * L.part_stride); wa.sc = sc; wa.q = q; wa.err = io->err;
     cudaStream_t ws_stream = ss->overlap ? ss->side : s;
     if (ss->overlap) {
@@ -1468,7 +1627,7 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
       if (e != cudaSuccess) return (int)e;
     }
   }
-  const int NC = 384 + L.np;
+  const int NC = L.nc0 + L.np;
   double* G = reinterpret_cast<double*>(ws + L.G);
   double* Y = reinterpret_cast<double*>(ws + L.Y);
   double* GSC = reinterpret_cast<double*>(ws + L.GSC);
@@ -1481,7 +1640,7 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
   for (int k = 0; k < cfg->nheads; ++k) atot += cfg->head_dim[k];
   f.O = cfg->O; f.nheads = cfg->nheads; f.atot = atot; f.npos = npos; f.np = L.np; f.WW = WW;
   for (int k = 0; k < IC3_MAX_HEADS; ++k) f.head_dim[k] = cfg->head_dim[k];
-  f.G = G; f.NC = NC; f.Y = Y; f.GSC = GSC; f.dC = dC;
+  f.G = G; f.NC = NC; f.Y = Y; f.ldy = L.np; f.GSC = GSC; f.dC = dC;
   f.g_w_ih = const_cast<float*>(grads->w_ih); f.g_w_hh = const_cast<float*>(grads->w_hh);
   f.g_b_ih = const_cast<float*>(grads->b_ih); f.g_b_hh = const_cast<float*>(grads->b_hh);
   f.g_enc_w = const_cast<float*>(grads->encoder_w); f.g_enc_b = const_cast<float*>(grads->encoder_b);
@@ -1498,18 +1657,34 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
   if (is_tj) f.tj = *p->tj_env;
   else f.pp = *p->pp_env;
   f.ones_col = npos + (is_tj ? WW + 3 : 2 * WW);     // the constant column of P is its last used column
+  if (L.tanh) {
+    // G = [G_h | Q]: affine2 from G_h and g1; affine1 through the observation layout with Y = Q (d x = dz)
+    f.g_f_w = const_cast<float*>(grads->f_w_pass[0]);
+    f.g_f_b = const_cast<float*>(grads->f_b_pass[0]);
+    if (!f.g_f_w || !f.g_f_b) return IC3_E_NULL;
+    bptt_reduce_partials_kernel<<<(L.ng * NC + 255) / 256, 256, 0, s>>>(
+        reinterpret_cast<const float*>(ws + L.partial), L.ng, L.nc0, L.j0, L.j1, G, NC);
+    IC3_LAUNCH_CHECK();
+    bptt_finish_tanh_kernel<<<(TC_H * TC_H + 255) / 256, 256, 0, s>>>(f);
+    IC3_LAUNCH_CHECK();
+    f.Y = G + L.nc0;
+    f.ldy = NC;
+    f.g_c_b = nullptr;
+    bptt_finish_misc_kernel<<<(finish_enc_items(f) * 128 + 255) / 256, 256, 0, s>>>(f);
+    IC3_LAUNCH_CHECK();
+  }
   // One fold per comm pass, in pass order, each ADDING its share: pass p's partials hold G_x, G_h and the P columns of
   // its units (summed over the passes by the additions) and its own S block / constant column, which go with
   // C_modules[p] (share_weights: every pass adds into the one module's gradient buffers).
-  for (int ps = 0; ps < L.P; ++ps) {
+  for (int ps = 0; ps < L.P && !L.tanh; ++ps) {
     const bool own = ps > 0;                           // pass 0 is c_w / c_b, as in ic3_policy_pack
     const float* c_w = own && params->c_w_pass[ps] ? params->c_w_pass[ps] : params->c_w;
     const float* c_b = own && params->c_b_pass[ps] ? params->c_b_pass[ps] : params->c_b;
     const float* g_c_w = own && grads->c_w_pass[ps] ? grads->c_w_pass[ps] : grads->c_w;
     const float* g_c_b = own && grads->c_b_pass[ps] ? grads->c_b_pass[ps] : grads->c_b;
     if (!c_w || !c_b || !g_c_w || !g_c_b) return IC3_E_NULL;
-    bptt_reduce_partials_kernel<<<(512 * NC + 255) / 256, 256, 0, s>>>(
-        reinterpret_cast<const float*>(ws + L.partial + (size_t)ps * L.part_stride), L.j0, L.j1, L.np, G, NC);
+    bptt_reduce_partials_kernel<<<(L.ng * NC + 255) / 256, 256, 0, s>>>(
+        reinterpret_cast<const float*>(ws + L.partial + (size_t)ps * L.part_stride), L.ng, L.nc0, L.j0, L.j1, G, NC);
     IC3_LAUNCH_CHECK();
     bptt_weights_f64_kernel<<<(512 * TC_H + 255) / 256, 256, 0, s>>>(params->w_ih, c_w, wj, cw);
     IC3_LAUNCH_CHECK();

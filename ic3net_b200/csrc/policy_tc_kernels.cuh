@@ -132,7 +132,7 @@ template <int XSRC, bool TAB, bool BWD = false>
 __global__ void __launch_bounds__(256) prep_kernel(ic3_policy_cfg cfg, ic3_policy_io io, __half* __restrict__ img,
                                                    PrepSrc src, PrepBwd bw) {
   static_assert(!(TAB && XSRC == XSRC_TENSOR), "the table belongs to the fused index encoder");
-  static_assert(!BWD || TAB, "the backward pass uses the per-position table form of the encoder");
+  static_assert(!BWD || TAB, "the backward pass uses the per-position table form of the encoder (table NULL: x = 0)");
   __shared__ float s_gate[PREP_ROWS + 64];
   __shared__ float s_den[PREP_ROWS + 64];
   // s_T: gated hidden-state sum of every environment touching this CTA's rows, [PREP_ROWS / N + 2][H] floats at the
@@ -365,7 +365,7 @@ __global__ void __launch_bounds__(256) prep_kernel(ic3_policy_cfg cfg, ic3_polic
         xv = __ldg(reinterpret_cast<const float4*>(io.x + (size_t)row * TC_H) + q);
       } else if (!TAB) {
         xv = *reinterpret_cast<const float4*>(&s_x[rl * TC_H + 4 * q]);
-      } else {
+      } else if (!BWD || src.table) {   // backward of the tanh cell: no table, x is no operand of its GEMMs (zero)
         // x = table[position] + (count / scalar terms in feature order): the same additions as the gather above
         const int pos = s_pos[rl];
         xv = __ldg(reinterpret_cast<const float4*>(pos >= 0 ? src.table + (size_t)pos * TC_H : src.bias) + q);

@@ -38,6 +38,9 @@ the other buffers (``RECORD_BYTES_LIMIT``, ``RECORD_MARGIN_BYTES``), ``record_mo
 only at every ``grad_window``-th step plus max |c| per step, and the backward re-runs the tensor-core policy step over
 one window at a time from its checkpoint into one of two window buffers, just ahead of the BPTT kernels of that window
 (``_recompute_window``).  The recompute is bit-exact, so the gradient equals the full records' bit for bit.
+The tanh RNN (models.RNN with rnn_type 'MLP', the IC / IRIC baselines, on the SIMT policy kernel) has no c: its records
+are h alone, (T+1) B N H 4 bytes (24.3 GB at predator-prey hard, 8192 slots, batch 500), and its windows are re-run with
+the index encoder and the SIMT step.
 """
 import ctypes as C
 import math
@@ -110,7 +113,8 @@ class Trainer(object):
         self.record_for_grad = bool(getattr(args, 'record_for_grad', False))
         self.grad_window = int(getattr(args, 'grad_window', 40))
         # compute_grad implementation: 'kernels' = hand-written BPTT (csrc/bptt_tc.cu; tensor-core policy path with the
-        # LSTM cell and 1..4 comm passes, at most 7 action logits, observation pattern of <= 512 columns), 'autograd' = windowed recompute under torch autograd,
+        # LSTM cell and 1..4 comm passes, or the tanh RNN without communication on the SIMT path; at most 7 action
+        # logits, observation pattern of <= 512 columns), 'autograd' = windowed recompute under torch autograd,
         # 'manual' = explicit formulas with torch GEMMs (bptt.py).  Default: kernels when the configuration allows.
         self.grad_impl = getattr(args, 'grad_impl', None) or 'auto'
         self.grad_kernels = False
@@ -127,8 +131,9 @@ class Trainer(object):
             ok = self._bptt_supported()
             if self.grad_impl == 'kernels' and not ok:
                 raise NotImplementedError("grad_impl='kernels' needs the tensor-core policy path (hid_size 128, LSTM "
-                                          "cell), the per-position encoder table, <= 7 action logits and a small "
-                                          "vision window")
+                                          "cell) with the per-position encoder table, or the tanh RNN without "
+                                          "communication at hid_size 128; <= 7 action logits and a small vision "
+                                          "window")
             self.grad_kernels = ok
         if self.grad_impl == 'auto':
             self.grad_impl = 'kernels' if self.grad_kernels else 'autograd'
@@ -136,16 +141,27 @@ class Trainer(object):
     def _bptt_supported(self):
         e, net = self.env.env, self.policy_net
         W = 2 * e.vision + 1
-        if not net.fuses_encoder(e) or 1 + sum(self.args.naction_heads) > 8:
+        if 1 + sum(self.args.naction_heads) > 8:
             return False
-        # the recurrent LSTM policies, any number of comm passes (share_weights included); not the tanh cells
-        if not net.tc_capable or net.comm_passes > _lib.MAX_PASSES:
+        if self._tanh_rnn():
+            # the tanh RNN runs on the SIMT kernel: no fused encoder, only the same window limit
+            if W * W > 25:
+                return False
+        # the recurrent LSTM policies, any number of comm passes (share_weights included)
+        elif not net.fuses_encoder(e) or not net.tc_capable or net.comm_passes > _lib.MAX_PASSES:
             return False
         if getattr(e, 'obs_layout', (0, 0, 0))[1] == 0:
             return False
         npos = e.obs_positions
         used = npos + ((W * W + 4) if self.is_tj else (2 * W * W + 1))
         return (used + 15) // 16 * 16 <= 512
+
+    def _tanh_rnn(self):
+        """The policy is the tanh recurrence without communication (models.RNN with rnn_type 'MLP': the IC / IRIC
+        baselines) at hid_size 128, which the BPTT kernels differentiate on the SIMT policy path."""
+        cp = self.policy_net._cfg_proto
+        return (cp['cell'] == _lib.CELL_TANH and not cp['x_tanh'] and not cp['h_from_x'] and cp['passes'] <= 1
+                and bool(cp['comm_mask_zero']) and not cp['hard_attn'] and cp['H'] == 128)
 
     def _encoder_table(self, cfg=None, w=None):
         """The policy's per-position encoder table for this environment (CommNetMLP.encoder_table), built from its
@@ -192,15 +208,21 @@ class Trainer(object):
             W = self.grad_window
             nw = (T + W - 1) // W
             self._record_mode = self._pick_record_mode(T) if self.grad_kernels else None
+            hc = not self._h_only_records()          # the tanh RNN's kernels keep h alone: it has no c
             if self._record_mode == 'full':
-                b.update(rec_h=torch.empty(T + 1, B * N, H, device=dev), rec_c=torch.empty(T + 1, B * N, H, device=dev))
+                b['rec_h'] = torch.empty(T + 1, B * N, H, device=dev)
+                if hc:
+                    b['rec_c'] = torch.empty(T + 1, B * N, H, device=dev)
             else:
-                b.update(ck_h=z(nw, B * N, H), ck_c=z(nw, B * N, H))
+                b['ck_h'] = z(nw, B * N, H)
+                if hc:
+                    b['ck_c'] = z(nw, B * N, H)
             if self._record_mode == 'window':
                 nb, L = min(nw, self._window_buffers()), min(W, T)      # window k lives in buffer k % _window_buffers()
                 e_ = lambda *s: torch.empty(*s, device=dev)
-                b.update(c_abs=z(T), win_h=[e_(L, B * N, H) for _ in range(nb)],
-                         win_c=[e_(L, B * N, H) for _ in range(nb)], win_value=e_(B * N), win_logp=e_(B * N, A))
+                b.update(win_h=[e_(L, B * N, H) for _ in range(nb)], win_value=e_(B * N), win_logp=e_(B * N, A))
+                if hc:
+                    b.update(c_abs=z(T), win_c=[e_(L, B * N, H) for _ in range(nb)])
         self._buf = b
         self._graph = None
         return b
@@ -230,12 +252,19 @@ class Trainer(object):
         # windows are re-run two ahead of the backward (_compute_grad_kernels); one-step windows need a third buffer
         return 2 if self.grad_window >= 2 else 3
 
+    def _h_only_records(self):
+        """The BPTT kernels of the tanh RNN record h alone (no c, no max |c|)."""
+        return self.grad_kernels and self._tanh_rnn()
+
     def _record_bytes(self, T):
-        """{'full': bytes of rec_h + rec_c, 'window': bytes of the checkpoints + window buffers} for T steps."""
+        """{'full': bytes of rec_h + rec_c, 'window': bytes of the checkpoints + window buffers} for T steps (h alone
+        for the tanh RNN)."""
         R, H, W = self.env.env.nenvs * self.args.nagents, self.args.hid_size, self.grad_window
         row = R * H * 4
         nw = (T + W - 1) // W
         nb = min(nw, self._window_buffers())
+        if self._h_only_records():
+            return dict(full=(T + 1) * row, window=nw * row + nb * min(W, T) * row)
         return dict(full=2 * (T + 1) * row, window=2 * nw * row + 2 * nb * min(W, T) * row + T * 4)
 
     def _bptt_extra_bytes(self):
@@ -312,6 +341,7 @@ class Trainer(object):
         rec = self.record_for_grad
         full = rec and self._record_mode == 'full'    # the policy step writes (h, c) straight into the records
         window = rec and self._record_mode == 'window'    # (h, c) checkpoints + max |c| per step (_alloc)
+        hc = not self._h_only_records()               # the tanh RNN's kernel records: h alone
         dense = self.obs_mode == 'dense'
         # dense observations written on a side stream while the policy step runs (see _overlap_obs)
         overlap = self._overlap_obs()
@@ -351,7 +381,8 @@ class Trainer(object):
                         b['s_loc'][0].copy_(e.loc)
                 if not full and t % self.grad_window == 0:
                     b['ck_h'][t // self.grad_window].copy_(b['h'])
-                    b['ck_c'][t // self.grad_window].copy_(b['c'])
+                    if hc:
+                        b['ck_c'][t // self.grad_window].copy_(b['c'])
             if overlap:
                 # the writer reads the state the previous env step left and must finish before this step's env step
                 # moves the agents (the join below)
@@ -371,8 +402,8 @@ class Trainer(object):
             else:
                 _lib.check(lib.ic3_pp_encoder_index(C.byref(e.cfg), C.byref(e.state), C.byref(cfg), C.byref(w),
                                                     b['x'].data_ptr(), s))
-            hin, cin = (b['rec_h'][t], b['rec_c'][t]) if full else (b['h'], b['c'])
-            hout, cout = (b['rec_h'][t + 1], b['rec_c'][t + 1]) if full else (b['h'], b['c'])
+            hin, hout = (b['rec_h'][t], b['rec_h'][t + 1]) if full else (b['h'], b['h'])
+            cin, cout = (b['rec_c'][t], b['rec_c'][t + 1]) if full and hc else (b['c'], b['c'])
             io = _lib.PolicyIO(x=None if fused_x else b['x'].data_ptr(), h=hin.data_ptr(), c=cin.data_ptr(),
                                comm_action=b['comm'].data_ptr() if hard else None, alive=b['alive'].data_ptr(),
                                fresh=b['fresh'].data_ptr(), tick=e.tick.data_ptr(), draws=None,
@@ -380,7 +411,7 @@ class Trainer(object):
                                logp=b['logp'][t].data_ptr(), action=b['action'][t].data_ptr(),
                                workspace=_lib.ptr(ws), err=b['err'].data_ptr(), **src)
             _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
-            if window:
+            if window and hc:
                 # max |c'| of this step: the backward's operand scale needs the bound over every step's c before it
                 # re-runs any window, the same value a full record gives (_compute_grad_kernels)
                 torch.linalg.vector_norm(b['c'], math.inf, out=b['c_abs'][t])
@@ -687,21 +718,23 @@ class Trainer(object):
         cfg = net.policy_cfg(B)
         cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
         w = net.packed()
-        table = self._encoder_table()
+        hc = not self._h_only_records()        # the tanh RNN: h alone, no encoder table (x is no operand of its GEMMs)
+        table = _lib.ptr(self._encoder_table()) if hc else None
         if self._bptt is None or self._bptt['B'] != B:
             plan = _lib.BpttPlan(cfg=C.pointer(cfg), w=C.pointer(w),
                                  pp_env=None if self.is_tj else C.pointer(e.cfg),
-                                 tj_env=C.pointer(e.cfg) if self.is_tj else None, x_table=table.data_ptr(),
+                                 tj_env=C.pointer(e.cfg) if self.is_tj else None, x_table=table,
                                  value_coeff=float(args.value_coeff), entr=float(args.entr), workspace=None)
             nbytes = int(lib.ic3_bptt_workspace_bytes(C.byref(plan)))
             if nbytes == 0:
                 raise NotImplementedError("this configuration is outside the BPTT kernels (use grad_impl='autograd')")
             self._bptt = dict(B=B, ws=torch.empty(nbytes, dtype=torch.uint8, device=e.device),
-                              dh=torch.zeros(B * N, H, device=e.device), dc=torch.zeros(B * N, H, device=e.device),
+                              dh=torch.zeros(B * N, H, device=e.device),
+                              dc=torch.zeros(B * N, H, device=e.device) if hc else None,
                               losses=torch.zeros(3, dtype=torch.float64, device=e.device))
         st = self._bptt
         plan = _lib.BpttPlan(cfg=C.pointer(cfg), w=C.pointer(w), pp_env=None if self.is_tj else C.pointer(e.cfg),
-                             tj_env=C.pointer(e.cfg) if self.is_tj else None, x_table=table.data_ptr(),
+                             tj_env=C.pointer(e.cfg) if self.is_tj else None, x_table=table,
                              value_coeff=float(args.value_coeff), entr=float(args.entr), workspace=st['ws'].data_ptr())
         hard = bool(args.hard_attn) and bool(args.commnet)
         adv = adv.contiguous()
@@ -710,7 +743,16 @@ class Trainer(object):
             cut = (((b['s_tep'] + 1) % args.detach_gap) == 0).to(torch.uint8).contiguous()
         window = self._record_mode == 'window'
         W = self.grad_window
-        if window:
+        if not hc:
+            cmax = 0.0                          # no cell state: the operand scale bounds |dh| alone
+
+            def state(t):                      # h entering step t and h' leaving it (window: in the window buffers)
+                if not window:
+                    return b['rec_h'][t], None, b['rec_h'][t + 1]
+                k, j = divmod(t, W)
+                wh = b['win_h'][k % self._window_buffers()]
+                return (b['ck_h'][k] if j == 0 else wh[j - 1]), None, wh[j]
+        elif window:
             cmax = float(b['c_abs'].max().item())                              # tracked per step by the rollout
             nb = self._window_buffers()
 
@@ -737,13 +779,14 @@ class Trainer(object):
 
         recompute_due(T)
         st['dh'].zero_()
-        st['dc'].zero_()
+        if hc:
+            st['dc'].zero_()
         _lib.check(lib.ic3_bptt_begin(C.byref(plan), cmax, s))
         value = b['value']
 
         def step_io(t):
             hp, cp, hn = state(t)
-            return _lib.BpttStepIO(t=t, h_prev=hp.data_ptr(), c_prev=cp.data_ptr(),
+            return _lib.BpttStepIO(t=t, h_prev=hp.data_ptr(), c_prev=_lib.ptr(cp),
                                    h_new=hn.data_ptr(), fresh=b['s_fresh'][t].data_ptr(),
                                    comm=b['s_comm'][t].data_ptr() if hard else None, alive=b['s_alive'][t].data_ptr(),
                                    cut=cut[t].data_ptr() if cut is not None else None,
@@ -755,7 +798,7 @@ class Trainer(object):
                                    logp=b['logp'][t].data_ptr(), action=b['action'][t].data_ptr(),
                                    value=value[t].data_ptr(), ret=ret[t].data_ptr(), adv=adv[t].data_ptr(),
                                    alive_post=b['ralive'][t].data_ptr(), valid=b['valid'][t].data_ptr(),
-                                   dh=st['dh'].data_ptr(), dc=st['dc'].data_ptr(), err=b['err'].data_ptr())
+                                   dh=st['dh'].data_ptr(), dc=_lib.ptr(st['dc']), err=b['err'].data_ptr())
         # look-ahead: the heads gradient and the operand images of step t - 1 do not depend on the recursion; they are
         # launched on the library's side stream before step t and overlap its tensor-core kernels
         nxt = step_io(T - 1) if T > 0 else None
@@ -780,7 +823,9 @@ class Trainer(object):
         fused index encoder with the per-position table); nothing is sampled and value / log-probs go to scratch.  The
         tensor-core policy step is deterministic and every encoder form gives the same x, so each row equals the
         rollout's (h', c') bit for bit -- except for slots that had already completed their batch (valid = 0), whose
-        inputs the env step no longer records; those rows carry no loss and no gradient."""
+        inputs the env step no longer records; those rows carry no loss and no gradient.
+        The tanh RNN (h alone, c is None): the index encoder from the recorded env state into the rollout's x buffer,
+        then the SIMT policy step, the same kernels and operands as the rollout."""
         b, e, net, args = self._buf, self.env.env, self.policy_net, self.args
         lib = _lib.load()
         B, W = e.nenvs, self.grad_window
@@ -788,12 +833,26 @@ class Trainer(object):
         cfg = net.policy_cfg(B)
         cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
         w = net.packed()
+        nb = self._window_buffers()
+        s = _lib.stream()
+        if self._h_only_records():
+            wh = b['win_h'][k % nb]
+            enc = lib.ic3_tj_encoder_index if self.is_tj else lib.ic3_pp_encoder_index
+            for t in range(t0, t1):
+                j = t - t0
+                hin = b['ck_h'][k] if j == 0 else wh[j - 1]
+                ecfg, est = self._record_state(t)
+                _lib.check(enc(C.byref(ecfg), C.byref(est), C.byref(cfg), C.byref(w), b['x'].data_ptr(), s))
+                io = _lib.PolicyIO(x=b['x'].data_ptr(), h=hin.data_ptr(), c=None, comm_action=None,
+                                   alive=b['s_alive'][t].data_ptr(), fresh=b['s_fresh'][t].data_ptr(), tick=None,
+                                   draws=None, h_out=wh[j].data_ptr(), c_out=None, value=b['win_value'].data_ptr(),
+                                   logp=b['win_logp'].data_ptr(), action=None, workspace=None, err=b['err'].data_ptr())
+                _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
+            return wh[:t1 - t0], None
         table = self._encoder_table()
         ws, _ = net.workspace(B)
         hard = bool(args.hard_attn) and bool(args.commnet)
-        nb = self._window_buffers()
         wh, wc = b['win_h'][k % nb], b['win_c'][k % nb]
-        s = _lib.stream()
         for t in range(t0, t1):
             j = t - t0
             hin, cin = (b['ck_h'][k], b['ck_c'][k]) if j == 0 else (wh[j - 1], wc[j - 1])
@@ -828,11 +887,13 @@ class Trainer(object):
             arr = lambda lst: (C.c_void_p * _lib.MAX_HEADS)(*([get(t) for t in lst] + [None] * (_lib.MAX_HEADS - len(lst))))
             # C_modules[p] per comm pass (share_weights: the same module, so the gradient pointers alias)
             parr = lambda lst: (C.c_void_p * _lib.MAX_PASSES)(*([get(t) for t in lst] + [None] * (_lib.MAX_PASSES - len(lst))))
+            # the LSTM cell's w_ih / w_hh / b_ih / b_hh, or the tanh cell's f_w / f_b per pass
+            cell = (dict(w_ih=get(w['w_ih']), w_hh=get(w['w_hh']), b_ih=get(w['b_ih']), b_hh=get(w['b_hh']))
+                    if 'w_ih' in w else dict(f_w_pass=parr(w['f_w']), f_b_pass=parr(w['f_b'])))
             return _lib.PolicyParams(encoder_w=get(w['enc_w']), encoder_b=get(w['enc_b']), c_w=get(w['c_w'][0]),
-                                     c_b=get(w['c_b'][0]), w_ih=get(w['w_ih']), w_hh=get(w['w_hh']), b_ih=get(w['b_ih']),
-                                     b_hh=get(w['b_hh']), value_w=get(w['value_w']), value_b=get(w['value_b']),
+                                     c_b=get(w['c_b'][0]), value_w=get(w['value_w']), value_b=get(w['value_b']),
                                      head_w=arr(w['head_w']), head_b=arr(w['head_b']),
-                                     c_w_pass=parr(w['c_w']), c_b_pass=parr(w['c_b']))
+                                     c_w_pass=parr(w['c_w']), c_b_pass=parr(w['c_b']), **cell)
         return mk(lambda p: p.data_ptr()), mk(grad_ptr)
 
     def _compute_grad_manual(self, adv, ret, W, nw):

@@ -392,7 +392,11 @@ int ic3_stat_reduce(int32_t B, int32_t N, const int32_t* stat_episodes, const in
  * Back-propagation through time of the rollout loss (Trainer.compute_grad, trainer.py:128-225;
  * utils.multinomials_log_density utils.py:42-46) over the records of a lock-step rollout, hid_size 128,
  * at most 7 action logits, the recurrent LSTM CommNet / IC3Net with 1 .. IC3_MAX_PASSES comm passes (share_weights
- * included; cfg->cell == IC3_CELL_LSTM, no x_tanh / h_from_x).  The host walks the lock-step iterations t = T-1 .. 0:
+ * included; cfg->cell == IC3_CELL_LSTM, no x_tanh / h_from_x), and the tanh recurrence without communication
+ * (models.RNN with rnn_type 'MLP', the IC / IRIC baselines: cfg->cell == IC3_CELL_TANH, one pass, comm_mask_zero,
+ * no hard_attn, no x_tanh / h_from_x; SIMT-packed weights, f_w_pass[0] / f_b_pass[0] in params and grads; no c:
+ * c_prev / dc may be NULL and c_abs_max is ignored).  Every other configuration gets a workspace of 0 bytes.
+ * The host walks the lock-step iterations t = T-1 .. 0:
  *     ic3_bptt_begin(plan, max |c| of the record, stream)
  *     for t in reversed(range(T)): ic3_bptt_step(plan, &io_t, stream)
  *     ic3_bptt_finish(plan, params, grads, losses, stream)
@@ -411,7 +415,8 @@ typedef struct {
   const ic3_policy_packed* w;
   const ic3_pp_cfg* pp_env;     /* exactly one of pp_env / tj_env */
   const ic3_tj_cfg* tj_env;
-  const float* x_table;         /* device: ic3_*_encoder_table of the CURRENT weights (required) */
+  const float* x_table;         /* device: ic3_*_encoder_table of the CURRENT weights (LSTM cell: required; tanh
+                                   cell: unused, may be NULL) */
   float value_coeff;            /* args.value_coeff (trainer.py:209) */
   float entr;                   /* args.entr (trainer.py:211-220) */
   void* workspace;              /* device scratch of ic3_bptt_workspace_bytes(plan) bytes */
