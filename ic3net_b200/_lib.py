@@ -16,6 +16,7 @@ MAX_AGENTS = 32
 MAX_HEADS = 4
 MAX_HEAD_DIM = 16
 MAX_PASSES = 4
+RANDOM_WORDS = 16
 CELL_LSTM, CELL_TANH = 0, 1
 LSTM_IMG_BYTES = 786432
 
@@ -148,6 +149,7 @@ SYMBOLS = {
     "ic3_policy_pass_states": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), C.POINTER(PolicyIO), C.c_int32,
                                          _PTR, _PTR, _PTR]),
     "ic3_sample_actions": (C.c_int, [C.POINTER(PolicyCfg), _PTR, _PTR, _PTR, _PTR, _PTR]),
+    "ic3_random_policy_step": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyIO), _PTR, _PTR]),
     "ic3_returns_scan": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, _PTR, _PTR, _PTR, _PTR,
                                    _PTR]),
     "ic3_bptt_workspace_bytes": (C.c_uint64, [C.POINTER(BpttPlan)]),

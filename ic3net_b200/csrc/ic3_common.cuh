@@ -29,8 +29,10 @@ extern unsigned long long g_ic3_launches;  // c_api.cu
 // Philox4x32-10 (Salmon et al., SC'11).  Same stream layout as oracle/philox.py:
 //   key = (seed_lo, seed_hi), counter = (env_id, tick, stream, index)
 // Every draw is reduced to 24 bits so u = u24 * 2^-24 is exact in fp32.
+// Stream 4 (the Random policy's value and logits, random_policy.cu): tick = env step counter, index = 4 * agent + block;
+// agent i's words u[0..15] are blocks 0..3 in order (IC3_RANDOM_WORDS).
 // ---------------------------------------------------------------------------
-enum { IC3_STREAM_PP_RESET = 1, IC3_STREAM_TJ_SPAWN = 2, IC3_STREAM_ACTION = 3 };
+enum { IC3_STREAM_PP_RESET = 1, IC3_STREAM_TJ_SPAWN = 2, IC3_STREAM_ACTION = 3, IC3_STREAM_RANDOM_POLICY = 4 };
 
 __host__ __device__ __forceinline__ void ic3_mulhilo(uint32_t a, uint32_t b, uint32_t& hi, uint32_t& lo) {
 #ifdef __CUDA_ARCH__

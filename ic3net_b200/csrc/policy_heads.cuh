@@ -1,6 +1,7 @@
 // Value / action heads, log-softmax and inverse-CDF sampling for one agent row, executed by
 // one warp (reference: comm.py:228-239, action_utils.py:32-36).  Shared by the fp32 SIMT
-// policy kernel (policy.cu) and the tensor-core policy path (policy_tc.cu).
+// policy kernel (policy.cu), the tensor-core policy path (policy_tc.cu) and the Random policy
+// step (random_policy.cu).
 #pragma once
 #include "ic3_common.cuh"
 
@@ -88,6 +89,53 @@ struct HeadsFinish {
   int32_t* action;        // [R, nheads] or NULL (no sampling)
 };
 
+// Log-softmax per head and inverse-CDF sampling of ONE agent row by ONE thread (action_utils.py:32-36): logit[1 + j] is
+// action logit j, heads concatenated (logit[0], the value, is not read), 1 + atot <= IC3_HEAD_PAD.  Head k samples with
+// word k of the action stream (env_id0 + e, tick[e], IC3_STREAM_ACTION, i) or draws[row, k]; action == NULL: no
+// sampling.  Shared by the tensor-core heads (heads_finish_row) and the Random policy step (random_policy.cu).
+__device__ __forceinline__ void heads_logp_sample_row(const float (&logit)[IC3_HEAD_PAD], int nheads,
+                                                      const int* head_dim, int atot, uint64_t seed, uint32_t env_id0,
+                                                      const uint32_t* tick, const uint32_t* draws, long row, int e,
+                                                      int i, float* logp, int32_t* action) {
+  const bool do_sample = action != nullptr;
+  uint4 d24 = make_uint4(0, 0, 0, 0);
+  if (do_sample && !draws)
+    d24 = ic3_draw24(seed, env_id0 + (uint32_t)e, tick ? tick[e] : 0u, IC3_STREAM_ACTION, (uint32_t)i);
+  int off = 1;
+  for (int k = 0; k < nheads; ++k) {
+    const int na = head_dim[k];
+    float m = -INFINITY;
+#pragma unroll
+    for (int o = 1; o < IC3_HEAD_PAD; ++o)
+      if (o >= off && o < off + na) m = fmaxf(m, logit[o]);
+    float ssum = 0.f;
+#pragma unroll
+    for (int o = 1; o < IC3_HEAD_PAD; ++o)
+      if (o >= off && o < off + na) ssum += expf(logit[o] - m);
+    const float lse = m + logf(ssum);
+    uint32_t u24 = 0;
+    if (do_sample) u24 = draws ? draws[(size_t)row * nheads + k] : ic3_word(d24, k);
+    const float u = (float)u24 * 5.9604644775390625e-08f;
+    float cdf = 0.f;
+    int act = na - 1;
+    bool found = false;
+#pragma unroll
+    for (int o = 1; o < IC3_HEAD_PAD; ++o) {
+      if (o >= off && o < off + na) {
+        const float lp = logit[o] - lse;
+        logp[(size_t)row * atot + (o - 1)] = lp;
+        cdf += expf(lp);
+        if (!found && cdf > u) {
+          act = o - off;
+          found = true;
+        }
+      }
+    }
+    if (do_sample) action[(size_t)row * nheads + k] = act;
+    off += na;
+  }
+}
+
 __device__ __forceinline__ void heads_finish_row(const HeadsFinish& f, long row, int e, int i) {
   float logit[IC3_HEAD_PAD];
   const float4* p4 = reinterpret_cast<const float4*>(f.partial + (size_t)row * IC3_HEAD_NSLOT * IC3_HEAD_PAD);
@@ -107,41 +155,6 @@ __device__ __forceinline__ void heads_finish_row(const HeadsFinish& f, long row,
 #pragma unroll
   for (int o = 0; o < IC3_HEAD_PAD; ++o) logit[o] += (o < 1 + atot) ? __ldg(f.head_b + o) : 0.f;
   f.value[row] = logit[0];
-  const bool do_sample = f.action != nullptr;
-  uint4 d24 = make_uint4(0, 0, 0, 0);
-  if (do_sample && !f.draws)
-    d24 = ic3_draw24(f.seed, f.env_id0 + (uint32_t)e, f.tick ? f.tick[e] : 0u, IC3_STREAM_ACTION, (uint32_t)i);
-  int off = 1;
-  for (int k = 0; k < f.nheads; ++k) {
-    const int na = f.head_dim[k];
-    float m = -INFINITY;
-#pragma unroll
-    for (int o = 1; o < IC3_HEAD_PAD; ++o)
-      if (o >= off && o < off + na) m = fmaxf(m, logit[o]);
-    float ssum = 0.f;
-#pragma unroll
-    for (int o = 1; o < IC3_HEAD_PAD; ++o)
-      if (o >= off && o < off + na) ssum += expf(logit[o] - m);
-    const float lse = m + logf(ssum);
-    uint32_t u24 = 0;
-    if (do_sample) u24 = f.draws ? f.draws[(size_t)row * f.nheads + k] : ic3_word(d24, k);
-    const float u = (float)u24 * 5.9604644775390625e-08f;
-    float cdf = 0.f;
-    int act = na - 1;
-    bool found = false;
-#pragma unroll
-    for (int o = 1; o < IC3_HEAD_PAD; ++o) {
-      if (o >= off && o < off + na) {
-        const float lp = logit[o] - lse;
-        f.logp[(size_t)row * atot + (o - 1)] = lp;
-        cdf += expf(lp);
-        if (!found && cdf > u) {
-          act = o - off;
-          found = true;
-        }
-      }
-    }
-    if (do_sample) f.action[(size_t)row * f.nheads + k] = act;
-    off += na;
-  }
+  heads_logp_sample_row(logit, f.nheads, f.head_dim, atot, f.seed, f.env_id0, f.tick, f.draws, row, e, i, f.logp,
+                        f.action);
 }

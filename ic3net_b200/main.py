@@ -4,7 +4,7 @@
         --max_steps 80 --hid_size 128 --ic3net --recurrent --nenvs 8192 --num_epochs 1
 
 Every reference flag is accepted with its meaning; flags of subsystems outside the accelerated
-path (``--plot``/visdom, ``--display``/curses, the MLP/RNN/Random baselines of models.py) are
+path (``--plot``/visdom, ``--display``/curses) are
 parsed and rejected with a clear message.  New flags: ``--nenvs`` (environment slots per GPU),
 ``--obs_mode`` (index | dense), ``--policy_impl`` (tc | simt), ``--use_graph``.
 Multi-GPU: launch with ``python -m torch.distributed.run --nproc-per-node N -m ic3net_b200.main ...``.

@@ -180,12 +180,15 @@ class MultiGPUTrainer(object):
     def train_batch(self, epoch):
         tr = self.trainer
         if hasattr(tr, 'stat_vector') and hasattr(tr.optimizer, 'flat_grads'):
+            learns = not getattr(tr, 'random_policy', False)     # models.Random: no gradient, no optimizer step
             T, quota = tr.batch_plan()
             batch = tr.rollout(T, epoch, quota=quota)            # statistics stay on the device up to reduce_device
-            tr.optimizer.zero_grad(set_to_none=False)
+            if learns:
+                tr.optimizer.zero_grad(set_to_none=False)
             loss_vec = tr.compute_grad_device(batch)
-            stat = self.reduce_device(loss_vec)
-            tr.optimizer.step(grad_div=stat['num_steps'])        # multi_processing.py:95-97 in one kernel
+            stat = self.reduce_device(loss_vec, with_grads=learns)
+            if learns:
+                tr.optimizer.step(grad_div=stat['num_steps'])    # multi_processing.py:95-97 in one kernel
             return stat
         batch, stat = tr.run_batch(epoch)
         tr.optimizer.zero_grad(set_to_none=False)

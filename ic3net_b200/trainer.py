@@ -50,6 +50,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
+from .models import Random
 from .optim import FlatRMSprop
 from .utils import merge_stat
 
@@ -96,9 +97,14 @@ def policy_forward_torch(net, x, h, c, g, n_alive):
 
 class Trainer(object):
     def __init__(self, args, policy_net, env):
-        if not hasattr(policy_net, 'packed'):
+        # models.Random (models.py:37-56): one ic3_random_policy_step per lock-step, no gradient (_enqueue_random)
+        self.random_policy = isinstance(policy_net, Random)
+        if self.random_policy and args.recurrent:
+            raise ValueError("models.Random is not recurrent: --random takes no --recurrent (the reference's "
+                             "Random.forward would receive [state, prev_hid] and fail on it)")
+        if not self.random_policy and not hasattr(policy_net, 'packed'):
             raise NotImplementedError("Trainer drives policies that run on the CUDA kernels (CommNetMLP, models.MLP, "
-                                      "models.RNN); models.Random has no kernel path")
+                                      "models.RNN, models.Random)")
         self.args = args
         self.policy_net = policy_net
         self.env = env                       # GymWrapper
@@ -124,6 +130,12 @@ class Trainer(object):
         self._graph = None
         self._graph_key = None
         self._side = None                    # stream of the dense observation writer (_overlap_obs)
+        if self.random_policy:
+            # nothing to record for a gradient: compute_grad reaches no parameter (trainer.py:223), so .grad stays None
+            self.record_for_grad = False
+            for p in self.params:
+                p.grad = None
+            return
         # encoder layout of this environment (class terms / counts summed separately, comm.py set_obs_layout); the
         # fused index encoder's per-position table of the class terms belongs to the policy (encoder_table)
         policy_net.set_obs_layout(*getattr(env.env, 'obs_layout', (0, 0, 0)))
@@ -177,8 +189,7 @@ class Trainer(object):
         nh = len(self.args.naction_heads)
         A = sum(self.args.naction_heads)
         z = lambda *s, dtype=torch.float32: torch.zeros(*s, dtype=dtype, device=dev)
-        b = dict(T=T, h=z(B * N, H), c=z(B * N, H), x=z(B * N, H),
-                 comm=z(B, N, dtype=torch.uint8), alive=torch.ones(B, N, dtype=torch.uint8, device=dev),
+        b = dict(T=T, comm=z(B, N, dtype=torch.uint8), alive=torch.ones(B, N, dtype=torch.uint8, device=dev),
                  fresh=torch.ones(B, dtype=torch.uint8, device=dev), t_ep=z(B, dtype=torch.int32),
                  action=z(T, B, N, nh, dtype=torch.int32), logp=z(T, B, N, A), value=z(T, B * N),
                  reward=z(T, B, N), emask=z(T, B, dtype=torch.uint8), mini=z(T, B, N, dtype=torch.uint8),
@@ -187,6 +198,10 @@ class Trainer(object):
                  stat_episodes=z(B, dtype=torch.int32), stat_steps=z(B, dtype=torch.int32),
                  err=z(1, dtype=torch.int32), halted=z(B, dtype=torch.uint8), valid=z(T, B, dtype=torch.uint8),
                  statvec=z(4 + 2 * N, dtype=torch.float64))
+        if self.random_policy:                # no encoder, observation or recurrent state
+            self._buf = b
+            return b
+        b.update(h=z(B * N, H), c=z(B * N, H), x=z(B * N, H))
         if self.obs_mode == 'dense':
             b['obs'] = torch.empty(B, N, self.env.observation_dim, dtype=torch.float32, device=dev)
         if self.record_for_grad:
@@ -328,10 +343,11 @@ class Trainer(object):
         """Enqueue T lock-step iterations on the current stream (no host sync).  quota > 0: reference batch
         boundary -- a slot halts at the first episode end with >= quota steps (ic3_rollout_io.batch_size);
         quota = 0: episodes still open at iteration T-1 are cut there."""
+        if self.random_policy:
+            return self._enqueue_random(T, quota)
         b, e, net, args = self._buf, self.env.env, self.policy_net, self.args
         lib = _lib.load()
-        B, N = e.nenvs, args.nagents
-        nh = len(args.naction_heads)
+        B = e.nenvs
         cfg = net.policy_cfg(B)
         cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
         w = net.packed()
@@ -417,23 +433,52 @@ class Trainer(object):
                 torch.linalg.vector_norm(b['c'], math.inf, out=b['c_abs'][t])
             if overlap:
                 main.wait_stream(side)
-            r = _lib.RolloutIO(t=t, max_steps=args.max_steps, nheads=nh, hard_attn=hard,
-                               comm_action_one=int(bool(args.comm_action_one)),
-                               last=int(t == T - 1 and quota <= 0), batch_size=int(quota),
-                               halted=b['halted'].data_ptr(), rec_valid=b['valid'].data_ptr(), **snap,
-                               action=b['action'][t].data_ptr(), t_ep=b['t_ep'].data_ptr(),
-                               fresh=b['fresh'].data_ptr(), comm_next=b['comm'].data_ptr(),
-                               alive_next=b['alive'].data_ptr(), rec_reward=b['reward'].data_ptr(),
-                               rec_episode_mask=b['emask'].data_ptr(), rec_mini_mask=b['mini'].data_ptr(),
-                               rec_alive=b['ralive'].data_ptr(), stat_reward=b['stat_reward'].data_ptr(),
-                               stat_comm=b['stat_comm'].data_ptr(), stat_success=b['stat_success'].data_ptr(),
-                               stat_episodes=b['stat_episodes'].data_ptr(), stat_steps=b['stat_steps'].data_ptr())
-            if self.is_tj:
-                _lib.check(lib.ic3_tj_step(C.byref(e.cfg), C.byref(e.state), b['action'][t].data_ptr(), nh, None,
-                                           b['step_reward'].data_ptr(), None, b['err'].data_ptr(), C.byref(r), s))
-            else:
-                _lib.check(lib.ic3_pp_step(C.byref(e.cfg), C.byref(e.state), b['action'][t].data_ptr(), nh,
-                                           b['step_reward'].data_ptr(), None, b['err'].data_ptr(), C.byref(r), s))
+            self._env_step(t, T, quota, snap, s)
+
+    def _env_step(self, t, T, quota, snap, s):
+        """Env step of lock-step iteration t on the actions the policy step wrote to the records, with the
+        Trainer.get_episode bookkeeping and auto-reset (ic3_rollout_io; ``snap``: its snap_* fields)."""
+        b, e, args = self._buf, self.env.env, self.args
+        lib = _lib.load()
+        nh = len(args.naction_heads)
+        hard = int(bool(args.hard_attn) and bool(args.commnet))
+        r = _lib.RolloutIO(t=t, max_steps=args.max_steps, nheads=nh, hard_attn=hard,
+                           comm_action_one=int(bool(args.comm_action_one)),
+                           last=int(t == T - 1 and quota <= 0), batch_size=int(quota),
+                           halted=b['halted'].data_ptr(), rec_valid=b['valid'].data_ptr(), **snap,
+                           action=b['action'][t].data_ptr(), t_ep=b['t_ep'].data_ptr(),
+                           fresh=b['fresh'].data_ptr(), comm_next=b['comm'].data_ptr(),
+                           alive_next=b['alive'].data_ptr(), rec_reward=b['reward'].data_ptr(),
+                           rec_episode_mask=b['emask'].data_ptr(), rec_mini_mask=b['mini'].data_ptr(),
+                           rec_alive=b['ralive'].data_ptr(), stat_reward=b['stat_reward'].data_ptr(),
+                           stat_comm=b['stat_comm'].data_ptr(), stat_success=b['stat_success'].data_ptr(),
+                           stat_episodes=b['stat_episodes'].data_ptr(), stat_steps=b['stat_steps'].data_ptr())
+        if self.is_tj:
+            _lib.check(lib.ic3_tj_step(C.byref(e.cfg), C.byref(e.state), b['action'][t].data_ptr(), nh, None,
+                                       b['step_reward'].data_ptr(), None, b['err'].data_ptr(), C.byref(r), s))
+        else:
+            _lib.check(lib.ic3_pp_step(C.byref(e.cfg), C.byref(e.state), b['action'][t].data_ptr(), nh,
+                                       b['step_reward'].data_ptr(), None, b['err'].data_ptr(), C.byref(r), s))
+
+    def random_cfg(self):
+        """ic3_policy_cfg of the Random policy step: the fields ic3_random_policy_step reads (B, N, heads, Philox key
+        and env ids of this GPU's slots)."""
+        e, heads = self.env.env, list(self.args.naction_heads)
+        return _lib.PolicyCfg(B=e.nenvs, N=self.args.nagents, nheads=len(heads),
+                              head_dim=(C.c_int32 * _lib.MAX_HEADS)(*heads), env_id0=e.cfg.env_id0, seed=e.cfg.seed)
+
+    def _enqueue_random(self, T, quota):
+        """_enqueue for models.Random: per lock-step iteration one ic3_random_policy_step (value, log-probs and actions
+        into the records, from the env's action tick) and the env step."""
+        b, e = self._buf, self.env.env
+        lib = _lib.load()
+        cfg = self.random_cfg()
+        s = _lib.stream()
+        for t in range(T):
+            io = _lib.PolicyIO(tick=e.tick.data_ptr(), value=b['value'][t].data_ptr(), logp=b['logp'][t].data_ptr(),
+                               action=b['action'][t].data_ptr())
+            _lib.check(lib.ic3_random_policy_step(C.byref(cfg), C.byref(io), None, s))
+            self._env_step(t, T, quota, {}, s)
 
     def _episode_boundary(self, epoch):
         e, b = self.env.env, self._buf
@@ -454,9 +499,10 @@ class Trainer(object):
         b = self._buf
         self._episode_boundary(epoch)             # trainer.py:28-32, 45-51
         b['err'].zero_()
-        w = self.policy_net.packed()              # (re)pack weights outside any graph capture
-        if self._fused_x():
-            self._encoder_table()                 # ... and the encoder table with them
+        if not self.random_policy:
+            self.policy_net.packed()              # (re)pack weights outside any graph capture
+            if self._fused_x():
+                self._encoder_table()             # ... and the encoder table with them
         if self.use_graph:
             # kernel arguments passed BY VALUE are frozen into a captured graph: everything of that kind that can
             # change between rollouts is part of the key (the TJ curriculum moves cfg.spawn_thr, traffic_junction_env.py:
@@ -468,7 +514,7 @@ class Trainer(object):
                 snap = e.snapshot()
                 keys = ('fresh', 'comm', 'alive', 't_ep', 'h', 'c', 'halted', 'stat_reward', 'stat_comm', 'stat_success',
                         'stat_episodes', 'stat_steps')
-                saved = {k: b[k].clone() for k in keys}
+                saved = {k: b[k].clone() for k in keys if k in b}
                 self._enqueue(T, quota)
                 torch.cuda.synchronize()
                 e.restore(snap)                   # env state, RNG ticks ...
@@ -667,7 +713,7 @@ class Trainer(object):
     def compute_grad_device(self, batch):
         """compute_grad without a host synchronisation: the three loss sums come back as a float64 DEVICE vector
         (LOSS_KEYS order) so the data-parallel trainer can reduce them together with the batch statistics."""
-        if not self.record_for_grad:
+        if not self.record_for_grad and not self.random_policy:
             raise RuntimeError("set args.record_for_grad = True before the rollout to use compute_grad")
         b, args = self._buf, self.args
         e = self.env.env
@@ -683,6 +729,8 @@ class Trainer(object):
             mean = (adv * v).sum((0, 2), keepdim=True) / cnt
             var = (((adv - mean) * v) ** 2).sum((0, 2), keepdim=True) / (cnt - 1)      # torch.std: unbiased
             adv = (adv - mean) / var.sqrt()
+        if self.random_policy:
+            return self._random_losses(adv, ret)
         if self.grad_kernels:
             return self._compute_grad_kernels(adv, ret)
         W = self.grad_window
@@ -705,6 +753,22 @@ class Trainer(object):
             dc = c0.grad.detach() if c0.grad is not None else torch.zeros_like(c0)
             tot += torch.stack([st[key] for key in self.LOSS_KEYS]).double()
         return tot
+
+    def _random_losses(self, adv, ret):
+        """compute_grad of models.Random (trainer.py:186-220): the three loss sums straight from the records, in float64;
+        no forward to re-run and no parameter to reach (Random's outputs are leaves of the graph)."""
+        b, args = self._buf, self.args
+        T, B, N = b['T'], self.env.env.nenvs, args.nagents
+        heads = list(args.naction_heads)
+        off = torch.tensor([sum(heads[:k]) for k in range(len(heads))], device=adv.device)
+        logp = b['logp'].double()                                                    # [T, B, N, sum(na)]
+        lp = logp.gather(-1, b['action'].long() + off).sum(-1)                       # utils.py:42-46
+        alive = b['ralive'].double()
+        ret = ret.double()
+        a_loss = (-adv.double() * lp * alive).sum()                                  # trainer.py:198-201
+        v_loss = ((b['value'].view(T, B, N).double() - ret) ** 2 * alive).sum()      # :205-208
+        ent = -(logp * logp.exp() * b['valid'].double().view(T, B, 1, 1)).sum()      # :213-217, real steps only
+        return torch.stack([a_loss, v_loss, ent])
 
     def _compute_grad_kernels(self, adv, ret):
         """Hand-written BPTT (csrc/bptt_tc.cu): one ic3_bptt_step per lock-step iteration, last to first (one host read
@@ -932,6 +996,11 @@ class Trainer(object):
     # only used when there is a single process (trainer.py:245-256)
     def train_batch(self, epoch):
         batch, stat = self.run_batch(epoch)
+        if self.random_policy:
+            # no gradient: the reference's step skips a parameter whose .grad is None (trainer.py:251-254), so the
+            # parameter and the optimizer state (state == {}) stay as they are
+            merge_stat(self.compute_grad(batch), stat)
+            return stat
         self.optimizer.zero_grad(set_to_none=False)
         s = self.compute_grad(batch)
         merge_stat(s, stat)

@@ -373,6 +373,23 @@ int ic3_sample_actions(const ic3_policy_cfg* cfg, const float* logp, const uint3
                        const uint32_t* draws, int32_t* action, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Random baseline  (models.py:45-56 Random.forward, action_utils.py:32-36 select_action)
+ * ---------------------------------------------------------------------- */
+/* The reference's Random policy ignores its observation apart from its shape: value = torch.rand(..., 1), one
+ * torch.randn logit vector per action head, log_softmax of each.  One thread per agent row of cfg->B x cfg->N (N counts
+ * the prey under --enemy_comm) draws them from Philox stream 4 and samples like ic3_policy_step:
+ *   u[0 .. 15]  24-bit words of counters (env_id0 + env, tick[env], 4, 4 * agent + 0 .. 3), or the low 24 bits of
+ *               random_draws[B, N, IC3_RANDOM_WORDS] when random_draws != NULL
+ *   value       u[0] * 2^-24                                                   (exact in fp32)
+ *   logit j     sqrt(-2 ln((u[1 + 2j] + 1) * 2^-24)) * cos(2 pi u[2 + 2j] * 2^-24)   (Box-Muller; heads concatenated)
+ *   logp        log_softmax per head;  action: inverse CDF on the action stream (3) or io->draws [B, N, nheads]
+ * Reads cfg->B, N, nheads, head_dim, env_id0, seed and io->tick, draws, value, logp, action (NULL: no sampling); every
+ * other field is ignored (Random needs no encoder, state or masks).  1 + sum(head_dim) <= 8. */
+#define IC3_RANDOM_WORDS 16
+int ic3_random_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_io* io, const uint32_t* random_draws,
+                           void* stream);
+
+/* ------------------------------------------------------------------------
  * REINFORCE returns  (trainer.py:160-173), the first step of Trainer.compute_grad
  * ---------------------------------------------------------------------- */
 /* reward, mini_mask: [T,B,N]; episode_mask: [T,B]; returns out: [T,B,N] float32 (float64 accumulation). */
