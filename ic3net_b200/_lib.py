@@ -114,6 +114,19 @@ class BpttStepIO(C.Structure):
                 ("valid", _p), ("dh", _p), ("dc", _p), ("err", _p)]
 
 
+class FfGradPlan(C.Structure):
+    _fields_ = [("cfg", C.POINTER(PolicyCfg)), ("w", C.POINTER(PolicyPacked)), ("pp_env", C.POINTER(PPCfg)),
+                ("tj_env", C.POINTER(TJCfg)), ("value_coeff", C.c_float), ("entr", C.c_float), ("max_rows", C.c_int32),
+                ("reserved0", C.c_int32), ("workspace", _p)]
+
+
+class FfGradIO(C.Structure):
+    _fields_ = [("nsteps", C.c_int32), ("reserved0", C.c_int32), ("fresh", _p), ("comm", _p), ("alive", _p),
+                ("pp_loc", _p), ("tj_loc", _p), ("tj_alive", _p), ("tj_last_act", _p), ("tj_route_id", _p),
+                ("logp", _p), ("action", _p), ("value", _p), ("ret", _p), ("adv", _p), ("alive_post", _p),
+                ("valid", _p)]
+
+
 # every symbol include/ic3net_b200.h declares: name -> (restype, argtypes)
 _PTR = C.c_void_p
 SYMBOLS = {
@@ -148,6 +161,8 @@ SYMBOLS = {
                                           C.POINTER(C.c_float)]),
     "ic3_policy_pass_states": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), C.POINTER(PolicyIO), C.c_int32,
                                          _PTR, _PTR, _PTR]),
+    "ic3_policy_ff_states": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyPacked), C.POINTER(PolicyIO), _PTR, _PTR,
+                                       _PTR]),
     "ic3_sample_actions": (C.c_int, [C.POINTER(PolicyCfg), _PTR, _PTR, _PTR, _PTR, _PTR]),
     "ic3_random_policy_step": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyIO), _PTR, _PTR]),
     "ic3_returns_scan": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, _PTR, _PTR, _PTR, _PTR,
@@ -157,6 +172,11 @@ SYMBOLS = {
     "ic3_bptt_step": (C.c_int, [C.POINTER(BpttPlan), C.POINTER(BpttStepIO), _PTR]),
     "ic3_bptt_prepare": (C.c_int, [C.POINTER(BpttPlan), C.POINTER(BpttStepIO), _PTR]),
     "ic3_bptt_finish": (C.c_int, [C.POINTER(BpttPlan), C.POINTER(PolicyParams), C.POINTER(PolicyParams), _PTR, _PTR]),
+    "ic3_ff_grad_workspace_bytes": (C.c_uint64, [C.POINTER(FfGradPlan)]),
+    "ic3_ff_grad_begin": (C.c_int, [C.POINTER(FfGradPlan), _PTR]),
+    "ic3_ff_grad_chunk": (C.c_int, [C.POINTER(FfGradPlan), C.POINTER(FfGradIO), _PTR]),
+    "ic3_ff_grad_finish": (C.c_int, [C.POINTER(FfGradPlan), C.POINTER(PolicyParams), C.POINTER(PolicyParams), _PTR,
+                                     _PTR]),
     "ic3_stat_reduce": (C.c_int, [C.c_int32, C.c_int32, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR]),
     "ic3_rmsprop_step": (C.c_int, [C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, _PTR, _PTR, _PTR, _PTR]),
 }

@@ -1707,3 +1707,652 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
   IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
+
+// ==================================================================================================================
+// Non-recurrent tanh policies (models.MLP, CommNet / IC3Net without --recurrent): ic3_ff_grad_*.  No state crosses a
+// step, so a chunk of K consecutive lock-steps is one batch of K*B env slots.  Per chunk:
+//   desc      observation pattern of every row (position, counts / scalars, constant)           [ff_desc_kernel]
+//   forward   index encoder + the SIMT step's pass-state form (ic3_policy_ff_states): tanh(x), h_1 .. h_P, S_0 .. S_{P-1}
+//   heads     d loss / d (value, logits), head weight gradients, loss sums                       [bptt_heads_kernel]
+//   pass p    dz = g (1 - h_{p+1}^2), dx += dz, g = dz F_p + comm^T(dz C_p)  (tile of whole envs) [ff_pass_kernel]
+//             G_F += dz^T h_p, G_C += dz^T S_p, g_b += sum dz  (fixed row blocks)               [ff_wgrad_kernel]
+//   encoder   dpre = (dx + g) (1 - tanh(x)^2);  Y += dpre^T P                                    [ff_dpre_kernel, ff_wgrad_kernel<true>]
+// ic3_ff_grad_finish sums the row-block partials in float64 and folds Y through the observation layout like the BPTT
+// finish (bptt_finish_misc_kernel).  All fp32 SIMT arithmetic; every sum has a fixed order.
+// ==================================================================================================================
+namespace {
+
+constexpr int FF_ROWS = 64;        // agent rows per CTA of ff_pass_kernel (whole envs, as in policy_step_kernel)
+constexpr int FF_NB = 256;         // row blocks of the weight-gradient sums (fixed: the partition does not depend on the card)
+constexpr int FF_WK = 16;          // rows staged per iteration of ff_wgrad_kernel
+
+struct FfGeom {
+  int npos, WW, is_tj, np, npad, ne;   // positions, window cells, env kind, pattern columns, padded to 128, columns >= npos
+  int P, comm, R;                      // passes, communication on, max rows
+  size_t x, hs, ss, g, dx, dz, dout, pos, ext, rloc, rroute, ralive, rlast, apost, fw, cw, fpart, cpart, bpart, ypart,
+      gw_part, gs_part, sc, Y, total;
+  int nhb;
+};
+
+int ff_geometry(const ic3_ff_grad_plan* p, FfGeom* G) {
+  if (!p || !p->cfg) return IC3_E_NULL;
+  const ic3_policy_cfg* cfg = p->cfg;
+  if (cfg->H != TC_H || cfg->cell != IC3_CELL_TANH || !cfg->x_tanh || !cfg->h_from_x) return IC3_E_UNSUPPORTED;
+  if (cfg->passes < 0 || cfg->passes > IC3_MAX_PASSES) return IC3_E_UNSUPPORTED;
+  if (cfg->N < 1 || cfg->N > IC3_MAX_AGENTS || cfg->B < 1 || cfg->nheads < 1 || cfg->nheads > IC3_MAX_HEADS)
+    return IC3_E_RANGE;
+  int nout = 1;
+  for (int k = 0; k < cfg->nheads; ++k) nout += cfg->head_dim[k];
+  if (nout > BP_HEADS) return IC3_E_UNSUPPORTED;
+  if (!!p->pp_env == !!p->tj_env) return IC3_E_NULL;
+  int W;
+  if (p->pp_env) {
+    W = 2 * p->pp_env->vision + 1;
+    G->npos = p->pp_env->dim * p->pp_env->dim;
+    G->is_tj = 0;
+    // the index encoder's limits (ic3_pp_encoder_index)
+    if (cfg->O != W * W * (G->npos + 4) || ic3_pp_agents(*p->pp_env) != cfg->N || p->pp_env->N >= IC3_MAX_AGENTS ||
+        ic3_pp_layout_check(p->pp_env, cfg))
+      return IC3_E_RANGE;
+  } else {
+    W = 2 * p->tj_env->vision + 1;
+    G->npos = p->tj_env->h * p->tj_env->w;
+    G->is_tj = 1;
+    if (cfg->O != 2 + W * W * p->tj_env->vocab || p->tj_env->N != cfg->N || ic3_tj_layout_check(p->tj_env, cfg))
+      return IC3_E_RANGE;
+    if (!p->tj_env->grid) return IC3_E_NULL;
+  }
+  G->WW = W * W;
+  if (G->WW > PREP_MAX_WW) return IC3_E_UNSUPPORTED;
+  G->ne = G->is_tj ? G->WW + 4 : 2 * G->WW + 1;
+  G->np = G->npos + G->ne;
+  if ((G->np + 15) / 16 * 16 > WG_MAX_NP) return IC3_E_UNSUPPORTED;
+  G->npad = (G->np + 127) / 128 * 128;
+  G->P = cfg->passes > 1 ? cfg->passes : 1;
+  G->comm = !cfg->comm_mask_zero;
+  if ((long)p->max_rows < (long)cfg->B * cfg->N) return IC3_E_RANGE;
+  G->R = p->max_rows;
+  const size_t R = (size_t)G->R, RH = R * TC_H * 4, HH = (size_t)TC_H * TC_H * 4;
+  G->nhb = (int)((R + HB_ROWS - 1) / HB_ROWS);
+  size_t off = 0;
+  auto take = [&](size_t bytes) { size_t o = off; off += (bytes + 1023) / 1024 * 1024; return o; };
+  G->x = take(RH);
+  G->hs = take((size_t)(G->P + 1) * RH);
+  G->ss = take(G->comm ? (size_t)G->P * RH : 0);
+  G->g = take(RH);
+  G->dx = take(RH);
+  G->dz = take(RH);
+  G->dout = take(R * BP_HEADS * 4);
+  G->pos = take(R * 4);
+  G->ext = take(R * G->ne * 4);
+  // the chunk's env records with the slots of valid = 0 replaced by an empty state (their recorded state is stale)
+  G->rloc = take(R * 16);                    // predator-prey [K*B, N_pred + 1, 2] or traffic junction [K*B*N, 2]
+  G->rroute = take(R * 4);
+  G->ralive = take(R);
+  G->rlast = take(R);
+  G->apost = take(R);                        // alive_post AND valid: what the heads backward reads
+  G->fw = take((size_t)G->P * HH);
+  G->cw = take(G->comm ? (size_t)G->P * HH : 0);
+  // accumulators, zeroed by ic3_ff_grad_begin (fpart .. end)
+  G->fpart = take((size_t)G->P * FF_NB * HH);
+  G->cpart = take(G->comm ? (size_t)G->P * FF_NB * HH : 0);
+  G->bpart = take((size_t)G->P * FF_NB * TC_H * 4);
+  G->ypart = take((size_t)FF_NB * TC_H * G->npad * 4);
+  G->gw_part = take((size_t)G->nhb * BP_HEADS * TC_H * 4);
+  G->gs_part = take((size_t)G->nhb * (BP_HEADS + 3) * 8);
+  G->sc = take(sizeof(BpttScalars));
+  G->Y = take((size_t)TC_H * G->npad * 8);
+  G->total = off;
+  return IC3_OK;
+}
+
+// out[p][n][k] = in[p][k][n]: the SIMT-packed K-major f_wT / c_wT back to the module layout [out unit n][in unit k]
+__global__ void ff_transpose_kernel(const float* __restrict__ in, float* __restrict__ out, int P) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= P * TC_H * TC_H) return;
+  const int p = idx / (TC_H * TC_H), r = idx - p * TC_H * TC_H, n = r >> 7, k = r & 127;
+  out[idx] = in[(size_t)p * TC_H * TC_H + k * TC_H + n];
+}
+
+// Observation pattern of every row (the columns of prep_kernel's P image): pos = one-hot column of the agent position
+// (-1: no class term -- a dead car, or a slot with valid = 0), ext = [prey, predator count per window cell, 1]
+// (predator-prey) or [car count per window cell, last_act, route ratio, 0, 1] (traffic junction).  Rows of slots with
+// valid = 0 get an all-zero pattern and never index the grid.
+struct DescArgs {
+  int R, N, ne, is_tj;
+  ic3_pp_cfg pp; ic3_tj_cfg tj;
+  const int32_t* pp_loc; const int32_t* tj_loc; const uint8_t* tj_alive; const uint8_t* tj_last_act;
+  const int32_t* tj_route_id; const uint8_t* valid;
+  int32_t* pos; float* ext;
+};
+
+__global__ void __launch_bounds__(256) ff_desc_kernel(DescArgs a) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= a.R) return;
+  const int e = row / a.N, i = row - e * a.N;
+  float* x = a.ext + (size_t)row * a.ne;
+  for (int c = 0; c < a.ne; ++c) x[c] = 0.f;
+  if (a.valid && !a.valid[e]) {
+    a.pos[row] = -1;
+    return;
+  }
+  if (!a.is_tj) {
+    const int D = a.pp.dim, v = a.pp.vision, W = 2 * v + 1, NP = a.pp.N;
+    const int* l = a.pp_loc + (size_t)e * (NP + 1) * 2;
+    a.pos[row] = l[2 * i] * D + l[2 * i + 1];
+    for (int w = 0; w < W * W; ++w) {
+      const int rr = l[2 * i] - v + w / W, cc = l[2 * i + 1] - v + w % W;
+      if (rr < 0 || rr >= D || cc < 0 || cc >= D) continue;
+      int npred = 0;
+      for (int j = 0; j < NP; ++j) npred += (l[2 * j] == rr && l[2 * j + 1] == cc);
+      x[2 * w] = (float)(l[2 * NP] == rr && l[2 * NP + 1] == cc);
+      x[2 * w + 1] = (float)npred;
+    }
+    x[2 * W * W] = 1.f;
+  } else {
+    const int v = a.tj.vision, W = 2 * v + 1, N = a.N;
+    x[W * W + 3] = 1.f;
+    if (!a.tj_alive[row]) {                      // dead car: all-zero observation
+      a.pos[row] = -1;
+      return;
+    }
+    const int* l = a.tj_loc + (size_t)e * N * 2;
+    a.pos[row] = l[2 * i] * a.tj.w + l[2 * i + 1];
+    for (int w = 0; w < W * W; ++w) {
+      const int rr = l[2 * i] - v + w / W, cc = l[2 * i + 1] - v + w % W;
+      if (rr < 0 || rr >= a.tj.h || cc < 0 || cc >= a.tj.w) continue;
+      int cnt = 0;
+      for (int j = 0; j < N; ++j) cnt += (l[2 * j] == rr && l[2 * j + 1] == cc);
+      x[w] = (float)cnt;
+    }
+    x[W * W] = (float)a.tj_last_act[row];
+    x[W * W + 1] = (float)a.tj_route_id[row] / (float)(a.tj.npath - 1);
+  }
+}
+
+// Per agent row of a chunk: the env records the forward re-run reads, with every slot of valid = 0 given an empty
+// state (all agents at (0, 0); traffic junction: no car alive), and alive_post masked by valid, so that such a slot
+// indexes nothing from its stale records and contributes exactly zero.
+struct RecArgs {
+  int R, N, NP, is_tj;
+  const int32_t* pp_loc; const int32_t* tj_loc; const uint8_t* tj_alive; const uint8_t* tj_last_act;
+  const int32_t* tj_route_id; const uint8_t* alive_post; const uint8_t* valid;
+  int32_t* loc; int32_t* route; uint8_t* alive; uint8_t* last; uint8_t* apost;
+};
+
+__global__ void __launch_bounds__(256) ff_records_kernel(RecArgs a) {
+  const int row = blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= a.R) return;
+  const int e = row / a.N, i = row - e * a.N;
+  const bool ok = !a.valid || a.valid[e];
+  a.apost[row] = ok && a.alive_post[row] ? 1 : 0;
+  if (!a.is_tj) {
+    if (i <= a.NP) {                           // rows 0 .. NP of env e carry its N_pred + 1 positions
+      const size_t o = ((size_t)e * (a.NP + 1) + i) * 2;
+      a.loc[o] = ok ? a.pp_loc[o] : 0;
+      a.loc[o + 1] = ok ? a.pp_loc[o + 1] : 0;
+    }
+    if (i == a.N - 1 && a.NP >= a.N) {         // N_pred + 1 > N rows: the prey's position goes with the last row
+      const size_t o = ((size_t)e * (a.NP + 1) + a.NP) * 2;
+      a.loc[o] = ok ? a.pp_loc[o] : 0;
+      a.loc[o + 1] = ok ? a.pp_loc[o + 1] : 0;
+    }
+  } else {
+    a.loc[2 * (size_t)row] = ok ? a.tj_loc[2 * (size_t)row] : 0;
+    a.loc[2 * (size_t)row + 1] = ok ? a.tj_loc[2 * (size_t)row + 1] : 0;
+    a.alive[row] = ok ? a.tj_alive[row] : 0;
+    a.last[row] = ok ? a.tj_last_act[row] : 0;
+    a.route[row] = ok ? a.tj_route_id[row] : 0;
+  }
+}
+
+// One backward pass p over a tile of whole environments: dz = g (1 - h_{p+1}^2) (g of the last pass: the heads'
+// dout . W_heads), dx (+)= dz, g <- dz F_p + comm^T(dz C_p) with the forward's gate and mean rules (policy_step_kernel).
+struct PassArgs {
+  int R, N, last, first_acc, comm, hard_attn, comm_avg, nout;
+  const float* h_out;        // [R, H] h_{p+1}
+  const float* dout;         // [R, 8]
+  const float* head_w;       // packed [1 + atot, H]
+  const float* fw;           // [H, H] F_p as f.weight [n][k]
+  const float* cw;           // [H, H] C_p as C.weight [n][k]
+  const uint8_t* fresh; const uint8_t* comm_action; const uint8_t* alive; const uint8_t* valid;
+  float* g; float* dx; float* dz;
+};
+
+__global__ void __launch_bounds__(256) ff_pass_kernel(PassArgs a) {
+  __shared__ __align__(16) float s_dz[FF_ROWS][TC_H];   // dz of the tile, then (after the GEMMs) dS = dz C_p
+  __shared__ float s_gate[FF_ROWS], s_gs[FF_ROWS];
+  const int N = a.N, epb = FF_ROWS / N;
+  const int e0 = blockIdx.x * epb;
+  const int nrows = min(epb * N, a.R - e0 * N);
+  const size_t row0 = (size_t)e0 * N;
+  const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
+  for (int idx = tid; idx < FF_ROWS * TC_H; idx += 256) {
+    const int r = idx >> 7, c = idx & 127;
+    float d = 0.f;
+    if (r < nrows && (!a.valid || a.valid[e0 + r / N])) {
+      const size_t o = (row0 + r) * TC_H + c;
+      float gin;
+      if (a.last) {
+        gin = 0.f;
+        for (int k = 0; k < a.nout; ++k) gin = fmaf(a.dout[(row0 + r) * BP_HEADS + k], __ldg(a.head_w + k * TC_H + c), gin);
+      } else {
+        gin = a.g[o];
+      }
+      const float h = a.h_out[o];
+      d = gin * (1.f - h * h);
+    }
+    s_dz[r][c] = d;
+    if (r < nrows) {
+      const size_t o = (row0 + r) * TC_H + c;
+      a.dz[o] = d;
+      a.dx[o] = a.first_acc ? d : a.dx[o] + d;
+    }
+  }
+  for (int r = tid; r < FF_ROWS; r += 256) {      // comm gate and mean factor, as policy_step_kernel stage A
+    float g = 0.f, den = 1.f;
+    if (r < nrows) {
+      const int el = r / N, e = e0 + el, i = r - el * N;
+      const bool fr = a.fresh && a.fresh[e];
+      int n_alive = N, al = 1;
+      if (a.alive && !fr) {
+        n_alive = 0;
+        for (int j = 0; j < N; ++j) n_alive += a.alive[(size_t)e * N + j] != 0;
+        al = a.alive[(size_t)e * N + i] != 0;
+      }
+      int cm = 1;
+      if (a.hard_attn) cm = fr ? 0 : (a.comm_action[(size_t)e * N + i] != 0);
+      g = (float)(al * cm);
+      if (a.comm_avg && n_alive > 1) den = (float)(n_alive - 1);
+    }
+    s_gate[r] = g;
+    s_gs[r] = g / den;
+  }
+  __syncthreads();
+  // thread: rows ty * 8 .. + 7, columns tx * 4 .. + 3
+  float af[8][4], ac[8][4];
+#pragma unroll
+  for (int r = 0; r < 8; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) af[r][c] = ac[r][c] = 0.f;
+  for (int n = 0; n < TC_H; n += 4) {
+    float4 av[8];
+#pragma unroll
+    for (int r = 0; r < 8; ++r) av[r] = *reinterpret_cast<const float4*>(&s_dz[ty * 8 + r][n]);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const float4 bf = __ldg(reinterpret_cast<const float4*>(a.fw + (size_t)(n + q) * TC_H) + tx);
+      float4 bc = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (a.comm) bc = __ldg(reinterpret_cast<const float4*>(a.cw + (size_t)(n + q) * TC_H) + tx);
+#pragma unroll
+      for (int r = 0; r < 8; ++r) {
+        const float v = q == 0 ? av[r].x : (q == 1 ? av[r].y : (q == 2 ? av[r].z : av[r].w));
+        af[r][0] = fmaf(v, bf.x, af[r][0]); af[r][1] = fmaf(v, bf.y, af[r][1]);
+        af[r][2] = fmaf(v, bf.z, af[r][2]); af[r][3] = fmaf(v, bf.w, af[r][3]);
+        ac[r][0] = fmaf(v, bc.x, ac[r][0]); ac[r][1] = fmaf(v, bc.y, ac[r][1]);
+        ac[r][2] = fmaf(v, bc.z, ac[r][2]); ac[r][3] = fmaf(v, bc.w, ac[r][3]);
+      }
+    }
+  }
+  __syncthreads();
+  float (*s_ds)[TC_H] = s_dz;
+  if (a.comm) {
+#pragma unroll
+    for (int r = 0; r < 8; ++r)
+      *reinterpret_cast<float4*>(&s_ds[ty * 8 + r][tx * 4]) = make_float4(ac[r][0], ac[r][1], ac[r][2], ac[r][3]);
+  }
+  __syncthreads();
+#pragma unroll
+  for (int r = 0; r < 8; ++r) {
+    const int row = ty * 8 + r;
+    if (row >= nrows) continue;
+    float o[4] = {af[r][0], af[r][1], af[r][2], af[r][3]};
+    if (a.comm && s_gate[row] != 0.f) {
+      // S[m] = gs[m] sum_{j != m, gate j} h[j]  ->  d h[row] += gate[row] sum_{m != row} gs[m] dS[m]
+      const int base = (row / N) * N;
+      float t[4] = {0.f, 0.f, 0.f, 0.f};
+      for (int m = base; m < base + N; ++m) {
+        if (m == row || s_gs[m] == 0.f) continue;
+        const float4 d = *reinterpret_cast<const float4*>(&s_ds[m][tx * 4]);
+        t[0] = fmaf(s_gs[m], d.x, t[0]); t[1] = fmaf(s_gs[m], d.y, t[1]);
+        t[2] = fmaf(s_gs[m], d.z, t[2]); t[3] = fmaf(s_gs[m], d.w, t[3]);
+      }
+#pragma unroll
+      for (int c = 0; c < 4; ++c) o[c] += t[c];
+    }
+    *reinterpret_cast<float4*>(a.g + (row0 + row) * TC_H + tx * 4) = make_float4(o[0], o[1], o[2], o[3]);
+  }
+}
+
+// dpre = (dx + g) (1 - xt^2) into dz (rows of slots with valid = 0 are zero already: dz, dx and g are)
+__global__ void __launch_bounds__(256) ff_dpre_kernel(size_t n4, const float4* __restrict__ xt, const float4* __restrict__ dx,
+                                                      const float4* __restrict__ g, float4* __restrict__ out) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
+    const float4 x = xt[i], d = dx[i], q = g[i];
+    out[i] = make_float4((d.x + q.x) * (1.f - x.x * x.x), (d.y + q.y) * (1.f - x.y * x.y), (d.z + q.z) * (1.f - x.z * x.z),
+                         (d.w + q.w) * (1.f - x.w * x.w));
+  }
+}
+
+// part[blk][n][ld] (+)= sum over the rows of block blk of A[r][n] * B[r][c]  (columns c of tile blockIdx.y), rows in
+// increasing order.  PAT: B is the observation pattern (pos, ext) of ff_desc_kernel; else B = b[blockIdx.y] dense [R, H].
+// bsum (dense, tile 0 only): bsum[blk][n] (+)= sum of A[r][n].
+struct WgradFfArgs {
+  int R, ld, npos, ne;
+  const float* A;
+  const float* b[2];
+  float* part[2];
+  size_t part_stride;        // floats per block
+  const int32_t* pos; const float* ext;
+  float* bsum;
+};
+
+template <bool PAT>
+__global__ void __launch_bounds__(256) ff_wgrad_kernel(WgradFfArgs a) {
+  __shared__ __align__(16) float s_a[FF_WK][TC_H];
+  __shared__ __align__(16) float s_b[FF_WK][TC_H];
+  const int tid = threadIdx.x, tn = tid >> 4, tc = tid & 15;
+  const int blk = blockIdx.x, y = blockIdx.y;
+  const long r0 = (long)a.R * blk / FF_NB, r1 = (long)a.R * (blk + 1) / FF_NB;
+  const float* B = PAT ? nullptr : a.b[y];
+  const int c0 = PAT ? y * TC_H : 0;
+  float acc[8][8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
+  float bs = 0.f;
+  for (long r = r0; r < r1; r += FF_WK) {
+    for (int idx = tid; idx < FF_WK * TC_H / 4; idx += 256) {
+      const int kk = idx >> 5, q = idx & 31;
+      const long row = r + kk;
+      float4 va = make_float4(0.f, 0.f, 0.f, 0.f), vb = va;
+      if (row < r1) {
+        va = __ldg(reinterpret_cast<const float4*>(a.A + (size_t)row * TC_H) + q);
+        if (PAT) {
+          const int p = a.pos[row];
+          float v[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const int c = c0 + 4 * q + j;
+            v[j] = c < a.npos ? (c == p ? 1.f : 0.f) : (c - a.npos < a.ne ? a.ext[(size_t)row * a.ne + c - a.npos] : 0.f);
+          }
+          vb = make_float4(v[0], v[1], v[2], v[3]);
+        } else {
+          vb = __ldg(reinterpret_cast<const float4*>(B + (size_t)row * TC_H) + q);
+        }
+      }
+      *reinterpret_cast<float4*>(&s_a[kk][4 * q]) = va;
+      *reinterpret_cast<float4*>(&s_b[kk][4 * q]) = vb;
+    }
+    __syncthreads();
+    if (!PAT && y == 0 && tid < TC_H) {
+#pragma unroll
+      for (int kk = 0; kk < FF_WK; ++kk) bs += s_a[kk][tid];
+    }
+#pragma unroll
+    for (int kk = 0; kk < FF_WK; ++kk) {
+      float av[8], bv[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) av[i] = s_a[kk][tn + 16 * i];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) bv[j] = s_b[kk][tc + 16 * j];
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+    }
+    __syncthreads();
+  }
+  float* out = (PAT ? a.part[0] + c0 : a.part[y]) + (size_t)blk * a.part_stride;
+#pragma unroll
+  for (int i = 0; i < 8; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) out[(size_t)(tn + 16 * i) * a.ld + tc + 16 * j] += acc[i][j];
+  if (!PAT && y == 0 && tid < TC_H) a.bsum[(size_t)blk * TC_H + tid] += bs;
+}
+
+// grad[i] += sum_blk part[blk][i] (float64, block order), i < n
+__global__ void ff_reduce_add_kernel(const float* __restrict__ part, size_t stride, int n, float* __restrict__ grad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double acc = 0.0;
+  for (int b = 0; b < FF_NB; ++b) acc += (double)part[(size_t)b * stride + i];
+  grad[i] += (float)acc;
+}
+
+// Y[n][c] = sum_blk ypart[blk][n][c]
+__global__ void ff_reduce_y_kernel(const float* __restrict__ part, int n, double* __restrict__ Y) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double acc = 0.0;
+  for (int b = 0; b < FF_NB; ++b) acc += (double)part[(size_t)b * n + i];
+  Y[i] = acc;
+}
+
+}  // namespace
+
+extern "C" uint64_t ic3_ff_grad_workspace_bytes(const ic3_ff_grad_plan* p) {
+  FfGeom G;
+  if (ff_geometry(p, &G)) return 0;
+  return (uint64_t)G.total;
+}
+
+extern "C" int ic3_ff_grad_begin(const ic3_ff_grad_plan* p, void* stream) {
+  FfGeom G;
+  int rc = ff_geometry(p, &G);
+  if (rc) return rc;
+  if (!p->w || !p->workspace || !p->w->f_wT || (G.comm && !p->w->c_wT)) return IC3_E_NULL;
+  cudaStream_t s = (cudaStream_t)stream;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
+  cudaError_t e = cudaMemsetAsync(ws + G.fpart, 0, G.total - G.fpart, s);
+  if (e != cudaSuccess) return (int)e;
+  const int n = G.P * TC_H * TC_H;
+  ff_transpose_kernel<<<(n + 255) / 256, 256, 0, s>>>(p->w->f_wT, reinterpret_cast<float*>(ws + G.fw), G.P);
+  IC3_LAUNCH_CHECK();
+  if (G.comm) {
+    ff_transpose_kernel<<<(n + 255) / 256, 256, 0, s>>>(p->w->c_wT, reinterpret_cast<float*>(ws + G.cw), G.P);
+    IC3_LAUNCH_CHECK();
+  }
+  return IC3_OK;
+}
+
+extern "C" int ic3_ff_grad_chunk(const ic3_ff_grad_plan* p, const ic3_ff_grad_io* io, void* stream) {
+  FfGeom G;
+  int rc = ff_geometry(p, &G);
+  if (rc) return rc;
+  if (!io || !p->w || !p->workspace || !p->w->head_w) return IC3_E_NULL;
+  const ic3_policy_cfg* cfg = p->cfg;
+  if (io->nsteps < 1 || (long)io->nsteps * cfg->B * cfg->N > (long)G.R) return IC3_E_RANGE;
+  if (!io->fresh || !io->logp || !io->action || !io->value || !io->ret || !io->adv || !io->alive_post) return IC3_E_NULL;
+  if (cfg->hard_attn && !io->comm) return IC3_E_NULL;
+  if (G.is_tj ? (!io->tj_loc || !io->tj_alive || !io->tj_last_act || !io->tj_route_id) : !io->pp_loc) return IC3_E_NULL;
+  cudaStream_t s = (cudaStream_t)stream;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
+  const int Bk = io->nsteps * cfg->B, N = cfg->N, R = Bk * N;
+  const size_t RHs = (size_t)R * TC_H;             // floats of one [R, H] block of this chunk
+  float* x = reinterpret_cast<float*>(ws + G.x);
+  float* hs = reinterpret_cast<float*>(ws + G.hs);
+  float* ss = G.comm ? reinterpret_cast<float*>(ws + G.ss) : nullptr;
+  float* g = reinterpret_cast<float*>(ws + G.g);
+  float* dx = reinterpret_cast<float*>(ws + G.dx);
+  float* dz = reinterpret_cast<float*>(ws + G.dz);
+  float* dout = reinterpret_cast<float*>(ws + G.dout);
+  int32_t* pos = reinterpret_cast<int32_t*>(ws + G.pos);
+  float* ext = reinterpret_cast<float*>(ws + G.ext);
+  RecArgs ra;
+  memset(&ra, 0, sizeof(ra));
+  ra.R = R; ra.N = N; ra.NP = G.is_tj ? N : p->pp_env->N; ra.is_tj = G.is_tj;
+  ra.pp_loc = io->pp_loc; ra.tj_loc = io->tj_loc; ra.tj_alive = io->tj_alive; ra.tj_last_act = io->tj_last_act;
+  ra.tj_route_id = io->tj_route_id; ra.alive_post = io->alive_post; ra.valid = io->valid;
+  ra.loc = reinterpret_cast<int32_t*>(ws + G.rloc); ra.route = reinterpret_cast<int32_t*>(ws + G.rroute);
+  ra.alive = ws + G.ralive; ra.last = ws + G.rlast; ra.apost = ws + G.apost;
+  ff_records_kernel<<<(R + 255) / 256, 256, 0, s>>>(ra);
+  IC3_LAUNCH_CHECK();
+  const int32_t* pp_loc = G.is_tj ? nullptr : ra.loc;
+  const int32_t* tj_loc = G.is_tj ? ra.loc : nullptr;
+  // observation pattern
+  DescArgs d;
+  memset(&d, 0, sizeof(d));
+  d.R = R; d.N = N; d.ne = G.ne; d.is_tj = G.is_tj;
+  if (G.is_tj) d.tj = *p->tj_env;
+  else d.pp = *p->pp_env;
+  d.pp_loc = pp_loc; d.tj_loc = tj_loc; d.tj_alive = ra.alive; d.tj_last_act = ra.last;
+  d.tj_route_id = ra.route; d.valid = io->valid; d.pos = pos; d.ext = ext;
+  ff_desc_kernel<<<(R + 255) / 256, 256, 0, s>>>(d);
+  IC3_LAUNCH_CHECK();
+  // forward: x from the recorded env state (the K steps as K*B env slots), then every pass state
+  ic3_policy_cfg ccfg = *cfg;
+  ccfg.B = Bk;
+  if (G.is_tj) {
+    ic3_tj_cfg env = *p->tj_env;
+    env.B = Bk;
+    ic3_tj_state st;
+    memset(&st, 0, sizeof(st));
+    st.loc = const_cast<int32_t*>(tj_loc); st.alive = ra.alive; st.last_act = ra.last; st.route_id = ra.route;
+    rc = ic3_tj_encoder_index(&env, &st, &ccfg, p->w, x, stream);
+  } else {
+    ic3_pp_cfg env = *p->pp_env;
+    env.B = Bk;
+    ic3_pp_state st;
+    memset(&st, 0, sizeof(st));
+    st.loc = const_cast<int32_t*>(pp_loc);
+    rc = ic3_pp_encoder_index(&env, &st, &ccfg, p->w, x, stream);
+  }
+  if (rc) return rc;
+  // pass blocks of this chunk: [p][R][H] with the chunk's own R (packed at the front of the capacity)
+  ic3_policy_io pio;
+  memset(&pio, 0, sizeof(pio));
+  pio.x = x; pio.comm_action = cfg->hard_attn ? io->comm : nullptr; pio.alive = io->alive; pio.fresh = io->fresh;
+  rc = ic3_policy_ff_states(&ccfg, p->w, &pio, hs, ss, stream);
+  if (rc) return rc;
+  // heads of the last pass
+  int atot = 0;
+  for (int k = 0; k < cfg->nheads; ++k) atot += cfg->head_dim[k];
+  HeadsArgs h;
+  memset(&h, 0, sizeof(h));
+  h.R = R; h.N = N; h.nheads = cfg->nheads; h.atot = atot;
+  for (int k = 0; k < IC3_MAX_HEADS; ++k) h.head_dim[k] = cfg->head_dim[k];
+  h.value_coeff = p->value_coeff; h.entr = p->entr;
+  h.logp = io->logp; h.action = io->action; h.value = io->value; h.ret = io->ret; h.adv = io->adv;
+  h.alive_post = ra.apost; h.valid = io->valid;
+  h.h_new = hs + (size_t)G.P * RHs;
+  h.head_w = p->w->head_w;
+  h.dout = dout;
+  h.gw_part = reinterpret_cast<float*>(ws + G.gw_part);
+  h.gs_part = reinterpret_cast<double*>(ws + G.gs_part);
+  h.sc = reinterpret_cast<BpttScalars*>(ws + G.sc);
+  h.q = 0;
+  bptt_heads_kernel<<<(R + HB_ROWS - 1) / HB_ROWS, 256, 0, s>>>(h);
+  IC3_LAUNCH_CHECK();
+  // passes P-1 .. 0
+  const int epb = FF_ROWS / N;
+  for (int ps = G.P - 1; ps >= 0; --ps) {
+    PassArgs a;
+    memset(&a, 0, sizeof(a));
+    a.R = R; a.N = N; a.last = ps == G.P - 1; a.first_acc = ps == G.P - 1; a.comm = G.comm;
+    a.hard_attn = cfg->hard_attn; a.comm_avg = cfg->comm_avg; a.nout = 1 + atot;
+    a.h_out = hs + (size_t)(ps + 1) * RHs;
+    a.dout = dout; a.head_w = p->w->head_w;
+    a.fw = reinterpret_cast<const float*>(ws + G.fw) + (size_t)ps * TC_H * TC_H;
+    a.cw = G.comm ? reinterpret_cast<const float*>(ws + G.cw) + (size_t)ps * TC_H * TC_H : nullptr;
+    a.fresh = io->fresh; a.comm_action = cfg->hard_attn ? io->comm : nullptr; a.alive = io->alive; a.valid = io->valid;
+    a.g = g; a.dx = dx; a.dz = dz;
+    ff_pass_kernel<<<(Bk + epb - 1) / epb, 256, 0, s>>>(a);
+    IC3_LAUNCH_CHECK();
+    WgradFfArgs w;
+    memset(&w, 0, sizeof(w));
+    w.R = R; w.ld = TC_H; w.A = dz;
+    w.b[0] = hs + (size_t)ps * RHs;
+    w.b[1] = G.comm ? ss + (size_t)ps * RHs : nullptr;
+    w.part[0] = reinterpret_cast<float*>(ws + G.fpart) + (size_t)ps * FF_NB * TC_H * TC_H;
+    w.part[1] = G.comm ? reinterpret_cast<float*>(ws + G.cpart) + (size_t)ps * FF_NB * TC_H * TC_H : nullptr;
+    w.part_stride = (size_t)TC_H * TC_H;
+    w.bsum = reinterpret_cast<float*>(ws + G.bpart) + (size_t)ps * FF_NB * TC_H;
+    ff_wgrad_kernel<false><<<dim3(FF_NB, G.comm ? 2 : 1), 256, 0, s>>>(w);
+    IC3_LAUNCH_CHECK();
+  }
+  // encoder: dpre, then dpre^T P
+  ff_dpre_kernel<<<1024, 256, 0, s>>>(RHs / 4, reinterpret_cast<const float4*>(hs), reinterpret_cast<const float4*>(dx),
+                                      reinterpret_cast<const float4*>(g), reinterpret_cast<float4*>(dz));
+  IC3_LAUNCH_CHECK();
+  WgradFfArgs w;
+  memset(&w, 0, sizeof(w));
+  w.R = R; w.ld = G.npad; w.npos = G.npos; w.ne = G.ne; w.A = dz;
+  w.part[0] = reinterpret_cast<float*>(ws + G.ypart);
+  w.part_stride = (size_t)TC_H * G.npad;
+  w.pos = pos; w.ext = ext;
+  ff_wgrad_kernel<true><<<dim3(FF_NB, G.npad / TC_H), 256, 0, s>>>(w);
+  IC3_LAUNCH_CHECK();
+  return IC3_OK;
+}
+
+extern "C" int ic3_ff_grad_finish(const ic3_ff_grad_plan* p, const ic3_policy_params* params, const ic3_policy_params* grads,
+                                  double* losses, void* stream) {
+  FfGeom G;
+  int rc = ff_geometry(p, &G);
+  if (rc) return rc;
+  if (!params || !grads || !losses || !p->workspace) return IC3_E_NULL;
+  if (!grads->encoder_w || !grads->encoder_b || !grads->value_w || !grads->value_b) return IC3_E_NULL;
+  const ic3_policy_cfg* cfg = p->cfg;
+  for (int k = 0; k < cfg->nheads; ++k)
+    if (!grads->head_w[k] || !grads->head_b[k]) return IC3_E_NULL;
+  for (int ps = 0; ps < G.P; ++ps) {
+    const float* g_c_w = ps > 0 && grads->c_w_pass[ps] ? grads->c_w_pass[ps] : grads->c_w;
+    const float* g_c_b = ps > 0 && grads->c_b_pass[ps] ? grads->c_b_pass[ps] : grads->c_b;
+    if (!grads->f_w_pass[ps] || !grads->f_b_pass[ps] || !g_c_b || (G.comm && !g_c_w)) return IC3_E_NULL;
+  }
+  cudaStream_t s = (cudaStream_t)stream;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
+  const size_t HH = (size_t)TC_H * TC_H;
+  // pass by pass, in order: with share_weights every pass adds into the one module's buffers
+  for (int ps = 0; ps < G.P; ++ps) {
+    float* g_c_w = const_cast<float*>(ps > 0 && grads->c_w_pass[ps] ? grads->c_w_pass[ps] : grads->c_w);
+    float* g_c_b = const_cast<float*>(ps > 0 && grads->c_b_pass[ps] ? grads->c_b_pass[ps] : grads->c_b);
+    const float* fp = reinterpret_cast<const float*>(ws + G.fpart) + (size_t)ps * FF_NB * HH;
+    const float* bp = reinterpret_cast<const float*>(ws + G.bpart) + (size_t)ps * FF_NB * TC_H;
+    ff_reduce_add_kernel<<<(int)(HH / 256), 256, 0, s>>>(fp, HH, (int)HH, const_cast<float*>(grads->f_w_pass[ps]));
+    IC3_LAUNCH_CHECK();
+    ff_reduce_add_kernel<<<1, TC_H, 0, s>>>(bp, TC_H, TC_H, const_cast<float*>(grads->f_b_pass[ps]));
+    IC3_LAUNCH_CHECK();
+    ff_reduce_add_kernel<<<1, TC_H, 0, s>>>(bp, TC_H, TC_H, g_c_b);      // c_b enters beside f_b: the same sum
+    IC3_LAUNCH_CHECK();
+    if (G.comm) {
+      const float* cp = reinterpret_cast<const float*>(ws + G.cpart) + (size_t)ps * FF_NB * HH;
+      ff_reduce_add_kernel<<<(int)(HH / 256), 256, 0, s>>>(cp, HH, (int)HH, g_c_w);
+      IC3_LAUNCH_CHECK();
+    }
+  }
+  // encoder through the observation layout, then the heads
+  double* Y = reinterpret_cast<double*>(ws + G.Y);
+  const int ny = TC_H * G.npad;
+  ff_reduce_y_kernel<<<(ny + 255) / 256, 256, 0, s>>>(reinterpret_cast<const float*>(ws + G.ypart), ny, Y);
+  IC3_LAUNCH_CHECK();
+  FinishArgs f;
+  memset(&f, 0, sizeof(f));
+  int atot = 0;
+  for (int k = 0; k < cfg->nheads; ++k) atot += cfg->head_dim[k];
+  f.O = cfg->O; f.nheads = cfg->nheads; f.atot = atot; f.npos = G.npos; f.np = G.npad; f.WW = G.WW;
+  for (int k = 0; k < IC3_MAX_HEADS; ++k) f.head_dim[k] = cfg->head_dim[k];
+  f.Y = Y; f.ldy = G.npad;
+  f.g_enc_w = const_cast<float*>(grads->encoder_w); f.g_enc_b = const_cast<float*>(grads->encoder_b);
+  f.g_c_b = nullptr;
+  f.g_value_w = const_cast<float*>(grads->value_w); f.g_value_b = const_cast<float*>(grads->value_b);
+  for (int k = 0; k < IC3_MAX_HEADS; ++k) {
+    f.g_head_w[k] = const_cast<float*>(grads->head_w[k]);
+    f.g_head_b[k] = const_cast<float*>(grads->head_b[k]);
+  }
+  f.gw_part = reinterpret_cast<const float*>(ws + G.gw_part);
+  f.gs_part = reinterpret_cast<const double*>(ws + G.gs_part);
+  f.nhb = G.nhb;
+  f.losses = losses;
+  f.is_tj = G.is_tj;
+  if (G.is_tj) f.tj = *p->tj_env;
+  else f.pp = *p->pp_env;
+  f.ones_col = G.np - 1;
+  bptt_finish_misc_kernel<<<(finish_enc_items(f) * 128 + 255) / 256, 256, 0, s>>>(f);
+  IC3_LAUNCH_CHECK();
+  bptt_finish_heads_kernel<<<(BP_HEADS * TC_H + 255) / 256, 256, 0, s>>>(f);
+  IC3_LAUNCH_CHECK();
+  return IC3_OK;
+}

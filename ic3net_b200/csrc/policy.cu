@@ -104,9 +104,13 @@ struct PolicyArgs {
   ic3_policy_cfg cfg;
   ic3_policy_packed w;
   ic3_policy_io io;
+  float* st_h;   // STATES: [passes + 1, B*N, H] the state entering pass 0 (x or tanh(x)), then h after every pass
+  float* st_s;   // STATES: [passes, B*N, H] the communication vector of every pass, or NULL
 };
 
-template <int H>
+// STATES: the pass-state form of the step for the non-recurrent backward (ic3_ff_grad_chunk): the same arithmetic,
+// every pass's input, communication vector and output written out, no heads.
+template <int H, bool STATES = false>
 __global__ void __launch_bounds__(NT) policy_step_kernel(PolicyArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   PolicySmem<H>& sm = *reinterpret_cast<PolicySmem<H>*>(smem_raw);
@@ -137,6 +141,7 @@ __global__ void __launch_bounds__(NT) policy_step_kernel(PolicyArgs a) {
       }
     }
     *reinterpret_cast<float4*>(&sm.hs[r][q * 4]) = v;
+    if (STATES && r < nrows) *(reinterpret_cast<float4*>(a.st_h + (row0 + r) * H) + q) = v;
   }
   for (int r = tid; r < ROWS; r += NT) {
     float g = 0.f, den = 1.f;
@@ -185,6 +190,8 @@ __global__ void __launch_bounds__(NT) policy_step_kernel(PolicyArgs a) {
         acc.x /= d; acc.y /= d; acc.z /= d; acc.w /= d;
       }
       *reinterpret_cast<float4*>(&sm.ss[r][q * 4]) = acc;
+      if (STATES && a.st_s && r < nrows)
+        *(reinterpret_cast<float4*>(a.st_s + ((size_t)ps * B * N + row0 + r) * H) + q) = acc;
     }
     __syncthreads();
 
@@ -233,7 +240,8 @@ __global__ void __launch_bounds__(NT) policy_step_kernel(PolicyArgs a) {
           float hn = 0.f;
           if (row < nrows) {
             hn = tanhf(sm.ss[row][col] + (acc[r][c] + __ldg(a.w.f_b + (size_t)ps * H + col)));
-            if (ps == npass - 1) io.h_out[(row0 + row) * H + col] = hn;
+            if (STATES) a.st_h[((size_t)(ps + 1) * B * N + row0 + row) * H + col] = hn;
+            else if (ps == npass - 1) io.h_out[(row0 + row) * H + col] = hn;
           }
           sm.h2[row][col] = hn;
         }
@@ -274,6 +282,7 @@ __global__ void __launch_bounds__(NT) policy_step_kernel(PolicyArgs a) {
     __syncthreads();
   }
 
+  if (STATES) return;
   // ---- E: heads, log-softmax, sampling (comm.py:228-239, action_utils.py:32-36) --
   const int warp = ty, lane = tx;
   for (int r = warp; r < nrows; r += NT / 32) {
@@ -601,17 +610,17 @@ int packed_check(const ic3_policy_packed* w) {
   return IC3_OK;
 }
 
-template <int H>
+template <int H, bool STATES = false>
 int launch_policy(const PolicyArgs& a, cudaStream_t s) {
   const size_t smem = sizeof(PolicySmem<H>);
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(policy_step_kernel<H>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(policy_step_kernel<H, STATES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
   const int epb = ROWS / a.cfg.N;
-  policy_step_kernel<H><<<(a.cfg.B + epb - 1) / epb, NT, smem, s>>>(a);
+  policy_step_kernel<H, STATES><<<(a.cfg.B + epb - 1) / epb, NT, smem, s>>>(a);
   IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
@@ -787,8 +796,22 @@ extern "C" int ic3_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packe
   }
   if (!io->x) return IC3_E_NULL;
   if (cfg->cell == IC3_CELL_TANH && (!w->f_wT || !w->f_b)) return IC3_E_NULL;
-  PolicyArgs a{*cfg, *w, *io};
+  PolicyArgs a{*cfg, *w, *io, nullptr, nullptr};
   IC3_DISPATCH_H(cfg->H, launch_policy<HH>(a, (cudaStream_t)stream));
+}
+
+extern "C" int ic3_policy_ff_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,
+                                    float* st_h, float* st_s, void* stream) {
+  int rc = policy_check(cfg);
+  if (rc) return rc;
+  rc = packed_check(w);
+  if (rc) return rc;
+  if (!io || !io->x || !st_h || (!cfg->comm_mask_zero && !st_s)) return IC3_E_NULL;
+  if (cfg->hard_attn && !io->comm_action) return IC3_E_NULL;
+  if (cfg->cell != IC3_CELL_TANH || !cfg->h_from_x || cfg->H != 128 || cfg->N > ROWS) return IC3_E_UNSUPPORTED;
+  if (!w->f_wT || !w->f_b) return IC3_E_NULL;
+  PolicyArgs a{*cfg, *w, *io, st_h, st_s};
+  return launch_policy<128, true>(a, (cudaStream_t)stream);
 }
 
 extern "C" int ic3_policy_pass_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,

@@ -81,9 +81,10 @@ def build_parser():
                         help='what env.reset/step hand back: the dense [nenvs,N,obs_dim] tensor, or a LazyObs handle on the '
                              'env state that CommNetMLP.forward consumes directly (lazy_obs.py)')
     parser.add_argument('--policy_impl', default=None, choices=['tc', 'simt'], help='wgmma tensor-core or fp32 SIMT policy kernels')
-    parser.add_argument('--grad_impl', default='auto', choices=['auto', 'kernels', 'autograd', 'manual'],
-                        help='compute_grad: hand-written BPTT kernels (auto: whenever the configuration allows), torch '
-                             'autograd recompute, or the explicit formulas with torch GEMMs')
+    parser.add_argument('--grad_impl', default='auto', choices=['auto', 'kernels', 'kernels_ff', 'autograd', 'manual'],
+                        help='compute_grad: hand-written BPTT kernels (auto: whenever the configuration allows), the '
+                             'hand-written kernels of the non-recurrent tanh policies (models.MLP, CommNet / IC3Net '
+                             'without --recurrent), torch autograd recompute, or the explicit formulas with torch GEMMs')
     parser.add_argument('--batch_boundary', default='reference', choices=['reference', 'cut'],
                         help='run_batch: whole episodes until >= batch_size steps per env slot (reference), or a fixed '
                              'number of lock-steps with open episodes cut at the end')

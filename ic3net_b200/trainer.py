@@ -41,6 +41,11 @@ one window at a time from its checkpoint into one of two window buffers, just ah
 The tanh RNN (models.RNN with rnn_type 'MLP', the IC / IRIC baselines, on the SIMT policy kernel) has no c: its records
 are h alone, (T+1) B N H 4 bytes (24.3 GB at predator-prey hard, 8192 slots, batch 500), and its windows are re-run with
 the index encoder and the SIMT step.
+
+The non-recurrent tanh policies (models.MLP, CommNet / IC3Net without --recurrent) carry nothing from one step to the
+next.  With ``grad_impl = 'kernels_ff'`` their gradient comes from the kernels of ic3_ff_grad_* (csrc/bptt_tc.cu): no
+hidden-state record or checkpoint at all; the backward re-runs the forward from the env-state records over chunks of K
+consecutive lock-steps (K*B env slots at once, K from the memory the device has left, ``FF_CHUNK_STEPS``).
 """
 import ctypes as C
 import math
@@ -149,6 +154,16 @@ class Trainer(object):
             self.grad_kernels = ok
         if self.grad_impl == 'auto':
             self.grad_impl = 'kernels' if self.grad_kernels else 'autograd'
+        # the non-recurrent tanh policies' kernels (ic3_ff_grad_*): no (h, c) records or checkpoints
+        self.grad_ff = self.record_for_grad and self.grad_impl == 'kernels_ff'
+        if self.grad_ff:
+            e = env.env
+            cfg = policy_net.policy_cfg(e.nenvs)
+            if int(_lib.load().ic3_ff_grad_workspace_bytes(C.byref(self._ff_plan(cfg, None, e.nenvs * args.nagents)))) == 0:
+                raise NotImplementedError("grad_impl='kernels_ff' covers the non-recurrent tanh policies (models.MLP, "
+                                          "CommNet / IC3Net without --recurrent, 1..%d comm passes) at hid_size 128 with "
+                                          "<= 7 action logits, a vision window of <= 5 x 5 cells and an observation "
+                                          "pattern of <= 512 columns" % _lib.MAX_PASSES)
 
     def _bptt_supported(self):
         e, net = self.env.env, self.policy_net
@@ -228,7 +243,7 @@ class Trainer(object):
                 b['rec_h'] = torch.empty(T + 1, B * N, H, device=dev)
                 if hc:
                     b['rec_c'] = torch.empty(T + 1, B * N, H, device=dev)
-            else:
+            elif not self.grad_ff:          # kernels_ff re-runs every step from the env-state records alone
                 b['ck_h'] = z(nw, B * N, H)
                 if hc:
                     b['ck_c'] = z(nw, B * N, H)
@@ -395,7 +410,7 @@ class Trainer(object):
                         b['s_tjroute'][0].copy_(e.route_id)
                     else:
                         b['s_loc'][0].copy_(e.loc)
-                if not full and t % self.grad_window == 0:
+                if not full and not self.grad_ff and t % self.grad_window == 0:
                     b['ck_h'][t // self.grad_window].copy_(b['h'])
                     if hc:
                         b['ck_c'][t // self.grad_window].copy_(b['c'])
@@ -733,6 +748,8 @@ class Trainer(object):
             return self._random_losses(adv, ret)
         if self.grad_kernels:
             return self._compute_grad_kernels(adv, ret)
+        if self.grad_ff:
+            return self._compute_grad_ff(adv, ret)
         W = self.grad_window
         nw = (T + W - 1) // W
         dh = dc = None
@@ -879,6 +896,76 @@ class Trainer(object):
         params, grads = self._param_structs()
         _lib.check(lib.ic3_bptt_finish(C.byref(plan), C.byref(params), C.byref(grads), st['losses'].data_ptr(), s))
         return st['losses']
+
+    # Lock-steps per chunk of the non-recurrent kernels: as many as the memory the device has left holds (measured like
+    # the BPTT records in _pick_record_mode), at most FF_CHUNK_ROWS agent rows (2^21: 25 steps, about 10 GB of workspace
+    # at predator-prey hard with 8192 slots and 2 passes; one step of that size already fills the card many times
+    # over), and at most FF_CHUNK_STEPS steps when set
+    FF_CHUNK_ROWS = 1 << 21
+    FF_CHUNK_STEPS = None
+
+    def _ff_plan(self, cfg, w, rows, workspace=None):
+        e, args = self.env.env, self.args
+        return _lib.FfGradPlan(cfg=C.pointer(cfg), w=None if w is None else C.pointer(w),
+                               pp_env=None if self.is_tj else C.pointer(e.cfg), tj_env=C.pointer(e.cfg) if self.is_tj else None,
+                               value_coeff=float(args.value_coeff), entr=float(args.entr), max_rows=rows,
+                               workspace=workspace)
+
+    def _ff_chunk_steps(self, T, cfg):
+        """Lock-steps per chunk K of ic3_ff_grad_chunk for a T-step rollout: what the workspace of K steps needs must fit
+        in the device's free memory plus the allocator's unused reserve, minus RECORD_MARGIN_BYTES; K * B * N is at most
+        FF_CHUNK_ROWS (at least one step)."""
+        e = self.env.env
+        lib = _lib.load()
+        rows = e.nenvs * self.args.nagents
+        nbytes = lambda k: int(lib.ic3_ff_grad_workspace_bytes(C.byref(self._ff_plan(cfg, None, k * rows))))
+        one = nbytes(1)
+        per_step = max(1, nbytes(2) - one)
+        free, _ = torch.cuda.mem_get_info(e.device)
+        free += torch.cuda.memory_reserved(e.device) - torch.cuda.memory_allocated(e.device)
+        k = max(1, min(T, (free - self.RECORD_MARGIN_BYTES - one) // per_step + 1, self.FF_CHUNK_ROWS // rows))
+        if self.FF_CHUNK_STEPS is not None:
+            k = max(1, min(k, int(self.FF_CHUNK_STEPS)))
+        return int(k)
+
+    def _compute_grad_ff(self, adv, ret):
+        """grad_impl 'kernels_ff' (ic3_ff_grad_*): the rollout's T lock-steps in chunks of K consecutive steps, each one
+        batch of K*B env slots (records are [T, B, ...]), in any order since no state crosses a step.  Returns the device
+        float64 vector of the three loss sums."""
+        b, net, args, e = self._buf, self.policy_net, self.args, self.env.env
+        lib = _lib.load()
+        T, B, N = b['T'], e.nenvs, args.nagents
+        s = _lib.stream()
+        cfg = net.policy_cfg(B)
+        cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
+        w = net.packed()
+        K = self._ff_chunk_steps(T, cfg)
+        plan = self._ff_plan(cfg, w, K * B * N)
+        nbytes = int(lib.ic3_ff_grad_workspace_bytes(C.byref(plan)))
+        if nbytes == 0:
+            raise NotImplementedError("this configuration is outside the non-recurrent gradient kernels")
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=e.device)     # stream-ordered: freed after the kernels ran
+        plan.workspace = ws.data_ptr()
+        losses = torch.zeros(3, dtype=torch.float64, device=e.device)
+        hard = bool(args.hard_attn) and bool(args.commnet)
+        adv = adv.contiguous()
+        _lib.check(lib.ic3_ff_grad_begin(C.byref(plan), s))
+        for t in range(0, T, K):
+            io = _lib.FfGradIO(nsteps=min(K, T - t), fresh=b['s_fresh'][t].data_ptr(),
+                               comm=b['s_comm'][t].data_ptr() if hard else None, alive=b['s_alive'][t].data_ptr(),
+                               pp_loc=None if self.is_tj else b['s_loc'][t].data_ptr(),
+                               tj_loc=b['s_tjloc'][t].data_ptr() if self.is_tj else None,
+                               tj_alive=b['s_tjalive'][t].data_ptr() if self.is_tj else None,
+                               tj_last_act=b['s_tjlast'][t].data_ptr() if self.is_tj else None,
+                               tj_route_id=b['s_tjroute'][t].data_ptr() if self.is_tj else None,
+                               logp=b['logp'][t].data_ptr(), action=b['action'][t].data_ptr(),
+                               value=b['value'][t].data_ptr(), ret=ret[t].data_ptr(), adv=adv[t].data_ptr(),
+                               alive_post=b['ralive'][t].data_ptr(), valid=b['valid'][t].data_ptr())
+            _lib.check(lib.ic3_ff_grad_chunk(C.byref(plan), C.byref(io), s))
+        params, grads = self._param_structs()
+        _lib.check(lib.ic3_ff_grad_finish(C.byref(plan), C.byref(params), C.byref(grads), losses.data_ptr(), s))
+        self.ff_chunk_steps = K
+        return losses
 
     def _recompute_window(self, k):
         """Window mode: re-run the policy step over steps [k W, min(T, (k+1) W)) from checkpoint k into the window

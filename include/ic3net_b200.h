@@ -368,6 +368,14 @@ int ic3_policy_step_profile(const ic3_policy_cfg* cfg, const ic3_policy_packed* 
  * The BPTT kernels re-run the intermediate passes this way. */
 int ic3_policy_pass_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,
                            int32_t npasses, float* h_pass, float* c_pass, void* stream);
+/* The non-recurrent tanh step (cfg->cell == IC3_CELL_TANH, x_tanh, h_from_x, hid_size 128: models.MLP and the
+ * non-recurrent CommNet / IC3Net, comm.py:127-129,179-224, models.py:23-25) on the fp32 SIMT kernel with every pass
+ * state written out and no heads: st_h [passes + 1, B*N, H] gets tanh(x) (the state entering pass 0), then h after each
+ * pass; st_s [passes, B*N, H] the communication vector of each pass (may be NULL with comm_mask_zero).  Reads io->x,
+ * comm_action, alive, fresh.  Same kernel code as ic3_policy_step, so block `passes` of st_h equals its h_out bit for
+ * bit.  The non-recurrent backward (ic3_ff_grad_chunk) re-runs the forward this way. */
+int ic3_policy_ff_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, float* st_h,
+                         float* st_s, void* stream);
 /* select_action alone (action_utils.py:32-36) on given log-probabilities. */
 int ic3_sample_actions(const ic3_policy_cfg* cfg, const float* logp, const uint32_t* tick,
                        const uint32_t* draws, int32_t* action, void* stream);
@@ -485,6 +493,70 @@ int ic3_bptt_prepare(const ic3_bptt_plan* plan, const ic3_bptt_step_io* io, void
  * losses: device double[3] = action_loss, value_loss, entropy sums (trainer.py:198-216). */
 int ic3_bptt_finish(const ic3_bptt_plan* plan, const ic3_policy_params* params, const ic3_policy_params* grads,
                     double* losses, void* stream);
+
+/* ------------------------------------------------------------------------
+ * Gradient of the rollout loss (Trainer.compute_grad, trainer.py:128-225) for the NON-RECURRENT tanh policies:
+ * models.MLP (models.py:23-25) and CommNet / IC3Net without --recurrent (comm.py:127-129, 179, 220-224), i.e.
+ * cfg->cell == IC3_CELL_TANH, x_tanh = h_from_x = 1, 1 .. IC3_MAX_PASSES passes (share_weights included), hard attention,
+ * comm_mode avg / sum and comm_mask_zero; hid_size 128, at most 7 action logits, a window of at most 5 x 5 cells and an
+ * observation pattern of at most 512 columns.  Every other configuration gets a workspace of 0 bytes and IC3_E_* from
+ * the other calls before any device work.
+ * Nothing is carried from one step to the next, so there is no recursion in time: K consecutive lock-steps of the
+ * [T, B, ...] records are one batch of K*B env slots.  The host calls
+ *     ic3_ff_grad_begin(plan, stream)
+ *     for each chunk of consecutive steps (any order, any sizes up to plan->max_rows agent rows):
+ *         ic3_ff_grad_chunk(plan, &io_chunk, stream)
+ *     ic3_ff_grad_finish(plan, params, grads, losses, stream)
+ * Per chunk: the forward is re-run from the recorded env state (index encoder, ic3_policy_ff_states: bit-identical to
+ * the rollout), then for p = P-1 .. 0, from g = d loss / d h_P of the heads (recorded log-probs / actions / advantages):
+ *     dz = g (1 - h_{p+1}^2);  dx += dz;  dF_p += dz^T h_p;  dC_p += dz^T S_p;  df_b,p += sum dz;  dc_b,p += sum dz;
+ *     g = dz F_p + comm^T (dz C_p)
+ * and  dpre = (dx + g) (1 - tanh(x)^2),  d encoder = dpre^T obs through the observation pattern (never materialised),
+ * d encoder bias = sum dpre.  fp32 SIMT kernels; the sums over agent rows go to fixed per-block partials (no atomics)
+ * and are finished in float64, so the gradient is bit-identical from run to run for the same chunk sizes.  Slots with
+ * valid = 0 contribute exactly zero.  Gradients are ADDED to the `grads` buffers like ic3_bptt_finish (c_w_pass /
+ * c_b_pass / f_w_pass / f_b_pass per pass; index 0 or NULL of c_*_pass: c_w / c_b; share_weights may alias them).
+ * ---------------------------------------------------------------------- */
+typedef struct {
+  const ic3_policy_cfg* cfg;    /* HOST pointers: the structs the rollout used (cfg->B = env slots of one lock-step) */
+  const ic3_policy_packed* w;   /* SIMT-packed weights of the CURRENT parameters */
+  const ic3_pp_cfg* pp_env;     /* exactly one of pp_env / tj_env */
+  const ic3_tj_cfg* tj_env;
+  float value_coeff;            /* args.value_coeff (trainer.py:209) */
+  float entr;                   /* args.entr (trainer.py:211-220) */
+  int32_t max_rows;             /* chunk capacity in agent rows (>= cfg->B * cfg->N) */
+  int32_t reserved0;
+  void* workspace;              /* device scratch of ic3_ff_grad_workspace_bytes(plan) bytes */
+} ic3_ff_grad_plan;
+
+typedef struct {
+  int32_t nsteps;               /* K lock-steps in this chunk, K * B * N <= plan->max_rows; every pointer below is the
+                                   record of the chunk's first step in the [T, B, ...] layouts of the rollout */
+  int32_t reserved0;
+  const uint8_t* fresh;         /* [K, B] */
+  const uint8_t* comm;          /* [K, B, N] info['comm_action'] (required with hard_attn) */
+  const uint8_t* alive;         /* [K, B, N] info['alive_mask'] or NULL */
+  const int32_t* pp_loc;        /* [K, B, N+1, 2] */
+  const int32_t* tj_loc;        /* [K, B, N, 2] */
+  const uint8_t* tj_alive;      /* [K, B, N] */
+  const uint8_t* tj_last_act;   /* [K, B, N] */
+  const int32_t* tj_route_id;   /* [K, B, N] */
+  const float* logp;            /* [K*B*N, sum(na)] */
+  const int32_t* action;        /* [K*B*N, nheads] */
+  const float* value;           /* [K*B*N] */
+  const float* ret;             /* [K*B*N] */
+  const float* adv;             /* [K*B*N] */
+  const uint8_t* alive_post;    /* [K*B*N] */
+  const uint8_t* valid;         /* [K, B] or NULL */
+} ic3_ff_grad_io;
+
+uint64_t ic3_ff_grad_workspace_bytes(const ic3_ff_grad_plan* plan);   /* 0 = configuration not supported */
+int ic3_ff_grad_begin(const ic3_ff_grad_plan* plan, void* stream);
+int ic3_ff_grad_chunk(const ic3_ff_grad_plan* plan, const ic3_ff_grad_io* io, void* stream);
+/* params: the CURRENT parameters; grads: the gradient buffers (reference layouts); losses: device double[3] =
+ * action_loss, value_loss, entropy sums (trainer.py:198-216). */
+int ic3_ff_grad_finish(const ic3_ff_grad_plan* plan, const ic3_policy_params* params, const ic3_policy_params* grads,
+                       double* losses, void* stream);
 
 /* ------------------------------------------------------------------------
  * Optimizer step  (trainer.py:21-22 RMSprop(lr, alpha=0.97, eps=1e-6); trainer.py:251-256 and
