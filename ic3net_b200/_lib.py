@@ -108,8 +108,9 @@ class BpttPlan(C.Structure):
 
 
 class BpttStepIO(C.Structure):
-    _fields_ = [("t", C.c_int32), ("pass_index", C.c_int32), ("h_prev", _p), ("c_prev", _p), ("h_new", _p), ("fresh", _p), ("comm", _p), ("alive", _p), ("cut", _p),
-                ("pp_loc", _p), ("tj_loc", _p), ("tj_alive", _p), ("tj_last_act", _p), ("tj_route_id", _p),
+    _fields_ = [("t", C.c_int32), ("reserved0", C.c_int32), ("h_prev", _p), ("c_prev", _p), ("h_new", _p),
+                ("fresh", _p), ("comm", _p), ("alive", _p), ("cut", _p),
+                ("pp_state", C.POINTER(PPState)), ("tj_state", C.POINTER(TJState)),
                 ("logp", _p), ("action", _p), ("value", _p), ("ret", _p), ("adv", _p), ("alive_post", _p),
                 ("valid", _p), ("dh", _p), ("dc", _p), ("err", _p)]
 
@@ -122,7 +123,7 @@ class FfGradPlan(C.Structure):
 
 class FfGradIO(C.Structure):
     _fields_ = [("nsteps", C.c_int32), ("reserved0", C.c_int32), ("fresh", _p), ("comm", _p), ("alive", _p),
-                ("pp_loc", _p), ("tj_loc", _p), ("tj_alive", _p), ("tj_last_act", _p), ("tj_route_id", _p),
+                ("pp_state", C.POINTER(PPState)), ("tj_state", C.POINTER(TJState)),
                 ("logp", _p), ("action", _p), ("value", _p), ("ret", _p), ("adv", _p), ("alive_post", _p),
                 ("valid", _p)]
 

@@ -1,12 +1,11 @@
 """Explicit backward pass (BPTT) of the rollout loss over the trainer's lock-step record buffers.
 
 ``Trainer.compute_grad`` (reference trainer.py:128-225) needs d(loss)/d(parameters) through the recurrent policy.
-The default implementation re-runs windows of the rollout under torch autograd.  This module does the same with the
-hand-derived per-step formulas (spelled out and pinned to the reference's gradients in ``oracle/bptt.py``): a window
-is re-run forward without a graph, keeping only the activations the backward needs, then walked backwards with
-batched GEMMs -- no autograd graph, no per-op bookkeeping, and exactly the arithmetic a fused backward kernel would
-perform.  It is selected with ``args.grad_impl = 'manual'`` (``--grad_impl manual``); plain torch ops on whatever
-device / dtype the records live on, so the CPU tests run it in float64 against the oracle.
+This module states that gradient for the one-pass LSTM CommNet / IC3Net with the hand-derived per-step formulas
+(spelled out and pinned to the reference's gradients in ``oracle/bptt.py``): a window is re-run forward without a
+graph, keeping only the activations the backward needs, then walked backwards with batched GEMMs -- exactly the
+arithmetic the hand-written BPTT kernels (csrc/bptt_tc.cu) perform.  No ``Trainer`` backend runs it: it is the float64
+reference the tests compare the kernels against, in plain torch ops on whatever device / dtype the records live on.
 
 Step t of the lock-step batch (rows = B env slots x N agents; ``fresh`` marks slots that start an episode):
 

@@ -1227,12 +1227,22 @@ int env_geometry(const ic3_bptt_plan* p, int* npos, int* WW, int* is_tj) {
   return IC3_OK;
 }
 
+// The recorded env state of ic3_bptt_step_io / ic3_ff_grad_io: the fields the backward reads must be set.
+int records_check(const ic3_pp_state* pp, const ic3_tj_state* tj, int is_tj) {
+  if (is_tj) return tj && tj->loc && tj->alive && tj->last_act && tj->route_id ? IC3_OK : IC3_E_NULL;
+  return pp && pp->loc ? IC3_OK : IC3_E_NULL;
+}
+
 }  // namespace
 
 extern "C" uint64_t ic3_bptt_workspace_bytes(const ic3_bptt_plan* p) {
   if (!p || !p->cfg || p->cfg->H != TC_H) return 0;
   int npos, WW, is_tj;
   if (env_geometry(p, &npos, &WW, &is_tj)) return 0;
+  // the operand images sum the class terms apart from the counts (ic3_policy_cfg.obs_vocab): the environment's own
+  // layout hint is required
+  if (p->cfg->obs_vocab == 0 || (is_tj ? ic3_tj_layout_check(p->tj_env, p->cfg) : ic3_pp_layout_check(p->pp_env, p->cfg)))
+    return 0;
   Layout L;
   if (plan_layout(p->cfg, npos, WW, is_tj, &L)) return 0;
   int nout = 1;
@@ -1308,7 +1318,6 @@ static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, c
   pio.h = h_in; pio.c = io->c_prev; pio.comm_action = io->comm; pio.alive = io->alive; pio.fresh = io->fresh;
   pio.err = io->err;
   pio.pass_index = ps;                 // a fresh slot's zero state and silent first pass apply to pass 0 only
-  if (cfg->hard_attn && !io->comm) return IC3_E_NULL;
   PrepSrc src;
   memset(&src, 0, sizeof(src));
   // tanh cell: x is no operand of its GEMMs (the x block of the image stays zero), so it needs no table
@@ -1323,20 +1332,13 @@ static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, c
   bw.npos = npos;
   const int ntiles = L.ntiles;
   if (!is_tj) {
-    if (!io->pp_loc) return IC3_E_NULL;
     src.pp = *p->pp_env;
-    memset(&src.pps, 0, sizeof(src.pps));
-    src.pps.loc = const_cast<int32_t*>(io->pp_loc);
+    src.pps = *io->pp_state;
     prep_kernel<XSRC_PP, true, true><<<2 * ntiles, PREP_THREADS, prep_T_bytes(cfg->N), s>>>(*cfg, pio, a_img, src, bw);
     IC3_LAUNCH_CHECK();
   } else {
-    if (!io->tj_loc || !io->tj_alive || !io->tj_last_act || !io->tj_route_id) return IC3_E_NULL;
     src.tj = *p->tj_env;
-    memset(&src.tjs, 0, sizeof(src.tjs));
-    src.tjs.loc = const_cast<int32_t*>(io->tj_loc);
-    src.tjs.alive = const_cast<uint8_t*>(io->tj_alive);
-    src.tjs.last_act = const_cast<uint8_t*>(io->tj_last_act);
-    src.tjs.route_id = const_cast<int32_t*>(io->tj_route_id);
+    src.tjs = *io->tj_state;
     prep_kernel<XSRC_TJ, true, true><<<2 * ntiles, PREP_THREADS, prep_T_bytes(cfg->N), s>>>(*cfg, pio, a_img, src, bw);
     IC3_LAUNCH_CHECK();
   }
@@ -1371,6 +1373,8 @@ static int bptt_common(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, Layou
   rc = plan_layout(p->cfg, *npos, WW, *is_tj, L);
   if (rc) return rc;
   if (!L->tanh && (!io->c_prev || !io->dc)) return IC3_E_NULL;     // the tanh cell has no c
+  if (p->cfg->hard_attn && !io->comm) return IC3_E_NULL;
+  if (records_check(io->pp_state, io->tj_state, *is_tj)) return IC3_E_NULL;
   int nout = 1;
   for (int k = 0; k < p->cfg->nheads; ++k) nout += p->cfg->head_dim[k];
   return nout > BP_HEADS ? IC3_E_UNSUPPORTED : IC3_OK;
@@ -1565,7 +1569,6 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
   int npos, is_tj;
   int rc = bptt_common(p, io, &L, &npos, &is_tj);
   if (rc) return rc;
-  if (io->pass_index != 0) return IC3_E_RANGE;
   cudaStream_t s = (cudaStream_t)stream;
   if (L.P == 1) return bptt_unit(p, io, L, npos, is_tj, s, io->t & 1, 0, io->h_prev, io->c_prev);
   const ic3_policy_cfg* cfg = p->cfg;
@@ -1578,23 +1581,11 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
   pio.h = io->h_prev; pio.c = io->c_prev; pio.comm_action = io->comm; pio.alive = io->alive; pio.fresh = io->fresh;
   pio.err = io->err; pio.x_table = p->x_table;
   pio.workspace = ws + L.tc_ws;
-  ic3_pp_state pps;
-  ic3_tj_state tjs;
-  memset(&pps, 0, sizeof(pps));
-  memset(&tjs, 0, sizeof(tjs));
   if (!is_tj) {
-    if (!io->pp_loc) return IC3_E_NULL;
-    pps.loc = const_cast<int32_t*>(io->pp_loc);
-    pio.pp_env = p->pp_env; pio.pp_state = &pps;
+    pio.pp_env = p->pp_env; pio.pp_state = io->pp_state;
   } else {
-    if (!io->tj_loc || !io->tj_alive || !io->tj_last_act || !io->tj_route_id) return IC3_E_NULL;
-    tjs.loc = const_cast<int32_t*>(io->tj_loc);
-    tjs.alive = const_cast<uint8_t*>(io->tj_alive);
-    tjs.last_act = const_cast<uint8_t*>(io->tj_last_act);
-    tjs.route_id = const_cast<int32_t*>(io->tj_route_id);
-    pio.tj_env = p->tj_env; pio.tj_state = &tjs;
+    pio.tj_env = p->tj_env; pio.tj_state = io->tj_state;
   }
-  if (cfg->hard_attn && !io->comm) return IC3_E_NULL;
   rc = ic3_tc_pass_states(cfg, p->w, &pio, L.P - 1, h_pass, c_pass, s);
   if (rc) return rc;
   for (int ps = L.P - 1; ps >= 0; --ps) {
@@ -1875,8 +1866,8 @@ __global__ void __launch_bounds__(256) ff_desc_kernel(DescArgs a) {
 // indexes nothing from its stale records and contributes exactly zero.
 struct RecArgs {
   int R, N, NP, is_tj;
-  const int32_t* pp_loc; const int32_t* tj_loc; const uint8_t* tj_alive; const uint8_t* tj_last_act;
-  const int32_t* tj_route_id; const uint8_t* alive_post; const uint8_t* valid;
+  ic3_pp_state pps; ic3_tj_state tjs;          // the records (ic3_ff_grad_io)
+  const uint8_t* alive_post; const uint8_t* valid;
   int32_t* loc; int32_t* route; uint8_t* alive; uint8_t* last; uint8_t* apost;
 };
 
@@ -1889,20 +1880,20 @@ __global__ void __launch_bounds__(256) ff_records_kernel(RecArgs a) {
   if (!a.is_tj) {
     if (i <= a.NP) {                           // rows 0 .. NP of env e carry its N_pred + 1 positions
       const size_t o = ((size_t)e * (a.NP + 1) + i) * 2;
-      a.loc[o] = ok ? a.pp_loc[o] : 0;
-      a.loc[o + 1] = ok ? a.pp_loc[o + 1] : 0;
+      a.loc[o] = ok ? a.pps.loc[o] : 0;
+      a.loc[o + 1] = ok ? a.pps.loc[o + 1] : 0;
     }
     if (i == a.N - 1 && a.NP >= a.N) {         // N_pred + 1 > N rows: the prey's position goes with the last row
       const size_t o = ((size_t)e * (a.NP + 1) + a.NP) * 2;
-      a.loc[o] = ok ? a.pp_loc[o] : 0;
-      a.loc[o + 1] = ok ? a.pp_loc[o + 1] : 0;
+      a.loc[o] = ok ? a.pps.loc[o] : 0;
+      a.loc[o + 1] = ok ? a.pps.loc[o + 1] : 0;
     }
   } else {
-    a.loc[2 * (size_t)row] = ok ? a.tj_loc[2 * (size_t)row] : 0;
-    a.loc[2 * (size_t)row + 1] = ok ? a.tj_loc[2 * (size_t)row + 1] : 0;
-    a.alive[row] = ok ? a.tj_alive[row] : 0;
-    a.last[row] = ok ? a.tj_last_act[row] : 0;
-    a.route[row] = ok ? a.tj_route_id[row] : 0;
+    a.loc[2 * (size_t)row] = ok ? a.tjs.loc[2 * (size_t)row] : 0;
+    a.loc[2 * (size_t)row + 1] = ok ? a.tjs.loc[2 * (size_t)row + 1] : 0;
+    a.alive[row] = ok ? a.tjs.alive[row] : 0;
+    a.last[row] = ok ? a.tjs.last_act[row] : 0;
+    a.route[row] = ok ? a.tjs.route_id[row] : 0;
   }
 }
 
@@ -2166,7 +2157,7 @@ extern "C" int ic3_ff_grad_chunk(const ic3_ff_grad_plan* p, const ic3_ff_grad_io
   if (io->nsteps < 1 || (long)io->nsteps * cfg->B * cfg->N > (long)G.R) return IC3_E_RANGE;
   if (!io->fresh || !io->logp || !io->action || !io->value || !io->ret || !io->adv || !io->alive_post) return IC3_E_NULL;
   if (cfg->hard_attn && !io->comm) return IC3_E_NULL;
-  if (G.is_tj ? (!io->tj_loc || !io->tj_alive || !io->tj_last_act || !io->tj_route_id) : !io->pp_loc) return IC3_E_NULL;
+  if (records_check(io->pp_state, io->tj_state, G.is_tj)) return IC3_E_NULL;
   cudaStream_t s = (cudaStream_t)stream;
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
   const int Bk = io->nsteps * cfg->B, N = cfg->N, R = Bk * N;
@@ -2183,8 +2174,9 @@ extern "C" int ic3_ff_grad_chunk(const ic3_ff_grad_plan* p, const ic3_ff_grad_io
   RecArgs ra;
   memset(&ra, 0, sizeof(ra));
   ra.R = R; ra.N = N; ra.NP = G.is_tj ? N : p->pp_env->N; ra.is_tj = G.is_tj;
-  ra.pp_loc = io->pp_loc; ra.tj_loc = io->tj_loc; ra.tj_alive = io->tj_alive; ra.tj_last_act = io->tj_last_act;
-  ra.tj_route_id = io->tj_route_id; ra.alive_post = io->alive_post; ra.valid = io->valid;
+  if (G.is_tj) ra.tjs = *io->tj_state;
+  else ra.pps = *io->pp_state;
+  ra.alive_post = io->alive_post; ra.valid = io->valid;
   ra.loc = reinterpret_cast<int32_t*>(ws + G.rloc); ra.route = reinterpret_cast<int32_t*>(ws + G.rroute);
   ra.alive = ws + G.ralive; ra.last = ws + G.rlast; ra.apost = ws + G.apost;
   ff_records_kernel<<<(R + 255) / 256, 256, 0, s>>>(ra);

@@ -65,6 +65,13 @@ Transition = namedtuple('Transition', ('state', 'action', 'action_out', 'value',
 RolloutBatch = namedtuple('RolloutBatch', ('action', 'logp', 'value', 'reward', 'episode_mask',
                                            'episode_mini_mask', 'alive_mask', 'valid'))
 
+# The env state a policy step's observation is taken from, recorded for compute_grad: record buffer [T, ...] ->
+# (env attribute holding the live state, ic3_*_state field, ic3_rollout_io field through which the env step records it)
+PP_RECORDS = (('s_loc', 'loc', 'loc', 'snap_pp_loc'),)
+TJ_RECORDS = (('s_tjloc', 'car_loc', 'loc', 'snap_tj_loc'), ('s_tjalive', 'alive_mask', 'alive', 'snap_tj_alive'),
+              ('s_tjlast', 'car_last_act', 'last_act', 'snap_tj_last_act'),
+              ('s_tjroute', 'route_id', 'route_id', 'snap_tj_route_id'))
+
 
 def policy_forward_torch(net, x, h, c, g, n_alive):
     """Differentiable torch restatement of the policy step the kernels run (comm.py:134-244 for every variant of
@@ -121,13 +128,18 @@ class Trainer(object):
         self.obs_mode = getattr(args, 'obs_mode', 'index')      # 'index' | 'dense'
         self.use_graph = bool(getattr(args, 'use_graph', False))
         self.is_tj = args.env_name == 'traffic_junction'
+        self._records = TJ_RECORDS if self.is_tj else PP_RECORDS
+        self.hard = bool(args.hard_attn) and bool(args.commnet)      # hard attention gates (trainer.py:70)
         self.record_for_grad = bool(getattr(args, 'record_for_grad', False))
         self.grad_window = int(getattr(args, 'grad_window', 40))
         # compute_grad implementation: 'kernels' = hand-written BPTT (csrc/bptt_tc.cu; tensor-core policy path with the
         # LSTM cell and 1..4 comm passes, or the tanh RNN without communication on the SIMT path; at most 7 action
-        # logits, observation pattern of <= 512 columns), 'autograd' = windowed recompute under torch autograd,
-        # 'manual' = explicit formulas with torch GEMMs (bptt.py).  Default: kernels when the configuration allows.
+        # logits, observation pattern of <= 512 columns), 'kernels_ff' = the non-recurrent tanh policies' kernels,
+        # 'autograd' = windowed recompute under torch autograd.  Default: kernels when the configuration allows.
         self.grad_impl = getattr(args, 'grad_impl', None) or 'auto'
+        if self.grad_impl not in ('auto', 'kernels', 'kernels_ff', 'autograd'):
+            raise ValueError("grad_impl must be 'auto', 'kernels', 'kernels_ff' or 'autograd', not %r"
+                             % (self.grad_impl,))
         self.grad_kernels = False
         self._bptt = None
         self._buf = None
@@ -145,7 +157,11 @@ class Trainer(object):
         # fused index encoder's per-position table of the class terms belongs to the policy (encoder_table)
         policy_net.set_obs_layout(*getattr(env.env, 'obs_layout', (0, 0, 0)))
         if self.record_for_grad and self.grad_impl in ('auto', 'kernels'):
-            ok = self._bptt_supported()
+            # the library decides which configurations its kernels cover; an LSTM cell also needs the tensor-core path,
+            # whose weight image and policy step the kernels re-use
+            cfg = policy_net.policy_cfg(env.env.nenvs)
+            ok = ((cfg.cell == _lib.CELL_TANH or policy_net.policy_impl == 'tc') and
+                  self._bptt_workspace_bytes(cfg) > 0)
             if self.grad_impl == 'kernels' and not ok:
                 raise NotImplementedError("grad_impl='kernels' needs the tensor-core policy path (hid_size 128, LSTM "
                                           "cell) with the per-position encoder table, or the tanh RNN without "
@@ -165,30 +181,22 @@ class Trainer(object):
                                           "<= 7 action logits, a vision window of <= 5 x 5 cells and an observation "
                                           "pattern of <= 512 columns" % _lib.MAX_PASSES)
 
-    def _bptt_supported(self):
-        e, net = self.env.env, self.policy_net
-        W = 2 * e.vision + 1
-        if 1 + sum(self.args.naction_heads) > 8:
-            return False
-        if self._tanh_rnn():
-            # the tanh RNN runs on the SIMT kernel: no fused encoder, only the same window limit
-            if W * W > 25:
-                return False
-        # the recurrent LSTM policies, any number of comm passes (share_weights included)
-        elif not net.fuses_encoder(e) or not net.tc_capable or net.comm_passes > _lib.MAX_PASSES:
-            return False
-        if getattr(e, 'obs_layout', (0, 0, 0))[1] == 0:
-            return False
-        npos = e.obs_positions
-        used = npos + ((W * W + 4) if self.is_tj else (2 * W * W + 1))
-        return (used + 15) // 16 * 16 <= 512
+    def _policy_cfg(self):
+        """ic3_policy_cfg of the policy step over this GPU's slots, with the env's Philox key and env ids."""
+        e = self.env.env
+        cfg = self.policy_net.policy_cfg(e.nenvs)
+        cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
+        return cfg
 
-    def _tanh_rnn(self):
-        """The policy is the tanh recurrence without communication (models.RNN with rnn_type 'MLP': the IC / IRIC
-        baselines) at hid_size 128, which the BPTT kernels differentiate on the SIMT policy path."""
-        cp = self.policy_net._cfg_proto
-        return (cp['cell'] == _lib.CELL_TANH and not cp['x_tanh'] and not cp['h_from_x'] and cp['passes'] <= 1
-                and bool(cp['comm_mask_zero']) and not cp['hard_attn'] and cp['H'] == 128)
+    def _bptt_plan(self, cfg, w=None, x_table=None):
+        e, args = self.env.env, self.args
+        return _lib.BpttPlan(cfg=C.pointer(cfg), w=None if w is None else C.pointer(w),
+                             pp_env=None if self.is_tj else C.pointer(e.cfg), tj_env=C.pointer(e.cfg) if self.is_tj else None,
+                             x_table=x_table, value_coeff=float(args.value_coeff), entr=float(args.entr), workspace=None)
+
+    def _bptt_workspace_bytes(self, cfg):
+        """ic3_bptt_workspace_bytes of the policy configuration cfg on this environment (0: not covered)."""
+        return int(_lib.load().ic3_bptt_workspace_bytes(C.byref(self._bptt_plan(cfg))))
 
     def _encoder_table(self, cfg=None, w=None):
         """The policy's per-position encoder table for this environment (CommNetMLP.encoder_table), built from its
@@ -230,11 +238,9 @@ class Trainer(object):
             #              window at a time (_recompute_window)
             b.update(s_fresh=z(T, B, dtype=torch.uint8), s_comm=z(T, B, N, dtype=torch.uint8),
                      s_alive=z(T, B, N, dtype=torch.uint8), s_tep=z(T, B, dtype=torch.int32))
-            if self.is_tj:
-                b.update(s_tjloc=z(T, B, N, 2, dtype=torch.int32), s_tjalive=z(T, B, N, dtype=torch.uint8),
-                         s_tjlast=z(T, B, N, dtype=torch.uint8), s_tjroute=z(T, B, N, dtype=torch.int32))
-            else:
-                b['s_loc'] = z(T, B, e.npredator + 1, 2, dtype=torch.int32)    # predators + the prey
+            for key, attr, _, _ in self._records:
+                live = getattr(e, attr)
+                b[key] = z(T, *live.shape, dtype=live.dtype)
             W = self.grad_window
             nw = (T + W - 1) // W
             self._record_mode = self._pick_record_mode(T) if self.grad_kernels else None
@@ -284,7 +290,7 @@ class Trainer(object):
 
     def _h_only_records(self):
         """The BPTT kernels of the tanh RNN record h alone (no c, no max |c|)."""
-        return self.grad_kernels and self._tanh_rnn()
+        return self.grad_kernels and self.policy_net._cfg_proto['cell'] == _lib.CELL_TANH
 
     def _record_bytes(self, T):
         """{'full': bytes of rec_h + rec_c, 'window': bytes of the checkpoints + window buffers} for T steps (h alone
@@ -302,25 +308,20 @@ class Trainer(object):
         per-pass states, weight images and partials of comm_passes > 1 (0 with one pass)."""
         if int(self.args.comm_passes) <= 1:
             return 0
-        e = self.env.env
-        lib = _lib.load()
-
-        def nbytes(cfg):
-            plan = _lib.BpttPlan(cfg=C.pointer(cfg), w=None, pp_env=None if self.is_tj else C.pointer(e.cfg),
-                                 tj_env=C.pointer(e.cfg) if self.is_tj else None, x_table=None,
-                                 value_coeff=float(self.args.value_coeff), entr=float(self.args.entr), workspace=None)
-            return int(lib.ic3_bptt_workspace_bytes(C.byref(plan)))
-        cfg = self.policy_net.policy_cfg(e.nenvs)
-        one = self.policy_net.policy_cfg(e.nenvs)
+        cfg = self.policy_net.policy_cfg(self.env.env.nenvs)
+        one = self.policy_net.policy_cfg(self.env.env.nenvs)
         one.passes = 1
-        return max(0, nbytes(cfg) - nbytes(one))
+        return max(0, self._bptt_workspace_bytes(cfg) - self._bptt_workspace_bytes(one))
+
+    def _device_bytes_free(self):
+        """The device's free memory plus the caching allocator's unused reserve."""
+        dev = self.env.env.device
+        free, _ = torch.cuda.mem_get_info(dev)
+        return free + torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
 
     def _pick_record_mode(self, T):
         need = self._record_bytes(T)
-        dev = self.env.env.device
-        free, _ = torch.cuda.mem_get_info(dev)
-        free += torch.cuda.memory_reserved(dev) - torch.cuda.memory_allocated(dev)
-        avail = (free - self.RECORD_MARGIN_BYTES - self._bptt_extra_bytes()
+        avail = (self._device_bytes_free() - self.RECORD_MARGIN_BYTES - self._bptt_extra_bytes()
                  - self.RECORD_TEMP_FACTOR * T * self.env.env.nenvs * self.args.nagents * 4)
         limit = avail if self.RECORD_BYTES_LIMIT is None else min(avail, self.RECORD_BYTES_LIMIT)
         if need['full'] <= limit:
@@ -360,13 +361,11 @@ class Trainer(object):
         quota = 0: episodes still open at iteration T-1 are cut there."""
         if self.random_policy:
             return self._enqueue_random(T, quota)
-        b, e, net, args = self._buf, self.env.env, self.policy_net, self.args
+        b, e, net = self._buf, self.env.env, self.policy_net
         lib = _lib.load()
         B = e.nenvs
-        cfg = net.policy_cfg(B)
-        cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
+        cfg = self._policy_cfg()
         w = net.packed()
-        hard = int(bool(args.hard_attn) and bool(args.commnet))
         s = _lib.stream()
         ws, _ = net.workspace(B)          # tensor-core path scratch (None for the fp32 SIMT kernel)
         rec = self.record_for_grad
@@ -390,12 +389,8 @@ class Trainer(object):
         snap = {}
         if rec:
             snap = dict(snap_T=T, snap_fresh=b['s_fresh'].data_ptr(), snap_comm=b['s_comm'].data_ptr(),
-                        snap_alive=b['s_alive'].data_ptr(), snap_tep=b['s_tep'].data_ptr())
-            if self.is_tj:
-                snap.update(snap_tj_loc=b['s_tjloc'].data_ptr(), snap_tj_alive=b['s_tjalive'].data_ptr(),
-                            snap_tj_last_act=b['s_tjlast'].data_ptr(), snap_tj_route_id=b['s_tjroute'].data_ptr())
-            else:
-                snap['snap_pp_loc'] = b['s_loc'].data_ptr()
+                        snap_alive=b['s_alive'].data_ptr(), snap_tep=b['s_tep'].data_ptr(),
+                        **{field: b[key].data_ptr() for key, _, _, field in self._records})
         for t in range(T):
             if rec:
                 if t == 0:          # inputs of the first step; the env step kernels record those of every later step
@@ -403,13 +398,8 @@ class Trainer(object):
                     b['s_comm'][0].copy_(b['comm'])
                     b['s_alive'][0].copy_(b['alive'])
                     b['s_tep'][0].copy_(b['t_ep'])
-                    if self.is_tj:
-                        b['s_tjloc'][0].copy_(e.car_loc)
-                        b['s_tjalive'][0].copy_(e.alive_mask)
-                        b['s_tjlast'][0].copy_(e.car_last_act)
-                        b['s_tjroute'][0].copy_(e.route_id)
-                    else:
-                        b['s_loc'][0].copy_(e.loc)
+                    for key, attr, _, _ in self._records:
+                        b[key][0].copy_(getattr(e, attr))
                 if not full and not self.grad_ff and t % self.grad_window == 0:
                     b['ck_h'][t // self.grad_window].copy_(b['h'])
                     if hc:
@@ -436,7 +426,7 @@ class Trainer(object):
             hin, hout = (b['rec_h'][t], b['rec_h'][t + 1]) if full else (b['h'], b['h'])
             cin, cout = (b['rec_c'][t], b['rec_c'][t + 1]) if full and hc else (b['c'], b['c'])
             io = _lib.PolicyIO(x=None if fused_x else b['x'].data_ptr(), h=hin.data_ptr(), c=cin.data_ptr(),
-                               comm_action=b['comm'].data_ptr() if hard else None, alive=b['alive'].data_ptr(),
+                               comm_action=b['comm'].data_ptr() if self.hard else None, alive=b['alive'].data_ptr(),
                                fresh=b['fresh'].data_ptr(), tick=e.tick.data_ptr(), draws=None,
                                h_out=hout.data_ptr(), c_out=cout.data_ptr(), value=b['value'][t].data_ptr(),
                                logp=b['logp'][t].data_ptr(), action=b['action'][t].data_ptr(),
@@ -456,8 +446,7 @@ class Trainer(object):
         b, e, args = self._buf, self.env.env, self.args
         lib = _lib.load()
         nh = len(args.naction_heads)
-        hard = int(bool(args.hard_attn) and bool(args.commnet))
-        r = _lib.RolloutIO(t=t, max_steps=args.max_steps, nheads=nh, hard_attn=hard,
+        r = _lib.RolloutIO(t=t, max_steps=args.max_steps, nheads=nh, hard_attn=int(self.hard),
                            comm_action_one=int(bool(args.comm_action_one)),
                            last=int(t == T - 1 and quota <= 0), batch_size=int(quota),
                            halted=b['halted'].data_ptr(), rec_valid=b['valid'].data_ptr(), **snap,
@@ -552,11 +541,10 @@ class Trainer(object):
         """Device float64 vector [num_episodes, num_steps, success, err flags, reward[N], comm_action[N]] of this
         GPU's slots (one kernel, csrc/returns.cu ic3_stat_reduce); no host synchronisation."""
         b, e = self._buf, self.env.env
-        hard = bool(self.args.hard_attn) and bool(self.args.commnet)
         _lib.check(_lib.load().ic3_stat_reduce(e.nenvs, self.args.nagents, b['stat_episodes'].data_ptr(),
                                                b['stat_steps'].data_ptr(), b['stat_success'].data_ptr(),
                                                b['err'].data_ptr(), b['stat_reward'].data_ptr(),
-                                               b['stat_comm'].data_ptr() if hard else None,
+                                               b['stat_comm'].data_ptr() if self.hard else None,
                                                b['statvec'].data_ptr(), _lib.stream()))
         return b['statvec']
 
@@ -629,12 +617,18 @@ class Trainer(object):
         e, b = self.env.env, self._buf
         k1 = e.nenvs if k1 is None else k1
         cfg, st = e.chunk_view(k0, k1)
-        rec = lambda key: b[key][t, k0:k1].data_ptr()
-        if self.is_tj:
-            st.loc, st.alive, st.last_act, st.route_id = rec('s_tjloc'), rec('s_tjalive'), rec('s_tjlast'), rec('s_tjroute')
-        else:
-            st.loc = rec('s_loc')
+        for key, _, field, _ in self._records:
+            setattr(st, field, b[key][t, k0:k1].data_ptr())
         return cfg, st
+
+    def _grad_state(self, t):
+        """{'pp_state' | 'tj_state': an ic3_*_state whose recorded fields point at step t of the records} for
+        ic3_bptt_step_io / ic3_ff_grad_io (a chunk's [K, ...] records start at its first step).  The other fields stay
+        NULL: the backward reads none of them."""
+        b = self._buf
+        st = (_lib.TJState if self.is_tj else _lib.PPState)(**{field: b[key][t].data_ptr()
+                                                               for key, _, field, _ in self._records})
+        return {'tj_state' if self.is_tj else 'pp_state': C.pointer(st)}
 
     def _tj_record_obs(self, t, k0=0, k1=None):
         """[k1 - k0, N, O] traffic-junction observation of step t for env slots [k0, k1), written by ic3_tj_obs from the
@@ -670,7 +664,6 @@ class Trainer(object):
         """Differentiable re-run of steps [t0, t1) for all slots; returns (loss, h, c, stats)."""
         b, net, args = self._buf, self.policy_net, self.args
         B, N, H = self.env.env.nenvs, args.nagents, args.hid_size
-        hard = bool(args.hard_attn) and bool(args.commnet)
         w = net._kernel_weights()
         w_e, b_e = w['enc_w'], w['enc_b']
         w_eT = None if self.is_tj else w_e.t().contiguous()
@@ -689,7 +682,7 @@ class Trainer(object):
             alive = torch.where(fresh, torch.ones_like(b['s_alive'][t]), b['s_alive'][t]).float()   # comm.py:99-112
             n_alive = alive.sum(1, keepdim=True)
             g = alive
-            if hard:
+            if self.hard:
                 g = g * torch.where(fresh, torch.zeros_like(b['s_comm'][t]), b['s_comm'][t]).float()  # :171-175
             h, c, value, logps = policy_forward_torch(net, x, h, c, g, n_alive)
             value = value.view(B, N)
@@ -753,9 +746,6 @@ class Trainer(object):
         W = self.grad_window
         nw = (T + W - 1) // W
         dh = dc = None
-        if self.grad_impl == 'manual':
-            tot = self._compute_grad_manual(adv, ret, W, nw)
-            return torch.tensor([tot[k] for k in self.LOSS_KEYS], dtype=torch.float64, device=e.device)
         tot = torch.zeros(3, dtype=torch.float64, device=e.device)
         for k in reversed(range(nw)):
             t0, t1 = k * W, min(T, (k + 1) * W)
@@ -796,16 +786,11 @@ class Trainer(object):
         lib = _lib.load()
         T, B, N, H = b['T'], e.nenvs, args.nagents, args.hid_size
         s = _lib.stream()
-        cfg = net.policy_cfg(B)
-        cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
+        cfg = self._policy_cfg()
         w = net.packed()
         hc = not self._h_only_records()        # the tanh RNN: h alone, no encoder table (x is no operand of its GEMMs)
-        table = _lib.ptr(self._encoder_table()) if hc else None
+        plan = self._bptt_plan(cfg, w, _lib.ptr(self._encoder_table()) if hc else None)
         if self._bptt is None or self._bptt['B'] != B:
-            plan = _lib.BpttPlan(cfg=C.pointer(cfg), w=C.pointer(w),
-                                 pp_env=None if self.is_tj else C.pointer(e.cfg),
-                                 tj_env=C.pointer(e.cfg) if self.is_tj else None, x_table=table,
-                                 value_coeff=float(args.value_coeff), entr=float(args.entr), workspace=None)
             nbytes = int(lib.ic3_bptt_workspace_bytes(C.byref(plan)))
             if nbytes == 0:
                 raise NotImplementedError("this configuration is outside the BPTT kernels (use grad_impl='autograd')")
@@ -814,40 +799,29 @@ class Trainer(object):
                               dc=torch.zeros(B * N, H, device=e.device) if hc else None,
                               losses=torch.zeros(3, dtype=torch.float64, device=e.device))
         st = self._bptt
-        plan = _lib.BpttPlan(cfg=C.pointer(cfg), w=C.pointer(w), pp_env=None if self.is_tj else C.pointer(e.cfg),
-                             tj_env=C.pointer(e.cfg) if self.is_tj else None, x_table=table,
-                             value_coeff=float(args.value_coeff), entr=float(args.entr), workspace=st['ws'].data_ptr())
-        hard = bool(args.hard_attn) and bool(args.commnet)
+        plan.workspace = st['ws'].data_ptr()
         adv = adv.contiguous()
         cut = None
         if args.detach_gap <= args.max_steps:                                  # trainer.py:56-60
             cut = (((b['s_tep'] + 1) % args.detach_gap) == 0).to(torch.uint8).contiguous()
         window = self._record_mode == 'window'
-        W = self.grad_window
+        W, nb = self.grad_window, self._window_buffers()
         if not hc:
             cmax = 0.0                          # no cell state: the operand scale bounds |dh| alone
-
-            def state(t):                      # h entering step t and h' leaving it (window: in the window buffers)
-                if not window:
-                    return b['rec_h'][t], None, b['rec_h'][t + 1]
-                k, j = divmod(t, W)
-                wh = b['win_h'][k % self._window_buffers()]
-                return (b['ck_h'][k] if j == 0 else wh[j - 1]), None, wh[j]
         elif window:
             cmax = float(b['c_abs'].max().item())                              # tracked per step by the rollout
-            nb = self._window_buffers()
-
-            def state(t):                      # (h, c) entering step t and h' leaving it, in the window buffers
-                k, j = divmod(t, W)
-                wh, wc = b['win_h'][k % nb], b['win_c'][k % nb]
-                hp, cp = (b['ck_h'][k], b['ck_c'][k]) if j == 0 else (wh[j - 1], wc[j - 1])
-                return hp, cp, wh[j]
         else:
             lo, hi = torch.aminmax(b['rec_c'][1:])                              # bound of |c| for the operand scale
             cmax = max(abs(float(lo.item())), abs(float(hi.item())))
 
-            def state(t):
-                return b['rec_h'][t], b['rec_c'][t], b['rec_h'][t + 1]
+        def state(t):                          # (h, c) entering step t and h' leaving it (c: None for the tanh RNN)
+            if not window:
+                return b['rec_h'][t], b['rec_c'][t] if hc else None, b['rec_h'][t + 1]
+            k, j = divmod(t, W)                # window mode: in the window buffers, entered from checkpoint k
+            wh = b['win_h'][k % nb]
+            if j == 0:
+                return b['ck_h'][k], b['ck_c'][k] if hc else None, wh[0]
+            return wh[j - 1], b['win_c'][k % nb][j - 1] if hc else None, wh[j]
         # window mode: window k, steps [t0, t1), is re-run on this stream right before ic3_bptt_step(t1 + 1) is issued
         # (before ic3_bptt_begin when there is no such step).  The look-ahead ic3_bptt_prepare(t) on the library's side
         # stream waits for this stream's work up to ic3_bptt_step(t + 2), so it sees every window it reads; and the
@@ -869,17 +843,13 @@ class Trainer(object):
             hp, cp, hn = state(t)
             return _lib.BpttStepIO(t=t, h_prev=hp.data_ptr(), c_prev=_lib.ptr(cp),
                                    h_new=hn.data_ptr(), fresh=b['s_fresh'][t].data_ptr(),
-                                   comm=b['s_comm'][t].data_ptr() if hard else None, alive=b['s_alive'][t].data_ptr(),
-                                   cut=cut[t].data_ptr() if cut is not None else None,
-                                   pp_loc=None if self.is_tj else b['s_loc'][t].data_ptr(),
-                                   tj_loc=b['s_tjloc'][t].data_ptr() if self.is_tj else None,
-                                   tj_alive=b['s_tjalive'][t].data_ptr() if self.is_tj else None,
-                                   tj_last_act=b['s_tjlast'][t].data_ptr() if self.is_tj else None,
-                                   tj_route_id=b['s_tjroute'][t].data_ptr() if self.is_tj else None,
+                                   comm=b['s_comm'][t].data_ptr() if self.hard else None,
+                                   alive=b['s_alive'][t].data_ptr(), cut=cut[t].data_ptr() if cut is not None else None,
                                    logp=b['logp'][t].data_ptr(), action=b['action'][t].data_ptr(),
                                    value=value[t].data_ptr(), ret=ret[t].data_ptr(), adv=adv[t].data_ptr(),
                                    alive_post=b['ralive'][t].data_ptr(), valid=b['valid'][t].data_ptr(),
-                                   dh=st['dh'].data_ptr(), dc=_lib.ptr(st['dc']), err=b['err'].data_ptr())
+                                   dh=st['dh'].data_ptr(), dc=_lib.ptr(st['dc']), err=b['err'].data_ptr(),
+                                   **self._grad_state(t))
         # look-ahead: the heads gradient and the operand images of step t - 1 do not depend on the recursion; they are
         # launched on the library's side stream before step t and overlap its tensor-core kernels
         nxt = step_io(T - 1) if T > 0 else None
@@ -921,8 +891,7 @@ class Trainer(object):
         nbytes = lambda k: int(lib.ic3_ff_grad_workspace_bytes(C.byref(self._ff_plan(cfg, None, k * rows))))
         one = nbytes(1)
         per_step = max(1, nbytes(2) - one)
-        free, _ = torch.cuda.mem_get_info(e.device)
-        free += torch.cuda.memory_reserved(e.device) - torch.cuda.memory_allocated(e.device)
+        free = self._device_bytes_free()
         k = max(1, min(T, (free - self.RECORD_MARGIN_BYTES - one) // per_step + 1, self.FF_CHUNK_ROWS // rows))
         if self.FF_CHUNK_STEPS is not None:
             k = max(1, min(k, int(self.FF_CHUNK_STEPS)))
@@ -936,8 +905,7 @@ class Trainer(object):
         lib = _lib.load()
         T, B, N = b['T'], e.nenvs, args.nagents
         s = _lib.stream()
-        cfg = net.policy_cfg(B)
-        cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
+        cfg = self._policy_cfg()
         w = net.packed()
         K = self._ff_chunk_steps(T, cfg)
         plan = self._ff_plan(cfg, w, K * B * N)
@@ -947,20 +915,15 @@ class Trainer(object):
         ws = torch.empty(nbytes, dtype=torch.uint8, device=e.device)     # stream-ordered: freed after the kernels ran
         plan.workspace = ws.data_ptr()
         losses = torch.zeros(3, dtype=torch.float64, device=e.device)
-        hard = bool(args.hard_attn) and bool(args.commnet)
         adv = adv.contiguous()
         _lib.check(lib.ic3_ff_grad_begin(C.byref(plan), s))
         for t in range(0, T, K):
             io = _lib.FfGradIO(nsteps=min(K, T - t), fresh=b['s_fresh'][t].data_ptr(),
-                               comm=b['s_comm'][t].data_ptr() if hard else None, alive=b['s_alive'][t].data_ptr(),
-                               pp_loc=None if self.is_tj else b['s_loc'][t].data_ptr(),
-                               tj_loc=b['s_tjloc'][t].data_ptr() if self.is_tj else None,
-                               tj_alive=b['s_tjalive'][t].data_ptr() if self.is_tj else None,
-                               tj_last_act=b['s_tjlast'][t].data_ptr() if self.is_tj else None,
-                               tj_route_id=b['s_tjroute'][t].data_ptr() if self.is_tj else None,
+                               comm=b['s_comm'][t].data_ptr() if self.hard else None, alive=b['s_alive'][t].data_ptr(),
                                logp=b['logp'][t].data_ptr(), action=b['action'][t].data_ptr(),
                                value=b['value'][t].data_ptr(), ret=ret[t].data_ptr(), adv=adv[t].data_ptr(),
-                               alive_post=b['ralive'][t].data_ptr(), valid=b['valid'][t].data_ptr())
+                               alive_post=b['ralive'][t].data_ptr(), valid=b['valid'][t].data_ptr(),
+                               **self._grad_state(t))
             _lib.check(lib.ic3_ff_grad_chunk(C.byref(plan), C.byref(io), s))
         params, grads = self._param_structs()
         _lib.check(lib.ic3_ff_grad_finish(C.byref(plan), C.byref(params), C.byref(grads), losses.data_ptr(), s))
@@ -977,46 +940,37 @@ class Trainer(object):
         inputs the env step no longer records; those rows carry no loss and no gradient.
         The tanh RNN (h alone, c is None): the index encoder from the recorded env state into the rollout's x buffer,
         then the SIMT policy step, the same kernels and operands as the rollout."""
-        b, e, net, args = self._buf, self.env.env, self.policy_net, self.args
+        b, e, net = self._buf, self.env.env, self.policy_net
         lib = _lib.load()
         B, W = e.nenvs, self.grad_window
         t0, t1 = k * W, min(b['T'], (k + 1) * W)
-        cfg = net.policy_cfg(B)
-        cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
+        cfg = self._policy_cfg()
         w = net.packed()
         nb = self._window_buffers()
         s = _lib.stream()
-        if self._h_only_records():
-            wh = b['win_h'][k % nb]
-            enc = lib.ic3_tj_encoder_index if self.is_tj else lib.ic3_pp_encoder_index
-            for t in range(t0, t1):
-                j = t - t0
-                hin = b['ck_h'][k] if j == 0 else wh[j - 1]
-                ecfg, est = self._record_state(t)
-                _lib.check(enc(C.byref(ecfg), C.byref(est), C.byref(cfg), C.byref(w), b['x'].data_ptr(), s))
-                io = _lib.PolicyIO(x=b['x'].data_ptr(), h=hin.data_ptr(), c=None, comm_action=None,
-                                   alive=b['s_alive'][t].data_ptr(), fresh=b['s_fresh'][t].data_ptr(), tick=None,
-                                   draws=None, h_out=wh[j].data_ptr(), c_out=None, value=b['win_value'].data_ptr(),
-                                   logp=b['win_logp'].data_ptr(), action=None, workspace=None, err=b['err'].data_ptr())
-                _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
-            return wh[:t1 - t0], None
-        table = self._encoder_table()
+        hc = not self._h_only_records()
+        wh, wc = b['win_h'][k % nb], b['win_c'][k % nb] if hc else None
+        table = self._encoder_table() if hc else None
+        enc = lib.ic3_tj_encoder_index if self.is_tj else lib.ic3_pp_encoder_index
         ws, _ = net.workspace(B)
-        hard = bool(args.hard_attn) and bool(args.commnet)
-        wh, wc = b['win_h'][k % nb], b['win_c'][k % nb]
         for t in range(t0, t1):
             j = t - t0
-            hin, cin = (b['ck_h'][k], b['ck_c'][k]) if j == 0 else (wh[j - 1], wc[j - 1])
+            hin = b['ck_h'][k] if j == 0 else wh[j - 1]
+            cin = None if not hc else b['ck_c'][k] if j == 0 else wc[j - 1]
             ecfg, est = self._record_state(t)          # held until the policy step below has read them
-            src = _lib.env_source(ecfg, est)
-            io = _lib.PolicyIO(x=None, h=hin.data_ptr(), c=cin.data_ptr(),
-                               comm_action=b['s_comm'][t].data_ptr() if hard else None,
+            if hc:       # the fused index encoder with the per-position table
+                src = dict(_lib.env_source(ecfg, est), x=None, x_table=table.data_ptr())
+            else:        # the index encoder into the rollout's x buffer
+                _lib.check(enc(C.byref(ecfg), C.byref(est), C.byref(cfg), C.byref(w), b['x'].data_ptr(), s))
+                src = dict(x=b['x'].data_ptr())
+            io = _lib.PolicyIO(h=hin.data_ptr(), c=_lib.ptr(cin),
+                               comm_action=b['s_comm'][t].data_ptr() if self.hard else None,
                                alive=b['s_alive'][t].data_ptr(), fresh=b['s_fresh'][t].data_ptr(), tick=None,
-                               draws=None, h_out=wh[j].data_ptr(), c_out=wc[j].data_ptr(),
+                               draws=None, h_out=wh[j].data_ptr(), c_out=wc[j].data_ptr() if hc else None,
                                value=b['win_value'].data_ptr(), logp=b['win_logp'].data_ptr(), action=None,
-                               workspace=_lib.ptr(ws), err=b['err'].data_ptr(), x_table=table.data_ptr(), **src)
+                               workspace=_lib.ptr(ws), err=b['err'].data_ptr(), **src)
             _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
-        return wh[:t1 - t0], wc[:t1 - t0]
+        return wh[:t1 - t0], wc[:t1 - t0] if hc else None
 
     def _param_structs(self):
         """ic3_policy_params of the parameters and of their gradient buffers (reference layouts), by kernel role."""
@@ -1046,39 +1000,6 @@ class Trainer(object):
                                      head_w=arr(w['head_w']), head_b=arr(w['head_b']),
                                      c_w_pass=parr(w['c_w']), c_b_pass=parr(w['c_b']), **cell)
         return mk(lambda p: p.data_ptr()), mk(grad_ptr)
-
-    def _compute_grad_manual(self, adv, ret, W, nw):
-        """``args.grad_impl == 'manual'``: the same gradient from the explicit backward formulas of bptt.py (no autograd
-        graph; validated in float64 against the oracle by tests/test_bptt_manual.py).  Opt-in until it has been
-        measured on the GPU."""
-        from . import bptt
-        b, net, args = self._buf, self.policy_net, self.args
-        if getattr(net, 'is_variant', False) or type(net).__name__ != 'CommNetMLP':
-            raise NotImplementedError("grad_impl='manual' covers the recurrent LSTM CommNet / IC3Net with one comm pass")
-        B, N = self.env.env.nenvs, args.nagents
-        T = b['T']
-        P, G = {}, {}
-        for name, p in net.named_parameters():
-            if p.grad is None:
-                p.grad = torch.zeros_like(p)
-            P[name], G[name] = p.detach(), p.grad
-        spec = bptt.Spec(N, args.hid_size, len(args.naction_heads), bool(args.hard_attn) and bool(args.commnet),
-                         getattr(args, 'comm_mode', 'avg') == 'avg', bool(args.comm_mask_zero), args.value_coeff,
-                         args.entr, args.detach_gap, args.max_steps)
-        if self.is_tj:
-            obs_fn = lambda t: self._tj_record_obs(t).reshape(B * N, -1)
-        else:
-            obs_fn = lambda t: self._pp_sparse_obs(b['s_loc'][t])
-        rec = dict(fresh=b['s_fresh'], comm=b['s_comm'], alive=b['s_alive'], t_ep=b['s_tep'], action=b['action'],
-                   alive_post=b['ralive'], obs=obs_fn, valid=b['valid'])
-        tot = dict(action_loss=0.0, value_loss=0.0, entropy=0.0)
-        dh = dc = None
-        for k in reversed(range(nw)):
-            t0, t1 = k * W, min(T, (k + 1) * W)
-            dh, dc, st = bptt.window_backward(P, G, spec, rec, t0, t1, b['ck_h'][k], b['ck_c'][k], adv, ret, dh, dc)
-            for key in tot:
-                tot[key] += st[key]
-        return tot
 
     # only used when there is a single process (trainer.py:245-256)
     def train_batch(self, epoch):

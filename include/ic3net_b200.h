@@ -420,7 +420,9 @@ int ic3_stat_reduce(int32_t B, int32_t N, const int32_t* stat_episodes, const in
  * included; cfg->cell == IC3_CELL_LSTM, no x_tanh / h_from_x), and the tanh recurrence without communication
  * (models.RNN with rnn_type 'MLP', the IC / IRIC baselines: cfg->cell == IC3_CELL_TANH, one pass, comm_mask_zero,
  * no hard_attn, no x_tanh / h_from_x; SIMT-packed weights, f_w_pass[0] / f_b_pass[0] in params and grads; no c:
- * c_prev / dc may be NULL and c_abs_max is ignored).  Every other configuration gets a workspace of 0 bytes.
+ * c_prev / dc may be NULL and c_abs_max is ignored); always with the environment's observation layout hint
+ * (cfg->obs_vocab > 0), a window of at most 5 x 5 cells and an observation pattern of at most 512 columns.  Every other
+ * configuration gets a workspace of 0 bytes.
  * The host walks the lock-step iterations t = T-1 .. 0:
  *     ic3_bptt_begin(plan, max |c| of the record, stream)
  *     for t in reversed(range(T)): ic3_bptt_step(plan, &io_t, stream)
@@ -450,7 +452,7 @@ typedef struct {
 typedef struct {
   int32_t t;                    /* lock-step index (the parity of the unit counter t * passes + p selects the
                                    operand-image set of unit (t, p)) */
-  int32_t pass_index;           /* callers pass 0: the library walks the passes of step t itself */
+  int32_t reserved0;
   /* state entering / leaving policy step t */
   const float* h_prev;          /* [B*N, H] h_{t-1} as fed to the step (ignored for fresh slots) */
   const float* c_prev;          /* [B*N, H] */
@@ -460,12 +462,10 @@ typedef struct {
   const uint8_t* comm;          /* [B, N] info['comm_action'] (required with hard_attn) */
   const uint8_t* alive;         /* [B, N] info['alive_mask'] or NULL */
   const uint8_t* cut;           /* [B] or NULL: (h', c') of step t were detached, (t_ep + 1) % detach_gap == 0 (trainer.py:56-60) */
-  /* environment state the observation of step t was taken from */
-  const int32_t* pp_loc;        /* [B, N+1, 2] */
-  const int32_t* tj_loc;        /* [B, N, 2] */
-  const uint8_t* tj_alive;      /* [B, N] */
-  const uint8_t* tj_last_act;   /* [B, N] */
-  const int32_t* tj_route_id;   /* [B, N] */
+  /* environment state the observation of step t was taken from (HOST pointer to a struct of device pointers; the one
+     matching the plan's env): predator-prey reads loc, traffic junction loc / alive / last_act / route_id */
+  const ic3_pp_state* pp_state;
+  const ic3_tj_state* tj_state;
   /* outputs of step t and their learning signals */
   const float* logp;            /* [B*N, sum(na)] */
   const int32_t* action;        /* [B*N, nheads] */
@@ -536,11 +536,9 @@ typedef struct {
   const uint8_t* fresh;         /* [K, B] */
   const uint8_t* comm;          /* [K, B, N] info['comm_action'] (required with hard_attn) */
   const uint8_t* alive;         /* [K, B, N] info['alive_mask'] or NULL */
-  const int32_t* pp_loc;        /* [K, B, N+1, 2] */
-  const int32_t* tj_loc;        /* [K, B, N, 2] */
-  const uint8_t* tj_alive;      /* [K, B, N] */
-  const uint8_t* tj_last_act;   /* [K, B, N] */
-  const int32_t* tj_route_id;   /* [K, B, N] */
+  /* recorded environment state as in ic3_bptt_step_io, each field [K, ...] (loc [K, B, N+1, 2] / [K, B, N, 2]) */
+  const ic3_pp_state* pp_state;
+  const ic3_tj_state* tj_state;
   const float* logp;            /* [K*B*N, sum(na)] */
   const int32_t* action;        /* [K*B*N, nheads] */
   const float* value;           /* [K*B*N] */

@@ -38,7 +38,8 @@ def test_struct_sizes_match_header(built_lib):
     names = {"ic3_pp_cfg": _lib.PPCfg, "ic3_pp_state": _lib.PPState, "ic3_rollout_io": _lib.RolloutIO,
              "ic3_tj_cfg": _lib.TJCfg, "ic3_tj_state": _lib.TJState, "ic3_policy_cfg": _lib.PolicyCfg,
              "ic3_policy_params": _lib.PolicyParams, "ic3_policy_packed": _lib.PolicyPacked,
-             "ic3_policy_io": _lib.PolicyIO, "ic3_bptt_plan": _lib.BpttPlan, "ic3_bptt_step_io": _lib.BpttStepIO}
+             "ic3_policy_io": _lib.PolicyIO, "ic3_bptt_plan": _lib.BpttPlan, "ic3_bptt_step_io": _lib.BpttStepIO,
+             "ic3_ff_grad_plan": _lib.FfGradPlan, "ic3_ff_grad_io": _lib.FfGradIO}
     prog = '#include <stdio.h>\n#include "ic3net_b200.h"\nint main(){' + "".join(
         'printf("%s %%zu\\n", sizeof(%s));' % (n, n) for n in names) + "return 0;}"
     with tempfile.TemporaryDirectory() as d:

@@ -74,8 +74,9 @@ def test_entry_points_check_arguments_before_device_work():
     plan.w = C.pointer(w)
     assert lib.ic3_ff_grad_chunk(C.byref(plan), None, None) == E_NULL
     assert lib.ic3_ff_grad_chunk(C.byref(plan), C.byref(io), None) == E_NULL  # no records
+    st = _lib.PPState(loc=0x1000)
     fake = dict(fresh=0x1000, logp=0x1000, action=0x1000, value=0x1000, ret=0x1000, adv=0x1000, alive_post=0x1000,
-                pp_loc=0x1000, comm=0x1000)
+                pp_state=C.pointer(st), comm=0x1000)
     assert lib.ic3_ff_grad_chunk(C.byref(plan), C.byref(_lib.FfGradIO(nsteps=2, **fake)), None) == E_RANGE  # > capacity
     assert lib.ic3_ff_grad_chunk(C.byref(plan), C.byref(_lib.FfGradIO(nsteps=0, **fake)), None) == E_RANGE
     assert lib.ic3_ff_grad_finish(C.byref(plan), None, None, None, None) == E_NULL

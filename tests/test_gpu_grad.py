@@ -39,7 +39,7 @@ def test_returns_scan_matches_oracle():
 
 
 @pytest.mark.parametrize("name", golden_names("grad_"))
-@pytest.mark.parametrize("impl,grad_impl", [("tc", "kernels"), ("tc", "autograd"), ("tc", "manual"), ("simt", "autograd")])
+@pytest.mark.parametrize("impl,grad_impl", [("tc", "kernels"), ("tc", "autograd"), ("simt", "autograd")])
 def test_compute_grad_matches_oracle(name, impl, grad_impl):
     from ic3net_b200 import data
     from ic3net_b200.comm import CommNetMLP
@@ -100,6 +100,22 @@ def test_train_batch_updates_parameters():
         assert c == (not n.startswith("hidd_encoder")), n      # the unused module gets no gradient (comm.py:57)
     stat2 = tr.train_batch(1)                                  # re-packed weights, second update runs
     assert 64 * args.batch_size <= stat2["num_steps"] <= 64 * tr.steps_per_batch()
+
+
+@pytest.mark.parametrize("grad_impl", ["manual", "kernel"])
+def test_unknown_grad_impl_is_refused(grad_impl):
+    """A grad_impl the Trainer does not implement is an error, not a silent autograd recompute."""
+    from ic3net_b200 import data
+    from ic3net_b200.comm import CommNetMLP
+    from ic3net_b200.trainer import Trainer
+    meta, _ = load_golden("grad_pp_easy_ic3net")
+    args = ns(meta["args"], nenvs=2, seed=3, env_id0=0, obs_mode="index", use_graph=False, record_for_grad=True,
+              grad_impl=grad_impl)
+    env = data.init(args.env_name, args)
+    finish_args(args, env)
+    net = CommNetMLP(args, args.num_inputs)
+    with pytest.raises(ValueError, match="grad_impl"):
+        Trainer(args, net, env)
 
 
 @pytest.mark.parametrize("grad_impl", ["auto", "autograd"])
