@@ -19,6 +19,7 @@ MAX_PASSES = 4
 RANDOM_WORDS = 16
 CELL_LSTM, CELL_TANH = 0, 1
 LSTM_IMG_BYTES = 786432
+RNN_IMG_BYTES = 65536
 
 ERR_EPISODE_DONE = 1
 ERR_ROUTE_OVERRUN = 2
@@ -82,7 +83,8 @@ class PolicyParams(C.Structure):
 
 class PolicyPacked(C.Structure):
     _fields_ = [("enc_wT", _p), ("enc_b", _p), ("c_wT", _p), ("c_b", _p), ("lstm_wT", _p), ("lstm_b", _p),
-                ("head_w", _p), ("head_b", _p), ("lstm_img", _p), ("bias_cat", _p), ("f_wT", _p), ("f_b", _p), ("flags", _p)]
+                ("head_w", _p), ("head_b", _p), ("lstm_img", _p), ("bias_cat", _p), ("f_wT", _p), ("f_b", _p), ("flags", _p),
+                ("rnn_img", _p)]
 
 
 class PolicyIO(C.Structure):

@@ -119,14 +119,21 @@ class CommNetMLP(nn.Module):
         self._packed = None
         self._packed_key = None
         # 'tc' = wgmma tensor-core path (csrc/policy_tc.cu: hid_size 128, LSTM cell on the encoded observation, any
-        # number of comm passes), 'simt' = fp32 CUDA-core kernel (every variant)
+        # number of comm passes), 'simt' = fp32 CUDA-core kernel (every variant), 'tc_tanh' = wgmma step of the tanh RNN
+        # without communication (csrc/rnn_tc.cu: models.RNN with the vanilla recurrence, hid_size 128); opt-in
         self.tc_capable = (var['cell'] == _lib.CELL_LSTM and not var['x_tanh'] and not var['h_from_x'])
         want = getattr(args, 'policy_impl', None)
         self.policy_impl = want or ('tc' if (H == 128 and self.tc_capable) else 'simt')
-        if self.policy_impl not in ('tc', 'simt'):
-            raise ValueError("policy_impl must be 'tc' or 'simt'")
-        if self.policy_impl == 'tc' and H != 128:
+        if self.policy_impl not in ('tc', 'simt', 'tc_tanh'):
+            raise ValueError("policy_impl must be 'tc', 'simt' or 'tc_tanh'")
+        if self.policy_impl != 'simt' and H != 128:
             raise NotImplementedError("the tensor-core policy path is specialised for hid_size 128")
+        if self.policy_impl == 'tc_tanh' and not (var['cell'] == _lib.CELL_TANH and var['passes'] == 1 and
+                                                  args.comm_mask_zero and not args.hard_attn and
+                                                  not var['x_tanh'] and not var['h_from_x']):
+            raise NotImplementedError("policy_impl='tc_tanh' implements the tanh RNN without communication (models.RNN "
+                                      "with rnn_type 'MLP': the IC / IRIC baselines); LSTM cells run on 'tc', models.MLP "
+                                      "and the non-recurrent CommNet / IC3Net on 'simt'")
         if self.policy_impl == 'tc' and not self.tc_capable:
             raise NotImplementedError("the tensor-core policy path implements the recurrent LSTM policy; the tanh-cell "
                                       "variants run on policy_impl='simt'")
@@ -168,8 +175,8 @@ class CommNetMLP(nn.Module):
         return _lib.PolicyCfg(B=B, **self._cfg_proto)
 
     def workspace(self, B):
-        """(scratch, err) tensors of the tensor-core path for a batch of B envs (None, None for 'simt')."""
-        if self.policy_impl != 'tc':
+        """(scratch, err) tensors of the tensor-core paths for a batch of B envs (None, None for 'simt')."""
+        if self.policy_impl == 'simt':
             return None, None
         if B not in self._ws:
             cfg = self.policy_cfg(B)
@@ -226,6 +233,9 @@ class CommNetMLP(nn.Module):
             if self.policy_impl == 'tc':
                 self._bufs['lstm_img'] = torch.empty(P * _lib.LSTM_IMG_BYTES, dtype=torch.uint8, device=dev)   # one per pass
                 self._bufs['bias_cat'] = torch.empty(P, 4 * H, device=dev)
+                self._bufs['flags'] = torch.zeros(1, dtype=torch.int32, device=dev)
+            if self.policy_impl == 'tc_tanh':
+                self._bufs['rnn_img'] = torch.empty(_lib.RNN_IMG_BYTES, dtype=torch.uint8, device=dev)
                 self._bufs['flags'] = torch.zeros(1, dtype=torch.int32, device=dev)
             self._packed = _lib.PolicyPacked(**{k: v.data_ptr() for k, v in self._bufs.items()})
         for p in ps:

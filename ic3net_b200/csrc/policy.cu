@@ -656,11 +656,13 @@ extern "C" int ic3_policy_pack(const ic3_policy_cfg* cfg, const ic3_policy_param
     for (int i = 0; i < (cfg->passes > 1 ? cfg->passes : 1); ++i)
       if (!p->f_w_pass[i] || !p->f_b_pass[i]) return IC3_E_NULL;
   }
-  if (!policy_tc_capable(cfg) && (out->lstm_img || out->bias_cat)) return IC3_E_UNSUPPORTED;  // tanh cells: SIMT kernel only
+  if (!policy_tc_capable(cfg) && (out->lstm_img || out->bias_cat)) return IC3_E_UNSUPPORTED;  // LSTM operand images
+  if (out->rnn_img && !ic3_rnn_tc_capable(cfg)) return IC3_E_UNSUPPORTED;                     // tanh RNN weight image
   for (int k = 0; k < cfg->nheads; ++k)
     if (!p->head_w[k] || !p->head_b[k]) return IC3_E_NULL;
   pack_kernel<<<296, 256, 0, (cudaStream_t)stream>>>(*cfg, *p, *out);
   IC3_LAUNCH_CHECK();
+  if (out->rnn_img) return ic3_rnn_tc_pack(cfg, p, out, (cudaStream_t)stream);
   if (out->lstm_img || out->bias_cat) {   // tensor-core operand images
     if (!out->lstm_img || !out->bias_cat) return IC3_E_NULL;
     return ic3_tc_pack(cfg, p, out, (cudaStream_t)stream);
@@ -668,7 +670,11 @@ extern "C" int ic3_policy_pack(const ic3_policy_cfg* cfg, const ic3_policy_param
   return IC3_OK;
 }
 
-extern "C" uint64_t ic3_policy_workspace_bytes(const ic3_policy_cfg* cfg) { return ic3_tc_workspace_bytes(cfg); }
+extern "C" uint64_t ic3_policy_workspace_bytes(const ic3_policy_cfg* cfg) {
+  // the tanh RNN's tensor-core step stages nothing through HBM; a non-NULL io->workspace is what selects it
+  if (cfg && ic3_rnn_tc_capable(cfg)) return 16;
+  return ic3_tc_workspace_bytes(cfg);
+}
 
 int ic3_encoder_check(const ic3_policy_cfg* cfg, const ic3_policy_packed* w) {
   const int rc = policy_check(cfg);
@@ -790,6 +796,8 @@ extern "C" int ic3_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packe
   if (cfg->cell == IC3_CELL_LSTM && (!io->c || !io->c_out)) return IC3_E_NULL;
   if (cfg->hard_attn && !io->comm_action) return IC3_E_NULL;
   if (cfg->N > ROWS) return IC3_E_RANGE;
+  if (io->workspace && w->rnn_img)        // tensor-core path of the tanh RNN (rnn_tc.cu)
+    return ic3_rnn_tc_policy_step(cfg, w, io, (cudaStream_t)stream);
   if (io->workspace && w->lstm_img) {     // tensor-core path (policy_tc.cu); otherwise the fp32 SIMT kernel below
     if (!policy_tc_capable(cfg)) return IC3_E_UNSUPPORTED;
     return ic3_tc_policy_step(cfg, w, io, (cudaStream_t)stream);

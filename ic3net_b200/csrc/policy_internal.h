@@ -10,6 +10,13 @@ int ic3_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3
 int ic3_tc_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, cudaStream_t s);
 int ic3_tc_pass_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, int npasses,
                        float* h_pass, float* c_pass, cudaStream_t s);
+// tensor-core step of the tanh RNN without communication (rnn_tc.cu): the configurations it covers, its weight image
+// (ic3_policy_packed.rnn_img) and the step itself
+bool ic3_rnn_tc_capable(const ic3_policy_cfg* cfg);
+int ic3_rnn_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3_policy_packed* out, cudaStream_t s);
+int ic3_rnn_tc_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, cudaStream_t s);
+// timing hook of ic3_policy_step_profile: records event i (0 .. 3) on s while a profiled step runs, else nothing
+void ic3_prof_mark(int i, cudaStream_t s);
 // grid of a persistent kernel `kern` (threads per CTA, dynamic shared memory smem) over nwork items that runs beside the
 // tensor-core LSTM kernel: min(nwork, SMs x the CTAs of kern that fit on one SM next to a resident lstm_tc_kernel CTA --
 // registers, shared memory, threads, CTA slots -- at least one per SM)

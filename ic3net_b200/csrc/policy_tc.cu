@@ -136,9 +136,10 @@ int ic3_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3
 // Per-kernel timing hook (ic3_policy_step_profile): when set, events are recorded on the stream before the first
 // kernel of the step and after each of its kernels.  Host-side only; nullptr in normal operation.
 static cudaEvent_t* g_prof_ev = nullptr;
-static inline void prof_mark(int i, cudaStream_t s) {
+void ic3_prof_mark(int i, cudaStream_t s) {
   if (g_prof_ev) cudaEventRecord(g_prof_ev[i], s);
 }
+static inline void prof_mark(int i, cudaStream_t s) { ic3_prof_mark(i, s); }
 
 extern "C" int ic3_policy_step_profile(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,
                                        void* stream, float* ms) {

@@ -415,18 +415,7 @@ __global__ void __launch_bounds__(256) prep_kernel(ic3_policy_cfg cfg, ic3_polic
 // 1e-5 budget of the hidden state (tests/test_gpu_policy.py, tests/test_gpu_rollout.py).  The epilogue is the
 // pacing stage of the kernel, so the forms are chosen for instruction count: the argument arrives already scaled
 // by -log2(e) (folded into the accumulator scale and the shared-memory bias copy), and both functions are
-// 1 / (1 + 2^t), see lstm_cell4.
-__device__ __forceinline__ float ex2_fast(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ float rcp_fast(float x) {
-  float y;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-constexpr float LOG2E = 1.4426950408889634f;
+// 1 / (1 + 2^t), see lstm_cell4 (ex2_fast, rcp_fast, LOG2E: tc_common.cuh).
 
 // Gate biases pre-multiplied like the accumulator scale: (i, f, o) * -log2(e), g * -2 log2(e); [4H] in shared memory.
 __device__ __forceinline__ void load_scaled_bias(float* s_bias, const float* __restrict__ bias_cat) {

@@ -939,7 +939,8 @@ class Trainer(object):
         rollout's (h', c') bit for bit -- except for slots that had already completed their batch (valid = 0), whose
         inputs the env step no longer records; those rows carry no loss and no gradient.
         The tanh RNN (h alone, c is None): the index encoder from the recorded env state into the rollout's x buffer,
-        then the SIMT policy step, the same kernels and operands as the rollout."""
+        then the policy step of the rollout's policy_impl ('simt' or 'tc_tanh': the policy's packed weights and workspace
+        select it, as in _enqueue), the same kernels and operands as the rollout."""
         b, e, net = self._buf, self.env.env, self.policy_net
         lib = _lib.load()
         B, W = e.nenvs, self.grad_window
