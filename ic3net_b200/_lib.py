@@ -21,6 +21,11 @@ CELL_LSTM, CELL_TANH = 0, 1
 LSTM_IMG_BYTES = 786432
 RNN_IMG_BYTES = 65536
 
+
+def ff_img_bytes(passes, comm):
+    """Bytes of PolicyPacked.ff_img (IC3_FF_IMG_BYTES): 64 KB per weight matrix (F, and C with communication) and pass."""
+    return max(1, int(passes)) * (131072 if comm else 65536)
+
 ERR_EPISODE_DONE = 1
 ERR_ROUTE_OVERRUN = 2
 ERR_BAD_ACTION = 4
@@ -84,7 +89,7 @@ class PolicyParams(C.Structure):
 class PolicyPacked(C.Structure):
     _fields_ = [("enc_wT", _p), ("enc_b", _p), ("c_wT", _p), ("c_b", _p), ("lstm_wT", _p), ("lstm_b", _p),
                 ("head_w", _p), ("head_b", _p), ("lstm_img", _p), ("bias_cat", _p), ("f_wT", _p), ("f_b", _p), ("flags", _p),
-                ("rnn_img", _p)]
+                ("ff_img", _p), ("rnn_img", _p)]
 
 
 class PolicyIO(C.Structure):

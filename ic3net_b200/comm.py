@@ -120,14 +120,20 @@ class CommNetMLP(nn.Module):
         self._packed_key = None
         # 'tc' = wgmma tensor-core path (csrc/policy_tc.cu: hid_size 128, LSTM cell on the encoded observation, any
         # number of comm passes), 'simt' = fp32 CUDA-core kernel (every variant), 'tc_tanh' = wgmma step of the tanh RNN
-        # without communication (csrc/rnn_tc.cu: models.RNN with the vanilla recurrence, hid_size 128); opt-in
+        # without communication (csrc/rnn_tc.cu: models.RNN with the vanilla recurrence, hid_size 128); opt-in;
+        # 'tc_ff' = wgmma step of the non-recurrent tanh policies (csrc/ff_tc.cu: models.MLP, CommNet / IC3Net without
+        # --recurrent, hid_size 128); opt-in
         self.tc_capable = (var['cell'] == _lib.CELL_LSTM and not var['x_tanh'] and not var['h_from_x'])
         want = getattr(args, 'policy_impl', None)
         self.policy_impl = want or ('tc' if (H == 128 and self.tc_capable) else 'simt')
-        if self.policy_impl not in ('tc', 'simt', 'tc_tanh'):
-            raise ValueError("policy_impl must be 'tc', 'simt' or 'tc_tanh'")
+        if self.policy_impl not in ('tc', 'simt', 'tc_tanh', 'tc_ff'):
+            raise ValueError("policy_impl must be 'tc', 'simt', 'tc_tanh' or 'tc_ff'")
         if self.policy_impl != 'simt' and H != 128:
             raise NotImplementedError("the tensor-core policy path is specialised for hid_size 128")
+        if self.policy_impl == 'tc_ff' and not (var['cell'] == _lib.CELL_TANH and var['x_tanh'] and var['h_from_x']):
+            raise NotImplementedError("policy_impl='tc_ff' implements the non-recurrent tanh step (models.MLP, CommNet / "
+                                      "IC3Net without --recurrent); recurrent LSTM cells run on 'tc', the tanh RNN "
+                                      "(IC / IRIC) on 'tc_tanh'")
         if self.policy_impl == 'tc_tanh' and not (var['cell'] == _lib.CELL_TANH and var['passes'] == 1 and
                                                   args.comm_mask_zero and not args.hard_attn and
                                                   not var['x_tanh'] and not var['h_from_x']):
@@ -236,6 +242,10 @@ class CommNetMLP(nn.Module):
                 self._bufs['flags'] = torch.zeros(1, dtype=torch.int32, device=dev)
             if self.policy_impl == 'tc_tanh':
                 self._bufs['rnn_img'] = torch.empty(_lib.RNN_IMG_BYTES, dtype=torch.uint8, device=dev)
+                self._bufs['flags'] = torch.zeros(1, dtype=torch.int32, device=dev)
+            if self.policy_impl == 'tc_ff':         # one F (and C) image per pass
+                nbytes = _lib.ff_img_bytes(P, not self._cfg_proto['comm_mask_zero'])
+                self._bufs['ff_img'] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
                 self._bufs['flags'] = torch.zeros(1, dtype=torch.int32, device=dev)
             self._packed = _lib.PolicyPacked(**{k: v.data_ptr() for k, v in self._bufs.items()})
         for p in ps:

@@ -658,11 +658,13 @@ extern "C" int ic3_policy_pack(const ic3_policy_cfg* cfg, const ic3_policy_param
   }
   if (!policy_tc_capable(cfg) && (out->lstm_img || out->bias_cat)) return IC3_E_UNSUPPORTED;  // LSTM operand images
   if (out->rnn_img && !ic3_rnn_tc_capable(cfg)) return IC3_E_UNSUPPORTED;                     // tanh RNN weight image
+  if (out->ff_img && !ic3_ff_tc_capable(cfg)) return IC3_E_UNSUPPORTED;                       // non-recurrent tanh image
   for (int k = 0; k < cfg->nheads; ++k)
     if (!p->head_w[k] || !p->head_b[k]) return IC3_E_NULL;
   pack_kernel<<<296, 256, 0, (cudaStream_t)stream>>>(*cfg, *p, *out);
   IC3_LAUNCH_CHECK();
   if (out->rnn_img) return ic3_rnn_tc_pack(cfg, p, out, (cudaStream_t)stream);
+  if (out->ff_img) return ic3_ff_tc_pack(cfg, p, out, (cudaStream_t)stream);
   if (out->lstm_img || out->bias_cat) {   // tensor-core operand images
     if (!out->lstm_img || !out->bias_cat) return IC3_E_NULL;
     return ic3_tc_pack(cfg, p, out, (cudaStream_t)stream);
@@ -673,6 +675,7 @@ extern "C" int ic3_policy_pack(const ic3_policy_cfg* cfg, const ic3_policy_param
 extern "C" uint64_t ic3_policy_workspace_bytes(const ic3_policy_cfg* cfg) {
   // the tanh RNN's tensor-core step stages nothing through HBM; a non-NULL io->workspace is what selects it
   if (cfg && ic3_rnn_tc_capable(cfg)) return 16;
+  if (cfg && ic3_ff_tc_capable(cfg)) return ic3_ff_tc_workspace_bytes(cfg);   // non-recurrent tanh step: h between passes
   return ic3_tc_workspace_bytes(cfg);
 }
 
@@ -798,6 +801,8 @@ extern "C" int ic3_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packe
   if (cfg->N > ROWS) return IC3_E_RANGE;
   if (io->workspace && w->rnn_img)        // tensor-core path of the tanh RNN (rnn_tc.cu)
     return ic3_rnn_tc_policy_step(cfg, w, io, (cudaStream_t)stream);
+  if (io->workspace && w->ff_img)         // tensor-core path of the non-recurrent tanh step (ff_tc.cu)
+    return ic3_ff_tc_policy_step(cfg, w, io, (cudaStream_t)stream);
   if (io->workspace && w->lstm_img) {     // tensor-core path (policy_tc.cu); otherwise the fp32 SIMT kernel below
     if (!policy_tc_capable(cfg)) return IC3_E_UNSUPPORTED;
     return ic3_tc_policy_step(cfg, w, io, (cudaStream_t)stream);
@@ -818,6 +823,8 @@ extern "C" int ic3_policy_ff_states(const ic3_policy_cfg* cfg, const ic3_policy_
   if (cfg->hard_attn && !io->comm_action) return IC3_E_NULL;
   if (cfg->cell != IC3_CELL_TANH || !cfg->h_from_x || cfg->H != 128 || cfg->N > ROWS) return IC3_E_UNSUPPORTED;
   if (!w->f_wT || !w->f_b) return IC3_E_NULL;
+  if (w->ff_img)                          // the rollout's tensor-core step (ff_tc.cu), in its pass-state form
+    return ic3_ff_tc_states(cfg, w, io, st_h, st_s, (cudaStream_t)stream);
   PolicyArgs a{*cfg, *w, *io, st_h, st_s};
   return launch_policy<128, true>(a, (cudaStream_t)stream);
 }

@@ -15,6 +15,14 @@ int ic3_tc_pass_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, co
 bool ic3_rnn_tc_capable(const ic3_policy_cfg* cfg);
 int ic3_rnn_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3_policy_packed* out, cudaStream_t s);
 int ic3_rnn_tc_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, cudaStream_t s);
+// tensor-core step of the non-recurrent tanh policies (ff_tc.cu): the configurations it covers, its scratch, its weight
+// image (ic3_policy_packed.ff_img), the step and its pass-state form
+bool ic3_ff_tc_capable(const ic3_policy_cfg* cfg);
+uint64_t ic3_ff_tc_workspace_bytes(const ic3_policy_cfg* cfg);
+int ic3_ff_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3_policy_packed* out, cudaStream_t s);
+int ic3_ff_tc_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, cudaStream_t s);
+int ic3_ff_tc_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, float* st_h,
+                     float* st_s, cudaStream_t s);
 // timing hook of ic3_policy_step_profile: records event i (0 .. 3) on s while a profiled step runs, else nothing
 void ic3_prof_mark(int i, cudaStream_t s);
 // grid of a persistent kernel `kern` (threads per CTA, dynamic shared memory smem) over nwork items that runs beside the

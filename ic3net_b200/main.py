@@ -6,7 +6,7 @@
 Every reference flag is accepted with its meaning; flags of subsystems outside the accelerated
 path (``--plot``/visdom, ``--display``/curses) are
 parsed and rejected with a clear message.  New flags: ``--nenvs`` (environment slots per GPU),
-``--obs_mode`` (index | dense), ``--policy_impl`` (tc | simt | tc_tanh), ``--use_graph``.
+``--obs_mode`` (index | dense), ``--policy_impl`` (tc | simt | tc_tanh | tc_ff), ``--use_graph``.
 Multi-GPU: launch with ``python -m torch.distributed.run --nproc-per-node N -m ic3net_b200.main ...``.
 """
 import argparse
@@ -80,9 +80,11 @@ def build_parser():
     parser.add_argument('--obs_api', default='dense', choices=['dense', 'handle'],
                         help='what env.reset/step hand back: the dense [nenvs,N,obs_dim] tensor, or a LazyObs handle on the '
                              'env state that CommNetMLP.forward consumes directly (lazy_obs.py)')
-    parser.add_argument('--policy_impl', default=None, choices=['tc', 'simt', 'tc_tanh'],
+    parser.add_argument('--policy_impl', default=None, choices=['tc', 'simt', 'tc_tanh', 'tc_ff'],
                         help='wgmma tensor-core or fp32 SIMT policy kernels; tc_tanh: the tensor-core step of the '
-                             'tanh RNN (IC / IRIC: --recurrent without --commnet, hid_size 128)')
+                             'tanh RNN (IC / IRIC: --recurrent without --commnet, hid_size 128); tc_ff: the tensor-core '
+                             'step of the non-recurrent tanh policies (MLP, CommNet / IC3Net without --recurrent, '
+                             'hid_size 128)')
     parser.add_argument('--grad_impl', default='auto', choices=['auto', 'kernels', 'kernels_ff', 'autograd'],
                         help='compute_grad: hand-written BPTT kernels (auto: whenever the configuration allows), the '
                              'hand-written kernels of the non-recurrent tanh policies (models.MLP, CommNet / IC3Net '

@@ -287,6 +287,13 @@ typedef struct {
   float* f_b;
   int32_t* flags;  /* device word written by ic3_policy_pack (IC3_ERR_FP16_RANGE when a folded weight does not fit the
                       operand split), OR-ed into ic3_policy_io.err by every policy step; may be NULL */
+  /* tensor-core path of the non-recurrent tanh step (IC3_CELL_TANH, x_tanh, h_from_x, H == 128: models.MLP and
+   * CommNet / IC3Net without --recurrent, 1..4 passes); NULL selects the fp32 SIMT kernel.
+   * ff_img: per pass, the fp16 hi/lo split of 256 * f_p.weight and, unless comm_mask_zero, of 256 * C_p.weight as
+   *   ready-made shared-memory images, [pass][F hi, F lo (, C hi, C lo)][core-matrix layout] =
+   *   IC3_FF_IMG_BYTES(passes, !comm_mask_zero) bytes; |weight| must stay below 255 (flags).  f_wT / f_b / c_wT / c_b
+   *   are packed as well.  (It sits in front of rnn_img, which stays the last member.) */
+  void* ff_img;
   /* tensor-core path of the tanh RNN without communication (IC3_CELL_TANH, one pass, comm_mask_zero, no hard attention,
    * x_tanh = h_from_x = 0, H == 128: models.RNN with the vanilla recurrence); NULL selects the fp32 SIMT kernel.
    * rnn_img: fp16 hi/lo split of 256 * f_0.weight as a ready-made shared-memory image, [hi,lo][core-matrix layout] =
@@ -296,6 +303,8 @@ typedef struct {
 
 #define IC3_LSTM_IMG_BYTES 786432
 #define IC3_RNN_IMG_BYTES 65536
+/* bytes of ic3_policy_packed.ff_img: 64 KB per weight matrix and pass (passes = 0 counts as one) */
+#define IC3_FF_IMG_BYTES(passes, comm) ((size_t)((passes) > 1 ? (passes) : 1) * ((comm) ? 131072u : 65536u))
 
 int ic3_policy_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p,
                     const ic3_policy_packed* out, void* stream);
@@ -357,7 +366,9 @@ typedef struct {
 } ic3_policy_io;
 
 /* Scratch the tensor-core policy path needs for a batch of cfg->B environments (0 when unsupported).  The tanh RNN's
- * tensor-core step needs none and reports a nominal 16 bytes: a non-NULL workspace is what selects the tensor-core path. */
+ * tensor-core step needs none and reports a nominal 16 bytes: a non-NULL workspace is what selects the tensor-core path.
+ * The non-recurrent tanh step (ff_img) reports the same 16 bytes for one pass and one [B*N, H] float32 buffer that
+ * carries h between passes otherwise. */
 uint64_t ic3_policy_workspace_bytes(const ic3_policy_cfg* cfg);
 
 /* One CommNetMLP.forward (recurrent branch, comm_passes = 1) + select_action. */
@@ -366,7 +377,8 @@ int ic3_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const
 /* Measurement aid (bench.py "roofline_tensor"): ic3_policy_step on the tensor-core path with CUDA events between its
  * kernels; synchronises the stream and returns ms[3] = device time of {operand preparation (+ fused encoder),
  * LSTM/comm tensor-core kernel, heads + sampling}.  The tanh RNN's tensor-core step (rnn_img) is one kernel, reported as
- * ms[1]; ms[0] = ms[2] = 0.  Not for the production loop. */
+ * ms[1]; ms[0] = ms[2] = 0.  So is the non-recurrent tanh step (ff_img): ms[1] is its per-pass launches together.  Not
+ * for the production loop. */
 int ic3_policy_step_profile(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,
                             void* stream, float* ms);
 /* The recurrent state after each of the first `npasses` comm passes (1 <= npasses <= cfg->passes) of ic3_policy_step on
@@ -377,11 +389,13 @@ int ic3_policy_step_profile(const ic3_policy_cfg* cfg, const ic3_policy_packed* 
 int ic3_policy_pass_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,
                            int32_t npasses, float* h_pass, float* c_pass, void* stream);
 /* The non-recurrent tanh step (cfg->cell == IC3_CELL_TANH, x_tanh, h_from_x, hid_size 128: models.MLP and the
- * non-recurrent CommNet / IC3Net, comm.py:127-129,179-224, models.py:23-25) on the fp32 SIMT kernel with every pass
- * state written out and no heads: st_h [passes + 1, B*N, H] gets tanh(x) (the state entering pass 0), then h after each
- * pass; st_s [passes, B*N, H] the communication vector of each pass (may be NULL with comm_mask_zero).  Reads io->x,
- * comm_action, alive, fresh.  Same kernel code as ic3_policy_step, so block `passes` of st_h equals its h_out bit for
- * bit.  The non-recurrent backward (ic3_ff_grad_chunk) re-runs the forward this way. */
+ * non-recurrent CommNet / IC3Net, comm.py:127-129,179-224, models.py:23-25) with every pass state written out and no
+ * heads: st_h [passes + 1, B*N, H] gets tanh(x) (the state entering pass 0), then h after each pass; st_s [passes, B*N, H]
+ * the communication vector of each pass (may be NULL with comm_mask_zero).  Reads io->x, comm_action, alive, fresh.
+ * The kernel is the one ic3_policy_step runs for these weights: the fp32 SIMT kernel, or -- when w->ff_img is set -- the
+ * tensor-core step of ff_img in its pass-state form (no workspace needed; io->workspace is not read).  Either way block
+ * `passes` of st_h equals that step's h_out bit for bit.  The non-recurrent backward (ic3_ff_grad_chunk) re-runs the
+ * forward this way. */
 int ic3_policy_ff_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, float* st_h,
                          float* st_s, void* stream);
 /* select_action alone (action_utils.py:32-36) on given log-probabilities. */
