@@ -63,7 +63,11 @@ class TJCfg(C.Structure):
     _fields_ = [("B", C.c_int32), ("N", C.c_int32), ("vision", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
                 ("G", C.c_int32), ("P", C.c_int32), ("Lmax", C.c_int32), ("outside_cls", C.c_int32),
                 ("car_cls", C.c_int32), ("vocab", C.c_int32), ("npath", C.c_int32), ("spawn_thr", C.c_uint32),
-                ("env_id0", C.c_uint32), ("seed", C.c_uint64), ("grid", _p), ("route_len", _p), ("route_cells", _p)]
+                ("env_id0", C.c_uint32), ("seed", C.c_uint64), ("grid", _p), ("route_len", _p), ("route_cells", _p),
+                ("vocab_type", C.c_int32), ("reserved0", C.c_int32)]
+
+
+TJ_VOCAB = {"bool": 0, "scalar": 1}          # TJCfg.vocab_type (IC3_TJ_VOCAB_BOOL / IC3_TJ_VOCAB_SCALAR)
 
 
 class TJState(C.Structure):

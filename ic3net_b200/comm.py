@@ -154,9 +154,10 @@ class CommNetMLP(nn.Module):
 
     def fuses_encoder(self, env):
         """Whether the policy step can form x from the env state itself (the fused index encoder): the tensor-core
-        path, with a vision window of at most 5x5."""
+        path, with a vision window of at most 5x5, on the traffic junction's bool vocabulary only (a scalar-vocabulary
+        env's x comes from the separate index / dense encoder)."""
         W = 2 * env.vision + 1
-        return self.policy_impl == 'tc' and W * W <= 25
+        return self.policy_impl == 'tc' and W * W <= 25 and getattr(env, 'vocab_type', 'bool') == 'bool'
 
     def encoder_table(self, env):
         """[positions, H] class part of x per agent position of env (ic3_*_encoder_table) for the current packed

@@ -69,11 +69,15 @@ __device__ __forceinline__ void pp_encode_row(CellFn cell, int WW, int V, const 
 
 // Traffic-junction row: [last_act, route_id/(npath-1), WW cells x V classes], all zero for a dead car (x = b).
 // cell(w) returns cls | count << 16 (tj_write_obs, tj_env.cu); the car count is feature car_cls > cls.
-template <int H, typename CellFn>
-__device__ __forceinline__ void tj_encode_row(bool alive, float la, float ri, CellFn cell, int WW, int V, int car_cls,
-                                              const float* __restrict__ wT, const float* __restrict__ bias, bool split,
-                                              float* __restrict__ xrow, int lane) {
+// SC (scalar vocabulary, never split: no layout hint): [last_act, route_id/(npath-1), pr, pc, WW cells x (ROAD, CAR)],
+// cell column q is class q + 1, so OUTSIDE has no column and every in-map cell contributes at most its ROAD term.
+template <int H, bool SC, typename CellFn>
+__device__ __forceinline__ void tj_encode_row(bool alive, float la, float ri, float pr, float pc, CellFn cell, int WW,
+                                              int V, int car_cls, const float* __restrict__ wT,
+                                              const float* __restrict__ bias, bool split, float* __restrict__ xrow,
+                                              int lane) {
   constexpr int CPT = H / 32;
+  constexpr int S = SC ? 4 : 2, C0 = SC ? 1 : 0;   // scalar features; class of cell column 0
   float acc[CPT], acc2s[CPT];
 #pragma unroll
   for (int c = 0; c < CPT; ++c) {
@@ -88,13 +92,15 @@ __device__ __forceinline__ void tj_encode_row(bool alive, float la, float ri, Ce
     } else {
       if (la != 0.f) axpy_row<CPT>(acc, la, wT, lane);
       if (ri != 0.f) axpy_row<CPT>(acc, ri, wT + H, lane);
+      if (SC && pr != 0.f) axpy_row<CPT>(acc, pr, wT + 2 * H, lane);
+      if (SC && pc != 0.f) axpy_row<CPT>(acc, pc, wT + 3 * H, lane);
     }
     for (int w = 0; w < WW; ++w) {
       const uint32_t info = cell(w);
       const int cls = (int)(info & 0xffffu), cnt = (int)(info >> 16);
-      const float* wcell = wT + (size_t)(2 + w * V) * H;
-      // dense order: class index ascending; cls < car_cls always (BASE+2)
-      axpy_row<CPT>(acc, 1.f, wcell + (size_t)cls * H, lane);
+      const float* wcell = wT + (size_t)(S + w * V - C0) * H;     // row of class k: wcell + k * H
+      // dense order: class index ascending; cls < car_cls always (BASE+2; scalar: ROAD 1 < CAR 2)
+      if (!SC || cls >= C0) axpy_row<CPT>(acc, 1.f, wcell + (size_t)cls * H, lane);
       if (cnt) {
         if (split) axpy_row<CPT>(acc2s, (float)cnt, wcell + (size_t)car_cls * H, lane);
         else axpy_row<CPT>(acc, (float)cnt, wcell + (size_t)car_cls * H, lane);

@@ -16,6 +16,23 @@
 // predator-prey: agent rows per environment (the prey is row N with --enemy_comm, predator_prey_env.py:203-207)
 __host__ __device__ __forceinline__ int ic3_pp_agents(const ic3_pp_cfg& c) { return c.N + (c.enemy_comm != 0 ? 1 : 0); }
 
+// traffic junction: scalar features in front of a car's window cells (last_act, route id; + row, col in the scalar
+// vocabulary) and the length of its observation row (ic3_tj_cfg.vocab_type)
+__host__ __device__ __forceinline__ int ic3_tj_scalars(const ic3_tj_cfg& c) {
+  return c.vocab_type == IC3_TJ_VOCAB_SCALAR ? 4 : 2;
+}
+__host__ __device__ __forceinline__ int ic3_tj_obs_dim(const ic3_tj_cfg& c) {
+  const int W = 2 * c.vision + 1;
+  return ic3_tj_scalars(c) + W * W * c.vocab;
+}
+// a known vocabulary; the scalar one has fixed classes (OUTSIDE 0, ROAD 1, CAR 2, no BASE: traffic_junction_env.py:139-141)
+// and p_norm divides by h - 1, w - 1 (:344)
+inline int ic3_tj_vocab_check(const ic3_tj_cfg& c) {
+  if (c.vocab_type == IC3_TJ_VOCAB_BOOL) return IC3_OK;
+  if (c.vocab_type != IC3_TJ_VOCAB_SCALAR) return IC3_E_RANGE;
+  return (c.outside_cls == 0 && c.car_cls == 2 && c.vocab == 2 && c.h >= 2 && c.w >= 2) ? IC3_OK : IC3_E_RANGE;
+}
+
 extern unsigned long long g_ic3_launches;  // c_api.cu
 
 #define IC3_LAUNCH_CHECK()                         \

@@ -462,7 +462,7 @@ __global__ void __launch_bounds__(256) pp_encoder_index_kernel(ic3_pp_cfg env, i
   pp_encode_row<H>(cell, W * W, V, wT, bias, split, x + (size_t)row * H, lane);
 }
 
-template <int H>
+template <int H, bool SC>
 __global__ void __launch_bounds__(256) tj_encoder_index_kernel(ic3_tj_cfg env, ic3_tj_state st,
                                                                const float* __restrict__ wT,
                                                                const float* __restrict__ bias, float* __restrict__ x,
@@ -490,7 +490,20 @@ __global__ void __launch_bounds__(256) tj_encoder_index_kernel(ic3_tj_cfg env, i
   const bool alive = st.alive[k] != 0;
   const float la = alive ? (float)st.last_act[k] : 0.f;
   const float ri = alive ? (float)st.route_id[k] / (float)(env.npath - 1) : 0.f;
-  tj_encode_row<H>(alive, la, ri, cell, W * W, V, env.car_cls, wT, bias, split, x + (size_t)row * H, lane);
+  const float pr = SC && alive ? (float)r0 / (float)(env.h - 1) : 0.f;      // p_norm of the scalar vocabulary
+  const float pc = SC && alive ? (float)c0 / (float)(env.w - 1) : 0.f;
+  tj_encode_row<H, SC>(alive, la, ri, pr, pc, cell, W * W, V, env.car_cls, wT, bias, split, x + (size_t)row * H, lane);
+}
+
+template <int H>
+int tj_encoder_index_launch(const ic3_tj_cfg& env, const ic3_tj_state& st, const ic3_policy_packed* w, float* x,
+                            bool split, int grid, cudaStream_t s) {
+  if (env.vocab_type == IC3_TJ_VOCAB_SCALAR)
+    tj_encoder_index_kernel<H, true><<<grid, 256, 0, s>>>(env, st, w->enc_wT, w->enc_b, x, split);
+  else
+    tj_encoder_index_kernel<H, false><<<grid, 256, 0, s>>>(env, st, w->enc_wT, w->enc_b, x, split);
+  IC3_LAUNCH_CHECK();
+  return IC3_OK;
 }
 
 // ---------------------------------------------------------------------------
@@ -691,7 +704,9 @@ int ic3_pp_layout_check(const ic3_pp_cfg* env, const ic3_policy_cfg* cfg) {
 }
 int ic3_tj_layout_check(const ic3_tj_cfg* env, const ic3_policy_cfg* cfg) {
   if (cfg->obs_vocab == 0) return IC3_OK;
-  return (cfg->obs_off == 2 && cfg->obs_vocab == env->vocab && cfg->obs_ncount == 1 && env->car_cls == env->vocab - 1)
+  // the bool vocabulary only: the scalar one takes no hint
+  return (env->vocab_type == IC3_TJ_VOCAB_BOOL && cfg->obs_off == 2 && cfg->obs_vocab == env->vocab &&
+          cfg->obs_ncount == 1 && env->car_cls == env->vocab - 1)
              ? IC3_OK : IC3_E_RANGE;
 }
 
@@ -720,7 +735,7 @@ extern "C" int ic3_tj_encoder_table(const ic3_tj_cfg* env, const ic3_policy_cfg*
   if (rc) return rc;
   if (!env || !env->grid || !table) return IC3_E_NULL;
   const int W = 2 * env->vision + 1;
-  if (cfg->O != 2 + W * W * env->vocab || cfg->obs_vocab == 0) return IC3_E_RANGE;
+  if (cfg->O != ic3_tj_obs_dim(*env) || cfg->obs_vocab == 0) return IC3_E_RANGE;
   rc = ic3_tj_layout_check(env, cfg);
   if (rc) return rc;
   tj_encoder_table_kernel<<<env->h * env->w, cfg->H, 0, (cudaStream_t)stream>>>(*env, cfg->H, w->enc_wT, w->enc_b, table);
@@ -771,21 +786,15 @@ extern "C" int ic3_tj_encoder_index(const ic3_tj_cfg* env, const ic3_tj_state* s
   if (rc) return rc;
   if (!env || !st || !st->loc || !st->alive || !st->last_act || !st->route_id || !env->grid || !x) return IC3_E_NULL;
   if (env->B != cfg->B || env->N != cfg->N) return IC3_E_RANGE;
-  const int W = 2 * env->vision + 1;
-  if (cfg->O != 2 + W * W * env->vocab) return IC3_E_RANGE;
+  rc = ic3_tj_vocab_check(*env);
+  if (rc) return rc;
+  if (cfg->O != ic3_tj_obs_dim(*env)) return IC3_E_RANGE;
   rc = ic3_tj_layout_check(env, cfg);
   if (rc) return rc;
   const bool split = cfg->obs_vocab > 0;
   const int rows = cfg->B * cfg->N, grid = (rows + 7) / 8;
   cudaStream_t s = (cudaStream_t)stream;
-  switch (cfg->H) {
-    case 32: tj_encoder_index_kernel<32><<<grid, 256, 0, s>>>(*env, *st, w->enc_wT, w->enc_b, x, split); break;
-    case 64: tj_encoder_index_kernel<64><<<grid, 256, 0, s>>>(*env, *st, w->enc_wT, w->enc_b, x, split); break;
-    case 128: tj_encoder_index_kernel<128><<<grid, 256, 0, s>>>(*env, *st, w->enc_wT, w->enc_b, x, split); break;
-    default: return IC3_E_UNSUPPORTED;
-  }
-  IC3_LAUNCH_CHECK();
-  return IC3_OK;
+  IC3_DISPATCH_H(cfg->H, tj_encoder_index_launch<HH>(*env, *st, w, x, split, grid, s));
 }
 
 extern "C" int ic3_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,

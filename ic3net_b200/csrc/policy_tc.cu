@@ -261,6 +261,8 @@ static int tc_pass(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const 
       IC3_LAUNCH_CHECK();
     }
   } else if (io->tj_env && io->tj_state) {       // fused index encoder, traffic junction
+    // bool vocabulary only: a scalar-vocabulary env's x comes from ic3_tj_encoder_index / ic3_tj_obs_encode
+    if (io->tj_env->vocab_type != IC3_TJ_VOCAB_BOOL) return IC3_E_UNSUPPORTED;
     const int W = 2 * io->tj_env->vision + 1;
     if (W * W > PREP_MAX_WW || io->tj_env->B != cfg->B || io->tj_env->N != cfg->N) return IC3_E_RANGE;
     if (cfg->O != 2 + W * W * io->tj_env->vocab) return IC3_E_RANGE;

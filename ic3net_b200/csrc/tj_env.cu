@@ -48,12 +48,16 @@ __global__ void tj_reset_kernel(TJArgs a, const uint8_t* __restrict__ mask) {
 
 // _get_obs (:321-366) + _flatten_obs (env_wrappers.py:88-98): row i =
 // [last_act, route_id/(npath-1), W*W cells x V classes]; all zero for dead cars.
+// SC (IC3_TJ_VOCAB_SCALAR, :139-148,331-332,344): [last_act, route_id/(npath-1), row/(h-1), col/(w-1), W*W cells x
+// (ROAD, CAR)] -- the OUTSIDE column is dropped, so cell column q holds class q + 1.
 // s_cell packs (cls | count << 16).
+template <bool SC>
 __device__ __forceinline__ void tj_write_obs(const ic3_tj_cfg& cfg, const int* s_r, const int* s_c,
                                             const int* s_alive, const int* s_rid, const int* s_lact,
                                             uint32_t* s_cell, float* __restrict__ obs_env, bool keep) {
+  constexpr int S = SC ? 4 : 2, C0 = SC ? 1 : 0;   // scalar features; class of cell column 0
   const int N = cfg.N, v = cfg.vision, W = 2 * v + 1, WW = W * W, V = cfg.vocab;
-  const int O = 2 + WW * V;
+  const int O = S + WW * V;
   const int ncell = N * WW;
   for (int c = threadIdx.x; c < ncell; c += blockDim.x) {
     const int i = c / WW, w = c - i * WW, dy = w / W, dx = w - dy * W;
@@ -74,10 +78,10 @@ __device__ __forceinline__ void tj_write_obs(const ic3_tj_cfg& cfg, const int* s
     const int cls = (int)(info & 0xffffu);
     const float cnt = (float)(info >> 16);
     const bool live = s_alive[i] != 0;
-    float* dst = obs_env + (size_t)i * O + 2 + (size_t)w * V;
+    float* dst = obs_env + (size_t)i * O + S + (size_t)w * V;
     for (int q = lane; q < V; q += 32) {
-      float o = (q == cls) ? 1.f : 0.f;
-      if (q == cfg.car_cls) o += cnt;
+      float o = (q + C0 == cls) ? 1.f : 0.f;
+      if (q + C0 == cfg.car_cls) o += cnt;
       ic3_st_obs(dst + q, live ? o : 0.f, keep);
     }
   }
@@ -86,9 +90,14 @@ __device__ __forceinline__ void tj_write_obs(const ic3_tj_cfg& cfg, const int* s
     float* dst = obs_env + (size_t)i * O;
     dst[0] = live ? (float)s_lact[i] : 0.f;                                    // / (naction-1) == 1
     dst[1] = live ? (float)s_rid[i] / (float)(cfg.npath - 1) : 0.f;            // :341
+    if (SC) {                                                                  // p_norm :344
+      dst[2] = live ? (float)s_r[i] / (float)(cfg.h - 1) : 0.f;
+      dst[3] = live ? (float)s_c[i] / (float)(cfg.w - 1) : 0.f;
+    }
   }
 }
 
+template <bool SC>
 __global__ void tj_step_kernel(TJArgs a, const int32_t* __restrict__ act, int act_stride,
                                const uint32_t* __restrict__ draws, float* __restrict__ reward,
                                float* __restrict__ obs, int32_t* err, RolloutOpt r, int do_step, int keep_l2) {
@@ -237,14 +246,14 @@ __global__ void tj_step_kernel(TJArgs a, const int32_t* __restrict__ act, int ac
   }
   if (obs == nullptr) return;
   __syncthreads();
-  const int W = 2 * cfg.vision + 1;
-  tj_write_obs(cfg, s_r, s_c, s_alive, s_rid, s_lact, s_cell, obs + (size_t)e * N * (2 + W * W * cfg.vocab), keep_l2 != 0);
+  const int W = 2 * cfg.vision + 1, S = SC ? 4 : 2;
+  tj_write_obs<SC>(cfg, s_r, s_c, s_alive, s_rid, s_lact, s_cell, obs + (size_t)e * N * (S + W * W * cfg.vocab), keep_l2 != 0);
 }
 
 // _get_obs + _flatten_obs + encoder (comm.py:119) in one pass: the observation block of the env is written exactly
 // as tj_step_kernel writes it, and x = W_e.obs + b of the env's cars is summed from the same per-cell records and
 // scalars (warp per row, tj_encode_row) -- the block is never read back.  One CTA per env.
-template <int H>
+template <int H, bool SC>
 __global__ void __launch_bounds__(128) tj_obs_encode_kernel(TJArgs a, float* __restrict__ obs,
                                                             const float* __restrict__ wT, const float* __restrict__ bias,
                                                             float* __restrict__ x, bool split, int keep_l2) {
@@ -252,7 +261,7 @@ __global__ void __launch_bounds__(128) tj_obs_encode_kernel(TJArgs a, float* __r
   __shared__ int s_r[IC3_MAX_AGENTS], s_c[IC3_MAX_AGENTS], s_alive[IC3_MAX_AGENTS], s_rid[IC3_MAX_AGENTS],
       s_lact[IC3_MAX_AGENTS];
   const ic3_tj_cfg& cfg = a.cfg;
-  const int N = cfg.N, W = 2 * cfg.vision + 1, WW = W * W, V = cfg.vocab;
+  const int N = cfg.N, W = 2 * cfg.vision + 1, WW = W * W, V = cfg.vocab, S = SC ? 4 : 2;
   const int e = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x < N) {
     const size_t i = (size_t)e * N + threadIdx.x;
@@ -263,28 +272,31 @@ __global__ void __launch_bounds__(128) tj_obs_encode_kernel(TJArgs a, float* __r
     s_lact[threadIdx.x] = a.st.last_act[i];
   }
   __syncthreads();
-  tj_write_obs(cfg, s_r, s_c, s_alive, s_rid, s_lact, s_cell, obs + (size_t)e * N * (2 + WW * V), keep_l2 != 0);
+  tj_write_obs<SC>(cfg, s_r, s_c, s_alive, s_rid, s_lact, s_cell, obs + (size_t)e * N * (S + WW * V), keep_l2 != 0);
   // s_cell: the records of all N * WW window cells (complete: tj_write_obs synchronised after building them)
   for (int i = warp; i < N; i += blockDim.x >> 5) {
     const uint32_t* rec = s_cell + i * WW;
     const bool alive = s_alive[i] != 0;
     const float la = alive ? (float)s_lact[i] : 0.f;
     const float ri = alive ? (float)s_rid[i] / (float)(cfg.npath - 1) : 0.f;
-    tj_encode_row<H>(alive, la, ri, [rec](int w) { return rec[w]; }, WW, V, cfg.car_cls, wT, bias, split,
-                     x + ((size_t)e * N + i) * H, lane);
+    const float pr = SC && alive ? (float)s_r[i] / (float)(cfg.h - 1) : 0.f;
+    const float pc = SC && alive ? (float)s_c[i] / (float)(cfg.w - 1) : 0.f;
+    tj_encode_row<H, SC>(alive, la, ri, pr, pc, [rec](int w) { return rec[w]; }, WW, V, cfg.car_cls, wT, bias, split,
+                         x + ((size_t)e * N + i) * H, lane);
   }
 }
 
 // The observation block of every env exactly as tj_step_kernel writes it (tj_write_obs, same store policy), no x, from
 // a persistent grid that strides over the envs (ic3_tj_obs_bounded); see pp_obs_writer_kernel.
+template <bool SC>
 __global__ void __launch_bounds__(IC3_OBS_WRITER_THREADS, IC3_OBS_WRITER_MIN_CTAS)
     tj_obs_writer_kernel(TJArgs a, float* __restrict__ obs, int keep_l2) {
   extern __shared__ uint32_t s_cell[];
   __shared__ int s_r[IC3_MAX_AGENTS], s_c[IC3_MAX_AGENTS], s_alive[IC3_MAX_AGENTS], s_rid[IC3_MAX_AGENTS],
       s_lact[IC3_MAX_AGENTS];
   const ic3_tj_cfg& cfg = a.cfg;
-  const int N = cfg.N, W = 2 * cfg.vision + 1, B = cfg.B;
-  const size_t per_env = (size_t)N * (2 + W * W * cfg.vocab);
+  const int N = cfg.N, W = 2 * cfg.vision + 1, B = cfg.B, S = SC ? 4 : 2;
+  const size_t per_env = (size_t)N * (S + W * W * cfg.vocab);
   const int k = threadIdx.x;
   int r = 0, c = 0, alive = 0, rid = 0, lact = 0;
   auto load = [&](int e) {
@@ -306,7 +318,7 @@ __global__ void __launch_bounds__(IC3_OBS_WRITER_THREADS, IC3_OBS_WRITER_MIN_CTA
       if (e + (int)gridDim.x < B) load(e + gridDim.x);
     }
     __syncthreads();
-    tj_write_obs(cfg, s_r, s_c, s_alive, s_rid, s_lact, s_cell, obs + (size_t)e * per_env, keep_l2 != 0);
+    tj_write_obs<SC>(cfg, s_r, s_c, s_alive, s_rid, s_lact, s_cell, obs + (size_t)e * per_env, keep_l2 != 0);
     __syncthreads();      // the per-car arrays and s_cell are rebuilt for the next env
   }
 }
@@ -322,7 +334,7 @@ int tj_check(const ic3_tj_cfg* cfg, const ic3_tj_state* st) {
   if (cfg->vision < 0 || cfg->vision > 7) return IC3_E_RANGE;
   if (cfg->G <= 0 || cfg->P <= 0 || cfg->Lmax <= 0 || cfg->npath < 2 || cfg->vocab <= 0 || cfg->vocab > 65535)
     return IC3_E_RANGE;
-  return IC3_OK;
+  return ic3_tj_vocab_check(*cfg);
 }
 
 int tj_launch(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const int32_t* act, int act_stride,
@@ -334,8 +346,11 @@ int tj_launch(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const int32_t* act,
   const int threads = obs ? 128 : 32 * IC3_ENV_WARPS;
   const int grid = obs ? cfg->B : (cfg->B + IC3_ENV_WARPS - 1) / IC3_ENV_WARPS;
   RolloutOpt ro = make_rollout_opt(r);
-  const int keep = obs && (size_t)cfg->B * cfg->N * (2 + W * W * cfg->vocab) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
-  tj_step_kernel<<<grid, threads, smem, s>>>(a, act, act_stride, draws, reward, obs, err, ro, do_step, keep);
+  const int keep = obs && (size_t)cfg->B * cfg->N * ic3_tj_obs_dim(*cfg) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
+  if (cfg->vocab_type == IC3_TJ_VOCAB_SCALAR)
+    tj_step_kernel<true><<<grid, threads, smem, s>>>(a, act, act_stride, draws, reward, obs, err, ro, do_step, keep);
+  else
+    tj_step_kernel<false><<<grid, threads, smem, s>>>(a, act, act_stride, draws, reward, obs, err, ro, do_step, keep);
   IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
@@ -348,8 +363,11 @@ int tj_obs_encode_launch(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const ic
   const size_t smem = (size_t)cfg->N * W * W * sizeof(uint32_t);
   const bool split = pcfg->obs_vocab > 0;
   // same store policy as ic3_tj_obs: batches that fit in L2 stay there for a reader that follows
-  const int keep = (size_t)cfg->B * cfg->N * (2 + W * W * cfg->vocab) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
-  tj_obs_encode_kernel<H><<<cfg->B, 128, smem, s>>>(a, obs, w->enc_wT, w->enc_b, x, split, keep);
+  const int keep = (size_t)cfg->B * cfg->N * ic3_tj_obs_dim(*cfg) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;
+  if (cfg->vocab_type == IC3_TJ_VOCAB_SCALAR)
+    tj_obs_encode_kernel<H, true><<<cfg->B, 128, smem, s>>>(a, obs, w->enc_wT, w->enc_b, x, split, keep);
+  else
+    tj_obs_encode_kernel<H, false><<<cfg->B, 128, smem, s>>>(a, obs, w->enc_wT, w->enc_b, x, split, keep);
   IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
@@ -363,11 +381,16 @@ extern "C" int ic3_tj_obs_bounded(const ic3_tj_cfg* cfg, const ic3_tj_state* st,
   TJArgs a{*cfg, *st};
   const int W = 2 * cfg->vision + 1;
   const size_t smem = (size_t)cfg->N * W * W * sizeof(uint32_t);
-  const int keep = (size_t)cfg->B * cfg->N * (2 + W * W * cfg->vocab) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;  // as ic3_tj_obs
+  const int keep = (size_t)cfg->B * cfg->N * ic3_tj_obs_dim(*cfg) * sizeof(float) <= IC3_OBS_L2_KEEP_BYTES;  // as ic3_tj_obs
+  const bool sc = cfg->vocab_type == IC3_TJ_VOCAB_SCALAR;
+  const void* kern = sc ? (const void*)tj_obs_writer_kernel<true> : (const void*)tj_obs_writer_kernel<false>;
   int grid = 0;
-  rc = ic3_grid_beside_lstm((const void*)tj_obs_writer_kernel, IC3_OBS_WRITER_THREADS, smem, cfg->B, &grid);
+  rc = ic3_grid_beside_lstm(kern, IC3_OBS_WRITER_THREADS, smem, cfg->B, &grid);
   if (rc) return rc;
-  tj_obs_writer_kernel<<<grid, IC3_OBS_WRITER_THREADS, smem, (cudaStream_t)stream>>>(a, obs, keep);
+  if (sc)
+    tj_obs_writer_kernel<true><<<grid, IC3_OBS_WRITER_THREADS, smem, (cudaStream_t)stream>>>(a, obs, keep);
+  else
+    tj_obs_writer_kernel<false><<<grid, IC3_OBS_WRITER_THREADS, smem, (cudaStream_t)stream>>>(a, obs, keep);
   IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
@@ -411,8 +434,7 @@ extern "C" int ic3_tj_obs_encode(const ic3_tj_cfg* env, const ic3_tj_state* st, 
   if (rc) return rc;
   if (!obs || !x) return IC3_E_NULL;
   if (env->B != cfg->B || env->N != cfg->N) return IC3_E_RANGE;
-  const int W = 2 * env->vision + 1;
-  if (cfg->O != 2 + W * W * env->vocab) return IC3_E_RANGE;
+  if (cfg->O != ic3_tj_obs_dim(*env)) return IC3_E_RANGE;
   rc = ic3_tj_layout_check(env, cfg);
   if (rc) return rc;
   IC3_DISPATCH_H(cfg->H, tj_obs_encode_launch<HH>(env, st, cfg, w, obs, x, (cudaStream_t)stream));

@@ -52,11 +52,24 @@ def road_blocks(h, w, difficulty):
             np.s_[:, w // 3 - 2:w // 3], np.s_[:, 2 * h // 3:2 * h // 3 + 2]]
 
 
-def build_grid(difficulty, dim):
+def scalar_constants():
+    """(OUTSIDE, ROAD, CAR, vocab) of vocab_type 'scalar' (:139-141): fixed classes, no BASE offset."""
+    return 0, 1, 2, 2
+
+
+def build_grid(difficulty, dim, vocab_type="bool"):
     """Road-id grid: every strip is numbered row-major in turn, later strips
-    overwrite the junction cells; everything else is OUTSIDE."""
+    overwrite the junction cells; everything else is OUTSIDE.  vocab_type 'scalar'
+    keeps the road-class grid instead (_set_grid :300-314 skips the numbering):
+    ROAD = 1 on every strip, OUTSIDE = 0."""
     dims, _, outside, _, _, _ = constants(difficulty, dim)
     h, w = dims
+    if vocab_type == "scalar":
+        outside, road = scalar_constants()[:2]
+        grid = np.full((h, w), outside, dtype=np.int64)
+        for blk in road_blocks(h, w, difficulty):
+            grid[blk] = road
+        return grid
     grid = np.full((h, w), outside, dtype=np.int64)
     start = 0
     for blk in road_blocks(h, w, difficulty):
@@ -142,16 +155,22 @@ def build_routes(difficulty, dim):
     return routes
 
 
-def build_tables(difficulty, dim, vision=0):
-    """Everything the kernels need, as numpy arrays (uploaded once by the env)."""
+def build_tables(difficulty, dim, vision=0, vocab_type="bool"):
+    """Everything the kernels need, as numpy arrays (uploaded once by the env).  The routes do not depend on
+    vocab_type: both vocabularies hand get_routes the same road-class grid (:309,510)."""
+    if vocab_type not in ("bool", "scalar"):
+        raise ValueError("vocab_type must be 'bool' or 'scalar'")
     dims, base, outside, car, vocab, npath = constants(difficulty, dim)
+    if vocab_type == "scalar":
+        base = None
+        outside, _, car, vocab = scalar_constants()
     if difficulty in ("easy", "medium"):          # traffic_junction_env.py:93-96
         assert dim % 2 == 0, "Only even dimension supported for now."
         assert dim >= 4 + vision, "Min dim: 4 + vision"
     if difficulty == "hard":                       # :98-100
         assert dim >= 9, "Min dim: 9"
         assert dim % 3 == 0, "Hard version works for multiple of 3. dim. only."
-    grid = build_grid(difficulty, dim)
+    grid = build_grid(difficulty, dim, vocab_type)
     routes = build_routes(difficulty, dim)
     G, P = len(routes), len(routes[0])
     assert all(len(g) == P for g in routes)

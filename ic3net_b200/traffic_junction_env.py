@@ -6,7 +6,9 @@ Same surface as the reference ``ic3net_envs/traffic_junction_env.py:TrafficJunct
 ``args.nenvs`` independent junctions per instance advanced by csrc/tj_env.cu.  The
 static tables (road-id grid, routes) are built once on the host
 (ic3net_b200/traffic_helper.py) and uploaded.  obs is ``[B, N, 2 + W*W*V]`` float32
-(already in the flattened order of env_wrappers.py:88-98).
+(already in the flattened order of env_wrappers.py:88-98); with ``vocab_type='scalar'``
+(:139-148,331-332,344) it is ``[B, N, 4 + W*W*2]``: last action, route id, the car's
+normalised position, then (is_road, car count) per window cell.
 """
 import ctypes as C
 import math
@@ -52,21 +54,26 @@ class TrafficJunctionEnv(object):
         for key in ('dim', 'vision', 'add_rate_min', 'add_rate_max', 'curr_start', 'curr_end', 'difficulty',
                     'vocab_type'):
             setattr(self, key, getattr(args, key))
-        if self.vocab_type != 'bool':
-            raise NotImplementedError("vocab_type='scalar' is outside the accelerated path")
+        if self.vocab_type not in _lib.TJ_VOCAB:
+            raise NotImplementedError("vocab_type must be 'bool' or 'scalar'")
+        scalar = self.vocab_type == 'scalar'
         self.ncar = N = args.nagents
-        t = traffic_helper.build_tables(self.difficulty, self.dim, self.vision)   # asserts of :93-100 inside
+        t = traffic_helper.build_tables(self.difficulty, self.dim, self.vision, self.vocab_type)   # asserts of :93-100
         self.dims = list(t['dims'])
         self.exact_rate = self.add_rate = self.add_rate_min
         self.epoch_last_update = 0
         self.naction = 2
         self.action_space = spaces.Discrete(self.naction)
         self.npath = t['npath']
-        self.BASE = t['BASE']
+        if not scalar:
+            self.BASE = t['BASE']              # the scalar vocabulary has none (:129-141)
         self.OUTSIDE_CLASS, self.CAR_CLASS, self.vocab_size = t['OUTSIDE'], t['CAR'], t['vocab']
         W = 2 * self.vision + 1
-        self.observation_space = spaces.Tuple((spaces.Discrete(self.naction), spaces.Discrete(self.npath),
-                                               spaces.MultiBinary((W, W, self.vocab_size))))
+        # scalar: the position member is MultiDiscrete of the dims as given (:147), before easy's +1 -- only its
+        # shape (2,) reaches observation_dim
+        pos = [spaces.MultiDiscrete((self.dim, self.dim))] if scalar else []
+        self.observation_space = spaces.Tuple([spaces.Discrete(self.naction), spaces.Discrete(self.npath)] + pos +
+                                              [spaces.MultiBinary((W, W, self.vocab_size))])
         self.grid = t['grid']
         self.routes = t['routes']
         self.tables = t
@@ -79,6 +86,7 @@ class TrafficJunctionEnv(object):
         self.cfg = _lib.TJCfg(B=B, N=N, vision=self.vision, h=self.dims[0], w=self.dims[1], G=t['G'], P=t['P'],
                               Lmax=t['Lmax'], outside_cls=self.OUTSIDE_CLASS, car_cls=self.CAR_CLASS,
                               vocab=self.vocab_size, npath=self.npath, spawn_thr=self._spawn_thr(),
+                              vocab_type=_lib.TJ_VOCAB[self.vocab_type],
                               env_id0=int(getattr(args, 'env_id0', 0)),
                               seed=int(getattr(args, 'seed', 0)) & 0xFFFFFFFFFFFFFFFF,
                               grid=self.d_grid.data_ptr(), route_len=self.d_route_len.data_ptr(),
@@ -99,9 +107,10 @@ class TrafficJunctionEnv(object):
                                   route_pos=self.car_route_loc.data_ptr(), last_act=self.car_last_act.data_ptr(),
                                   completed=self.is_completed.data_ptr(), cars_in_sys=self.cars_in_sys.data_ptr(),
                                   has_failed=self.has_failed.data_ptr(), tick=self.tick.data_ptr())
-        self.obs_dim = 2 + W * W * self.vocab_size
-        # encoder layout hint: two scalars, then cells of V entries whose last one (CAR) is a count
-        self.obs_layout = (2, self.vocab_size, 1) if self.CAR_CLASS == self.vocab_size - 1 else (0, 0, 0)
+        self.obs_dim = (4 if scalar else 2) + W * W * self.vocab_size
+        # encoder layout hint: two scalars, then cells of V entries whose last one (CAR) is a count; the scalar
+        # vocabulary takes none (one plain sum: no per-position table, no fused index encoder, no BPTT kernels)
+        self.obs_layout = (2, self.vocab_size, 1) if not scalar and self.CAR_CLASS == self.vocab_size - 1 else (0, 0, 0)
         self.obs_positions = self.dims[0] * self.dims[1]
         self.obs_shape = (B, N, self.obs_dim)
         self.stat = dict()

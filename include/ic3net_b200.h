@@ -175,7 +175,19 @@ typedef struct {
   const int32_t* grid;        /* [h, w] road ids / OUTSIDE (:300-316) */
   const int32_t* route_len;   /* [G, P] */
   const int32_t* route_cells; /* [G, P, Lmax] (row << 16 | col) (traffic_helper.py:156-209) */
+  /* IC3_TJ_VOCAB_BOOL: grid holds road ids, OUTSIDE = BASE, CAR = BASE + 2, vocab = BASE + 3; a car's row is
+   *   [last_act, route_id/(npath-1), W*W cells x vocab classes].
+   * IC3_TJ_VOCAB_SCALAR (:139-148,331-332,344): grid holds OUTSIDE = 0 / ROAD = 1, CAR = 2, vocab = 2 (outside_cls 0,
+   *   car_cls 2, anything else is IC3_E_RANGE); a car's row is
+   *   [last_act, route_id/(npath-1), row/(h-1), col/(w-1), W*W cells x (is_road, car count)].
+   * Every TJ entry point takes the row layout from this field; the encoder layout hint (ic3_policy_cfg.obs_vocab),
+   * the per-position encoder table, the fused index encoder of the tensor-core step and the BPTT / ff-grad kernels
+   * cover the bool layout only. */
+  int32_t vocab_type;
+  int32_t reserved0;
 } ic3_tj_cfg;
+#define IC3_TJ_VOCAB_BOOL 0
+#define IC3_TJ_VOCAB_SCALAR 1
 
 typedef struct {
   int32_t* loc;        /* [B, N, 2] car_loc; dead cars sit at (0,0) (:185,565) */
@@ -201,7 +213,7 @@ int ic3_tj_step(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const int32_t* ac
                 const uint32_t* draws, float* reward, float* obs, int32_t* err,
                 const ic3_rollout_io* r, void* stream);
 /* _get_obs + _flatten_obs: traffic_junction_env.py:321-366, env_wrappers.py:88-100.
- * obs: [B, N, 2 + W*W*V] float32. */
+ * obs: [B, N, 2 + W*W*V] float32 (IC3_TJ_VOCAB_SCALAR: [B, N, 4 + W*W*2]). */
 int ic3_tj_obs(const ic3_tj_cfg* cfg, const ic3_tj_state* st, float* obs, void* stream);
 /* The same obs as ic3_tj_obs from a grid that shares every SM with the policy step (see ic3_pp_obs_bounded). */
 int ic3_tj_obs_bounded(const ic3_tj_cfg* cfg, const ic3_tj_state* st, float* obs, void* stream);
