@@ -35,6 +35,7 @@
 // 2^-35 of the step's largest element); products are unscaled when they leave the accumulator registers.
 #include <cuda.h>
 
+#include "ff_grad_tc.h"
 #include "policy_tc_kernels.cuh"
 
 namespace {
@@ -1710,6 +1711,8 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
 //   encoder   dpre = (dx + g) (1 - tanh(x)^2);  Y += dpre^T P                                    [ff_dpre_kernel, ff_wgrad_kernel<true>]
 // ic3_ff_grad_finish sums the row-block partials in float64 and folds Y through the observation layout like the BPTT
 // finish (bptt_finish_misc_kernel).  All fp32 SIMT arithmetic; every sum has a fixed order.
+// plan->impl == IC3_FF_GRAD_TC replaces the pass and encoder kernels by the tensor-core ones of ff_grad_tc.cu (same
+// records, forward, heads, partials and finish).
 // ==================================================================================================================
 namespace {
 
@@ -1722,11 +1725,14 @@ struct FfGeom {
   int P, comm, R;                      // passes, communication on, max rows
   size_t x, hs, ss, g, dx, dz, dout, pos, ext, rloc, rroute, ralive, rlast, apost, fw, cw, fpart, cpart, bpart, ypart,
       gw_part, gs_part, sc, Y, total;
-  int nhb;
+  size_t tc;                           // IC3_FF_GRAD_TC: weight images and operand-scale words (ff_grad_tc.cu)
+  int nhb, impl;
 };
 
 int ff_geometry(const ic3_ff_grad_plan* p, FfGeom* G) {
   if (!p || !p->cfg) return IC3_E_NULL;
+  if (p->impl != IC3_FF_GRAD_SIMT && p->impl != IC3_FF_GRAD_TC) return IC3_E_UNSUPPORTED;
+  G->impl = p->impl;
   const ic3_policy_cfg* cfg = p->cfg;
   if (cfg->H != TC_H || cfg->cell != IC3_CELL_TANH || !cfg->x_tanh || !cfg->h_from_x) return IC3_E_UNSUPPORTED;
   if (cfg->passes < 0 || cfg->passes > IC3_MAX_PASSES) return IC3_E_UNSUPPORTED;
@@ -1784,6 +1790,7 @@ int ff_geometry(const ic3_ff_grad_plan* p, FfGeom* G) {
   G->apost = take(R);                        // alive_post AND valid: what the heads backward reads
   G->fw = take((size_t)G->P * HH);
   G->cw = take(G->comm ? (size_t)G->P * HH : 0);
+  G->tc = take(G->impl == IC3_FF_GRAD_TC ? ic3_ff_grad_tc_bytes(G->P, G->comm) : 0);
   // accumulators, zeroed by ic3_ff_grad_begin (fpart .. end)
   G->fpart = take((size_t)G->P * FF_NB * HH);
   G->cpart = take(G->comm ? (size_t)G->P * FF_NB * HH : 0);
@@ -2145,6 +2152,7 @@ extern "C" int ic3_ff_grad_begin(const ic3_ff_grad_plan* p, void* stream) {
     ff_transpose_kernel<<<(n + 255) / 256, 256, 0, s>>>(p->w->c_wT, reinterpret_cast<float*>(ws + G.cw), G.P);
     IC3_LAUNCH_CHECK();
   }
+  if (G.impl == IC3_FF_GRAD_TC) return ic3_ff_grad_tc_pack(G.P, G.comm, p->w->f_wT, p->w->c_wT, ws + G.tc, s);
   return IC3_OK;
 }
 
@@ -2237,6 +2245,22 @@ extern "C" int ic3_ff_grad_chunk(const ic3_ff_grad_plan* p, const ic3_ff_grad_io
   h.q = 0;
   bptt_heads_kernel<<<(R + HB_ROWS - 1) / HB_ROWS, 256, 0, s>>>(h);
   IC3_LAUNCH_CHECK();
+  if (G.impl == IC3_FF_GRAD_TC) {
+    FfGradTcChunk c;
+    memset(&c, 0, sizeof(c));
+    c.R = R; c.N = N; c.Bk = Bk; c.P = G.P; c.comm = G.comm; c.hard_attn = cfg->hard_attn; c.comm_avg = cfg->comm_avg;
+    c.nout = 1 + atot; c.npos = G.npos; c.ne = G.ne; c.npad = G.npad; c.is_tj = G.is_tj;
+    c.hs = hs; c.ss = ss; c.dout = dout; c.head_w = p->w->head_w;
+    c.fresh = io->fresh; c.comm_action = cfg->hard_attn ? io->comm : nullptr; c.alive = io->alive; c.valid = io->valid;
+    c.g = g; c.dx = dx; c.dz = dz; c.pos = pos; c.ext = ext;
+    c.fpart = reinterpret_cast<float*>(ws + G.fpart);
+    c.cpart = G.comm ? reinterpret_cast<float*>(ws + G.cpart) : nullptr;
+    c.bpart = reinterpret_cast<float*>(ws + G.bpart);
+    c.ypart = reinterpret_cast<float*>(ws + G.ypart);
+    c.nb = FF_NB;
+    c.tc = ws + G.tc;
+    return ic3_ff_grad_tc_chunk(&c, s);
+  }
   // passes P-1 .. 0
   const int epb = FF_ROWS / N;
   for (int ps = G.P - 1; ps >= 0; --ps) {

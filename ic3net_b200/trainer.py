@@ -46,6 +46,8 @@ The non-recurrent tanh policies (models.MLP, CommNet / IC3Net without --recurren
 next.  With ``grad_impl = 'kernels_ff'`` their gradient comes from the kernels of ic3_ff_grad_* (csrc/bptt_tc.cu): no
 hidden-state record or checkpoint at all; the backward re-runs the forward from the env-state records over chunks of K
 consecutive lock-steps (K*B env slots at once, K from the memory the device has left, ``FF_CHUNK_STEPS``).
+``grad_impl = 'kernels_ff_tc'`` is the same path with the products of the backward on the tensor cores
+(ic3_ff_grad_plan.impl = IC3_FF_GRAD_TC, csrc/ff_grad_tc.cu); chunking, records and the finish are shared.
 """
 import ctypes as C
 import math
@@ -135,11 +137,14 @@ class Trainer(object):
         # compute_grad implementation: 'kernels' = hand-written BPTT (csrc/bptt_tc.cu; tensor-core policy path with the
         # LSTM cell and 1..4 comm passes, or the tanh RNN without communication on the SIMT path; at most 7 action
         # logits, observation pattern of <= 512 columns), 'kernels_ff' = the non-recurrent tanh policies' kernels,
-        # 'autograd' = windowed recompute under torch autograd.  Default: kernels when the configuration allows.
+        # 'kernels_ff_tc' = the same with the backward's products on the tensor cores, 'autograd' = windowed recompute
+        # under torch autograd.  Default: kernels when the configuration allows.
         self.grad_impl = getattr(args, 'grad_impl', None) or 'auto'
-        if self.grad_impl not in ('auto', 'kernels', 'kernels_ff', 'autograd'):
-            raise ValueError("grad_impl must be 'auto', 'kernels', 'kernels_ff' or 'autograd', not %r"
+        if self.grad_impl not in ('auto', 'kernels', 'kernels_ff', 'kernels_ff_tc', 'autograd'):
+            raise ValueError("grad_impl must be 'auto', 'kernels', 'kernels_ff', 'kernels_ff_tc' or 'autograd', not %r"
                              % (self.grad_impl,))
+        # ic3_ff_grad_plan.impl of the non-recurrent kernels
+        self._ff_impl = _lib.FF_GRAD_TC if self.grad_impl == 'kernels_ff_tc' else _lib.FF_GRAD_SIMT
         self.grad_kernels = False
         self._bptt = None
         self._buf = None
@@ -171,15 +176,15 @@ class Trainer(object):
         if self.grad_impl == 'auto':
             self.grad_impl = 'kernels' if self.grad_kernels else 'autograd'
         # the non-recurrent tanh policies' kernels (ic3_ff_grad_*): no (h, c) records or checkpoints
-        self.grad_ff = self.record_for_grad and self.grad_impl == 'kernels_ff'
+        self.grad_ff = self.record_for_grad and self.grad_impl in ('kernels_ff', 'kernels_ff_tc')
         if self.grad_ff:
             e = env.env
             cfg = policy_net.policy_cfg(e.nenvs)
             if int(_lib.load().ic3_ff_grad_workspace_bytes(C.byref(self._ff_plan(cfg, None, e.nenvs * args.nagents)))) == 0:
-                raise NotImplementedError("grad_impl='kernels_ff' covers the non-recurrent tanh policies (models.MLP, "
+                raise NotImplementedError("grad_impl=%r covers the non-recurrent tanh policies (models.MLP, "
                                           "CommNet / IC3Net without --recurrent, 1..%d comm passes) at hid_size 128 with "
                                           "<= 7 action logits, a vision window of <= 5 x 5 cells and an observation "
-                                          "pattern of <= 512 columns" % _lib.MAX_PASSES)
+                                          "pattern of <= 512 columns" % (self.grad_impl, _lib.MAX_PASSES))
 
     def _policy_cfg(self):
         """ic3_policy_cfg of the policy step over this GPU's slots, with the env's Philox key and env ids."""
@@ -879,7 +884,7 @@ class Trainer(object):
         return _lib.FfGradPlan(cfg=C.pointer(cfg), w=None if w is None else C.pointer(w),
                                pp_env=None if self.is_tj else C.pointer(e.cfg), tj_env=C.pointer(e.cfg) if self.is_tj else None,
                                value_coeff=float(args.value_coeff), entr=float(args.entr), max_rows=rows,
-                               workspace=workspace)
+                               impl=self._ff_impl, workspace=workspace)
 
     def _ff_chunk_steps(self, T, cfg):
         """Lock-steps per chunk K of ic3_ff_grad_chunk for a T-step rollout: what the workspace of K steps needs must fit
@@ -898,7 +903,7 @@ class Trainer(object):
         return int(k)
 
     def _compute_grad_ff(self, adv, ret):
-        """grad_impl 'kernels_ff' (ic3_ff_grad_*): the rollout's T lock-steps in chunks of K consecutive steps, each one
+        """grad_impl 'kernels_ff' / 'kernels_ff_tc' (ic3_ff_grad_*): the rollout's T lock-steps in chunks of K consecutive steps, each one
         batch of K*B env slots (records are [T, B, ...]), in any order since no state crosses a step.  Returns the device
         float64 vector of the three loss sums."""
         b, net, args, e = self._buf, self.policy_net, self.args, self.env.env
