@@ -120,7 +120,7 @@ class CommNetMLP(nn.Module):
         self._packed_key = None
         # 'tc' = wgmma tensor-core path (csrc/policy_tc.cu: hid_size 128, LSTM cell on the encoded observation, any
         # number of comm passes), 'simt' = fp32 CUDA-core kernel (every variant), 'tc_tanh' = wgmma step of the tanh RNN
-        # without communication (csrc/rnn_tc.cu: models.RNN with the vanilla recurrence, hid_size 128); opt-in;
+        # without communication (csrc/ff_tc.cu: models.RNN with the vanilla recurrence, hid_size 128); opt-in;
         # 'tc_ff' = wgmma step of the non-recurrent tanh policies (csrc/ff_tc.cu: models.MLP, CommNet / IC3Net without
         # --recurrent, hid_size 128); opt-in
         self.tc_capable = (var['cell'] == _lib.CELL_LSTM and not var['x_tanh'] and not var['h_from_x'])
@@ -241,10 +241,7 @@ class CommNetMLP(nn.Module):
                 self._bufs['lstm_img'] = torch.empty(P * _lib.LSTM_IMG_BYTES, dtype=torch.uint8, device=dev)   # one per pass
                 self._bufs['bias_cat'] = torch.empty(P, 4 * H, device=dev)
                 self._bufs['flags'] = torch.zeros(1, dtype=torch.int32, device=dev)
-            if self.policy_impl == 'tc_tanh':
-                self._bufs['rnn_img'] = torch.empty(_lib.RNN_IMG_BYTES, dtype=torch.uint8, device=dev)
-                self._bufs['flags'] = torch.zeros(1, dtype=torch.int32, device=dev)
-            if self.policy_impl == 'tc_ff':         # one F (and C) image per pass
+            if self.policy_impl in ('tc_tanh', 'tc_ff'):     # one F (and C) image per pass
                 nbytes = _lib.ff_img_bytes(P, not self._cfg_proto['comm_mask_zero'])
                 self._bufs['ff_img'] = torch.empty(nbytes, dtype=torch.uint8, device=dev)
                 self._bufs['flags'] = torch.zeros(1, dtype=torch.int32, device=dev)

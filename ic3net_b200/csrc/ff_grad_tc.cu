@@ -76,8 +76,6 @@ __device__ __forceinline__ float max4(const float4& v) {
   return fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w)));
 }
 
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
 // weight image of one pass and part, in halfs: element (output column n, contraction index k) -- K-major B operand
 __host__ __device__ __forceinline__ size_t w_off(int nout, int n, int k) {
   return ((size_t)(k >> 3) * (nout / 8) + (n >> 3)) * 64 + (n & 7) * 8 + (k & 7);

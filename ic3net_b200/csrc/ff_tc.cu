@@ -1,23 +1,28 @@
-// Policy step of the non-recurrent tanh policies (models.MLP and CommNet / IC3Net without --recurrent: comm.py:127-129,
-// 179-224, models.py:23-25) on the Hopper tensor cores, H = 128:
-//   x~ = tanh(x),  h_0 = x~
-//   pass p:  S_p = gated mean of h_p over the env's other agents (zero with comm_mask_zero)
-//            h_{p+1} = tanh(x~ + c_b,p + S_p . C_p^T + h_p . F_p^T + f_b,p)
-//   value / action heads, log-softmax and sampling of h_P.
+// Policy step of the tanh policies without a recurrent LSTM cell on the Hopper tensor cores, H = 128, in two forms:
+//  - non-recurrent (models.MLP and CommNet / IC3Net without --recurrent: comm.py:127-129, 179-224, models.py:23-25):
+//      x~ = tanh(x),  h_0 = x~
+//      pass p:  S_p = gated mean of h_p over the env's other agents (zero with comm_mask_zero)
+//               h_{p+1} = tanh(x~ + c_b,p + S_p . C_p^T + h_p . F_p^T + f_b,p)
+//  - recurrent (models.RNN with the vanilla recurrence, the IC and IRIC baselines: models.py:83-85): one pass without
+//    communication, x~ = x and h_0 = the previous step's h (zero for slots starting an episode)
+//  then value / action heads, log-softmax and sampling of h_P.
 //
 // One launch per pass.  The pass's weight image -- the fp16 hi/lo split of 256 * F_p (and of 256 * C_p unless
 // comm_mask_zero) in the no-swizzle K-major core-matrix layout, 64 KB per matrix -- stays in shared memory for the whole
 // launch; only activations stream.  With communication the two products are one K = 256 contraction of [h | S] against
-// [F_p ; C_p] into the same 64 x 128 accumulator.  Persistent CTAs of one warpgroup (two per SM without communication,
-// one with) loop over 64-row tiles of whole envs (floor(64 / N) envs per tile, padding rows at the end):
-//   A  x~ of the thread's accumulator fragment (tanh on the SFU), kept in registers for C; gate and divisor per row
-//   A  h_p (x~ on pass 0) -> hi/lo fp16 (x 16) into the core-matrix layout in shared memory; with communication one
-//      thread per (env, column quad) also sums the gated rows (T) and writes S = g (T - h) / den into the S image
+// [F_p ; C_p] into the same 64 x 128 accumulator.  Persistent CTAs of one warpgroup loop over 64-row tiles: two CTAs
+// per SM and 64 consecutive rows per tile without communication, one CTA per SM and whole envs per tile with it
+// (floor(64 / N) envs, padding rows at the end):
+//   A  x~ of the thread's accumulator fragment (tanh on the SFU unless recurrent), kept in registers for C; gate and
+//      divisor per row
+//   A  h_p -> hi/lo fp16 (x 16) into the core-matrix layout in shared memory; with communication one thread per
+//      (env, column quad) also sums the gated rows (T) and writes S = g (T - h) / den into the S image
 //   B  8 k-steps x 3 wgmma m64n128k16 (hi.hi + lo.hi + hi.lo, tc_common.cuh) per product, fp32 accumulator
 //   C  h_{p+1} = tanh((x~ + c_b) + acc / 4096 + f_b) on the SFU -> HBM; last pass: also as fp32 over the A image
 //   D  last pass: heads of the tile's rows from shared memory, one warp per row (policy_heads.cuh)
 // Between passes h travels through a workspace buffer in place (a tile reads only its own rows, before it writes them).
-// The pass-state form (ic3_policy_ff_states) is the same kernel with tanh(x), S_p and h_{p+1} written out and no heads.
+// The pass-state form (ic3_policy_ff_states) is the non-recurrent kernel with tanh(x), S_p and h_{p+1} written out and
+// no heads.
 #include "ic3_common.cuh"
 #include "policy_heads.cuh"
 #include "policy_internal.h"
@@ -71,26 +76,25 @@ struct FfTcArgs {
   ic3_policy_io io;      // x, comm_action, alive, fresh; heads: tick, draws, value, logp, action, err
   const __half* w_img;   // this pass's image
   const float* f_b;      // this pass's biases
-  const float* c_b;
+  const float* c_b;      // recurrent form: bias of the (zero) comm projection, x + C(0) = x + c_b as the SIMT kernel adds it
   const float* head_w;
   const float* head_b;
   const int32_t* wflags;
-  const float* h_in;     // h_p, or NULL on pass 0 (h_0 = tanh(x)); may alias h_out
+  const float* h_in;     // h_p, or NULL on pass 0 (h_0 = tanh(x)); recurrent form: io.h; may alias h_out
   float* h_out;          // h_{p+1}
   float* st_x;           // pass-state form, pass 0: tanh(x), else NULL
   float* st_s;           // pass-state form: S_p, else NULL
   int heads;             // last pass of the step: heads and sampling
-  int epb, ntiles;       // envs per tile, tiles
+  int epb, ntiles;       // with communication: envs per tile; tiles
 };
-
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ float4 tanh4(float4 v) {
   return make_float4(tanh_fast(v.x), tanh_fast(v.y), tanh_fast(v.z), tanh_fast(v.w));
 }
 
-template <bool COMM>
+template <bool COMM, bool RECUR>
 __global__ void __launch_bounds__(FT_THREADS, COMM ? 1 : 2) ff_tc_kernel(FfTcArgs a) {
+  static_assert(!(COMM && RECUR), "the recurrent form has no communication");
   using L = FtLayout<COMM>;
   extern __shared__ __align__(1024) unsigned char smem[];
   __half* s_a = reinterpret_cast<__half*>(smem + L::W_BYTES);
@@ -113,8 +117,16 @@ __global__ void __launch_bounds__(FT_THREADS, COMM ? 1 : 2) ff_tc_kernel(FfTcArg
   const uint64_t dA = make_desc(smem_base + L::W_BYTES, (FT_M / 8) * 128, 128);
   const uint64_t dB = make_desc(smem_base, (FT_H / 8) * 128, 128);
   const int fr = lane >> 2, fc = 2 * (lane & 3);       // accumulator fragment: rows 16 warp + fr + 8 i, columns 8 j + fc + {0, 1}
-  // h_p of tile-local row rl, float4 column q (plain loads: h_in may alias h_out)
+  // the recurrent form is a rollout step: heads, no pass states
+  const bool heads = RECUR || a.heads;
+  float* const st_x = RECUR ? nullptr : a.st_x;
+  float* const st_s = RECUR ? nullptr : a.st_s;
+  // h_p of row `row`, float4 column q (plain loads: h_in may alias h_out)
   auto load_h = [&](long row, int q) -> float4 {
+    if (RECUR) {     // an episode start enters with h = 0 whatever io.h holds (trainer.py:50-51)
+      if (io.fresh && io.fresh[row / N]) return make_float4(0.f, 0.f, 0.f, 0.f);
+      return *(reinterpret_cast<const float4*>(a.h_in + row * FT_H) + q);
+    }
     if (a.h_in) return *(reinterpret_cast<const float4*>(a.h_in + row * FT_H) + q);
     return tanh4(__ldg(reinterpret_cast<const float4*>(io.x + row * FT_H) + q));
   };
@@ -124,9 +136,10 @@ __global__ void __launch_bounds__(FT_THREADS, COMM ? 1 : 2) ff_tc_kernel(FfTcArg
   };
 
   for (int tile = blockIdx.x; tile < a.ntiles; tile += gridDim.x) {
-    const int e0 = tile * a.epb;
-    const int nrows = min(a.epb, B - e0) * N;
-    const long row0 = (long)e0 * N;
+    // with communication a tile holds whole envs; without, 64 consecutive rows (each row's product is its own)
+    const int e0 = COMM ? tile * a.epb : 0;
+    const long row0 = COMM ? (long)e0 * N : (long)tile * FT_M;
+    const int nrows = COMM ? min(a.epb, B - e0) * N : (int)min((long)FT_M, (long)B * N - row0);
     // ---- A: x~ of this thread's fragment; gate and divisor per row (as policy_step_kernel) -------------
     float2 xv[32];
 #pragma unroll
@@ -136,7 +149,7 @@ __global__ void __launch_bounds__(FT_THREADS, COMM ? 1 : 2) ff_tc_kernel(FfTcArg
       for (int j = 0; j < 16; ++j) {
         float2 v = make_float2(0.f, 0.f);
         if (rl < nrows) v = __ldg(reinterpret_cast<const float2*>(io.x + (row0 + rl) * FT_H + 8 * j + fc));
-        xv[16 * i + j] = make_float2(tanh_fast(v.x), tanh_fast(v.y));
+        xv[16 * i + j] = RECUR ? v : make_float2(tanh_fast(v.x), tanh_fast(v.y));
       }
     }
     if (COMM && tid < FT_M) {
@@ -169,8 +182,8 @@ __global__ void __launch_bounds__(FT_THREADS, COMM ? 1 : 2) ff_tc_kernel(FfTcArg
         float4 hv = make_float4(0.f, 0.f, 0.f, 0.f);
         if (rl < nrows) {
           hv = load_h(row0 + rl, q);
-          if (a.st_x) *(reinterpret_cast<float4*>(a.st_x + (row0 + rl) * FT_H) + q) = hv;
-          if (a.st_s) *(reinterpret_cast<float4*>(a.st_s + (row0 + rl) * FT_H) + q) = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (st_x) *(reinterpret_cast<float4*>(st_x + (row0 + rl) * FT_H) + q) = hv;
+          if (st_s) *(reinterpret_cast<float4*>(st_s + (row0 + rl) * FT_H) + q) = make_float4(0.f, 0.f, 0.f, 0.f);
         }
         range_check(hv);
         store_split4(s_a, ft_a_off(rl, q), FT_A_PART / 2 + ft_a_off(rl, q), hv, SCALE_A);
@@ -193,7 +206,7 @@ __global__ void __launch_bounds__(FT_THREADS, COMM ? 1 : 2) ff_tc_kernel(FfTcArg
           for (int u = 0; u < 4; ++u) {
             if (j0 + u >= N) break;
             const int rl = rb + j0 + u;
-            if (a.st_x) *(reinterpret_cast<float4*>(a.st_x + (row0 + rl) * FT_H) + q) = hv[u];
+            if (st_x) *(reinterpret_cast<float4*>(st_x + (row0 + rl) * FT_H) + q) = hv[u];
             if (s_gate[rl] != 0.f) { T.x += hv[u].x; T.y += hv[u].y; T.z += hv[u].z; T.w += hv[u].w; }
             range_check(hv[u]);
             store_split4(s_a, ft_a_off(rl, q), FT_A_PART / 2 + ft_a_off(rl, q), hv[u], SCALE_A);
@@ -213,7 +226,7 @@ __global__ void __launch_bounds__(FT_THREADS, COMM ? 1 : 2) ff_tc_kernel(FfTcArg
               const float d = s_den[rl];
               sv = make_float4((T.x - hv[u].x) / d, (T.y - hv[u].y) / d, (T.z - hv[u].z) / d, (T.w - hv[u].w) / d);
             }
-            if (a.st_s) *(reinterpret_cast<float4*>(a.st_s + (row0 + rl) * FT_H) + q) = sv;
+            if (st_s) *(reinterpret_cast<float4*>(st_s + (row0 + rl) * FT_H) + q) = sv;
             range_check(sv);
             store_split4(s_s, ft_a_off(rl, q), FT_A_PART / 2 + ft_a_off(rl, q), sv, SCALE_A);
           }
@@ -265,10 +278,10 @@ __global__ void __launch_bounds__(FT_THREADS, COMM ? 1 : 2) ff_tc_kernel(FfTcArg
         hn.x = tanh_fast((xv[16 * i + j].x + cb.x) + fmaf(d[4 * j + 2 * i + 0], INV_SCALE, fb.x));
         hn.y = tanh_fast((xv[16 * i + j].y + cb.y) + fmaf(d[4 * j + 2 * i + 1], INV_SCALE, fb.y));
         if (rl < nrows) *reinterpret_cast<float2*>(a.h_out + row * FT_H + col) = hn;
-        if (a.heads) *reinterpret_cast<float2*>(s_hp + rl * FT_HP_LD + col) = hn;
+        if (heads) *reinterpret_cast<float2*>(s_hp + rl * FT_HP_LD + col) = hn;
       }
     }
-    if (!a.heads) continue;       // the next tile's image writes follow the MMA barrier above
+    if (!heads) continue;       // the next tile's image writes follow the MMA barrier above
     __syncthreads();
 
     // ---- D: heads, log-softmax, sampling (comm.py:228-239, action_utils.py:32-36) --------------------
@@ -285,20 +298,13 @@ __global__ void __launch_bounds__(FT_THREADS, COMM ? 1 : 2) ff_tc_kernel(FfTcArg
   }
 }
 
-template <bool COMM>
+template <bool COMM, bool RECUR>
 int ff_tc_launch(const FfTcArgs& a, cudaStream_t s) {
-  static int max_ctas = 0;
   const size_t smem = FtLayout<COMM>::SMEM;
-  if (max_ctas == 0) {
-    cudaError_t e = cudaFuncSetAttribute(ff_tc_kernel<COMM>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    int per_sm = 0, dev = 0, nsm = 0;
-    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ff_tc_kernel<COMM>, FT_THREADS, smem);
-    if (e == cudaSuccess) e = cudaGetDevice(&dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
-    if (e != cudaSuccess || per_sm <= 0) return e != cudaSuccess ? (int)e : IC3_E_RANGE;
-    max_ctas = per_sm * nsm;                                        // persistent grid: every CTA resident
-  }
-  ff_tc_kernel<COMM><<<a.ntiles < max_ctas ? a.ntiles : max_ctas, FT_THREADS, smem, s>>>(a);
+  int grid = 0;
+  const int rc = ic3_persistent_grid((const void*)ff_tc_kernel<COMM, RECUR>, FT_THREADS, smem, a.ntiles, &grid);
+  if (rc) return rc;
+  ff_tc_kernel<COMM, RECUR><<<grid, FT_THREADS, smem, s>>>(a);
   IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
@@ -308,7 +314,7 @@ int ff_tc_launch(const FfTcArgs& a, cudaStream_t s) {
 int ff_tc_run(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, float* carry, float* st_h,
               float* st_s, cudaStream_t s) {
   const int P = cfg->passes > 1 ? cfg->passes : 1;
-  const bool comm = !cfg->comm_mask_zero;
+  const bool comm = !cfg->comm_mask_zero, recur = !cfg->h_from_x;
   const size_t RH = (size_t)cfg->B * cfg->N * FT_H;
   FfTcArgs a;
   a.cfg = *cfg;
@@ -317,7 +323,7 @@ int ff_tc_run(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_p
   a.head_b = w->head_b;
   a.wflags = w->flags;
   a.epb = FT_M / cfg->N;
-  a.ntiles = (cfg->B + a.epb - 1) / a.epb;
+  a.ntiles = comm ? (cfg->B + a.epb - 1) / a.epb : (int)((RH / FT_H + FT_M - 1) / FT_M);
   const size_t img_pass = IC3_FF_IMG_BYTES(1, comm ? 1 : 0);
   for (int ps = 0; ps < P; ++ps) {
     a.w_img = reinterpret_cast<const __half*>(reinterpret_cast<const unsigned char*>(w->ff_img) + ps * img_pass);
@@ -330,12 +336,13 @@ int ff_tc_run(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_p
       a.st_s = st_s ? st_s + ps * RH : nullptr;
       a.heads = 0;
     } else {
-      a.h_in = ps == 0 ? nullptr : carry;
+      a.h_in = ps > 0 ? carry : recur ? io->h : nullptr;
       a.h_out = ps == P - 1 ? io->h_out : carry;
       a.st_x = a.st_s = nullptr;
       a.heads = ps == P - 1;
     }
-    const int rc = comm ? ff_tc_launch<true>(a, s) : ff_tc_launch<false>(a, s);
+    const int rc = comm ? ff_tc_launch<true, false>(a, s) : recur ? ff_tc_launch<false, true>(a, s)
+                                                                  : ff_tc_launch<false, false>(a, s);
     if (rc) return rc;
   }
   return IC3_OK;
@@ -344,13 +351,15 @@ int ff_tc_run(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_p
 }  // namespace
 
 bool ic3_ff_tc_capable(const ic3_policy_cfg* cfg) {
-  return cfg->cell == IC3_CELL_TANH && cfg->x_tanh && cfg->h_from_x && cfg->H == FT_H && cfg->N <= IC3_MAX_AGENTS &&
-         cfg->passes <= IC3_MAX_PASSES;
+  if (cfg->cell != IC3_CELL_TANH || cfg->H != FT_H) return false;
+  if (!cfg->x_tanh && !cfg->h_from_x)     // the tanh RNN: one pass without communication
+    return cfg->passes <= 1 && cfg->comm_mask_zero && !cfg->hard_attn;
+  return cfg->x_tanh && cfg->h_from_x && cfg->N <= IC3_MAX_AGENTS && cfg->passes <= IC3_MAX_PASSES;
 }
 
 uint64_t ic3_ff_tc_workspace_bytes(const ic3_policy_cfg* cfg) {
-  // one [R, H] buffer carries h from pass to pass; one pass needs none, and reports a nominal 16 bytes: a non-NULL
-  // workspace is what selects the tensor-core path
+  // one [R, H] buffer carries h from pass to pass; one pass (the tanh RNN's too) needs none, and reports a nominal
+  // 16 bytes: a non-NULL workspace is what selects the tensor-core path
   if (cfg->passes <= 1) return 16;
   return (uint64_t)cfg->B * cfg->N * FT_H * sizeof(float);
 }

@@ -10,13 +10,9 @@ int ic3_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3
 int ic3_tc_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, cudaStream_t s);
 int ic3_tc_pass_states(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, int npasses,
                        float* h_pass, float* c_pass, cudaStream_t s);
-// tensor-core step of the tanh RNN without communication (rnn_tc.cu): the configurations it covers, its weight image
-// (ic3_policy_packed.rnn_img) and the step itself
-bool ic3_rnn_tc_capable(const ic3_policy_cfg* cfg);
-int ic3_rnn_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3_policy_packed* out, cudaStream_t s);
-int ic3_rnn_tc_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io, cudaStream_t s);
-// tensor-core step of the non-recurrent tanh policies (ff_tc.cu): the configurations it covers, its scratch, its weight
-// image (ic3_policy_packed.ff_img), the step and its pass-state form
+// tensor-core step of the non-recurrent tanh policies and of the one-pass tanh RNN without communication (ff_tc.cu):
+// the configurations it covers, its scratch, its weight image (ic3_policy_packed.ff_img), the step and its pass-state
+// form (non-recurrent only)
 bool ic3_ff_tc_capable(const ic3_policy_cfg* cfg);
 uint64_t ic3_ff_tc_workspace_bytes(const ic3_policy_cfg* cfg);
 int ic3_ff_tc_pack(const ic3_policy_cfg* cfg, const ic3_policy_params* p, const ic3_policy_packed* out, cudaStream_t s);
@@ -29,6 +25,9 @@ void ic3_prof_mark(int i, cudaStream_t s);
 // tensor-core LSTM kernel: min(nwork, SMs x the CTAs of kern that fit on one SM next to a resident lstm_tc_kernel CTA --
 // registers, shared memory, threads, CTA slots -- at least one per SM)
 int ic3_grid_beside_lstm(const void* kern, int threads, size_t smem, int nwork, int* grid);
+// grid of a persistent kernel `kern` (threads per CTA, dynamic shared memory smem, which it allows kern to use) over
+// nwork items with every CTA resident: min(nwork, SMs x the CTAs of kern that fit on one SM)
+int ic3_persistent_grid(const void* kern, int threads, size_t smem, int nwork, int* grid);
 // return CALL with the compile-time hid_size HH = Hval (32 | 64 | 128)
 #define IC3_DISPATCH_H(Hval, CALL)          \
   switch (Hval) {                           \

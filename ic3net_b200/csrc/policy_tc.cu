@@ -59,7 +59,10 @@ static int ctas_beside_lstm(const void* kern, int threads, size_t smem, int* per
   return IC3_OK;
 }
 
-int ic3_grid_beside_lstm(const void* kern, int threads, size_t smem, int nwork, int* grid) {
+// min(nwork, CTAs of kern), the CTA count worked out by `count(&ctas)` on the first call for (kern, threads, smem) and
+// cached; each caller (a distinct Count type) keeps its own cache
+template <class Count>
+static int cached_grid(const void* kern, int threads, size_t smem, int nwork, int* grid, Count count) {
   struct Entry { const void* kern; int threads; size_t smem; int ctas; };
   static Entry cache[8];
   static int ncache = 0;
@@ -67,6 +70,16 @@ int ic3_grid_beside_lstm(const void* kern, int threads, size_t smem, int nwork, 
   for (int i = 0; i < ncache; ++i)
     if (cache[i].kern == kern && cache[i].threads == threads && cache[i].smem == smem) ctas = cache[i].ctas;
   if (ctas == 0) {
+    const int rc = count(&ctas);
+    if (rc) return rc;
+    if (ncache < 8) cache[ncache++] = Entry{kern, threads, smem, ctas};
+  }
+  *grid = nwork < ctas ? nwork : ctas;
+  return IC3_OK;
+}
+
+int ic3_grid_beside_lstm(const void* kern, int threads, size_t smem, int nwork, int* grid) {
+  return cached_grid(kern, threads, smem, nwork, grid, [&](int* ctas) -> int {
     // an SM configured for a kernel that needs little shared memory keeps that L1 / shared split while any of its
     // CTAs is resident, and the LSTM kernel's 198 KB CTA cannot start there: ask for the largest shared carveout
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -74,30 +87,33 @@ int ic3_grid_beside_lstm(const void* kern, int threads, size_t smem, int nwork, 
     int per_sm = 0, nsm = 0;
     const int rc = ctas_beside_lstm(kern, threads, smem, &per_sm, &nsm);
     if (rc) return rc;
-    ctas = per_sm * nsm;
-    if (ncache < 8) cache[ncache++] = Entry{kern, threads, smem, ctas};
-  }
-  *grid = nwork < ctas ? nwork : ctas;
-  return IC3_OK;
+    *ctas = per_sm * nsm;
+    return IC3_OK;
+  });
+}
+
+int ic3_persistent_grid(const void* kern, int threads, size_t smem, int nwork, int* grid) {
+  return cached_grid(kern, threads, smem, nwork, grid, [&](int* ctas) -> int {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    int per_sm = 0, dev = 0, nsm = 0;
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem);
+    if (e == cudaSuccess) e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess || per_sm <= 0) return e != cudaSuccess ? (int)e : IC3_E_RANGE;
+    *ctas = per_sm * nsm;                                           // every CTA resident
+    return IC3_OK;
+  });
 }
 
 static int launch_lstm(const ic3_policy_cfg* cfg, const ic3_policy_io* io, const ic3_policy_packed* w, const __half* a_img,
                        int ntiles_pad, size_t smem, int nout, float* partial, cudaStream_t s) {
-  static int max_ctas = 0;
   auto kern = lstm_tc_kernel;
-  if (max_ctas == 0) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return (int)e;
-    int per_sm = 0, dev = 0, nsm = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, TC_P_THREADS, smem);
-    if (e == cudaSuccess) e = cudaGetDevice(&dev);
-    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
-    if (e != cudaSuccess || per_sm <= 0) return e != cudaSuccess ? (int)e : IC3_E_RANGE;
-    max_ctas = per_sm * nsm;                                        // persistent grid: every CTA resident
-  }
   const int nitems = 2 * ntiles_pad;                                // (tile, column half)
+  int grid = 0;
+  const int rc = ic3_persistent_grid((const void*)kern, TC_P_THREADS, smem, nitems, &grid);
+  if (rc) return rc;
   const __half* b_img = reinterpret_cast<const __half*>(w->lstm_img) + (size_t)io->pass_index * B_IMG_HALFS;
-  kern<<<nitems < max_ctas ? nitems : max_ctas, TC_P_THREADS, smem, s>>>(
+  kern<<<grid, TC_P_THREADS, smem, s>>>(
       *cfg, *io, a_img, b_img, w->bias_cat + (size_t)io->pass_index * 4 * TC_H, nitems, w->head_w, nout, partial);
   IC3_LAUNCH_CHECK();
   return IC3_OK;

@@ -96,6 +96,8 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
   return d;                               // base_offset = 0, layout_type = no swizzle (0)
 }
+// makes shared memory written through the generic proxy (plain stores) visible to the MMAs that read it
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>

@@ -299,22 +299,18 @@ typedef struct {
   float* f_b;
   int32_t* flags;  /* device word written by ic3_policy_pack (IC3_ERR_FP16_RANGE when a folded weight does not fit the
                       operand split), OR-ed into ic3_policy_io.err by every policy step; may be NULL */
-  /* tensor-core path of the non-recurrent tanh step (IC3_CELL_TANH, x_tanh, h_from_x, H == 128: models.MLP and
-   * CommNet / IC3Net without --recurrent, 1..4 passes); NULL selects the fp32 SIMT kernel.
+  /* tensor-core path of the tanh cell at H == 128 (IC3_CELL_TANH): the non-recurrent step (x_tanh, h_from_x: models.MLP
+   * and CommNet / IC3Net without --recurrent, 1..4 passes) and the tanh RNN without communication (one pass,
+   * comm_mask_zero, no hard attention, x_tanh = h_from_x = 0: models.RNN with the vanilla recurrence); NULL selects the
+   * fp32 SIMT kernel.
    * ff_img: per pass, the fp16 hi/lo split of 256 * f_p.weight and, unless comm_mask_zero, of 256 * C_p.weight as
    *   ready-made shared-memory images, [pass][F hi, F lo (, C hi, C lo)][core-matrix layout] =
    *   IC3_FF_IMG_BYTES(passes, !comm_mask_zero) bytes; |weight| must stay below 255 (flags).  f_wT / f_b / c_wT / c_b
-   *   are packed as well.  (It sits in front of rnn_img, which stays the last member.) */
+   *   are packed as well. */
   void* ff_img;
-  /* tensor-core path of the tanh RNN without communication (IC3_CELL_TANH, one pass, comm_mask_zero, no hard attention,
-   * x_tanh = h_from_x = 0, H == 128: models.RNN with the vanilla recurrence); NULL selects the fp32 SIMT kernel.
-   * rnn_img: fp16 hi/lo split of 256 * f_0.weight as a ready-made shared-memory image, [hi,lo][core-matrix layout] =
-   *   IC3_RNN_IMG_BYTES bytes; |weight| must stay below 255 (flags).  f_wT / f_b are packed as well. */
-  void* rnn_img;
 } ic3_policy_packed;
 
 #define IC3_LSTM_IMG_BYTES 786432
-#define IC3_RNN_IMG_BYTES 65536
 /* bytes of ic3_policy_packed.ff_img: 64 KB per weight matrix and pass (passes = 0 counts as one) */
 #define IC3_FF_IMG_BYTES(passes, comm) ((size_t)((passes) > 1 ? (passes) : 1) * ((comm) ? 131072u : 65536u))
 
@@ -377,10 +373,10 @@ typedef struct {
                                  zero state applies to pass 0 only; its masks to every pass, comm.py:179-218) */
 } ic3_policy_io;
 
-/* Scratch the tensor-core policy path needs for a batch of cfg->B environments (0 when unsupported).  The tanh RNN's
- * tensor-core step needs none and reports a nominal 16 bytes: a non-NULL workspace is what selects the tensor-core path.
- * The non-recurrent tanh step (ff_img) reports the same 16 bytes for one pass and one [B*N, H] float32 buffer that
- * carries h between passes otherwise. */
+/* Scratch the tensor-core policy path needs for a batch of cfg->B environments (0 when unsupported).  The tanh step
+ * (ff_img) needs none for one pass, the tanh RNN's included, and reports a nominal 16 bytes: a non-NULL workspace is
+ * what selects the tensor-core path.  With several passes it reports one [B*N, H] float32 buffer that carries h
+ * between passes. */
 uint64_t ic3_policy_workspace_bytes(const ic3_policy_cfg* cfg);
 
 /* One CommNetMLP.forward (recurrent branch, comm_passes = 1) + select_action. */
@@ -388,9 +384,8 @@ int ic3_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const
                     void* stream);
 /* Measurement aid (bench.py "roofline_tensor"): ic3_policy_step on the tensor-core path with CUDA events between its
  * kernels; synchronises the stream and returns ms[3] = device time of {operand preparation (+ fused encoder),
- * LSTM/comm tensor-core kernel, heads + sampling}.  The tanh RNN's tensor-core step (rnn_img) is one kernel, reported as
- * ms[1]; ms[0] = ms[2] = 0.  So is the non-recurrent tanh step (ff_img): ms[1] is its per-pass launches together.  Not
- * for the production loop. */
+ * LSTM/comm tensor-core kernel, heads + sampling}.  The tanh step (ff_img) is one kernel per pass, reported together as
+ * ms[1]; ms[0] = ms[2] = 0.  Not for the production loop. */
 int ic3_policy_step_profile(const ic3_policy_cfg* cfg, const ic3_policy_packed* w, const ic3_policy_io* io,
                             void* stream, float* ms);
 /* The recurrent state after each of the first `npasses` comm passes (1 <= npasses <= cfg->passes) of ic3_policy_step on

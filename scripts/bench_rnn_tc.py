@@ -1,5 +1,5 @@
 """The IC baseline's policy step (models.RNN with the tanh recurrence, rnn_type 'MLP') on the fp32 SIMT kernel
-(policy_impl 'simt', the default) against the tensor-core kernel (policy_impl 'tc_tanh', csrc/rnn_tc.cu), alternated in
+(policy_impl 'simt', the default) against the tensor-core kernel (policy_impl 'tc_tanh', the recurrent form of ff_tc_kernel in csrc/ff_tc.cu), alternated in
 one process: predator-prey hard (10 agents, dim 20, vision 1, 8192 env slots) and traffic-junction hard (20 agents,
 4096 env slots), index observations, grad_impl 'kernels'.
 

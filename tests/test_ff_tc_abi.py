@@ -1,6 +1,6 @@
-"""CPU test of the C boundary of the non-recurrent tanh policies' tensor-core step: ic3_policy_packed grew by one pointer
-(ff_img, just in front of rnn_img, the last member); its ctypes mirror must have the header's size and field offsets, and the image size rule
-IC3_FF_IMG_BYTES must be that of _lib.ff_img_bytes."""
+"""CPU test of the C boundary of the tanh policies' tensor-core step (models.MLP, the non-recurrent CommNet / IC3Net and
+the tanh RNN): ic3_policy_packed grew by one pointer (ff_img, the last member); its ctypes mirror must have the header's
+size and field offsets, and the image size rule IC3_FF_IMG_BYTES must be that of _lib.ff_img_bytes."""
 import ctypes
 import os
 import re
@@ -13,7 +13,7 @@ CASES = [(p, c) for p in range(0, 5) for c in (0, 1)]
 def test_policy_packed_layout_and_image_size_match_header(tmp_path):
     from ic3net_b200 import _lib
     fields = [f for f, _ in _lib.PolicyPacked._fields_]
-    assert fields[-2:] == ["ff_img", "rnn_img"]
+    assert fields[-1] == "ff_img"
     src = open(os.path.join(ROOT, "include", "ic3net_b200.h")).read()
     body = re.search(r"typedef struct \{((?:(?!typedef struct).)*?)\} ic3_policy_packed;", src, flags=re.S).group(1)
     body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
@@ -56,6 +56,22 @@ def test_workspace_and_pack_validate_the_configuration(built_lib):
                                head_b=(ctypes.c_void_p * _lib.MAX_HEADS)(fake, None, None, None),
                                f_w_pass=(ctypes.c_void_p * _lib.MAX_PASSES)(*[fake] * _lib.MAX_PASSES),
                                f_b_pass=(ctypes.c_void_p * _lib.MAX_PASSES)(*[fake] * _lib.MAX_PASSES))
-    w = _lib.PolicyPacked(**{f: fake for f, _ in _lib.PolicyPacked._fields_ if f not in ("lstm_img", "bias_cat", "rnn_img")})
+    w = _lib.PolicyPacked(**{f: fake for f, _ in _lib.PolicyPacked._fields_ if f not in ("lstm_img", "bias_cat")})
     for bad in (dict(x_tanh=0, h_from_x=0), dict(H=64)):
         assert lib.ic3_policy_pack(ctypes.byref(_policy(**bad)), ctypes.byref(params), ctypes.byref(w), None) == -3, bad
+
+
+def test_workspace_and_step_validate_the_tanh_configuration(built_lib):
+    """Host-side checks only (nothing is launched): the tanh RNN (recurrent form of the step) reports a workspace; an
+    ff_img on a recurrent configuration outside its scope is refused as unsupported."""
+    from ic3net_b200 import _lib
+    lib = _lib.load()
+    pol = dict(comm_mask_zero=1, passes=1, x_tanh=0, h_from_x=0)
+    assert lib.ic3_policy_workspace_bytes(ctypes.byref(_policy(**pol))) > 0
+    fake = 0x1000                      # never dereferenced: validation fails first
+    w = _lib.PolicyPacked(**{f: fake for f, _ in _lib.PolicyPacked._fields_})
+    io = _lib.PolicyIO(x=fake, h=fake, c=fake, comm_action=fake, h_out=fake, c_out=fake, value=fake, logp=fake,
+                       workspace=fake)
+    for bad in (dict(comm_mask_zero=0), dict(passes=2), dict(H=64), dict(hard_attn=1), dict(cell=_lib.CELL_LSTM)):
+        cfg = _policy(**dict(pol, **bad))
+        assert lib.ic3_policy_step(ctypes.byref(cfg), ctypes.byref(w), ctypes.byref(io), None) == -3, bad

@@ -1,5 +1,5 @@
-"""GPU tests of the tanh RNN's tensor-core policy step (csrc/rnn_tc.cu, policy_impl 'tc_tanh': models.RNN with the vanilla
-recurrence, the IC / IRIC baselines).
+"""GPU tests of the tanh RNN's tensor-core policy step (the recurrent form of ff_tc_kernel in csrc/ff_tc.cu, policy_impl
+'tc_tanh': models.RNN with the vanilla recurrence, the IC / IRIC baselines).
 
 Covered: every row of every step of a rollout with episode resets at the full batch sizes against a float64 step; the
 reference's forward fixture and gradient fixtures at the bars of the SIMT path; sampling with explicit draws against the
