@@ -126,6 +126,12 @@ class BpttStepIO(C.Structure):
                 ("valid", _p), ("dh", _p), ("dc", _p), ("err", _p)]
 
 
+class PolicyBwdIO(C.Structure):
+    _fields_ = [("h_prev", _p), ("c_prev", _p), ("h_new", _p), ("logp", _p), ("comm", _p), ("alive", _p),
+                ("pp_state", C.POINTER(PPState)), ("tj_state", C.POINTER(TJState)), ("dlogp", _p), ("dvalue", _p),
+                ("dh_new", _p), ("dc_new", _p), ("dh_prev", _p), ("dc_prev", _p), ("err", _p)]
+
+
 class FfGradPlan(C.Structure):
     _fields_ = [("cfg", C.POINTER(PolicyCfg)), ("w", C.POINTER(PolicyPacked)), ("pp_env", C.POINTER(PPCfg)),
                 ("tj_env", C.POINTER(TJCfg)), ("value_coeff", C.c_float), ("entr", C.c_float), ("max_rows", C.c_int32),
@@ -187,6 +193,8 @@ SYMBOLS = {
     "ic3_bptt_step": (C.c_int, [C.POINTER(BpttPlan), C.POINTER(BpttStepIO), _PTR]),
     "ic3_bptt_prepare": (C.c_int, [C.POINTER(BpttPlan), C.POINTER(BpttStepIO), _PTR]),
     "ic3_bptt_finish": (C.c_int, [C.POINTER(BpttPlan), C.POINTER(PolicyParams), C.POINTER(PolicyParams), _PTR, _PTR]),
+    "ic3_policy_step_backward": (C.c_int, [C.POINTER(BpttPlan), C.POINTER(PolicyBwdIO), C.POINTER(PolicyParams),
+                                           C.POINTER(PolicyParams), _PTR]),
     "ic3_ff_grad_workspace_bytes": (C.c_uint64, [C.POINTER(FfGradPlan)]),
     "ic3_ff_grad_begin": (C.c_int, [C.POINTER(FfGradPlan), _PTR]),
     "ic3_ff_grad_chunk": (C.c_int, [C.POINTER(FfGradPlan), C.POINTER(FfGradIO), _PTR]),

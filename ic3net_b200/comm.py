@@ -9,8 +9,13 @@ The forward pass runs the hand-written kernels of csrc/policy.cu through the C A
 whole batch ``[B, N, .]`` of environments.  The recurrent (LSTM) branch with one comm pass -- the
 branch every BASELINE config uses -- runs on the wgmma tensor-core kernels; ``comm_passes > 1``,
 ``share_weights`` and the non-recurrent tanh branch (comm.py:63-70,127-131,220-224) run on the
-fp32 SIMT kernel.  The rollout forward is inference-only (the reference detaches what it samples
-from, action_utils.py:35); gradients are taken by the trainer.
+fp32 SIMT kernel.  By default ``forward`` is inference-only (the reference detaches what it samples from,
+action_utils.py:35) and gradients are taken by the trainer.  With ``args.forward_grad = 'kernels'`` its outputs carry
+a ``grad_fn`` whenever grad mode is on and a parameter requires grad: the backward of the step runs on the hand-written
+BPTT kernels (ic3_policy_step_backward, csrc/bptt_tc.cu), so a driver can differentiate its own loss through the
+module as the reference's Trainer does (trainer.py:54-60,223).  It covers what those kernels cover at hid_size 128 --
+the LSTM CommNet / IC3Net on policy_impl 'tc' (1..4 comm passes, share_weights), models.RNN with the LSTM cell, and the
+tanh RNN of the IC / IRIC baselines -- on observation handles (LazyObs, args.obs_api = 'handle').
 """
 import ctypes as C
 import weakref
@@ -18,6 +23,7 @@ import weakref
 import numpy as np
 import torch
 from torch import nn
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 from .lazy_obs import LazyObs
@@ -145,6 +151,21 @@ class CommNetMLP(nn.Module):
                                       "variants run on policy_impl='simt'")
         self._ws = {}
         self._enc_tables = weakref.WeakKeyDictionary()     # env -> (packed-weights key, encoder_table(env))
+        # differentiable forward on the BPTT kernels (ic3_policy_step_backward); None = inference-only forward
+        self.forward_grad = getattr(args, 'forward_grad', None)
+        if self.forward_grad not in (None, 'kernels'):
+            raise ValueError("forward_grad must be None or 'kernels'")
+        if self.forward_grad:
+            lstm_tc = var['cell'] == _lib.CELL_LSTM and self.policy_impl == 'tc'
+            tanh_rnn = (var['cell'] == _lib.CELL_TANH and not var['x_tanh'] and not var['h_from_x'] and
+                        var['passes'] == 1 and args.comm_mask_zero and not args.hard_attn and
+                        self.policy_impl in ('simt', 'tc_tanh'))
+            if H != 128 or not (lstm_tc or tanh_rnn):
+                raise NotImplementedError("forward_grad='kernels' covers the recurrent LSTM CommNet / IC3Net on "
+                                          "policy_impl='tc' (1..%d comm passes), models.RNN and the tanh RNN of the IC / "
+                                          "IRIC baselines, at hid_size 128; models.MLP and the non-recurrent CommNet / "
+                                          "IC3Net have no differentiable forward" % _lib.MAX_PASSES)
+        self._bwd_ws = {}                                   # B -> workspace of ic3_policy_step_backward
 
     def set_obs_layout(self, off, vocab, ncount):
         """Observation layout hint (include/ic3net_b200.h, ic3_policy_cfg.obs_vocab): lets the encoder sum the
@@ -265,6 +286,21 @@ class CommNetMLP(nn.Module):
         self._packed_key = key
         return self._packed
 
+    def policy_params(self, get):
+        """ic3_policy_params with get(tensor) for every kernel-side tensor by role: get = data_ptr gives the parameters,
+        a map to gradient buffers gives the gradient struct of ic3_bptt_finish / ic3_policy_step_backward."""
+        w = self._kernel_weights()
+        arr = lambda lst: (C.c_void_p * _lib.MAX_HEADS)(*([get(t) for t in lst] + [None] * (_lib.MAX_HEADS - len(lst))))
+        # C_modules[p] per comm pass (share_weights: the same module, so the gradient pointers alias)
+        parr = lambda lst: (C.c_void_p * _lib.MAX_PASSES)(*([get(t) for t in lst] + [None] * (_lib.MAX_PASSES - len(lst))))
+        # the LSTM cell's w_ih / w_hh / b_ih / b_hh, or the tanh cell's f_w / f_b per pass
+        cell = (dict(w_ih=get(w['w_ih']), w_hh=get(w['w_hh']), b_ih=get(w['b_ih']), b_hh=get(w['b_hh']))
+                if 'w_ih' in w else dict(f_w_pass=parr(w['f_w']), f_b_pass=parr(w['f_b'])))
+        return _lib.PolicyParams(encoder_w=get(w['enc_w']), encoder_b=get(w['enc_b']), c_w=get(w['c_w'][0]),
+                                 c_b=get(w['c_b'][0]), value_w=get(w['value_w']), value_b=get(w['value_b']),
+                                 head_w=arr(w['head_w']), head_b=arr(w['head_b']),
+                                 c_w_pass=parr(w['c_w']), c_b_pass=parr(w['c_b']), **cell)
+
     def check_errors(self):
         """Raise if a forward() of this module set a device-side error flag (tensor-core path: pipeline watchdog, fp16
         operand range).  One host synchronisation; the trainer checks its own flag word in collect_stat."""
@@ -285,6 +321,28 @@ class CommNetMLP(nn.Module):
             h, c = hid if lstm else (hid, None)
         else:
             state, h, c = x, None, None
+        B = state.shape[0]
+        if self.forward_grad and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            if not isinstance(state, LazyObs):
+                raise NotImplementedError("forward_grad='kernels' differentiates observation handles only (LazyObs: "
+                                          "args.obs_api='handle'); the backward rebuilds the observation from the env "
+                                          "state")
+            h = h.to(self._dev, torch.float32).reshape(B * self.nagents, self.hid_size)
+            c = c.to(self._dev, torch.float32) if c is not None else None
+            params = self._grad_params()
+            out = _PolicyStep.apply(self, state, info, h, c, *params)
+            action = list(torch.split(out[0], list(self.args.naction_heads), dim=-1))
+            return action, out[1], ((out[2], out[3]) if lstm else out[2])
+        logp, value, h2, c2, _ = self._step(state, h, c, info)
+        action = list(torch.split(logp, list(self.args.naction_heads), dim=-1))
+        if not carries:
+            return action, value.view(B, self.nagents, 1)          # comm.py:243-244
+        return action, value, ((h2, c2) if lstm else h2)
+
+    def _step(self, state, h, c, info):
+        """One ic3_policy_step on detached inputs: (log-probs [B, N, sum(na)], value [B*N, 1], h', c' or None, and the
+        (policy cfg, comm_action, alive_mask) the kernel read)."""
+        lstm = self._cfg_proto['cell'] == _lib.CELL_LSTM
         B, N, H = state.shape[0], self.nagents, self.hid_size
         dev = state.device
         lazy = isinstance(state, LazyObs)            # observation handle (lazy_obs.py): encoder from the env state
@@ -318,10 +376,33 @@ class CommNetMLP(nn.Module):
                            c_out=_lib.ptr(c2), value=value.data_ptr(), logp=logp.data_ptr(), action=None,
                            workspace=_lib.ptr(ws), err=_lib.ptr(err), **src)
         _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), _lib.stream()))
-        action = list(torch.split(logp, list(self.args.naction_heads), dim=-1))
-        if not carries:
-            return action, value.view(B, N, 1)                     # comm.py:243-244
-        return action, value, ((h2, c2) if lstm else h2)
+        return logp, value, h2, c2, (cfg, comm, alive)
+
+    def _grad_params(self):
+        """The distinct Parameters among the kernel-side tensors (share_weights aliases once; frozen buffers left out):
+        the inputs through which autograd hands ic3_policy_step_backward's gradients to them."""
+        seen, out = set(), []
+        for p in self._param_list():
+            if isinstance(p, nn.Parameter) and id(p) not in seen:
+                seen.add(id(p))
+                out.append(p)
+        return out
+
+    def _bwd_plan(self, env, cfg, w):
+        """ic3_bptt_plan of a differentiable step on env (the workspace is set by the backward); NotImplementedError
+        where the BPTT kernels do not cover the policy on this environment."""
+        table = self.encoder_table(env) if self._cfg_proto['cell'] == _lib.CELL_LSTM else None
+        tj = isinstance(env.cfg, _lib.TJCfg)
+        ecfg = type(env.cfg).from_buffer_copy(env.cfg)
+        plan = _lib.BpttPlan(cfg=C.pointer(cfg), w=C.pointer(w), pp_env=None if tj else C.pointer(ecfg),
+                             tj_env=C.pointer(ecfg) if tj else None, x_table=_lib.ptr(table), value_coeff=0.0,
+                             entr=0.0, workspace=None)
+        nbytes = int(_lib.load().ic3_bptt_workspace_bytes(C.byref(plan)))
+        if nbytes == 0 or (self._cfg_proto['cell'] == _lib.CELL_LSTM and table is None):
+            raise NotImplementedError("forward_grad='kernels' does not cover this environment: the BPTT kernels need a "
+                                      "vision window of at most 5 x 5 cells, the traffic junction's bool vocabulary and "
+                                      "at most 7 action logits")
+        return plan, nbytes, (ecfg, table)
 
     def _index_encoder(self, obs, B):
         """Encoder input for an observation HANDLE: returns (cfg, packed weights, PolicyIO source fields, x tensor or
@@ -347,3 +428,80 @@ class CommNetMLP(nn.Module):
         dev = self._dev
         return tuple((torch.zeros(batch_size * self.nagents, self.hid_size, device=dev),
                       torch.zeros(batch_size * self.nagents, self.hid_size, device=dev)))
+
+
+# env state fields the backward reads (ic3_policy_bwd_io.pp_state / tj_state): env attribute -> ic3_*_state field
+_PP_BWD_STATE = (('loc', 'loc'),)
+_TJ_BWD_STATE = (('car_loc', 'loc'), ('alive_mask', 'alive'), ('car_last_act', 'last_act'), ('route_id', 'route_id'))
+
+
+class _PolicyStep(torch.autograd.Function):
+    """CommNetMLP.forward with forward_grad='kernels': the module's own policy step forward (outputs bit-identical to
+    the inference-only forward), ic3_policy_step_backward backward.  Saves the step's inputs and outputs and a copy of
+    the env-state fields the backward reads (an observation handle is only valid until its env's next step); the packed
+    weights and encoder table are the module's, checked unchanged through the parameters' data_ptr / _version."""
+
+    @staticmethod
+    def forward(ctx, net, obs, info, h, c, *params):
+        logp, value, h2, c2, (cfg, comm, alive) = net._step(obs, h, c, info)
+        env = obs.env
+        w = net.packed()
+        ctx.plan, ctx.nbytes, ctx.keep = net._bwd_plan(env, cfg, w)
+        ctx.cfg, ctx.w, ctx.env = cfg, w, env
+        ctx.key = net._packed_key
+        tj = isinstance(env.cfg, _lib.TJCfg)
+        copies = {field: getattr(env, attr).clone() for attr, field in (_TJ_BWD_STATE if tj else _PP_BWD_STATE)}
+        ctx.state = (_lib.TJState if tj else _lib.PPState)(**{f: t.data_ptr() for f, t in copies.items()})
+        ctx.tj = tj
+        ctx.copies = copies
+        ctx.comm = None if comm is None else comm.clone()
+        ctx.alive = None if alive is None else alive.clone()
+        ctx.net, ctx.nparams = net, len(params)
+        ctx.set_materialize_grads(False)
+        outs = (logp, value, h2) + ((c2,) if c2 is not None else ())
+        ctx.save_for_backward(h, c, h2, logp)
+        return outs
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dlogp, dvalue, dh2, *rest):
+        net = ctx.net
+        if tuple((p.data_ptr(), p._version) for p in net._param_list()) != ctx.key:
+            raise RuntimeError("a parameter of the policy was modified in place (e.g. by an optimizer step) between "
+                               "this forward and its backward; the backward needs the weights of the forward")
+        h, c, h2, logp = ctx.saved_tensors
+        dc2 = rest[0] if rest else None
+        R, H = h2.shape
+        dev = h2.device
+        ws = net._bwd_ws.get(R)
+        if ws is None or ws.numel() < ctx.nbytes:
+            ws = torch.empty(ctx.nbytes, dtype=torch.uint8, device=dev)
+            net._bwd_ws[R] = ws
+        plan = ctx.plan
+        plan.workspace = ws.data_ptr()
+        lstm = c is not None
+        dh = torch.empty(R, H, device=dev)
+        dc = torch.empty(R, H, device=dev) if lstm else None
+        params = net._grad_params()
+        grads = {id(p): torch.zeros_like(p) for p in params}
+        scratch = {}                     # frozen kernel-side buffers (models.py zero comm projection): discarded
+
+        def grad_ptr(t):
+            g = grads.get(id(t))
+            if g is None:
+                g = scratch.setdefault(id(t), torch.zeros_like(t))
+            return g.data_ptr()
+        prm, grd = net.policy_params(lambda t: t.data_ptr()), net.policy_params(grad_ptr)
+        # every tensor the call reads stays referenced here until it has been enqueued
+        cont = lambda t: None if t is None else t.to(torch.float32).contiguous()
+        h, c, dlogp, dvalue, dh2, dc2 = cont(h), cont(c), cont(dlogp), cont(dvalue), cont(dh2), cont(dc2)
+        st = C.pointer(ctx.state)
+        _, err = net.workspace(R // net.nagents)
+        io = _lib.PolicyBwdIO(h_prev=h.data_ptr(), c_prev=_lib.ptr(c), h_new=h2.data_ptr(),
+                              logp=logp.data_ptr(), comm=_lib.ptr(ctx.comm), alive=_lib.ptr(ctx.alive),
+                              tj_state=st if ctx.tj else None, pp_state=None if ctx.tj else st,
+                              dlogp=_lib.ptr(dlogp), dvalue=_lib.ptr(dvalue), dh_new=_lib.ptr(dh2), dc_new=_lib.ptr(dc2),
+                              dh_prev=dh.data_ptr(), dc_prev=_lib.ptr(dc), err=_lib.ptr(err))
+        _lib.check(_lib.load().ic3_policy_step_backward(C.byref(plan), C.byref(io), C.byref(prm), C.byref(grd),
+                                                        _lib.stream()))
+        return (None, None, None, dh, dc) + tuple(grads[id(p)] for p in params)

@@ -75,12 +75,19 @@ struct HeadsArgs {
   double* gs_part;            // [nblocks][8 + 3] per-block: d head biases (8), action_loss, value_loss, entropy
   BpttScalars* sc;
   int q;                      // t & 1
+  // upstream form (ic3_policy_step_backward): d loss / d (log-probs, value) given by the caller, NULL = zero
+  const float* dlogp;         // [R, atot]
+  const float* dvalue;        // [R]
 };
 
 constexpr int HB_ROWS = 256;   // rows per block of the heads kernel
 
 // <= 40 registers: one CTA of this kernel fits beside a resident bptt_gates_kernel CTA (288 threads x 168 registers), so it
 // overlaps the tensor-core kernels of the previous step when launched ahead on the side stream (ic3_bptt_prepare)
+// UPSTREAM = false: d outputs from the records (the rollout loss).  UPSTREAM = true: from the caller's upstream gradients,
+//   dout_0 = dvalue,  dlogit_j = dlogp_j - p_j sum_k dlogp_k per head (log_softmax backward, p = exp of the saved
+//   log-probs); no loss sums.  Everything after d outputs (bound, bias / weight partials) is shared.
+template <bool UPSTREAM>
 __global__ void __launch_bounds__(256, 6) bptt_heads_kernel(HeadsArgs a) {
   __shared__ __align__(16) float s_dout[HB_ROWS][BP_HEADS];
   __shared__ float s_wmax[BP_HEADS];
@@ -98,7 +105,24 @@ __global__ void __launch_bounds__(256, 6) bptt_heads_kernel(HeadsArgs a) {
 #pragma unroll
   for (int o = 0; o < BP_HEADS; ++o) d[o] = 0.f;
   double al = 0.0, vl = 0.0, en = 0.0;
-  if (row < a.R) {
+  if (UPSTREAM && row < a.R) {
+    d[0] = a.dvalue ? a.dvalue[row] : 0.f;
+    int off = 0;
+    for (int m = 0; a.dlogp && m < a.nheads; ++m) {
+      const int na = a.head_dim[m];
+      const float* dl = a.dlogp + (size_t)row * a.atot + off;
+      float sum = 0.f;
+      for (int j = 0; j < na; ++j) sum += dl[j];
+      for (int j = 0; j < na; ++j) {
+        const float pj = __expf(a.logp[(size_t)row * a.atot + off + j]);
+        if (1 + off + j < BP_HEADS) d[1 + off + j] = fmaf(-pj, sum, dl[j]);
+      }
+      off += na;
+    }
+    *reinterpret_cast<float4*>(a.dout + (size_t)row * BP_HEADS) = make_float4(d[0], d[1], d[2], d[3]);
+    *reinterpret_cast<float4*>(a.dout + (size_t)row * BP_HEADS + 4) = make_float4(d[4], d[5], d[6], d[7]);
+  }
+  if (!UPSTREAM && row < a.R) {
     const float alive = a.alive_post[row] ? 1.f : 0.f;
     const float vmask = (a.valid == nullptr || a.valid[row / a.N]) ? 1.f : 0.f;
     const float value = a.value[row], ret = a.ret[row], adv = a.adv[row];
@@ -216,6 +240,42 @@ __global__ void bptt_scale_kernel(BpttScalars* sc, int q) {
   sc->dhmax = 0u;
   sc->dcmax = 0u;
   sc->hbound[q] = 0u;
+}
+
+// ic3_policy_step_backward: the recursion's inputs from the caller's upstream gradients.  dh = dh_new, dc = dc_new (NULL:
+// zero), and the maxima the scale kernel reads are reduced here on the device instead of coming from the host:
+// dhmax = max |dh_new|, dcmax = max |dc_new|, cmax = max |c_prev| + cadd (cadd = passes - 1, see ic3_bptt_begin).  The
+// scalars were zeroed before; the maxima are non-negative, so their bit patterns order like the values.
+__global__ void bptt_upstream_kernel(size_t n4, const float4* __restrict__ dh_new, const float4* __restrict__ dc_new,
+                                     const float4* __restrict__ c_prev, float4* __restrict__ dh, float4* __restrict__ dc,
+                                     float cadd, BpttScalars* sc) {
+  float mh = 0.f, mc = 0.f, mp = 0.f;
+  const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
+    const float4 h = dh_new ? dh_new[i] : z;
+    dh[i] = h;
+    mh = fmaxf(mh, fmaxf(fmaxf(fabsf(h.x), fabsf(h.y)), fmaxf(fabsf(h.z), fabsf(h.w))));
+    if (dc) {
+      const float4 c = dc_new ? dc_new[i] : z;
+      dc[i] = c;
+      mc = fmaxf(mc, fmaxf(fmaxf(fabsf(c.x), fabsf(c.y)), fmaxf(fabsf(c.z), fabsf(c.w))));
+    }
+    if (c_prev) {
+      const float4 c = c_prev[i];
+      mp = fmaxf(mp, fmaxf(fmaxf(fabsf(c.x) + cadd, fabsf(c.y) + cadd), fmaxf(fabsf(c.z) + cadd, fabsf(c.w) + cadd)));
+    }
+  }
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1) {
+    mh = fmaxf(mh, __shfl_xor_sync(IC3_FULL_MASK, mh, s));
+    mc = fmaxf(mc, __shfl_xor_sync(IC3_FULL_MASK, mc, s));
+    mp = fmaxf(mp, __shfl_xor_sync(IC3_FULL_MASK, mp, s));
+  }
+  if ((threadIdx.x & 31) == 0) {
+    atomicMax(&sc->dhmax, __float_as_uint(mh));
+    atomicMax(&sc->dcmax, __float_as_uint(mc));
+    atomicMax(reinterpret_cast<unsigned*>(&sc->cmax), __float_as_uint(mp));
+  }
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1252,23 +1312,12 @@ extern "C" uint64_t ic3_bptt_workspace_bytes(const ic3_bptt_plan* p) {
   return (uint64_t)L.total;
 }
 
-// Start of a compute_grad: zero the accumulators, build the dgrad weight image, set max |c|.
-extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) {
-  if (!p || !p->cfg || !p->w || !p->workspace) return IC3_E_NULL;
-  int npos, WW, is_tj;
-  int rc = env_geometry(p, &npos, &WW, &is_tj);
-  if (rc) return rc;
-  Layout L;
-  rc = plan_layout(p->cfg, npos, WW, is_tj, &L);
-  if (rc) return rc;
-  cudaStream_t s = (cudaStream_t)stream;
+// Zero the accumulators and scalars (partial .. end of the workspace) and build the dgrad weight image(s).
+static int bptt_reset(const ic3_bptt_plan* p, const Layout& L, cudaStream_t s) {
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
   cudaError_t e = cudaMemsetAsync(ws + L.partial, 0, L.total - L.partial, s);   // partial .. end: all accumulators / scalars
   if (e != cudaSuccess) return (int)e;
-  e = cudaMemsetAsync(ws + L.a_img, 0, L.w2_img - L.a_img, s);                  // both image sets
-  if (e != cudaSuccess) return (int)e;
   if (L.tanh) {                                // SIMT-packed weights: no forward image, the dgrad image comes from f_wT
-    if (!p->w->f_wT) return IC3_E_NULL;
     bptt_pack_w2_tanh_kernel<<<(256 * TC_H + 255) / 256, 256, 0, s>>>(p->w->f_wT, reinterpret_cast<__half*>(ws + L.w2_img));
     IC3_LAUNCH_CHECK();
   }
@@ -1281,6 +1330,26 @@ extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) 
   BpttStreams* ss = bptt_streams();
   if (!ss) return IC3_E_UNSUPPORTED;
   ss->prepared_t[0] = ss->prepared_t[1] = -1;
+  return IC3_OK;
+}
+
+// Start of a compute_grad: zero the accumulators and both operand-image sets, build the dgrad weight image, set max |c|.
+extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) {
+  if (!p || !p->cfg || !p->w || !p->workspace) return IC3_E_NULL;
+  int npos, WW, is_tj;
+  int rc = env_geometry(p, &npos, &WW, &is_tj);
+  if (rc) return rc;
+  Layout L;
+  rc = plan_layout(p->cfg, npos, WW, is_tj, &L);
+  if (rc) return rc;
+  if (L.tanh && !p->w->f_wT) return IC3_E_NULL;
+  cudaStream_t s = (cudaStream_t)stream;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
+  rc = bptt_reset(p, L, s);
+  if (rc) return rc;
+  cudaError_t e = cudaMemsetAsync(ws + L.a_img, 0, L.w2_img - L.a_img, s);      // both image sets
+  if (e != cudaSuccess) return (int)e;
+  BpttStreams* ss = bptt_streams();
   BpttScalars init;
   memset(&init, 0, sizeof(init));
   // the cell states entering passes 1 .. P-1 are not in the record: each pass changes |c| by at most 1
@@ -1302,8 +1371,9 @@ extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) 
 // Recursion-independent part of a backward unit (step t, comm pass ps): the operand images of the pass (prep) from
 // the state h_in entering it, and -- for the last pass only -- d loss / d outputs from the records (heads).  Runs on
 // `s` into buffer set q (parity of the unit counter t * P + ps).
+// up != NULL: the heads take the caller's upstream gradients (ic3_policy_step_backward) instead of the records.
 static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const Layout& L, int npos, int is_tj,
-                           cudaStream_t s, int q, int ps, const float* h_in) {
+                           cudaStream_t s, int q, int ps, const float* h_in, const ic3_policy_bwd_io* up) {
   const ic3_policy_cfg* cfg = p->cfg;
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
   const int R = cfg->B * cfg->N;
@@ -1357,7 +1427,12 @@ static int bptt_prepare_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, c
   ha.gs_part = reinterpret_cast<double*>(ws + L.gs_part);
   ha.sc = sc;
   ha.q = q;
-  bptt_heads_kernel<<<L.nhb, 256, 0, s>>>(ha);
+  if (up) {
+    ha.dlogp = up->dlogp; ha.dvalue = up->dvalue;
+    bptt_heads_kernel<true><<<L.nhb, 256, 0, s>>>(ha);
+  } else {
+    bptt_heads_kernel<false><<<L.nhb, 256, 0, s>>>(ha);
+  }
   IC3_LAUNCH_CHECK();
   return IC3_OK;
 }
@@ -1401,7 +1476,7 @@ extern "C" int ic3_bptt_prepare(const ic3_bptt_plan* p, const ic3_bptt_step_io* 
   // its weight-gradient kernel (side stream, already ordered before this call)
   cudaError_t e = cudaStreamWaitEvent(ss->side, ss->main_done[q], 0);
   if (e != cudaSuccess) return (int)e;
-  rc = bptt_prepare_on(p, io, L, npos, is_tj, ss->side, q, 0, io->h_prev);
+  rc = bptt_prepare_on(p, io, L, npos, is_tj, ss->side, q, 0, io->h_prev, nullptr);
   if (rc) return rc;
   e = cudaEventRecord(ss->prep_done[q], ss->side);
   if (e != cudaSuccess) return (int)e;
@@ -1412,7 +1487,7 @@ extern "C" int ic3_bptt_prepare(const ic3_bptt_plan* p, const ic3_bptt_step_io* 
 // One backward unit: comm pass ps of step io->t, entered with state (h_in, c_in), on buffer set q.  The incoming
 // io->dh / io->dc are d loss / d (h, c) leaving the pass; they are replaced by d loss / d (h_in, c_in).
 static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const Layout& L, int npos, int is_tj,
-                     cudaStream_t s, int q, int ps, const float* h_in, const float* c_in) {
+                     cudaStream_t s, int q, int ps, const float* h_in, const float* c_in, const ic3_policy_bwd_io* up) {
   int rc;
   const ic3_policy_cfg* cfg = p->cfg;
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
@@ -1435,7 +1510,7 @@ static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const L
     if (se != cudaSuccess) return (int)se;
     ss->prepared_t[q] = -1;
   } else {
-    rc = bptt_prepare_on(p, io, L, npos, is_tj, s, q, ps, h_in);
+    rc = bptt_prepare_on(p, io, L, npos, is_tj, s, q, ps, h_in, up);
     if (rc) return rc;
   }
   bptt_scale_kernel<<<1, 1, 0, s>>>(sc, q);
@@ -1528,7 +1603,8 @@ static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const L
       cudaError_t e = cudaFuncSetAttribute(bptt_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
       if (e != cudaSuccess) return (int)e;
       prefer_max_smem(bptt_wgrad_kernel);
-      prefer_max_smem(bptt_heads_kernel);
+      prefer_max_smem(bptt_heads_kernel<false>);
+      prefer_max_smem(bptt_heads_kernel<true>);
       prefer_max_smem(bptt_comm_kernel);
       prefer_max_smem(prep_kernel<XSRC_PP, true, true>);
       prefer_max_smem(prep_kernel<XSRC_TJ, true, true>);
@@ -1565,13 +1641,10 @@ static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const L
 
 // Step t = the units (t, P-1) .. (t, 0).  With P > 1 comm passes the states entering passes 1 .. P-1 are re-run first
 // from the record (h_{t-1}, c_{t-1}) with the rollout's own kernels (ic3_tc_pass_states).
-extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, void* stream) {
-  Layout L;
-  int npos, is_tj;
-  int rc = bptt_common(p, io, &L, &npos, &is_tj);
-  if (rc) return rc;
-  cudaStream_t s = (cudaStream_t)stream;
-  if (L.P == 1) return bptt_unit(p, io, L, npos, is_tj, s, io->t & 1, 0, io->h_prev, io->c_prev);
+static int bptt_step_on(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const Layout& L, int npos, int is_tj,
+                        cudaStream_t s, const ic3_policy_bwd_io* up) {
+  int rc;
+  if (L.P == 1) return bptt_unit(p, io, L, npos, is_tj, s, io->t & 1, 0, io->h_prev, io->c_prev, up);
   const ic3_policy_cfg* cfg = p->cfg;
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
   const size_t RH = (size_t)cfg->B * cfg->N * TC_H;
@@ -1593,10 +1666,18 @@ extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io,
     const int q = (io->t * L.P + ps) & 1;                 // unit counter parity: consecutive units alternate sets
     const float* h_in = ps == 0 ? io->h_prev : h_pass + (size_t)(ps - 1) * RH;
     const float* c_in = ps == 0 ? io->c_prev : c_pass + (size_t)(ps - 1) * RH;
-    rc = bptt_unit(p, io, L, npos, is_tj, s, q, ps, h_in, c_in);
+    rc = bptt_unit(p, io, L, npos, is_tj, s, q, ps, h_in, c_in, up);
     if (rc) return rc;
   }
   return IC3_OK;
+}
+
+extern "C" int ic3_bptt_step(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, void* stream) {
+  Layout L;
+  int npos, is_tj;
+  int rc = bptt_common(p, io, &L, &npos, &is_tj);
+  if (rc) return rc;
+  return bptt_step_on(p, io, L, npos, is_tj, (cudaStream_t)stream, nullptr);
 }
 
 // After step 0: fold the accumulators into the parameter gradients (added to what the buffers hold) and return the
@@ -1698,6 +1779,74 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
   bptt_finish_heads_kernel<<<(BP_HEADS * TC_H + 255) / 256, 256, 0, s>>>(f);
   IC3_LAUNCH_CHECK();
   return IC3_OK;
+}
+
+namespace {
+// the parameter / gradient pointers ic3_bptt_finish reads for the plan's cell
+int finish_args_check(const ic3_policy_cfg* cfg, const Layout& L, const ic3_policy_params* params,
+                      const ic3_policy_params* grads) {
+  if (!grads->encoder_w || !grads->encoder_b || !grads->value_w || !grads->value_b) return IC3_E_NULL;
+  for (int k = 0; k < cfg->nheads; ++k)
+    if (!grads->head_w[k] || !grads->head_b[k]) return IC3_E_NULL;
+  if (L.tanh) return grads->f_w_pass[0] && grads->f_b_pass[0] ? IC3_OK : IC3_E_NULL;
+  if (!params->w_ih || !params->c_w || !params->c_b || !grads->w_ih || !grads->w_hh || !grads->b_ih || !grads->b_hh ||
+      !grads->c_w || !grads->c_b)
+    return IC3_E_NULL;
+  return IC3_OK;
+}
+}  // namespace
+
+// The backward of one ic3_policy_step under caller-given upstream gradients: the BPTT unit chain of ic3_bptt_step with
+// the heads in their upstream form, between a reset of the accumulators and ic3_bptt_finish.  dh_prev / dc_prev carry
+// the recursion (in: d / d (h', c'), out: d / d (h, c)).  No host synchronisation: the operand-scale bound is reduced on
+// the device (bptt_upstream_kernel).  The operand images are not cleared: the preparation, gate and tanh kernels write
+// every row of every tile they cover, padding rows included.
+extern "C" int ic3_policy_step_backward(const ic3_bptt_plan* p, const ic3_policy_bwd_io* io,
+                                        const ic3_policy_params* params, const ic3_policy_params* grads, void* stream) {
+  if (!p || !io || !params || !grads || !p->cfg || !p->w || !p->workspace) return IC3_E_NULL;
+  const ic3_policy_cfg* cfg = p->cfg;
+  if (cfg->H != TC_H) return IC3_E_UNSUPPORTED;
+  int npos, WW, is_tj;
+  int rc = env_geometry(p, &npos, &WW, &is_tj);
+  if (rc) return rc;
+  if (cfg->obs_vocab == 0 || (is_tj ? ic3_tj_layout_check(p->tj_env, cfg) : ic3_pp_layout_check(p->pp_env, cfg)))
+    return IC3_E_UNSUPPORTED;
+  Layout L;
+  rc = plan_layout(cfg, npos, WW, is_tj, &L);
+  if (rc) return rc;
+  int nout = 1;
+  for (int k = 0; k < cfg->nheads; ++k) nout += cfg->head_dim[k];
+  if (nout > BP_HEADS) return IC3_E_UNSUPPORTED;
+  if (!io->h_prev || !io->h_new || !io->logp || !io->dh_prev) return IC3_E_NULL;
+  if (!L.tanh && (!io->c_prev || !io->dc_prev || !p->x_table || !p->w->lstm_img || !p->w->bias_cat)) return IC3_E_NULL;
+  if (L.tanh && !p->w->f_wT) return IC3_E_NULL;
+  if (!p->w->head_w || !p->w->enc_wT || !p->w->enc_b) return IC3_E_NULL;
+  if (cfg->hard_attn && !io->comm) return IC3_E_NULL;
+  rc = records_check(io->pp_state, io->tj_state, is_tj);
+  if (rc) return rc;
+  rc = finish_args_check(cfg, L, params, grads);
+  if (rc) return rc;
+
+  cudaStream_t s = (cudaStream_t)stream;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
+  rc = bptt_reset(p, L, s);
+  if (rc) return rc;
+  const size_t n4 = (size_t)cfg->B * cfg->N * TC_H / 4;
+  const size_t nblk = (n4 + 255) / 256, cap = (size_t)4 * sm_count();
+  bptt_upstream_kernel<<<(int)(nblk < cap ? nblk : cap), 256, 0, s>>>(
+      n4, reinterpret_cast<const float4*>(io->dh_new), L.tanh ? nullptr : reinterpret_cast<const float4*>(io->dc_new),
+      L.tanh ? nullptr : reinterpret_cast<const float4*>(io->c_prev), reinterpret_cast<float4*>(io->dh_prev),
+      L.tanh ? nullptr : reinterpret_cast<float4*>(io->dc_prev), (float)(L.P - 1),
+      reinterpret_cast<BpttScalars*>(ws + L.sc));
+  IC3_LAUNCH_CHECK();
+  ic3_bptt_step_io st;
+  memset(&st, 0, sizeof(st));
+  st.h_prev = io->h_prev; st.c_prev = L.tanh ? nullptr : io->c_prev; st.h_new = io->h_new;
+  st.comm = io->comm; st.alive = io->alive; st.pp_state = io->pp_state; st.tj_state = io->tj_state;
+  st.logp = io->logp; st.dh = io->dh_prev; st.dc = L.tanh ? nullptr : io->dc_prev; st.err = io->err;
+  rc = bptt_step_on(p, &st, L, npos, is_tj, s, io);
+  if (rc) return rc;
+  return ic3_bptt_finish(p, params, grads, reinterpret_cast<double*>(ws + L.losses), s);
 }
 
 // ==================================================================================================================
@@ -2243,7 +2392,7 @@ extern "C" int ic3_ff_grad_chunk(const ic3_ff_grad_plan* p, const ic3_ff_grad_io
   h.gs_part = reinterpret_cast<double*>(ws + G.gs_part);
   h.sc = reinterpret_cast<BpttScalars*>(ws + G.sc);
   h.q = 0;
-  bptt_heads_kernel<<<(R + HB_ROWS - 1) / HB_ROWS, 256, 0, s>>>(h);
+  bptt_heads_kernel<false><<<(R + HB_ROWS - 1) / HB_ROWS, 256, 0, s>>>(h);
   IC3_LAUNCH_CHECK();
   if (G.impl == IC3_FF_GRAD_TC) {
     FfGradTcChunk c;

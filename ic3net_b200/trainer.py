@@ -981,7 +981,6 @@ class Trainer(object):
     def _param_structs(self):
         """ic3_policy_params of the parameters and of their gradient buffers (reference layouts), by kernel role."""
         net = self.policy_net
-        w = net._kernel_weights()
         scratch = self.__dict__.setdefault('_grad_scratch', {})
 
         def grad_ptr(p):
@@ -994,18 +993,7 @@ class Trainer(object):
                 scratch[key] = torch.zeros_like(p)
             return scratch[key].data_ptr()
 
-        def mk(get):
-            arr = lambda lst: (C.c_void_p * _lib.MAX_HEADS)(*([get(t) for t in lst] + [None] * (_lib.MAX_HEADS - len(lst))))
-            # C_modules[p] per comm pass (share_weights: the same module, so the gradient pointers alias)
-            parr = lambda lst: (C.c_void_p * _lib.MAX_PASSES)(*([get(t) for t in lst] + [None] * (_lib.MAX_PASSES - len(lst))))
-            # the LSTM cell's w_ih / w_hh / b_ih / b_hh, or the tanh cell's f_w / f_b per pass
-            cell = (dict(w_ih=get(w['w_ih']), w_hh=get(w['w_hh']), b_ih=get(w['b_ih']), b_hh=get(w['b_hh']))
-                    if 'w_ih' in w else dict(f_w_pass=parr(w['f_w']), f_b_pass=parr(w['f_b'])))
-            return _lib.PolicyParams(encoder_w=get(w['enc_w']), encoder_b=get(w['enc_b']), c_w=get(w['c_w'][0]),
-                                     c_b=get(w['c_b'][0]), value_w=get(w['value_w']), value_b=get(w['value_b']),
-                                     head_w=arr(w['head_w']), head_b=arr(w['head_b']),
-                                     c_w_pass=parr(w['c_w']), c_b_pass=parr(w['c_b']), **cell)
-        return mk(lambda p: p.data_ptr()), mk(grad_ptr)
+        return net.policy_params(lambda p: p.data_ptr()), net.policy_params(grad_ptr)
 
     # only used when there is a single process (trainer.py:245-256)
     def train_batch(self, epoch):

@@ -524,6 +524,43 @@ int ic3_bptt_finish(const ic3_bptt_plan* plan, const ic3_policy_params* params, 
                     double* losses, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Backward of ONE policy step (one CommNetMLP.forward, comm.py:134-244) under upstream gradients of its outputs, for
+ * an autograd graph built around the module (args.forward_grad = 'kernels').  Same coverage, plan and workspace as the
+ * BPTT kernels above (ic3_bptt_workspace_bytes(plan) bytes; plan->value_coeff and plan->entr are ignored): the kernels
+ * of ic3_bptt_step with d (value, logits) taken from the caller instead of the records --
+ *     d value = dvalue,  d logit_j = dlogp_j - p_j sum_k dlogp_k per head (p = exp of the step's log-probs),
+ * then ic3_bptt_finish.  The step ran without `fresh` (a caller zeroes the state itself) and nothing is cut inside it.
+ * Writes d / d (h_prev, c_prev) and ADDS the parameter gradients into `grads` like ic3_bptt_finish (share_weights may
+ * alias c_w_pass / c_b_pass).  Bad arguments return IC3_E_* before any device work; the call never synchronises with
+ * the host (the operand-scale bound max |c_prev|, max |dh_new|, max |dc_new| is reduced on the device).
+ * ---------------------------------------------------------------------- */
+typedef struct {
+  /* the step's inputs and outputs (device) */
+  const float* h_prev;          /* [B*N, H] state entering the step */
+  const float* c_prev;          /* [B*N, H] LSTM cell (ignored for the tanh cell) */
+  const float* h_new;           /* [B*N, H] h' the step returned */
+  const float* logp;            /* [B*N, sum(na)] log-probs the step returned */
+  const uint8_t* comm;          /* [B, N] info['comm_action'] (required with hard_attn) */
+  const uint8_t* alive;         /* [B, N] info['alive_mask'] or NULL */
+  /* environment state the observation was taken from (HOST pointer to a struct of device pointers, the one matching
+     the plan's env): predator-prey reads loc, traffic junction loc / alive / last_act / route_id */
+  const ic3_pp_state* pp_state;
+  const ic3_tj_state* tj_state;
+  /* upstream gradients d loss / d outputs; NULL = zero */
+  const float* dlogp;           /* [B*N, sum(na)] */
+  const float* dvalue;          /* [B*N] */
+  const float* dh_new;          /* [B*N, H] */
+  const float* dc_new;          /* [B*N, H] (ignored for the tanh cell) */
+  /* outputs */
+  float* dh_prev;               /* [B*N, H] d loss / d h_prev */
+  float* dc_prev;               /* [B*N, H] d loss / d c_prev (LSTM cell: required; tanh cell: ignored) */
+  int32_t* err;                 /* device flag word (IC3_ERR_PIPELINE / IC3_ERR_FP16_RANGE), may be NULL */
+} ic3_policy_bwd_io;
+
+int ic3_policy_step_backward(const ic3_bptt_plan* plan, const ic3_policy_bwd_io* io, const ic3_policy_params* params,
+                             const ic3_policy_params* grads, void* stream);
+
+/* ------------------------------------------------------------------------
  * Gradient of the rollout loss (Trainer.compute_grad, trainer.py:128-225) for the NON-RECURRENT tanh policies:
  * models.MLP (models.py:23-25) and CommNet / IC3Net without --recurrent (comm.py:127-129, 179, 220-224), i.e.
  * cfg->cell == IC3_CELL_TANH, x_tanh = h_from_x = 1, 1 .. IC3_MAX_PASSES passes (share_weights included), hard attention,
