@@ -135,10 +135,7 @@ class PolicyBwdIO(C.Structure):
 class FfGradPlan(C.Structure):
     _fields_ = [("cfg", C.POINTER(PolicyCfg)), ("w", C.POINTER(PolicyPacked)), ("pp_env", C.POINTER(PPCfg)),
                 ("tj_env", C.POINTER(TJCfg)), ("value_coeff", C.c_float), ("entr", C.c_float), ("max_rows", C.c_int32),
-                ("impl", C.c_int32), ("workspace", _p)]
-
-
-FF_GRAD_SIMT, FF_GRAD_TC = 0, 1          # FfGradPlan.impl (IC3_FF_GRAD_SIMT / IC3_FF_GRAD_TC)
+                ("reserved0", C.c_int32), ("workspace", _p)]
 
 
 class FfGradIO(C.Structure):

@@ -1852,36 +1852,32 @@ extern "C" int ic3_policy_step_backward(const ic3_bptt_plan* p, const ic3_policy
 // ==================================================================================================================
 // Non-recurrent tanh policies (models.MLP, CommNet / IC3Net without --recurrent): ic3_ff_grad_*.  No state crosses a
 // step, so a chunk of K consecutive lock-steps is one batch of K*B env slots.  Per chunk:
+//   records   the chunk's env records, slots of valid = 0 given an empty state                   [ff_records_kernel]
 //   desc      observation pattern of every row (position, counts / scalars, constant)           [ff_desc_kernel]
 //   forward   index encoder + the SIMT step's pass-state form (ic3_policy_ff_states): tanh(x), h_1 .. h_P, S_0 .. S_{P-1}
 //   heads     d loss / d (value, logits), head weight gradients, loss sums                       [bptt_heads_kernel]
-//   pass p    dz = g (1 - h_{p+1}^2), dx += dz, g = dz F_p + comm^T(dz C_p)  (tile of whole envs) [ff_pass_kernel]
-//             G_F += dz^T h_p, G_C += dz^T S_p, g_b += sum dz  (fixed row blocks)               [ff_wgrad_kernel]
-//   encoder   dpre = (dx + g) (1 - tanh(x)^2);  Y += dpre^T P                                    [ff_dpre_kernel, ff_wgrad_kernel<true>]
+//   pass p    dz = g (1 - h_{p+1}^2), dx += dz, g = dz F_p + comm^T(dz C_p)  (tiles of whole envs)
+//             G_F += dz^T h_p, G_C += dz^T S_p, g_b += sum dz  (fixed row blocks)
+//   encoder   dpre = (dx + g) (1 - tanh(x)^2);  Y += dpre^T P
+// The pass and encoder products run on the tensor cores (ff_grad_tc.cu; ic3_ff_grad_begin packs their weight images).
 // ic3_ff_grad_finish sums the row-block partials in float64 and folds Y through the observation layout like the BPTT
-// finish (bptt_finish_misc_kernel).  All fp32 SIMT arithmetic; every sum has a fixed order.
-// plan->impl == IC3_FF_GRAD_TC replaces the pass and encoder kernels by the tensor-core ones of ff_grad_tc.cu (same
-// records, forward, heads, partials and finish).
+// finish (bptt_finish_misc_kernel).  Every sum has a fixed order.
 // ==================================================================================================================
 namespace {
 
-constexpr int FF_ROWS = 64;        // agent rows per CTA of ff_pass_kernel (whole envs, as in policy_step_kernel)
 constexpr int FF_NB = 256;         // row blocks of the weight-gradient sums (fixed: the partition does not depend on the card)
-constexpr int FF_WK = 16;          // rows staged per iteration of ff_wgrad_kernel
 
 struct FfGeom {
   int npos, WW, is_tj, np, npad, ne;   // positions, window cells, env kind, pattern columns, padded to 128, columns >= npos
   int P, comm, R;                      // passes, communication on, max rows
-  size_t x, hs, ss, g, dx, dz, dout, pos, ext, rloc, rroute, ralive, rlast, apost, fw, cw, fpart, cpart, bpart, ypart,
+  size_t x, hs, ss, g, dx, dz, dout, pos, ext, rloc, rroute, ralive, rlast, apost, fpart, cpart, bpart, ypart,
       gw_part, gs_part, sc, Y, total;
-  size_t tc;                           // IC3_FF_GRAD_TC: weight images and operand-scale words (ff_grad_tc.cu)
-  int nhb, impl;
+  size_t tc;                           // weight images and operand-scale words (ff_grad_tc.cu)
+  int nhb;
 };
 
 int ff_geometry(const ic3_ff_grad_plan* p, FfGeom* G) {
   if (!p || !p->cfg) return IC3_E_NULL;
-  if (p->impl != IC3_FF_GRAD_SIMT && p->impl != IC3_FF_GRAD_TC) return IC3_E_UNSUPPORTED;
-  G->impl = p->impl;
   const ic3_policy_cfg* cfg = p->cfg;
   if (cfg->H != TC_H || cfg->cell != IC3_CELL_TANH || !cfg->x_tanh || !cfg->h_from_x) return IC3_E_UNSUPPORTED;
   if (cfg->passes < 0 || cfg->passes > IC3_MAX_PASSES) return IC3_E_UNSUPPORTED;
@@ -1937,9 +1933,7 @@ int ff_geometry(const ic3_ff_grad_plan* p, FfGeom* G) {
   G->ralive = take(R);
   G->rlast = take(R);
   G->apost = take(R);                        // alive_post AND valid: what the heads backward reads
-  G->fw = take((size_t)G->P * HH);
-  G->cw = take(G->comm ? (size_t)G->P * HH : 0);
-  G->tc = take(G->impl == IC3_FF_GRAD_TC ? ic3_ff_grad_tc_bytes(G->P, G->comm) : 0);
+  G->tc = take(ic3_ff_grad_tc_bytes(G->P, G->comm));
   // accumulators, zeroed by ic3_ff_grad_begin (fpart .. end)
   G->fpart = take((size_t)G->P * FF_NB * HH);
   G->cpart = take(G->comm ? (size_t)G->P * FF_NB * HH : 0);
@@ -1951,14 +1945,6 @@ int ff_geometry(const ic3_ff_grad_plan* p, FfGeom* G) {
   G->Y = take((size_t)TC_H * G->npad * 8);
   G->total = off;
   return IC3_OK;
-}
-
-// out[p][n][k] = in[p][k][n]: the SIMT-packed K-major f_wT / c_wT back to the module layout [out unit n][in unit k]
-__global__ void ff_transpose_kernel(const float* __restrict__ in, float* __restrict__ out, int P) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= P * TC_H * TC_H) return;
-  const int p = idx / (TC_H * TC_H), r = idx - p * TC_H * TC_H, n = r >> 7, k = r & 127;
-  out[idx] = in[(size_t)p * TC_H * TC_H + k * TC_H + n];
 }
 
 // Observation pattern of every row (the columns of prep_kernel's P image): pos = one-hot column of the agent position
@@ -2053,212 +2039,6 @@ __global__ void __launch_bounds__(256) ff_records_kernel(RecArgs a) {
   }
 }
 
-// One backward pass p over a tile of whole environments: dz = g (1 - h_{p+1}^2) (g of the last pass: the heads'
-// dout . W_heads), dx (+)= dz, g <- dz F_p + comm^T(dz C_p) with the forward's gate and mean rules (policy_step_kernel).
-struct PassArgs {
-  int R, N, last, first_acc, comm, hard_attn, comm_avg, nout;
-  const float* h_out;        // [R, H] h_{p+1}
-  const float* dout;         // [R, 8]
-  const float* head_w;       // packed [1 + atot, H]
-  const float* fw;           // [H, H] F_p as f.weight [n][k]
-  const float* cw;           // [H, H] C_p as C.weight [n][k]
-  const uint8_t* fresh; const uint8_t* comm_action; const uint8_t* alive; const uint8_t* valid;
-  float* g; float* dx; float* dz;
-};
-
-__global__ void __launch_bounds__(256) ff_pass_kernel(PassArgs a) {
-  __shared__ __align__(16) float s_dz[FF_ROWS][TC_H];   // dz of the tile, then (after the GEMMs) dS = dz C_p
-  __shared__ float s_gate[FF_ROWS], s_gs[FF_ROWS];
-  const int N = a.N, epb = FF_ROWS / N;
-  const int e0 = blockIdx.x * epb;
-  const int nrows = min(epb * N, a.R - e0 * N);
-  const size_t row0 = (size_t)e0 * N;
-  const int tid = threadIdx.x, tx = tid & 31, ty = tid >> 5;
-  for (int idx = tid; idx < FF_ROWS * TC_H; idx += 256) {
-    const int r = idx >> 7, c = idx & 127;
-    float d = 0.f;
-    if (r < nrows && (!a.valid || a.valid[e0 + r / N])) {
-      const size_t o = (row0 + r) * TC_H + c;
-      float gin;
-      if (a.last) {
-        gin = 0.f;
-        for (int k = 0; k < a.nout; ++k) gin = fmaf(a.dout[(row0 + r) * BP_HEADS + k], __ldg(a.head_w + k * TC_H + c), gin);
-      } else {
-        gin = a.g[o];
-      }
-      const float h = a.h_out[o];
-      d = gin * (1.f - h * h);
-    }
-    s_dz[r][c] = d;
-    if (r < nrows) {
-      const size_t o = (row0 + r) * TC_H + c;
-      a.dz[o] = d;
-      a.dx[o] = a.first_acc ? d : a.dx[o] + d;
-    }
-  }
-  for (int r = tid; r < FF_ROWS; r += 256) {      // comm gate and mean factor, as policy_step_kernel stage A
-    float g = 0.f, den = 1.f;
-    if (r < nrows) {
-      const int el = r / N, e = e0 + el, i = r - el * N;
-      const bool fr = a.fresh && a.fresh[e];
-      int n_alive = N, al = 1;
-      if (a.alive && !fr) {
-        n_alive = 0;
-        for (int j = 0; j < N; ++j) n_alive += a.alive[(size_t)e * N + j] != 0;
-        al = a.alive[(size_t)e * N + i] != 0;
-      }
-      int cm = 1;
-      if (a.hard_attn) cm = fr ? 0 : (a.comm_action[(size_t)e * N + i] != 0);
-      g = (float)(al * cm);
-      if (a.comm_avg && n_alive > 1) den = (float)(n_alive - 1);
-    }
-    s_gate[r] = g;
-    s_gs[r] = g / den;
-  }
-  __syncthreads();
-  // thread: rows ty * 8 .. + 7, columns tx * 4 .. + 3
-  float af[8][4], ac[8][4];
-#pragma unroll
-  for (int r = 0; r < 8; ++r)
-#pragma unroll
-    for (int c = 0; c < 4; ++c) af[r][c] = ac[r][c] = 0.f;
-  for (int n = 0; n < TC_H; n += 4) {
-    float4 av[8];
-#pragma unroll
-    for (int r = 0; r < 8; ++r) av[r] = *reinterpret_cast<const float4*>(&s_dz[ty * 8 + r][n]);
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const float4 bf = __ldg(reinterpret_cast<const float4*>(a.fw + (size_t)(n + q) * TC_H) + tx);
-      float4 bc = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (a.comm) bc = __ldg(reinterpret_cast<const float4*>(a.cw + (size_t)(n + q) * TC_H) + tx);
-#pragma unroll
-      for (int r = 0; r < 8; ++r) {
-        const float v = q == 0 ? av[r].x : (q == 1 ? av[r].y : (q == 2 ? av[r].z : av[r].w));
-        af[r][0] = fmaf(v, bf.x, af[r][0]); af[r][1] = fmaf(v, bf.y, af[r][1]);
-        af[r][2] = fmaf(v, bf.z, af[r][2]); af[r][3] = fmaf(v, bf.w, af[r][3]);
-        ac[r][0] = fmaf(v, bc.x, ac[r][0]); ac[r][1] = fmaf(v, bc.y, ac[r][1]);
-        ac[r][2] = fmaf(v, bc.z, ac[r][2]); ac[r][3] = fmaf(v, bc.w, ac[r][3]);
-      }
-    }
-  }
-  __syncthreads();
-  float (*s_ds)[TC_H] = s_dz;
-  if (a.comm) {
-#pragma unroll
-    for (int r = 0; r < 8; ++r)
-      *reinterpret_cast<float4*>(&s_ds[ty * 8 + r][tx * 4]) = make_float4(ac[r][0], ac[r][1], ac[r][2], ac[r][3]);
-  }
-  __syncthreads();
-#pragma unroll
-  for (int r = 0; r < 8; ++r) {
-    const int row = ty * 8 + r;
-    if (row >= nrows) continue;
-    float o[4] = {af[r][0], af[r][1], af[r][2], af[r][3]};
-    if (a.comm && s_gate[row] != 0.f) {
-      // S[m] = gs[m] sum_{j != m, gate j} h[j]  ->  d h[row] += gate[row] sum_{m != row} gs[m] dS[m]
-      const int base = (row / N) * N;
-      float t[4] = {0.f, 0.f, 0.f, 0.f};
-      for (int m = base; m < base + N; ++m) {
-        if (m == row || s_gs[m] == 0.f) continue;
-        const float4 d = *reinterpret_cast<const float4*>(&s_ds[m][tx * 4]);
-        t[0] = fmaf(s_gs[m], d.x, t[0]); t[1] = fmaf(s_gs[m], d.y, t[1]);
-        t[2] = fmaf(s_gs[m], d.z, t[2]); t[3] = fmaf(s_gs[m], d.w, t[3]);
-      }
-#pragma unroll
-      for (int c = 0; c < 4; ++c) o[c] += t[c];
-    }
-    *reinterpret_cast<float4*>(a.g + (row0 + row) * TC_H + tx * 4) = make_float4(o[0], o[1], o[2], o[3]);
-  }
-}
-
-// dpre = (dx + g) (1 - xt^2) into dz (rows of slots with valid = 0 are zero already: dz, dx and g are)
-__global__ void __launch_bounds__(256) ff_dpre_kernel(size_t n4, const float4* __restrict__ xt, const float4* __restrict__ dx,
-                                                      const float4* __restrict__ g, float4* __restrict__ out) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-    const float4 x = xt[i], d = dx[i], q = g[i];
-    out[i] = make_float4((d.x + q.x) * (1.f - x.x * x.x), (d.y + q.y) * (1.f - x.y * x.y), (d.z + q.z) * (1.f - x.z * x.z),
-                         (d.w + q.w) * (1.f - x.w * x.w));
-  }
-}
-
-// part[blk][n][ld] (+)= sum over the rows of block blk of A[r][n] * B[r][c]  (columns c of tile blockIdx.y), rows in
-// increasing order.  PAT: B is the observation pattern (pos, ext) of ff_desc_kernel; else B = b[blockIdx.y] dense [R, H].
-// bsum (dense, tile 0 only): bsum[blk][n] (+)= sum of A[r][n].
-struct WgradFfArgs {
-  int R, ld, npos, ne;
-  const float* A;
-  const float* b[2];
-  float* part[2];
-  size_t part_stride;        // floats per block
-  const int32_t* pos; const float* ext;
-  float* bsum;
-};
-
-template <bool PAT>
-__global__ void __launch_bounds__(256) ff_wgrad_kernel(WgradFfArgs a) {
-  __shared__ __align__(16) float s_a[FF_WK][TC_H];
-  __shared__ __align__(16) float s_b[FF_WK][TC_H];
-  const int tid = threadIdx.x, tn = tid >> 4, tc = tid & 15;
-  const int blk = blockIdx.x, y = blockIdx.y;
-  const long r0 = (long)a.R * blk / FF_NB, r1 = (long)a.R * (blk + 1) / FF_NB;
-  const float* B = PAT ? nullptr : a.b[y];
-  const int c0 = PAT ? y * TC_H : 0;
-  float acc[8][8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-  float bs = 0.f;
-  for (long r = r0; r < r1; r += FF_WK) {
-    for (int idx = tid; idx < FF_WK * TC_H / 4; idx += 256) {
-      const int kk = idx >> 5, q = idx & 31;
-      const long row = r + kk;
-      float4 va = make_float4(0.f, 0.f, 0.f, 0.f), vb = va;
-      if (row < r1) {
-        va = __ldg(reinterpret_cast<const float4*>(a.A + (size_t)row * TC_H) + q);
-        if (PAT) {
-          const int p = a.pos[row];
-          float v[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int c = c0 + 4 * q + j;
-            v[j] = c < a.npos ? (c == p ? 1.f : 0.f) : (c - a.npos < a.ne ? a.ext[(size_t)row * a.ne + c - a.npos] : 0.f);
-          }
-          vb = make_float4(v[0], v[1], v[2], v[3]);
-        } else {
-          vb = __ldg(reinterpret_cast<const float4*>(B + (size_t)row * TC_H) + q);
-        }
-      }
-      *reinterpret_cast<float4*>(&s_a[kk][4 * q]) = va;
-      *reinterpret_cast<float4*>(&s_b[kk][4 * q]) = vb;
-    }
-    __syncthreads();
-    if (!PAT && y == 0 && tid < TC_H) {
-#pragma unroll
-      for (int kk = 0; kk < FF_WK; ++kk) bs += s_a[kk][tid];
-    }
-#pragma unroll
-    for (int kk = 0; kk < FF_WK; ++kk) {
-      float av[8], bv[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) av[i] = s_a[kk][tn + 16 * i];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) bv[j] = s_b[kk][tc + 16 * j];
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-  float* out = (PAT ? a.part[0] + c0 : a.part[y]) + (size_t)blk * a.part_stride;
-#pragma unroll
-  for (int i = 0; i < 8; ++i)
-#pragma unroll
-    for (int j = 0; j < 8; ++j) out[(size_t)(tn + 16 * i) * a.ld + tc + 16 * j] += acc[i][j];
-  if (!PAT && y == 0 && tid < TC_H) a.bsum[(size_t)blk * TC_H + tid] += bs;
-}
-
 // grad[i] += sum_blk part[blk][i] (float64, block order), i < n
 __global__ void ff_reduce_add_kernel(const float* __restrict__ part, size_t stride, int n, float* __restrict__ grad) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2294,15 +2074,7 @@ extern "C" int ic3_ff_grad_begin(const ic3_ff_grad_plan* p, void* stream) {
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
   cudaError_t e = cudaMemsetAsync(ws + G.fpart, 0, G.total - G.fpart, s);
   if (e != cudaSuccess) return (int)e;
-  const int n = G.P * TC_H * TC_H;
-  ff_transpose_kernel<<<(n + 255) / 256, 256, 0, s>>>(p->w->f_wT, reinterpret_cast<float*>(ws + G.fw), G.P);
-  IC3_LAUNCH_CHECK();
-  if (G.comm) {
-    ff_transpose_kernel<<<(n + 255) / 256, 256, 0, s>>>(p->w->c_wT, reinterpret_cast<float*>(ws + G.cw), G.P);
-    IC3_LAUNCH_CHECK();
-  }
-  if (G.impl == IC3_FF_GRAD_TC) return ic3_ff_grad_tc_pack(G.P, G.comm, p->w->f_wT, p->w->c_wT, ws + G.tc, s);
-  return IC3_OK;
+  return ic3_ff_grad_tc_pack(G.P, G.comm, p->w->f_wT, p->w->c_wT, ws + G.tc, s);
 }
 
 extern "C" int ic3_ff_grad_chunk(const ic3_ff_grad_plan* p, const ic3_ff_grad_io* io, void* stream) {
@@ -2394,62 +2166,20 @@ extern "C" int ic3_ff_grad_chunk(const ic3_ff_grad_plan* p, const ic3_ff_grad_io
   h.q = 0;
   bptt_heads_kernel<false><<<(R + HB_ROWS - 1) / HB_ROWS, 256, 0, s>>>(h);
   IC3_LAUNCH_CHECK();
-  if (G.impl == IC3_FF_GRAD_TC) {
-    FfGradTcChunk c;
-    memset(&c, 0, sizeof(c));
-    c.R = R; c.N = N; c.Bk = Bk; c.P = G.P; c.comm = G.comm; c.hard_attn = cfg->hard_attn; c.comm_avg = cfg->comm_avg;
-    c.nout = 1 + atot; c.npos = G.npos; c.ne = G.ne; c.npad = G.npad; c.is_tj = G.is_tj;
-    c.hs = hs; c.ss = ss; c.dout = dout; c.head_w = p->w->head_w;
-    c.fresh = io->fresh; c.comm_action = cfg->hard_attn ? io->comm : nullptr; c.alive = io->alive; c.valid = io->valid;
-    c.g = g; c.dx = dx; c.dz = dz; c.pos = pos; c.ext = ext;
-    c.fpart = reinterpret_cast<float*>(ws + G.fpart);
-    c.cpart = G.comm ? reinterpret_cast<float*>(ws + G.cpart) : nullptr;
-    c.bpart = reinterpret_cast<float*>(ws + G.bpart);
-    c.ypart = reinterpret_cast<float*>(ws + G.ypart);
-    c.nb = FF_NB;
-    c.tc = ws + G.tc;
-    return ic3_ff_grad_tc_chunk(&c, s);
-  }
-  // passes P-1 .. 0
-  const int epb = FF_ROWS / N;
-  for (int ps = G.P - 1; ps >= 0; --ps) {
-    PassArgs a;
-    memset(&a, 0, sizeof(a));
-    a.R = R; a.N = N; a.last = ps == G.P - 1; a.first_acc = ps == G.P - 1; a.comm = G.comm;
-    a.hard_attn = cfg->hard_attn; a.comm_avg = cfg->comm_avg; a.nout = 1 + atot;
-    a.h_out = hs + (size_t)(ps + 1) * RHs;
-    a.dout = dout; a.head_w = p->w->head_w;
-    a.fw = reinterpret_cast<const float*>(ws + G.fw) + (size_t)ps * TC_H * TC_H;
-    a.cw = G.comm ? reinterpret_cast<const float*>(ws + G.cw) + (size_t)ps * TC_H * TC_H : nullptr;
-    a.fresh = io->fresh; a.comm_action = cfg->hard_attn ? io->comm : nullptr; a.alive = io->alive; a.valid = io->valid;
-    a.g = g; a.dx = dx; a.dz = dz;
-    ff_pass_kernel<<<(Bk + epb - 1) / epb, 256, 0, s>>>(a);
-    IC3_LAUNCH_CHECK();
-    WgradFfArgs w;
-    memset(&w, 0, sizeof(w));
-    w.R = R; w.ld = TC_H; w.A = dz;
-    w.b[0] = hs + (size_t)ps * RHs;
-    w.b[1] = G.comm ? ss + (size_t)ps * RHs : nullptr;
-    w.part[0] = reinterpret_cast<float*>(ws + G.fpart) + (size_t)ps * FF_NB * TC_H * TC_H;
-    w.part[1] = G.comm ? reinterpret_cast<float*>(ws + G.cpart) + (size_t)ps * FF_NB * TC_H * TC_H : nullptr;
-    w.part_stride = (size_t)TC_H * TC_H;
-    w.bsum = reinterpret_cast<float*>(ws + G.bpart) + (size_t)ps * FF_NB * TC_H;
-    ff_wgrad_kernel<false><<<dim3(FF_NB, G.comm ? 2 : 1), 256, 0, s>>>(w);
-    IC3_LAUNCH_CHECK();
-  }
-  // encoder: dpre, then dpre^T P
-  ff_dpre_kernel<<<1024, 256, 0, s>>>(RHs / 4, reinterpret_cast<const float4*>(hs), reinterpret_cast<const float4*>(dx),
-                                      reinterpret_cast<const float4*>(g), reinterpret_cast<float4*>(dz));
-  IC3_LAUNCH_CHECK();
-  WgradFfArgs w;
-  memset(&w, 0, sizeof(w));
-  w.R = R; w.ld = G.npad; w.npos = G.npos; w.ne = G.ne; w.A = dz;
-  w.part[0] = reinterpret_cast<float*>(ws + G.ypart);
-  w.part_stride = (size_t)TC_H * G.npad;
-  w.pos = pos; w.ext = ext;
-  ff_wgrad_kernel<true><<<dim3(FF_NB, G.npad / TC_H), 256, 0, s>>>(w);
-  IC3_LAUNCH_CHECK();
-  return IC3_OK;
+  FfGradTcChunk c;
+  memset(&c, 0, sizeof(c));
+  c.R = R; c.N = N; c.Bk = Bk; c.P = G.P; c.comm = G.comm; c.hard_attn = cfg->hard_attn; c.comm_avg = cfg->comm_avg;
+  c.nout = 1 + atot; c.npos = G.npos; c.ne = G.ne; c.npad = G.npad; c.is_tj = G.is_tj;
+  c.hs = hs; c.ss = ss; c.dout = dout; c.head_w = p->w->head_w;
+  c.fresh = io->fresh; c.comm_action = cfg->hard_attn ? io->comm : nullptr; c.alive = io->alive; c.valid = io->valid;
+  c.g = g; c.dx = dx; c.dz = dz; c.pos = pos; c.ext = ext;
+  c.fpart = reinterpret_cast<float*>(ws + G.fpart);
+  c.cpart = G.comm ? reinterpret_cast<float*>(ws + G.cpart) : nullptr;
+  c.bpart = reinterpret_cast<float*>(ws + G.bpart);
+  c.ypart = reinterpret_cast<float*>(ws + G.ypart);
+  c.nb = FF_NB;
+  c.tc = ws + G.tc;
+  return ic3_ff_grad_tc_chunk(&c, s);
 }
 
 extern "C" int ic3_ff_grad_finish(const ic3_ff_grad_plan* p, const ic3_policy_params* params, const ic3_policy_params* grads,

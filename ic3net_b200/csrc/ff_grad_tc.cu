@@ -1,7 +1,7 @@
 // Backward of the non-recurrent tanh policies (models.MLP, CommNet / IC3Net without --recurrent) on the Hopper tensor
-// cores: ic3_ff_grad_* with plan->impl == IC3_FF_GRAD_TC.  The forward re-run, the observation pattern, the heads
-// backward and the float64 finish are those of the SIMT path (bptt_tc.cu); this file replaces its three fp32 SIMT
-// stages.  Per chunk, for p = P-1 .. 0:
+// cores, called from ic3_ff_grad_* (bptt_tc.cu).  The forward re-run, the observation pattern, the heads backward and
+// the float64 finish run in bptt_tc.cu; this file computes the three products of the backward after them.  Per chunk,
+// for p = P-1 .. 0:
 //   dgrad   dz = g (1 - h_{p+1}^2) (g of the last pass: dout . W_heads), dx += dz, then one wgmma product
 //           [dz F_p | dz C_p] (N = 128 without communication, 256 with it) over 128-row tiles of whole envs; the comm
 //           scatter  g += gate (sum_{m != row} gs_m dS_m)  runs in the epilogue from shared memory.  On pass 0 the
@@ -19,8 +19,8 @@
 //             gathers with atomicMax on the bits of non-negative floats
 //   h, S, P   fixed 16 (|h| <= 1, |S| <= N - 1, counts <= N): the predator-prey pattern (one-hot, counts, 1) is exact
 //             in fp16 and needs no lo half; the traffic-junction route ratio is not, so its P is split as well.
-// The weight-gradient row partition is that of the SIMT path (nb fixed blocks, rows in increasing order within a
-// block, fp32 partials summed in float64 in block order by ic3_ff_grad_finish): bit-identical run to run.
+// The weight-gradient row partition is fixed (nb blocks that do not depend on the card, rows in increasing order within
+// a block, fp32 partials summed in float64 in block order by ic3_ff_grad_finish): bit-identical run to run.
 #include <cstddef>
 #include <cstring>
 

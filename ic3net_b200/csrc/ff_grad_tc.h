@@ -1,5 +1,5 @@
 // Internal (non-ABI) interface of the tensor-core backward of the non-recurrent tanh policies (ff_grad_tc.cu), called
-// from ic3_ff_grad_* (bptt_tc.cu) when ic3_ff_grad_plan.impl == IC3_FF_GRAD_TC.
+// from ic3_ff_grad_* (bptt_tc.cu).
 #pragma once
 #include <cuda_runtime.h>
 

@@ -85,11 +85,10 @@ def build_parser():
                              'tanh RNN (IC / IRIC: --recurrent without --commnet, hid_size 128); tc_ff: the tensor-core '
                              'step of the non-recurrent tanh policies (MLP, CommNet / IC3Net without --recurrent, '
                              'hid_size 128)')
-    parser.add_argument('--grad_impl', default='auto', choices=['auto', 'kernels', 'kernels_ff', 'kernels_ff_tc', 'autograd'],
+    parser.add_argument('--grad_impl', default='auto', choices=['auto', 'kernels', 'kernels_ff', 'autograd'],
                         help='compute_grad: hand-written BPTT kernels (auto: whenever the configuration allows), the '
-                             'hand-written kernels of the non-recurrent tanh policies (models.MLP, CommNet / IC3Net '
-                             'without --recurrent; kernels_ff_tc: the same on the tensor cores), or torch autograd '
-                             'recompute')
+                             'hand-written tensor-core kernels of the non-recurrent tanh policies (kernels_ff: '
+                             'models.MLP, CommNet / IC3Net without --recurrent), or torch autograd recompute')
     parser.add_argument('--batch_boundary', default='reference', choices=['reference', 'cut'],
                         help='run_batch: whole episodes until >= batch_size steps per env slot (reference), or a fixed '
                              'number of lock-steps with open episodes cut at the end')

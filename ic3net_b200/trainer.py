@@ -45,9 +45,8 @@ the index encoder and the SIMT step.
 The non-recurrent tanh policies (models.MLP, CommNet / IC3Net without --recurrent) carry nothing from one step to the
 next.  With ``grad_impl = 'kernels_ff'`` their gradient comes from the kernels of ic3_ff_grad_* (csrc/bptt_tc.cu): no
 hidden-state record or checkpoint at all; the backward re-runs the forward from the env-state records over chunks of K
-consecutive lock-steps (K*B env slots at once, K from the memory the device has left, ``FF_CHUNK_STEPS``).
-``grad_impl = 'kernels_ff_tc'`` is the same path with the products of the backward on the tensor cores
-(ic3_ff_grad_plan.impl = IC3_FF_GRAD_TC, csrc/ff_grad_tc.cu); chunking, records and the finish are shared.
+consecutive lock-steps (K*B env slots at once, K from the memory the device has left, ``FF_CHUNK_STEPS``), with the
+products of the backward on the tensor cores (csrc/ff_grad_tc.cu).
 """
 import ctypes as C
 import math
@@ -137,14 +136,10 @@ class Trainer(object):
         # compute_grad implementation: 'kernels' = hand-written BPTT (csrc/bptt_tc.cu; tensor-core policy path with the
         # LSTM cell and 1..4 comm passes, or the tanh RNN without communication on the SIMT path; at most 7 action
         # logits, observation pattern of <= 512 columns), 'kernels_ff' = the non-recurrent tanh policies' kernels,
-        # 'kernels_ff_tc' = the same with the backward's products on the tensor cores, 'autograd' = windowed recompute
-        # under torch autograd.  Default: kernels when the configuration allows.
+        # 'autograd' = windowed recompute under torch autograd.  Default: kernels when the configuration allows.
         self.grad_impl = getattr(args, 'grad_impl', None) or 'auto'
-        if self.grad_impl not in ('auto', 'kernels', 'kernels_ff', 'kernels_ff_tc', 'autograd'):
-            raise ValueError("grad_impl must be 'auto', 'kernels', 'kernels_ff', 'kernels_ff_tc' or 'autograd', not %r"
-                             % (self.grad_impl,))
-        # ic3_ff_grad_plan.impl of the non-recurrent kernels
-        self._ff_impl = _lib.FF_GRAD_TC if self.grad_impl == 'kernels_ff_tc' else _lib.FF_GRAD_SIMT
+        if self.grad_impl not in ('auto', 'kernels', 'kernels_ff', 'autograd'):
+            raise ValueError("grad_impl must be 'auto', 'kernels', 'kernels_ff' or 'autograd', not %r" % (self.grad_impl,))
         self.grad_kernels = False
         self._bptt = None
         self._buf = None
@@ -176,7 +171,7 @@ class Trainer(object):
         if self.grad_impl == 'auto':
             self.grad_impl = 'kernels' if self.grad_kernels else 'autograd'
         # the non-recurrent tanh policies' kernels (ic3_ff_grad_*): no (h, c) records or checkpoints
-        self.grad_ff = self.record_for_grad and self.grad_impl in ('kernels_ff', 'kernels_ff_tc')
+        self.grad_ff = self.record_for_grad and self.grad_impl == 'kernels_ff'
         if self.grad_ff:
             e = env.env
             cfg = policy_net.policy_cfg(e.nenvs)
@@ -884,7 +879,7 @@ class Trainer(object):
         return _lib.FfGradPlan(cfg=C.pointer(cfg), w=None if w is None else C.pointer(w),
                                pp_env=None if self.is_tj else C.pointer(e.cfg), tj_env=C.pointer(e.cfg) if self.is_tj else None,
                                value_coeff=float(args.value_coeff), entr=float(args.entr), max_rows=rows,
-                               impl=self._ff_impl, workspace=workspace)
+                               workspace=workspace)
 
     def _ff_chunk_steps(self, T, cfg):
         """Lock-steps per chunk K of ic3_ff_grad_chunk for a T-step rollout: what the workspace of K steps needs must fit
@@ -903,9 +898,9 @@ class Trainer(object):
         return int(k)
 
     def _compute_grad_ff(self, adv, ret):
-        """grad_impl 'kernels_ff' / 'kernels_ff_tc' (ic3_ff_grad_*): the rollout's T lock-steps in chunks of K consecutive steps, each one
-        batch of K*B env slots (records are [T, B, ...]), in any order since no state crosses a step.  Returns the device
-        float64 vector of the three loss sums."""
+        """grad_impl 'kernels_ff' (ic3_ff_grad_*): the rollout's T lock-steps in chunks of K consecutive steps, each one
+        batch of K*B env slots (records are [T, B, ...]), in any order since no state crosses a step; the backward's
+        products run on the tensor cores.  Returns the device float64 vector of the three loss sums."""
         b, net, args, e = self._buf, self.policy_net, self.args, self.env.env
         lib = _lib.load()
         T, B, N = b['T'], e.nenvs, args.nagents

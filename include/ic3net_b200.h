@@ -578,19 +578,13 @@ int ic3_policy_step_backward(const ic3_bptt_plan* plan, const ic3_policy_bwd_io*
  *     dz = g (1 - h_{p+1}^2);  dx += dz;  dF_p += dz^T h_p;  dC_p += dz^T S_p;  df_b,p += sum dz;  dc_b,p += sum dz;
  *     g = dz F_p + comm^T (dz C_p)
  * and  dpre = (dx + g) (1 - tanh(x)^2),  d encoder = dpre^T obs through the observation pattern (never materialised),
- * d encoder bias = sum dpre.  fp32 SIMT kernels; the sums over agent rows go to fixed per-block partials (no atomics)
- * and are finished in float64, so the gradient is bit-identical from run to run for the same chunk sizes.
- * impl = IC3_FF_GRAD_TC computes the three products of every pass (dz [F_p | C_p], dz^T [h_p | S_p]) and dpre^T obs on
- * the tensor cores (fp16 hi/lo split, three MMAs, fp32 accumulate, power-of-two operand scales); everything else, the
- * coverage, the row partition and the determinism are those of impl 0.  Any other impl: a workspace of 0 bytes.  Slots with
- * valid = 0 contribute exactly zero.  Gradients are ADDED to the `grads` buffers like ic3_bptt_finish (c_w_pass /
- * c_b_pass / f_w_pass / f_b_pass per pass; index 0 or NULL of c_*_pass: c_w / c_b; share_weights may alias them).
+ * d encoder bias = sum dpre.  The three products of every pass (dz [F_p | C_p], dz^T [h_p | S_p]) and dpre^T obs run on
+ * the tensor cores: fp16 hi/lo split, three MMAs, fp32 accumulate, power-of-two operand scales.  The sums over agent
+ * rows go to a fixed partition of row blocks (it does not depend on the card; no atomics) and are finished in float64,
+ * so the gradient is bit-identical from run to run for the same chunk sizes.  Slots with valid = 0 contribute exactly
+ * zero.  Gradients are ADDED to the `grads` buffers like ic3_bptt_finish (c_w_pass / c_b_pass / f_w_pass / f_b_pass
+ * per pass; index 0 or NULL of c_*_pass: c_w / c_b; share_weights may alias them).
  * ---------------------------------------------------------------------- */
-enum {
-  IC3_FF_GRAD_SIMT = 0,
-  IC3_FF_GRAD_TC = 1
-};
-
 typedef struct {
   const ic3_policy_cfg* cfg;    /* HOST pointers: the structs the rollout used (cfg->B = env slots of one lock-step) */
   const ic3_policy_packed* w;   /* SIMT-packed weights of the CURRENT parameters */
@@ -599,7 +593,7 @@ typedef struct {
   float value_coeff;            /* args.value_coeff (trainer.py:209) */
   float entr;                   /* args.entr (trainer.py:211-220) */
   int32_t max_rows;             /* chunk capacity in agent rows (>= cfg->B * cfg->N) */
-  int32_t impl;                 /* IC3_FF_GRAD_SIMT (0): fp32 SIMT kernels; IC3_FF_GRAD_TC (1): tensor-core kernels */
+  int32_t reserved0;
   void* workspace;              /* device scratch of ic3_ff_grad_workspace_bytes(plan) bytes */
 } ic3_ff_grad_plan;
 

@@ -1,9 +1,12 @@
-"""CPU tests of the non-recurrent gradient entry points (ic3_ff_grad_*): zero workspaces for the configurations the kernels
-do not implement and IC3_E_* codes from the host-side checks, with no device work."""
+"""CPU tests of the non-recurrent gradient entry points (ic3_ff_grad_*): the plan's layout, zero workspaces for the
+configurations the kernels do not implement and IC3_E_* codes from the host-side checks, with no device work."""
 import ctypes as C
+import os
+import subprocess
 
 import pytest
 
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 E_NULL, E_RANGE, E_UNSUPPORTED = -1, -2, -3
 
 
@@ -28,9 +31,24 @@ def nbytes(_lib, lib, pol, env, rows=80, **kw):
     return int(lib.ic3_ff_grad_workspace_bytes(C.byref(plan))), plan, (cfg, pp)
 
 
+def test_plan_layout_matches_header(tmp_path):
+    from ic3net_b200 import _lib
+    prog = ('#include <stdio.h>\n#include <stddef.h>\n#include "ic3net_b200.h"\n'
+            'int main(){printf("%zu %zu %zu\\n", sizeof(ic3_ff_grad_plan), offsetof(ic3_ff_grad_plan, reserved0),'
+            ' offsetof(ic3_ff_grad_plan, workspace)); return 0;}')
+    c = tmp_path / "p.c"
+    c.write_text(prog)
+    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(c), "-o", str(tmp_path / "p")])
+    size, off, off_ws = map(int, subprocess.check_output([str(tmp_path / "p")]).split())
+    assert size == C.sizeof(_lib.FfGradPlan)
+    assert off == _lib.FfGradPlan.reserved0.offset and off_ws == _lib.FfGradPlan.workspace.offset
+    assert off == _lib.FfGradPlan.max_rows.offset + 4 and off_ws == off + 4
+
+
 def test_supported_configurations_get_a_workspace():
     _lib, lib, pol, env = setup()
-    for kw in (dict(), dict(passes=1), dict(passes=4), dict(hard_attn=0, comm_avg=0), dict(comm_mask_zero=1, passes=1)):
+    for kw in (dict(), dict(passes=1), dict(passes=4), dict(hard_attn=0, comm_avg=0), dict(comm_mask_zero=1, passes=1),
+               dict(comm_mask_zero=1, passes=3)):
         assert nbytes(_lib, lib, pol, env, **kw)[0] > 0, kw
     small, _, _ = nbytes(_lib, lib, pol, env, rows=80)
     big, _, _ = nbytes(_lib, lib, pol, env, rows=800)

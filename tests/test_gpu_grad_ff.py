@@ -1,5 +1,5 @@
-"""The gradient kernels of the non-recurrent tanh policies (ic3_ff_grad_*, grad_impl 'kernels_ff'): models.MLP and the
-CommNet / IC3Net without --recurrent.
+"""The gradient kernels of the non-recurrent tanh policies (ic3_ff_grad_*, grad_impl 'kernels_ff', the backward's
+products on the tensor cores in csrc/ff_grad_tc.cu): models.MLP and the CommNet / IC3Net without --recurrent.
 
 Covered:
   - the kernels against the float64 oracle of tests/ff_oracle.py (pinned to the unmodified reference by
@@ -7,14 +7,17 @@ Covered:
     fixture; one slot with a fixture's seed and env id against the reference's stored gradient arrays;
   - the kernels against a float64 backward over the trainer's own records (ff_oracle.records_reference): predator-prey
     hard with 8192 slots and traffic-junction hard with 4096 slots, 1, 2 and 4 passes with and without share_weights,
-    and row counts around every threshold the path uses (64-row env tiles, 256-row heads blocks, the 256-block row
-    partition of the weight-gradient sums, its 16-row slabs);
+    comm_mode sum; row counts around every threshold the path uses (128-row dgrad tiles, 256-row heads blocks, the
+    256-block row partition of the weight-gradient sums, the persistent grid) with the workspace poisoned (NaN) past
+    the rows of each chunk, and 1 .. 32 agents per env; gradients around 1e-6 and 1e2 (both ends of the operand
+    scaling);
   - a cross-check against the torch-autograd recompute of the same rollout;
   - chunk sizes K = 1, a K that does not divide T, and K >= T; bit-identical gradients run to run;
   - the pass-state recompute (ic3_policy_ff_states): every h block against ic3_policy_step with that many passes, bit
     for bit, and every S block against the gated mean of the block before it;
   - slots that completed their batch (valid = 0) contribute exactly nothing, whatever their records hold;
-  - train_batch end to end for each family on both environments with no device error flag.
+  - train_batch end to end for each family on both environments with no device error flag, and the command line;
+  - refusals: NotImplementedError outside the kernels' coverage, ValueError for unknown grad_impl values.
 
 Bar (that of tests/test_gpu_bptt_rnn.py): per tensor 1e-4 of its largest entry, the encoder weight also per input column,
 the action heads also 2^-20 of their sum of |terms|; loss sums rtol 2e-4."""
@@ -216,26 +219,93 @@ def test_gradient_matches_float64_records(name, family, over):
     check_records(tr, "%s %s %s" % (name, family, over))
 
 
-@pytest.mark.parametrize("name,family,over", [(PP, "ic3net", dict(comm_passes=2)), (TJ, "ic3net", dict(comm_passes=2)),
-                                              (PP, "mlp", {})])
+@pytest.mark.parametrize("name,family,over", [
+    (PP, "ic3net", dict(comm_passes=2)),
+    (TJ, "ic3net", dict(comm_passes=2)),
+    (PP, "mlp", {}),
+    (PP, "ic3net", {}),
+    (PP, "commnet", dict(comm_passes=2)),
+    (PP, "commnet", dict(comm_passes=2, share_weights=True)),
+    (PP, "ic3net", dict(comm_passes=4)),
+    (PP, "ic3net", dict(comm_passes=4, share_weights=True)),
+    (TJ, "commnet", dict(comm_passes=3, share_weights=True, comm_mode="sum")),
+])
 def test_full_size_gradient_matches_float64(name, family, over):
-    """81 920 rows per step at predator-prey hard (8192 slots), 81 920 at traffic-junction hard (4096 slots)."""
+    """81 920 rows per step at predator-prey hard (8192 slots), 81 920 at traffic-junction hard (4096 slots).
+    tests/test_gpu_ff_tc.py runs it on the tc_ff forward."""
     B = 8192 if name == PP else 4096
     tr = make_trainer(name, B, family, seed=5, id0=0, batch_size=10, **over)
     tr.run_batch(0)
     check_records(tr, "%s B=%d %s %s" % (name, B, family, over))
 
 
-@pytest.mark.parametrize("B", [1, 7, 26, 411])
-def test_row_counts_around_thresholds(B):
-    """One step per chunk (R = 10 B rows at predator-prey hard): B = 1 (fewer rows than one 16-row slab and than the
-    256 row blocks: most blocks empty), 7 (two 64-row env tiles of 6 envs, the second partial), 26 (260 rows: a second
-    heads block of 4 rows), 411 (4110 rows: 16 or 17 rows per row block, slab tails of 0 or 1 row)."""
+class _PoisonedWorkspace:
+    """Stands in for the trainer module's torch: byte buffers (the gradient workspace) start as 0xFF, a NaN in every
+    float lane, so nothing the kernels read past a chunk's rows (or before they write it) goes unnoticed."""
+
+    def __getattr__(self, k):
+        return getattr(torch, k)
+
+    @staticmethod
+    def empty(*a, **kw):
+        t = torch.empty(*a, **kw)
+        if kw.get("dtype") == torch.uint8:
+            t.fill_(0xFF)
+        return t
+
+
+def poisoned_check(tr, monkeypatch, K, label):
+    from ic3net_b200 import trainer as trainer_mod
+    tr.FF_CHUNK_STEPS = K
+    with monkeypatch.context() as m:
+        m.setattr(trainer_mod, "torch", _PoisonedWorkspace())
+        check_records(tr, label)
+    assert tr.ff_chunk_steps == min(K, tr._buf["T"])
+
+
+@pytest.mark.parametrize("B", [1, 7, 12, 13, 25, 26, 411, 819, 821, "grid", "grid+1"])
+def test_row_counts_around_thresholds(B, monkeypatch):
+    """Env counts at predator-prey hard (10 agents: 12 envs = 120 rows per 128-row dgrad tile): one env, one tile, one
+    tile + 1 env, fewer rows than the 256 row blocks, 32-row slabs at the block size, the persistent grid (one tile per
+    SM: 'grid') and one env past it; 7 envs fill part of one tile, 26 envs (260 rows) give a second heads block of 4
+    rows, 411 (4110 rows) 16 or 17 rows per row block.  Each with a chunk size that leaves a ragged last chunk, and with
+    one step per chunk."""
+    if isinstance(B, str):
+        B = 12 * torch.cuda.get_device_properties(0).multi_processor_count + (B == "grid+1")
     tr = make_trainer(PP, B, "ic3net", comm_passes=2, seed=77, id0=3, batch_size=14, max_steps=10)
-    tr.FF_CHUNK_STEPS = 1
     tr.run_batch(0)
-    check_records(tr, "B=%d R=%d" % (B, B * tr.args.nagents))
-    assert tr.ff_chunk_steps == 1
+    T = tr._buf["T"]
+    K = next((k for k in range(2, T) if T % k), 1)          # a ragged last chunk: rows past R in the workspace
+    poisoned_check(tr, monkeypatch, K, "B=%d R=%d K=%d" % (B, B * tr.args.nagents, K))
+    poisoned_check(tr, monkeypatch, 1, "B=%d K=1" % B)
+
+
+@pytest.mark.parametrize("name,N", [(PP, 1), (PP, 2), (PP, 3), (PP, 11), (PP, 31), (TJ, 32)])
+@pytest.mark.parametrize("family,over", [("ic3net", dict(comm_passes=2)), ("commnet", dict(comm_passes=3, comm_mode="sum")),
+                                         ("mlp", {})])
+def test_agents_per_env(name, N, family, over, monkeypatch):
+    """floor(128 / N) envs per dgrad tile, 128 mod N padding rows, 37 envs: a ragged last tile."""
+    agents = dict(nagents=N, nfriendly=N) if name == PP else dict(nagents=N)
+    tr = make_trainer(name, 37, family, batch_size=6, **agents, **over)
+    tr.run_batch(0)
+    poisoned_check(tr, monkeypatch, 3, "%s N=%d %s %s" % (name, N, family, over))
+
+
+@pytest.mark.parametrize("factor", [1e-5, 1e3])
+@pytest.mark.parametrize("family,over", [("ic3net", dict(comm_passes=2)), ("mlp", {})])
+def test_small_and_large_gradients(factor, family, over):
+    """The head weights are scaled after the rollout: d loss / d h_P, and with it every dz, dpre and every gradient but
+    the heads', scales by the same factor (|dz| around 1e-6 and 1e2); the records stay as they are."""
+    tr = make_trainer(PP, 96, family, **over)
+    tr.run_batch(0)
+    with torch.no_grad():
+        for k, p in tr.policy_net.named_parameters():
+            if k.endswith(".weight") and ("heads." in k or "value_head" in k):
+                p.mul_(factor)
+    got, ref = check_records(tr, "%s %s x%g" % (family, over, factor))
+    enc = encoder_name(got)
+    scale = float(ref[enc].abs().max())
+    assert 1e-9 < scale < 1e6, scale
 
 
 CASES = [
@@ -388,3 +458,47 @@ def test_train_batch(name, family):
     assert stat["num_steps"] > 0 and all(k in stat for k in ("action_loss", "value_loss", "entropy"))
     changed = [not torch.equal(a, p.detach()) for a, p in zip(before, tr.policy_net.parameters())]
     assert any(changed)
+
+
+def test_command_line(capsys):
+    from ic3net_b200 import main as cli
+    rc = cli.main(["--env_name", "predator_prey", "--nagents", "3", "--dim", "5", "--max_steps", "20", "--hid_size", "128",
+                   "--commnet", "--comm_passes", "2", "--grad_impl", "kernels_ff", "--nenvs", "64", "--num_epochs", "1",
+                   "--epoch_size", "1", "--batch_size", "40"])
+    out = capsys.readouterr().out
+    assert rc == 0 and "Epoch" in out, out[-2000:]
+
+
+def test_refusals():
+    from ic3net_b200 import data, models
+    from ic3net_b200.trainer import Trainer
+    import test_gpu_tj_scalar as ts
+    with pytest.raises(NotImplementedError, match="kernels_ff"):      # CommNet / IC3Net with the LSTM cell
+        make_trainer(PP, 4, "ic3net", recurrent=True, rnn_type="LSTM")
+    with pytest.raises(NotImplementedError, match="kernels_ff"):      # recurrent tanh CommNet
+        make_trainer(PP, 4, "commnet", recurrent=True, rnn_type="MLP")
+    with pytest.raises(NotImplementedError, match="kernels_ff"):      # hid_size 64
+        make_trainer(PP, 4, "ic3net", hid_size=64)
+    with pytest.raises(NotImplementedError, match="kernels_ff"):      # vision 3: a 7 x 7 window
+        make_trainer(PP, 4, "mlp", vision=3)
+    # the IC / IRIC baselines (models.RNN, tanh recurrence)
+    meta, _ = load_golden(PP)
+    args = ns(meta["args"], nenvs=4, seed=1, env_id0=0, obs_mode="index", use_graph=False, policy_impl=None,
+              record_for_grad=True, grad_impl="kernels_ff", commnet=False, ic3net=False, hard_attn=False,
+              recurrent=True, rnn_type="MLP", comm_passes=1, share_weights=False, comm_mask_zero=False)
+    env = data.init(args.env_name, args)
+    finish_args(args, env)
+    with pytest.raises(NotImplementedError, match="kernels_ff"):
+        Trainer(args, models.RNN(args, args.num_inputs), env)
+    # the scalar traffic-junction vocabulary, on the non-recurrent CommNet it would cover with the bool one
+    m, _ = load_golden(ts.GRAD)
+    kw = dict(recurrent=False, rnn_type="MLP", commnet=True, ic3net=False, hard_attn=False, comm_action_one=False)
+    with pytest.raises(NotImplementedError):
+        ts.build(dict(m, args=dict(m["args"], **kw)), 4, "index", "simt", weights=False, record_for_grad=True,
+                 grad_window=16, grad_impl="kernels_ff")
+    # 'auto' still takes autograd for these families; unknown values raise
+    tr = make_trainer(PP, 4, "ic3net", grad_impl="auto")
+    assert tr.grad_impl == "autograd" and not tr.grad_ff
+    for bad in ("kernels_ff_tc", "kernels_ff_tensor"):
+        with pytest.raises(ValueError):
+            make_trainer(PP, 4, "ic3net", grad_impl=bad)
