@@ -1288,6 +1288,28 @@ int env_geometry(const ic3_bptt_plan* p, int* npos, int* WW, int* is_tj) {
   return IC3_OK;
 }
 
+// The plan's agent geometry, with the rules of ff_geometry: one environment, 1 .. IC3_MAX_AGENTS agent rows per env
+// that are the environment's own (the kernels read N rows of recorded env state per slot), the environment's
+// observation width (the row stride of the encoder-weight gradient ic3_bptt_finish writes), 1 .. IC3_MAX_HEADS action
+// heads.  Every entry point calls it before any device work.
+int plan_geometry(const ic3_bptt_plan* p) {
+  const ic3_policy_cfg* cfg = p->cfg;
+  if (!!p->pp_env == !!p->tj_env) return IC3_E_NULL;
+  if (cfg->N < 1 || cfg->N > IC3_MAX_AGENTS || cfg->B < 1 || cfg->nheads < 1 || cfg->nheads > IC3_MAX_HEADS)
+    return IC3_E_RANGE;
+  if (p->pp_env) {
+    const int W = 2 * p->pp_env->vision + 1;
+    // the predator-prey env kernels take fewer than IC3_MAX_AGENTS predators (the prey's row makes 32 with enemy_comm)
+    if (cfg->O != W * W * (p->pp_env->dim * p->pp_env->dim + 4) || ic3_pp_agents(*p->pp_env) != cfg->N ||
+        p->pp_env->N >= IC3_MAX_AGENTS)
+      return IC3_E_RANGE;
+  } else {
+    const int W = 2 * p->tj_env->vision + 1;
+    if (cfg->O != 2 + W * W * p->tj_env->vocab || p->tj_env->N != cfg->N) return IC3_E_RANGE;
+  }
+  return IC3_OK;
+}
+
 // The recorded env state of ic3_bptt_step_io / ic3_ff_grad_io: the fields the backward reads must be set.
 int records_check(const ic3_pp_state* pp, const ic3_tj_state* tj, int is_tj) {
   if (is_tj) return tj && tj->loc && tj->alive && tj->last_act && tj->route_id ? IC3_OK : IC3_E_NULL;
@@ -1297,7 +1319,7 @@ int records_check(const ic3_pp_state* pp, const ic3_tj_state* tj, int is_tj) {
 }  // namespace
 
 extern "C" uint64_t ic3_bptt_workspace_bytes(const ic3_bptt_plan* p) {
-  if (!p || !p->cfg || p->cfg->H != TC_H) return 0;
+  if (!p || !p->cfg || p->cfg->H != TC_H || plan_geometry(p)) return 0;
   int npos, WW, is_tj;
   if (env_geometry(p, &npos, &WW, &is_tj)) return 0;
   // the operand images sum the class terms apart from the counts (ic3_policy_cfg.obs_vocab): the environment's own
@@ -1336,8 +1358,10 @@ static int bptt_reset(const ic3_bptt_plan* p, const Layout& L, cudaStream_t s) {
 // Start of a compute_grad: zero the accumulators and both operand-image sets, build the dgrad weight image, set max |c|.
 extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) {
   if (!p || !p->cfg || !p->w || !p->workspace) return IC3_E_NULL;
+  int rc = plan_geometry(p);
+  if (rc) return rc;
   int npos, WW, is_tj;
-  int rc = env_geometry(p, &npos, &WW, &is_tj);
+  rc = env_geometry(p, &npos, &WW, &is_tj);
   if (rc) return rc;
   Layout L;
   rc = plan_layout(p->cfg, npos, WW, is_tj, &L);
@@ -1443,8 +1467,10 @@ static int bptt_common(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, Layou
       !io->dh)
     return IC3_E_NULL;
   if (p->cfg->H != TC_H) return IC3_E_UNSUPPORTED;
+  int rc = plan_geometry(p);
+  if (rc) return rc;
   int WW;
-  int rc = env_geometry(p, npos, &WW, is_tj);
+  rc = env_geometry(p, npos, &WW, is_tj);
   if (rc) return rc;
   rc = plan_layout(p->cfg, *npos, WW, *is_tj, L);
   if (rc) return rc;
@@ -1686,8 +1712,10 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
                                double* losses, void* stream) {
   if (!p || !params || !grads || !losses || !p->cfg || !p->workspace) return IC3_E_NULL;
   const ic3_policy_cfg* cfg = p->cfg;
+  int rc = plan_geometry(p);
+  if (rc) return rc;
   int npos, WW, is_tj;
-  int rc = env_geometry(p, &npos, &WW, &is_tj);
+  rc = env_geometry(p, &npos, &WW, &is_tj);
   if (rc) return rc;
   Layout L;
   rc = plan_layout(cfg, npos, WW, is_tj, &L);
@@ -1786,7 +1814,7 @@ namespace {
 int finish_args_check(const ic3_policy_cfg* cfg, const Layout& L, const ic3_policy_params* params,
                       const ic3_policy_params* grads) {
   if (!grads->encoder_w || !grads->encoder_b || !grads->value_w || !grads->value_b) return IC3_E_NULL;
-  for (int k = 0; k < cfg->nheads; ++k)
+  for (int k = 0; k < cfg->nheads && k < IC3_MAX_HEADS; ++k)   // the head count is checked by plan_geometry
     if (!grads->head_w[k] || !grads->head_b[k]) return IC3_E_NULL;
   if (L.tanh) return grads->f_w_pass[0] && grads->f_b_pass[0] ? IC3_OK : IC3_E_NULL;
   if (!params->w_ih || !params->c_w || !params->c_b || !grads->w_ih || !grads->w_hh || !grads->b_ih || !grads->b_hh ||
@@ -1814,9 +1842,6 @@ extern "C" int ic3_policy_step_backward(const ic3_bptt_plan* p, const ic3_policy
   Layout L;
   rc = plan_layout(cfg, npos, WW, is_tj, &L);
   if (rc) return rc;
-  int nout = 1;
-  for (int k = 0; k < cfg->nheads; ++k) nout += cfg->head_dim[k];
-  if (nout > BP_HEADS) return IC3_E_UNSUPPORTED;
   if (!io->h_prev || !io->h_new || !io->logp || !io->dh_prev) return IC3_E_NULL;
   if (!L.tanh && (!io->c_prev || !io->dc_prev || !p->x_table || !p->w->lstm_img || !p->w->bias_cat)) return IC3_E_NULL;
   if (L.tanh && !p->w->f_wT) return IC3_E_NULL;
@@ -1826,6 +1851,11 @@ extern "C" int ic3_policy_step_backward(const ic3_bptt_plan* p, const ic3_policy
   if (rc) return rc;
   rc = finish_args_check(cfg, L, params, grads);
   if (rc) return rc;
+  rc = plan_geometry(p);
+  if (rc) return rc;
+  int nout = 1;
+  for (int k = 0; k < cfg->nheads; ++k) nout += cfg->head_dim[k];
+  if (nout > BP_HEADS) return IC3_E_UNSUPPORTED;
 
   cudaStream_t s = (cudaStream_t)stream;
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);

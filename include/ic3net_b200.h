@@ -509,6 +509,10 @@ typedef struct {
   int32_t* err;                 /* device flag word (IC3_ERR_PIPELINE / IC3_ERR_FP16_RANGE), may be NULL */
 } ic3_bptt_step_io;
 
+/* Every entry point below checks the plan's geometry before any device work: B >= 1; cfg->N in 1 .. IC3_MAX_AGENTS
+ * and equal to the environment's agent rows (predator-prey: pp_env->N < IC3_MAX_AGENTS predators, + 1 with
+ * enemy_comm; traffic junction: tj_env->N); cfg->O the environment's observation width; nheads in 1 .. IC3_MAX_HEADS.
+ * A plan that fails gets 0 bytes and IC3_E_RANGE (neither or both environments: IC3_E_NULL). */
 uint64_t ic3_bptt_workspace_bytes(const ic3_bptt_plan* plan);   /* 0 = configuration not supported by the kernels */
 int ic3_bptt_begin(const ic3_bptt_plan* plan, float c_abs_max, void* stream);
 int ic3_bptt_step(const ic3_bptt_plan* plan, const ic3_bptt_step_io* io, void* stream);

@@ -454,7 +454,7 @@ def test_tanh_cell_with_communication_gets_no_workspace():
     from ic3net_b200 import _lib
     lib = _lib.load()
     hd = (C.c_int32 * _lib.MAX_HEADS)(5, 0, 0, 0)
-    pol = dict(B=4, N=3, H=128, O=99, nheads=1, head_dim=hd, hard_attn=0, comm_avg=1, comm_mask_zero=1, env_id0=0, seed=1,
+    pol = dict(B=4, N=3, H=128, O=9 * 13, nheads=1, head_dim=hd, hard_attn=0, comm_avg=1, comm_mask_zero=1, env_id0=0, seed=1,
                obs_off=0, obs_vocab=13, obs_ncount=2, cell=_lib.CELL_TANH, passes=1, x_tanh=0, h_from_x=0)
     env = _lib.PPCfg(B=4, N=3, dim=3, vision=1, mode=0, naction=5, env_id0=0, enemy_comm=0, seed=1)
 
