@@ -31,6 +31,7 @@ ERR_ROUTE_OVERRUN = 2
 ERR_BAD_ACTION = 4
 ERR_PIPELINE = 0x100
 ERR_FP16_RANGE = 0x200
+ERR_GRAD_DIV = 0x400
 
 PP_MODES = {"mixed": 0, "cooperative": 1, "competitive": 2}
 
@@ -187,6 +188,7 @@ SYMBOLS = {
                                    _PTR]),
     "ic3_bptt_workspace_bytes": (C.c_uint64, [C.POINTER(BpttPlan)]),
     "ic3_bptt_begin": (C.c_int, [C.POINTER(BpttPlan), C.c_float, _PTR]),
+    "ic3_bptt_begin_dev": (C.c_int, [C.POINTER(BpttPlan), _PTR, C.c_int64, _PTR]),
     "ic3_bptt_step": (C.c_int, [C.POINTER(BpttPlan), C.POINTER(BpttStepIO), _PTR]),
     "ic3_bptt_prepare": (C.c_int, [C.POINTER(BpttPlan), C.POINTER(BpttStepIO), _PTR]),
     "ic3_bptt_finish": (C.c_int, [C.POINTER(BpttPlan), C.POINTER(PolicyParams), C.POINTER(PolicyParams), _PTR, _PTR]),
@@ -199,6 +201,7 @@ SYMBOLS = {
                                      _PTR]),
     "ic3_stat_reduce": (C.c_int, [C.c_int32, C.c_int32, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR]),
     "ic3_rmsprop_step": (C.c_int, [C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, _PTR, _PTR, _PTR, _PTR]),
+    "ic3_rmsprop_step_dev": (C.c_int, [C.c_int64, C.c_float, C.c_float, C.c_float, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR]),
 }
 
 _lib = None

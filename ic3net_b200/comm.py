@@ -180,17 +180,18 @@ class CommNetMLP(nn.Module):
         W = 2 * env.vision + 1
         return self.policy_impl == 'tc' and W * W <= 25 and getattr(env, 'vocab_type', 'bool') == 'bool'
 
-    def encoder_table(self, env):
+    def encoder_table(self, env, force=False):
         """[positions, H] class part of x per agent position of env (ic3_*_encoder_table) for the current packed
-        weights, rebuilt when they change; one table per environment.  None where the fused index encoder takes no
-        table: no fused encoder (fuses_encoder), or a layout without separate class terms (obs_vocab = 0)."""
+        weights, rebuilt when they change (force: always, for a CUDA graph that replays the build); one table per
+        environment.  None where the fused index encoder takes no table: no fused encoder (fuses_encoder), or a layout
+        without separate class terms (obs_vocab = 0)."""
         if not self.fuses_encoder(env) or self._cfg_proto['obs_vocab'] == 0:
             return None
         w = self.packed()
         key, table = self._enc_tables.get(env, (None, None))
         if table is None:
             table = torch.empty(env.obs_positions, self.hid_size, device=self._dev)
-        if key != self._packed_key:
+        if force or key != self._packed_key:
             lib = _lib.load()
             fn = lib.ic3_tj_encoder_table if isinstance(env.cfg, _lib.TJCfg) else lib.ic3_pp_encoder_table
             cfg = self.policy_cfg(env.nenvs)
@@ -239,11 +240,12 @@ class CommNetMLP(nn.Module):
         self.invalidate_packed()             # assign=True installs new Parameter objects
         return out
 
-    def packed(self):
-        """K-major kernel layout of the parameters; re-packed (one kernel) when any parameter changed."""
+    def packed(self, force=False):
+        """K-major kernel layout of the parameters; re-packed (one kernel) when any parameter changed, or always with
+        force (a CUDA graph capturing the pack, Trainer graph_update)."""
         ps = self._param_list()
         key = tuple((p.data_ptr(), p._version) for p in ps)
-        if self._packed is not None and key == self._packed_key:
+        if self._packed is not None and key == self._packed_key and not force:
             return self._packed
         H, O, P = self.hid_size, self.num_inputs, self.comm_passes
         dev = ps[0].device
@@ -285,6 +287,15 @@ class CommNetMLP(nn.Module):
         _lib.check(_lib.load().ic3_policy_pack(C.byref(cfg), C.byref(params), C.byref(self._packed), _lib.stream()))
         self._packed_key = key
         return self._packed
+
+    def mark_packed_current(self):
+        """A replayed CUDA graph has just re-packed the current parameters (and re-built the encoder tables) on the
+        device: take the parameters' present version counters as the key, so packed() does not pack them again."""
+        key = tuple((p.data_ptr(), p._version) for p in self._param_list())
+        for env, (k, table) in list(self._enc_tables.items()):
+            if k == self._packed_key:
+                self._enc_tables[env] = (key, table)
+        self._packed_key = key
 
     def policy_params(self, get):
         """ic3_policy_params with get(tensor) for every kernel-side tensor by role: get = data_ptr gives the parameters,

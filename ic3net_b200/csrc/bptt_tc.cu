@@ -278,6 +278,29 @@ __global__ void bptt_upstream_kernel(size_t n4, const float4* __restrict__ dh_ne
   }
 }
 
+// ic3_bptt_begin_dev: cmax = max |c[i]| + cadd over n floats (the scalars were zeroed before).  Rounding is monotone, so
+// max(|c| + cadd) is the float ic3_bptt_begin forms from the host maximum, (max |c|) + cadd.
+__global__ void bptt_cmax_kernel(int64_t n, const float* __restrict__ c, float cadd, BpttScalars* sc) {
+  float m = 0.f;
+  const int64_t n4 = (uintptr_t)c & 15 ? 0 : n >> 2;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
+    const float4 v = reinterpret_cast<const float4*>(c)[i];
+    m = fmaxf(m, fmaxf(fmaxf(fabsf(v.x) + cadd, fabsf(v.y) + cadd), fmaxf(fabsf(v.z) + cadd, fabsf(v.w) + cadd)));
+  }
+  for (int64_t i = (n4 << 2) + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+    m = fmaxf(m, fabsf(c[i]) + cadd);
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1) m = fmaxf(m, __shfl_xor_sync(IC3_FULL_MASK, m, s));
+  if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<unsigned*>(&sc->cmax), __float_as_uint(m));
+}
+
+// the scales ic3_bptt_begin copies from the host
+__global__ void bptt_init_scales_kernel(BpttScalars* sc) {
+  sc->scale[0] = sc->scale[1] = 1.f;
+  sc->inv_scale[0] = sc->inv_scale[1] = 1.f;
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // gates: forward gate GEMM re-computed + LSTM cell backward in the epilogue
 // ------------------------------------------------------------------------------------------------------------------
@@ -1159,6 +1182,10 @@ struct BpttStreams {
   cudaEvent_t gates_done[2], wgrad_done[2], prep_done[2], main_done[2];
   bool overlap;
   int prepared_t[2];         // lock-step index whose heads / operand images occupy buffer set q (-1: none)
+  // wgrad_done[q] was recorded since the last reset.  An older record belongs to a backward whose ic3_bptt_finish has
+  // already joined it into the caller's stream, so waiting on it orders nothing; skipping it keeps a captured backward
+  // from depending on an event recorded outside its capture.
+  bool wgrad_live[2];
 };
 
 BpttStreams* bptt_streams() {
@@ -1352,28 +1379,46 @@ static int bptt_reset(const ic3_bptt_plan* p, const Layout& L, cudaStream_t s) {
   BpttStreams* ss = bptt_streams();
   if (!ss) return IC3_E_UNSUPPORTED;
   ss->prepared_t[0] = ss->prepared_t[1] = -1;
+  ss->wgrad_live[0] = ss->wgrad_live[1] = false;
   return IC3_OK;
 }
 
-// Start of a compute_grad: zero the accumulators and both operand-image sets, build the dgrad weight image, set max |c|.
-extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) {
+// Start of a compute_grad: zero the accumulators and both operand-image sets, build the dgrad weight image.  The scalars
+// (max |c|, operand scales) are set by the caller, between this and the fork of the side stream (bptt_begin_fork).
+static int bptt_begin_common(const ic3_bptt_plan* p, Layout* L, cudaStream_t s) {
   if (!p || !p->cfg || !p->w || !p->workspace) return IC3_E_NULL;
   int rc = plan_geometry(p);
   if (rc) return rc;
   int npos, WW, is_tj;
   rc = env_geometry(p, &npos, &WW, &is_tj);
   if (rc) return rc;
-  Layout L;
-  rc = plan_layout(p->cfg, npos, WW, is_tj, &L);
+  rc = plan_layout(p->cfg, npos, WW, is_tj, L);
   if (rc) return rc;
-  if (L.tanh && !p->w->f_wT) return IC3_E_NULL;
-  cudaStream_t s = (cudaStream_t)stream;
+  if (L->tanh && !p->w->f_wT) return IC3_E_NULL;
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
-  rc = bptt_reset(p, L, s);
+  rc = bptt_reset(p, *L, s);
   if (rc) return rc;
-  cudaError_t e = cudaMemsetAsync(ws + L.a_img, 0, L.w2_img - L.a_img, s);      // both image sets
-  if (e != cudaSuccess) return (int)e;
+  cudaError_t e = cudaMemsetAsync(ws + L->a_img, 0, L->w2_img - L->a_img, s);      // both image sets
+  return e == cudaSuccess ? IC3_OK : (int)e;
+}
+
+// the look-ahead kernels of the first two steps (side stream) must see the zeroed accumulators -- and everything the
+// caller enqueued before ic3_bptt_begin (returns, advantages, the rollout records)
+static int bptt_begin_fork(cudaStream_t s) {
   BpttStreams* ss = bptt_streams();
+  for (int k = 0; k < 2; ++k) {
+    cudaError_t e = cudaEventRecord(ss->main_done[k], s);
+    if (e != cudaSuccess) return (int)e;
+  }
+  return IC3_OK;
+}
+
+extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) {
+  cudaStream_t s = (cudaStream_t)stream;
+  Layout L;
+  int rc = bptt_begin_common(p, &L, s);
+  if (rc) return rc;
+  unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
   BpttScalars init;
   memset(&init, 0, sizeof(init));
   // the cell states entering passes 1 .. P-1 are not in the record: each pass changes |c| by at most 1
@@ -1381,15 +1426,32 @@ extern "C" int ic3_bptt_begin(const ic3_bptt_plan* p, float cmax, void* stream) 
   init.cmax = L.P > 1 ? cmax + (float)(L.P - 1) : cmax;
   init.scale[0] = init.scale[1] = 1.f;
   init.inv_scale[0] = init.inv_scale[1] = 1.f;
-  e = cudaMemcpyAsync(ws + L.sc, &init, sizeof(init), cudaMemcpyHostToDevice, s);
+  cudaError_t e = cudaMemcpyAsync(ws + L.sc, &init, sizeof(init), cudaMemcpyHostToDevice, s);
   if (e != cudaSuccess) return (int)e;
-  // the look-ahead kernels of the first two steps (side stream) must see the zeroed accumulators -- and everything the
-  // caller enqueued before this call (returns, advantages, the rollout records)
-  for (int k = 0; k < 2; ++k) {
-    e = cudaEventRecord(ss->main_done[k], s);
-    if (e != cudaSuccess) return (int)e;
+  return bptt_begin_fork(s);
+}
+
+extern "C" int ic3_bptt_begin_dev(const ic3_bptt_plan* p, const float* c, int64_t n, void* stream) {
+  if (!p || !p->cfg) return IC3_E_NULL;
+  if (n < 0) return IC3_E_RANGE;
+  const bool lstm = p->cfg->cell == IC3_CELL_LSTM;
+  if (lstm && !c) return IC3_E_NULL;
+  if (lstm && n == 0) return IC3_E_RANGE;
+  cudaStream_t s = (cudaStream_t)stream;
+  Layout L;
+  int rc = bptt_begin_common(p, &L, s);
+  if (rc) return rc;
+  BpttScalars* sc = reinterpret_cast<BpttScalars*>(reinterpret_cast<unsigned char*>(p->workspace) + L.sc);
+  bptt_init_scales_kernel<<<1, 1, 0, s>>>(sc);       // bptt_reset zeroed the rest, cmax included
+  IC3_LAUNCH_CHECK();
+  if (!L.tanh && n > 0) {                            // the tanh cell has no c: cmax stays 0, as ic3_bptt_begin(plan, 0)
+    const int64_t n4 = (n + 3) / 4;
+    const int64_t cap = (int64_t)4 * sm_count();
+    const int64_t blocks = (n4 + 255) / 256 < cap ? (n4 + 255) / 256 : cap;
+    bptt_cmax_kernel<<<(int)blocks, 256, 0, s>>>(n, c, (float)(L.P - 1), sc);
+    IC3_LAUNCH_CHECK();
   }
-  return IC3_OK;
+  return bptt_begin_fork(s);
 }
 
 // Recursion-independent part of a backward unit (step t, comm pass ps): the operand images of the pass (prep) from
@@ -1529,7 +1591,7 @@ static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const L
   BpttStreams* ss = bptt_streams();
   if (!ss) return IC3_E_UNSUPPORTED;
   // buffer set q (images, scale) was last read by the weight-gradient kernel of unit u + 2 (side stream)
-  cudaError_t se = cudaStreamWaitEvent(s, ss->wgrad_done[q], 0);
+  cudaError_t se = ss->wgrad_live[q] ? cudaStreamWaitEvent(s, ss->wgrad_done[q], 0) : cudaSuccess;
   if (se != cudaSuccess) return (int)se;
   if (L.P == 1 && ss->prepared_t[q] == io->t) {    // heads + images were launched ahead (ic3_bptt_prepare)
     se = cudaStreamWaitEvent(s, ss->prep_done[q], 0);
@@ -1661,6 +1723,7 @@ static int bptt_unit(const ic3_bptt_plan* p, const ic3_bptt_step_io* io, const L
     IC3_LAUNCH_CHECK();
     se = cudaEventRecord(ss->wgrad_done[q], ws_stream);
     if (se != cudaSuccess) return (int)se;
+    ss->wgrad_live[q] = true;
   }
   return IC3_OK;
 }
@@ -1724,6 +1787,7 @@ extern "C" int ic3_bptt_finish(const ic3_bptt_plan* p, const ic3_policy_params* 
   unsigned char* ws = reinterpret_cast<unsigned char*>(p->workspace);
   if (BpttStreams* ss = bptt_streams()) {       // the last weight-gradient kernels may still run on the side stream
     for (int k = 0; k < 2; ++k) {
+      if (!ss->wgrad_live[k]) continue;
       cudaError_t e = cudaStreamWaitEvent(s, ss->wgrad_done[k], 0);
       if (e != cudaSuccess) return (int)e;
     }

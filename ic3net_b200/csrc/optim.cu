@@ -11,8 +11,9 @@
 
 namespace {
 
-__global__ void rmsprop_kernel(long n, float lr, float alpha, float eps, float inv_div, float* __restrict__ grad,
-                               float* __restrict__ param, float* __restrict__ sq) {
+// The update of elements i (float4 groups) and the < 4-element tail, shared by both entry points.
+__device__ __forceinline__ void rmsprop_apply(long n, float lr, float alpha, float eps, float inv_div,
+                                              float* __restrict__ grad, float* __restrict__ param, float* __restrict__ sq) {
   const long stride = (long)gridDim.x * blockDim.x;
   const long n4 = n >> 2;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += stride) {
@@ -40,6 +41,35 @@ __global__ void rmsprop_kernel(long n, float lr, float alpha, float eps, float i
   }
 }
 
+__global__ void rmsprop_kernel(long n, float lr, float alpha, float eps, float inv_div, float* __restrict__ grad,
+                               float* __restrict__ param, float* __restrict__ sq) {
+  rmsprop_apply(n, lr, alpha, eps, inv_div, grad, param, sq);
+}
+
+// ic3_rmsprop_step_dev: the divisor is the step count of the statistics vector (stat[1]), read on the device.  A rollout
+// that raised a device error flag (stat[3] != 0) updates nothing: the host raises on those flags, as before the update
+// in the eager path.  A count that is not a positive finite number updates nothing and raises IC3_ERR_GRAD_DIV in err
+// (the host form refuses it with IC3_E_RANGE; inside a CUDA graph nobody is there to see a return code).
+__global__ void rmsprop_dev_kernel(long n, float lr, float alpha, float eps, const double* __restrict__ stat,
+                                   float* __restrict__ grad, float* __restrict__ param, float* __restrict__ sq,
+                                   int32_t* __restrict__ err) {
+  if (stat[3] != 0.0) return;
+  const float div = (float)stat[1];
+  if (!(div > 0.f) || !isfinite(div)) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) atomicOr(err, IC3_ERR_GRAD_DIV);
+    return;
+  }
+  rmsprop_apply(n, lr, alpha, eps, 1.f / div, grad, param, sq);
+}
+
+static int rmsprop_grid(int64_t n) {
+  const int threads = 256;
+  long blocks = ((n >> 2) + threads - 1) / threads;
+  if (blocks < 1) blocks = 1;
+  if (blocks > 132 * 8) blocks = 132 * 8;
+  return (int)blocks;
+}
+
 }  // namespace
 
 extern "C" int ic3_rmsprop_step(int64_t n, float lr, float alpha, float eps, float grad_div, float* grad, float* param,
@@ -47,12 +77,19 @@ extern "C" int ic3_rmsprop_step(int64_t n, float lr, float alpha, float eps, flo
   if (!grad || !param || !square_avg) return IC3_E_NULL;
   if (n <= 0 || !(grad_div > 0.f) || !(eps > 0.f)) return IC3_E_RANGE;
   if (((uintptr_t)grad | (uintptr_t)param | (uintptr_t)square_avg) & 15) return IC3_E_RANGE;   // float4 path
-  const int threads = 256;
-  long blocks = ((n >> 2) + threads - 1) / threads;
-  if (blocks < 1) blocks = 1;
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  rmsprop_kernel<<<(int)blocks, threads, 0, (cudaStream_t)stream>>>((long)n, lr, alpha, eps, 1.f / grad_div, grad, param,
-                                                                    square_avg);
+  rmsprop_kernel<<<rmsprop_grid(n), 256, 0, (cudaStream_t)stream>>>((long)n, lr, alpha, eps, 1.f / grad_div, grad, param,
+                                                                   square_avg);
+  IC3_LAUNCH_CHECK();
+  return IC3_OK;
+}
+
+extern "C" int ic3_rmsprop_step_dev(int64_t n, float lr, float alpha, float eps, const double* stat, float* grad,
+                                    float* param, float* square_avg, int32_t* err, void* stream) {
+  if (!stat || !grad || !param || !square_avg || !err) return IC3_E_NULL;
+  if (n <= 0 || !(eps > 0.f)) return IC3_E_RANGE;
+  if (((uintptr_t)grad | (uintptr_t)param | (uintptr_t)square_avg) & 15) return IC3_E_RANGE;   // float4 path
+  rmsprop_dev_kernel<<<rmsprop_grid(n), 256, 0, (cudaStream_t)stream>>>((long)n, lr, alpha, eps, stat, grad, param,
+                                                                       square_avg, err);
   IC3_LAUNCH_CHECK();
   return IC3_OK;
 }

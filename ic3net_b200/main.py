@@ -6,7 +6,7 @@
 Every reference flag is accepted with its meaning; flags of subsystems outside the accelerated
 path (``--plot``/visdom, ``--display``/curses) are
 parsed and rejected with a clear message.  New flags: ``--nenvs`` (environment slots per GPU),
-``--obs_mode`` (index | dense), ``--policy_impl`` (tc | simt | tc_tanh | tc_ff), ``--use_graph``.
+``--obs_mode`` (index | dense), ``--policy_impl`` (tc | simt | tc_tanh | tc_ff), ``--use_graph``, ``--graph_update``.
 Multi-GPU: launch with ``python -m torch.distributed.run --nproc-per-node N -m ic3net_b200.main ...``.
 """
 import argparse
@@ -93,6 +93,9 @@ def build_parser():
                         help='run_batch: whole episodes until >= batch_size steps per env slot (reference), or a fixed '
                              'number of lock-steps with open episodes cut at the end')
     parser.add_argument('--use_graph', action='store_true', default=False, help='replay the rollout as a CUDA graph')
+    parser.add_argument('--graph_update', action='store_true', default=False,
+                        help='replay each whole training update (rollout, gradient kernels, RMSprop, weight pack) from '
+                             'CUDA graphs with one host read per update; needs grad_impl kernels or kernels_ff')
     parser.add_argument('--rollout_only', action='store_true', default=False,
                         help='collect batches and statistics without the optimizer step')
     return parser

@@ -170,6 +170,13 @@ class MultiGPUTrainer(object):
                 stat[k] = float(host[nstat + i])
         return stat
 
+    def _reduce_in_place(self, vec):
+        """graph_update: all-reduce(sum) the flat gradient buffer and the device vector [statistics | loss sums | ...]
+        in place (multi_processing.py:86-94)."""
+        dist.all_reduce(self.trainer.optimizer.flat_grads, op=dist.ReduceOp.SUM)
+        self.collectives += 1
+        dist.all_reduce(vec, op=dist.ReduceOp.SUM)
+
     def run_batch(self, epoch):
         """Rollout only (``--rollout_only``): every rank collects its batch; statistics merged over ranks."""
         tr = self.trainer
@@ -179,6 +186,11 @@ class MultiGPUTrainer(object):
 
     def train_batch(self, epoch):
         tr = self.trainer
+        if getattr(tr, 'graph_update', False):
+            # the update replayed from CUDA graphs; with several ranks the two all-reduces run eagerly between the head
+            # graph (rollout .. gradients) and the tail graph (optimizer step, weight pack): NCCL calls stay outside
+            # any capture
+            return tr.train_batch_graph(epoch, self._reduce_in_place if _dist_on() else None)
         if hasattr(tr, 'stat_vector') and hasattr(tr.optimizer, 'flat_grads'):
             learns = not getattr(tr, 'random_policy', False)     # models.Random: no gradient, no optimizer step
             T, quota = tr.batch_plan()

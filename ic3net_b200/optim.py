@@ -75,6 +75,16 @@ class FlatRMSprop(object):
         self.mark_params_changed()
         self.steps += 1
 
+    def step_dev(self, stat, err):
+        """Enqueue the update of step() with grad_div = stat[1], the step count of the device float64 statistics vector
+        stat (ic3_rmsprop_step_dev; nothing happens when stat[3] holds error flags, IC3_ERR_GRAD_DIV goes to the int32
+        device word err when the count is not positive).  No host read, so a CUDA graph can hold it; the caller advances
+        ``steps`` and calls mark_params_changed() once the update has run."""
+        self._check_attached()
+        _lib.check(_lib.load().ic3_rmsprop_step_dev(self.numel, self.lr, self.alpha, self.eps, stat.data_ptr(),
+                                                    self.flat_grads.data_ptr(), self.flat_params.data_ptr(),
+                                                    self.flat_square_avg.data_ptr(), err.data_ptr(), _lib.stream()))
+
     def mark_params_changed(self):
         """The flat parameter buffer was written through raw pointers / collectives: bump the version counters so
         that caches keyed on (data_ptr, _version) -- CommNetMLP.packed() -- see the new weights."""

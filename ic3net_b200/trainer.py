@@ -144,9 +144,18 @@ class Trainer(object):
         self._bptt = None
         self._buf = None
         self._record_mode = None             # 'full' | 'window' per allocation (record_mode)
+        self._ff_K = None                    # graph_update: kernels_ff chunk length frozen into the captured update
         self._graph = None
         self._graph_key = None
         self._side = None                    # stream of the dense observation writer (_overlap_obs)
+        # graph_update: train_batch replays the whole update from CUDA graphs (train_batch_graph)
+        self.graph_update = bool(getattr(args, 'graph_update', False))
+        self._ugraphs = None
+        self._ugraph_key = None
+        self.update_captures = 0             # graph_update: how often the update was captured
+        if self.random_policy and self.graph_update:
+            raise NotImplementedError("graph_update replays a gradient update; models.Random has neither gradient nor "
+                                      "optimizer step, and its rollout is replayed by use_graph")
         if self.random_policy:
             # nothing to record for a gradient: compute_grad reaches no parameter (trainer.py:223), so .grad stays None
             self.record_for_grad = False
@@ -170,6 +179,12 @@ class Trainer(object):
             self.grad_kernels = ok
         if self.grad_impl == 'auto':
             self.grad_impl = 'kernels' if self.grad_kernels else 'autograd'
+        if self.graph_update and self.record_for_grad and self.grad_impl == 'autograd':
+            raise NotImplementedError("graph_update needs the gradient kernels (grad_impl 'kernels' or 'kernels_ff'): "
+                                      "the torch recompute of grad_impl='autograd' cannot be captured into a CUDA graph")
+        if self.graph_update and getattr(policy_net, 'forward_grad', None) == 'kernels':
+            raise NotImplementedError("graph_update does not cover forward_grad='kernels': that policy's forward is "
+                                      "differentiated by torch autograd, which cannot be captured into a CUDA graph")
         # the non-recurrent tanh policies' kernels (ic3_ff_grad_*): no (h, c) records or checkpoints
         self.grad_ff = self.record_for_grad and self.grad_impl == 'kernels_ff'
         if self.grad_ff:
@@ -205,7 +220,8 @@ class Trainer(object):
 
     # ------------------------------------------------------------------ buffers
     def _alloc(self, T):
-        self._buf = self._graph = None       # the previous buffers go back to the allocator before the records are sized
+        # the previous buffers go back to the allocator before the records are sized
+        self._buf = self._graph = self._ugraphs = None
         e = self.env.env
         B, N, H = e.nenvs, self.args.nagents, self.args.hid_size
         dev = e.device
@@ -723,6 +739,12 @@ class Trainer(object):
         (LOSS_KEYS order) so the data-parallel trainer can reduce them together with the batch statistics."""
         if not self.record_for_grad and not self.random_policy:
             raise RuntimeError("set args.record_for_grad = True before the rollout to use compute_grad")
+        return self._losses_device()
+
+    def _losses_device(self, graph=False):
+        """compute_grad_device after its check.  graph: the form a CUDA graph can hold (graph_update): the BPTT kernels
+        take max |c| from the device (ic3_bptt_begin_dev) and kernels_ff runs with the chunk length frozen at capture
+        (self._ff_K); the gradient is the same bit for bit."""
         b, args = self._buf, self.args
         e = self.env.env
         T, B, N = b['T'], e.nenvs, args.nagents
@@ -740,9 +762,9 @@ class Trainer(object):
         if self.random_policy:
             return self._random_losses(adv, ret)
         if self.grad_kernels:
-            return self._compute_grad_kernels(adv, ret)
+            return self._compute_grad_kernels(adv, ret, dev_cmax=graph)
         if self.grad_ff:
-            return self._compute_grad_ff(adv, ret)
+            return self._compute_grad_ff(adv, ret, K=self._ff_K if graph else None)
         W = self.grad_window
         nw = (T + W - 1) // W
         dh = dc = None
@@ -777,9 +799,10 @@ class Trainer(object):
         ent = -(logp * logp.exp() * b['valid'].double().view(T, B, 1, 1)).sum()      # :213-217, real steps only
         return torch.stack([a_loss, v_loss, ent])
 
-    def _compute_grad_kernels(self, adv, ret):
+    def _compute_grad_kernels(self, adv, ret, dev_cmax=False):
         """Hand-written BPTT (csrc/bptt_tc.cu): one ic3_bptt_step per lock-step iteration, last to first (one host read
-        up front: max |c| of the record, the bound behind the operand scale).  In window mode (record_mode) the policy
+        up front: max |c| of the record, the bound behind the operand scale; dev_cmax: none, ic3_bptt_begin_dev reduces
+        it on the device).  In window mode (record_mode) the policy
         step re-runs each window from its checkpoint just ahead of the backward (_recompute_window); the gradient is
         bit-identical to full records'.  Returns the device float64 vector of the three loss sums."""
         b, net, args, e = self._buf, self.policy_net, self.args, self.env.env
@@ -806,7 +829,10 @@ class Trainer(object):
             cut = (((b['s_tep'] + 1) % args.detach_gap) == 0).to(torch.uint8).contiguous()
         window = self._record_mode == 'window'
         W, nb = self.grad_window, self._window_buffers()
-        if not hc:
+        if dev_cmax:
+            cmax = None                         # from the device: the same values as below (ic3_bptt_begin_dev)
+            csrc = None if not hc else b['c_abs'] if window else b['rec_c'][1:]
+        elif not hc:
             cmax = 0.0                          # no cell state: the operand scale bounds |dh| alone
         elif window:
             cmax = float(b['c_abs'].max().item())                              # tracked per step by the rollout
@@ -836,7 +862,10 @@ class Trainer(object):
         st['dh'].zero_()
         if hc:
             st['dc'].zero_()
-        _lib.check(lib.ic3_bptt_begin(C.byref(plan), cmax, s))
+        if dev_cmax:
+            _lib.check(lib.ic3_bptt_begin_dev(C.byref(plan), _lib.ptr(csrc), 0 if csrc is None else csrc.numel(), s))
+        else:
+            _lib.check(lib.ic3_bptt_begin(C.byref(plan), cmax, s))
         value = b['value']
 
         def step_io(t):
@@ -897,17 +926,19 @@ class Trainer(object):
             k = max(1, min(k, int(self.FF_CHUNK_STEPS)))
         return int(k)
 
-    def _compute_grad_ff(self, adv, ret):
+    def _compute_grad_ff(self, adv, ret, K=None):
         """grad_impl 'kernels_ff' (ic3_ff_grad_*): the rollout's T lock-steps in chunks of K consecutive steps, each one
         batch of K*B env slots (records are [T, B, ...]), in any order since no state crosses a step; the backward's
-        products run on the tensor cores.  Returns the device float64 vector of the three loss sums."""
+        products run on the tensor cores.  K: None = _ff_chunk_steps.  Returns the device float64 vector of the three
+        loss sums."""
         b, net, args, e = self._buf, self.policy_net, self.args, self.env.env
         lib = _lib.load()
         T, B, N = b['T'], e.nenvs, args.nagents
         s = _lib.stream()
         cfg = self._policy_cfg()
         w = net.packed()
-        K = self._ff_chunk_steps(T, cfg)
+        if K is None:
+            K = self._ff_chunk_steps(T, cfg)
         plan = self._ff_plan(cfg, w, K * B * N)
         nbytes = int(lib.ic3_ff_grad_workspace_bytes(C.byref(plan)))
         if nbytes == 0:
@@ -992,6 +1023,8 @@ class Trainer(object):
 
     # only used when there is a single process (trainer.py:245-256)
     def train_batch(self, epoch):
+        if self.graph_update:
+            return self.train_batch_graph(epoch)
         batch, stat = self.run_batch(epoch)
         if self.random_policy:
             # no gradient: the reference's step skips a parameter whose .grad is None (trainer.py:251-254), so the
@@ -1002,6 +1035,119 @@ class Trainer(object):
         s = self.compute_grad(batch)
         merge_stat(s, stat)
         self.optimizer.step(grad_div=stat['num_steps'])      # grad /= num_steps, then the update (trainer.py:251-254)
+        return stat
+
+    # ------------------------------------------------------------------ graph_update
+    # The update as CUDA graphs: head = gradient zeroing, rollout, ic3_stat_reduce, returns, advantages, gradient kernels
+    # and their finish, all into the float64 vector out = [statistics | loss sums | optimizer flags]; tail = RMSprop with
+    # the divisor read from out (ic3_rmsprop_step_dev), then the weight pack and encoder table of the updated parameters,
+    # which the next update's rollout uses.  One graph holds both; with a reduce between them (MultiGPUTrainer: the
+    # all-reduces of the gradients and of out stay eager) each is a graph of its own.  The episode boundary (env reset,
+    # TJ curriculum) runs eagerly before the replay, and the host reads out once after it.
+
+    def _update_head(self, T, quota):
+        b, opt = self._buf, self.optimizer
+        opt.flat_grads.zero_()
+        self._enqueue(T, quota)
+        vec = self.stat_vector()
+        losses = self._losses_device(graph=True)
+        b['opt_err'].zero_()
+        return torch.cat([vec, losses.to(vec.dtype), torch.zeros(1, dtype=vec.dtype, device=vec.device)])
+
+    def _update_tail(self, out):
+        b = self._buf
+        self.optimizer.step_dev(out, b['opt_err'])
+        out[-1:].copy_(b['opt_err'])
+        self.policy_net.packed(force=True)
+        if self._fused_x():
+            self.policy_net.encoder_table(self.env.env, force=True)
+
+    def _update_key(self, T, quota):
+        """Everything a captured update freezes by value that can change between updates: a change re-captures."""
+        e, opt = self.env.env, self.optimizer
+        return (T, int(quota), int(getattr(e.cfg, 'spawn_thr', 0)), int(e.cfg.seed), int(e.cfg.env_id0), e.nenvs,
+                self._record_mode, self._ff_K, opt.lr, opt.alpha, opt.eps)
+
+    def _capture_update(self, T, quota, reduce):
+        """Warm-up pass (lazy library state, allocator, the gradient kernels' workspaces), rewound so that it leaves no
+        trace (env state and RNG ticks, episode state, parameters, gradients, second moments, packed weights), then the
+        capture.  Nothing runs in the capture: the caller replays it."""
+        b, e, opt, net = self._buf, self.env.env, self.optimizer, self.policy_net
+        if self.grad_ff:
+            self._ff_K = self._ff_chunk_steps(T, self._policy_cfg())
+        snap = e.snapshot()
+        keys = ('fresh', 'comm', 'alive', 't_ep', 'h', 'c', 'halted', 'stat_reward', 'stat_comm', 'stat_success',
+                'stat_episodes', 'stat_steps', 'err')
+        saved = {k: b[k].clone() for k in keys if k in b}
+        flat = [opt.flat_params, opt.flat_grads, opt.flat_square_avg]
+        saved_flat = [t.clone() for t in flat]
+        out = self._update_head(T, quota)
+        if reduce is not None:
+            reduce(out)
+        self._update_tail(out)
+        torch.cuda.synchronize()
+        e.restore(snap)
+        for k, v in saved.items():
+            b[k].copy_(v)
+        for t, v in zip(flat, saved_flat):
+            t.copy_(v)
+        net.packed(force=True)                # the weights the warm-up packed were the updated ones
+        if self._fused_x():
+            net.encoder_table(e, force=True)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            out = self._update_head(T, quota)
+            if reduce is None:
+                self._update_tail(out)
+        graphs = [g]
+        if reduce is not None:
+            g2 = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g2, pool=g.pool()):
+                self._update_tail(out)
+            graphs.append(g2)
+        self._ugraphs, self._uout = graphs, out
+        self.update_captures += 1
+
+    def train_batch_graph(self, epoch, reduce=None):
+        """train_batch replayed from CUDA graphs (graph_update); one host read per update.  reduce(out), if given, runs
+        eagerly between the head and the tail graph (the data-parallel all-reduces of the flat gradients and of out,
+        in place).  Returns the stat dict train_batch returns."""
+        if not self.record_for_grad:
+            raise RuntimeError("set args.record_for_grad = True before the rollout to use compute_grad")
+        e, net, opt = self.env.env, self.policy_net, self.optimizer
+        T, quota = self.batch_plan()
+        if self._buf is None or self._buf['T'] != T:
+            self._alloc(T)
+            self._ff_K = None
+        b = self._buf
+        if 'opt_err' not in b:
+            b['opt_err'] = torch.zeros(1, dtype=torch.int32, device=e.device)
+        self._episode_boundary(epoch)             # trainer.py:28-32, 45-51 (TJ curriculum: may move spawn_thr)
+        b['err'].zero_()
+        net.packed()                              # no-ops when the last replay left the pack current
+        if self._fused_x():
+            self._encoder_table()
+        if self._ugraphs is None or self._update_key(T, quota) != self._ugraph_key:
+            self._ff_K = None
+            self._capture_update(T, quota, reduce)
+            self._ugraph_key = self._update_key(T, quota)
+        self._ugraphs[0].replay()
+        if reduce is not None:
+            reduce(self._uout)
+            self._ugraphs[1].replay()
+        host = self._uout.cpu().numpy()
+        nstat = host.size - 4
+        stat = self.stat_from_vector(host[:nstat])    # raises on the rollout's flags; the update then changed nothing
+        if int(host[-1]):
+            raise RuntimeError("device-side error flag %#x in the optimizer step (step count %r)" % (int(host[-1]),
+                                                                                                host[1]))
+        opt.steps += 1
+        opt.mark_params_changed()
+        net.mark_packed_current()
+        if self.grad_ff:
+            self.ff_chunk_steps = self._ff_K
+        merge_stat({k: float(host[nstat + i]) for i, k in enumerate(self.LOSS_KEYS)}, stat)
+        self.stats = stat
         return stat
 
     def state_dict(self):

@@ -51,9 +51,11 @@ enum {
   IC3_ERR_ROUTE_OVERRUN = 2,
   IC3_ERR_BAD_ACTION = 4,   /* action > naction (reference asserts, :137 / :228) */
   IC3_ERR_PIPELINE = 0x100, /* tensor-core path: an mbarrier wait ran into its watchdog (mis-programmed pipeline) */
-  IC3_ERR_FP16_RANGE = 0x200 /* tensor-core path: an activation (|a| >= 4094) or folded weight (|w| >= 255) left the range of
+  IC3_ERR_FP16_RANGE = 0x200, /* tensor-core path: an activation (|a| >= 4094) or folded weight (|w| >= 255) left the range of
                                the fp16 hi/lo operand split; results of that step are not trustworthy -> use the
                                fp32 SIMT kernels (policy_impl = 'simt') for such a model */
+  IC3_ERR_GRAD_DIV = 0x400  /* ic3_rmsprop_step_dev: the step count it divides by was not a positive finite number; the
+                               parameters, gradients and second moments were left unchanged */
 };
 
 enum { IC3_PP_MIXED = 0, IC3_PP_COOPERATIVE = 1, IC3_PP_COMPETITIVE = 2 };
@@ -515,6 +517,11 @@ typedef struct {
  * A plan that fails gets 0 bytes and IC3_E_RANGE (neither or both environments: IC3_E_NULL). */
 uint64_t ic3_bptt_workspace_bytes(const ic3_bptt_plan* plan);   /* 0 = configuration not supported by the kernels */
 int ic3_bptt_begin(const ic3_bptt_plan* plan, float c_abs_max, void* stream);
+/* ic3_bptt_begin with max |c| reduced on the device from the n floats at c (device): every step's cell state of a full
+ * record (rec_c[1:]), or the per-step maxima of a windowed one.  The operand-scale state is formed on the device with the
+ * same float arithmetic as ic3_bptt_begin(plan, max |c[i]|), so the gradients are bit-identical; no host read, no
+ * pageable copy: the call can be captured into a CUDA graph.  The tanh cell has no c: c = NULL, n = 0. */
+int ic3_bptt_begin_dev(const ic3_bptt_plan* plan, const float* c, int64_t n, void* stream);
 int ic3_bptt_step(const ic3_bptt_plan* plan, const ic3_bptt_step_io* io, void* stream);
 /* Optional look-ahead: launches the recursion-independent kernels of step io->t (heads gradient, operand images) on the
  * library's side stream so that they overlap the tensor-core kernels of step t + 1; call it for step t - 1 right before
@@ -637,6 +644,12 @@ int ic3_ff_grad_finish(const ic3_ff_grad_plan* plan, const ic3_policy_params* pa
  * square_avg = alpha*square_avg + (1-alpha)*g*g;  param -= lr * g / (sqrt(square_avg) + eps). */
 int ic3_rmsprop_step(int64_t n, float lr, float alpha, float eps, float grad_div, float* grad,
                      float* param, float* square_avg, void* stream);
+/* The same step with grad_div = (float)stat[1] read on the device; stat: the float64 statistics vector of
+ * ic3_stat_reduce (out[1] = num_steps, out[3] = error flags), after any all-reduce.  Nonzero flags: nothing is updated
+ * (the caller raises on them).  A count that is not a positive finite number updates nothing and ORs IC3_ERR_GRAD_DIV
+ * into the device word err.  No host read: the call can be captured into a CUDA graph. */
+int ic3_rmsprop_step_dev(int64_t n, float lr, float alpha, float eps, const double* stat, float* grad,
+                         float* param, float* square_avg, int32_t* err, void* stream);
 
 #ifdef __cplusplus
 }

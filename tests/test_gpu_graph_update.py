@@ -1,0 +1,198 @@
+"""graph_update: the whole training update (rollout, statistics, returns, advantages, gradient kernels, RMSprop, weight
+pack) replayed from CUDA graphs (Trainer.train_batch_graph).  Each case trains the same seed and initial weights for K
+updates eagerly and with graph_update and asserts bit-identical flat parameters, second moments, the last update's
+gradients and the stat dicts; plus the fp16-range flag after a replay, the refusals, the CLI with --save / --load, and
+the re-capture rule of the traffic-junction curriculum."""
+import os
+import subprocess
+import sys
+
+import numpy as np
+import pytest
+import torch
+
+from helpers import finish_args, load_golden, ns
+
+pytestmark = pytest.mark.gpu
+
+PP, TJ = "grad_pp_hard_ic3net_h128", "grad_tj_hard_ic3net_h128"
+K = 3
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def make_trainer(name, B, graph, model="commnet", windows=False, ff_chunk=None, **over):
+    from ic3net_b200 import data, models
+    from ic3net_b200.comm import CommNetMLP
+    from ic3net_b200.trainer import Trainer
+    meta, _ = load_golden(name)
+    kw = dict(nenvs=B, seed=808, env_id0=30, obs_mode="index", use_graph=False, policy_impl="tc",
+              record_for_grad=True, grad_impl="kernels", graph_update=graph, lrate=1e-3)
+    kw.update(over)
+    args = ns(meta["args"], **kw)
+    env = data.init(args.env_name, args)
+    finish_args(args, env)
+    torch.manual_seed(meta["weights_seed"])
+    net = {"rnn": models.RNN, "mlp": models.MLP, "commnet": CommNetMLP}[model](args, args.num_inputs)
+    tr = Trainer(args, net, env)
+    if windows:
+        tr.RECORD_BYTES_LIMIT = 0
+    if ff_chunk is not None:
+        tr.FF_CHUNK_STEPS = ff_chunk
+    return tr
+
+
+def same_stat(a, b):
+    assert sorted(a) == sorted(b)
+    for k in a:
+        assert np.array_equal(np.asarray(a[k]), np.asarray(b[k])), k
+
+
+def train_both(name, B, epochs=None, **over):
+    """(eager trainer, graph trainer) after K updates each, asserting identical stat dicts along the way."""
+    eager, graph = make_trainer(name, B, False, **over), make_trainer(name, B, True, **over)
+    for ep in (epochs or range(K)):
+        same_stat(eager.train_batch(ep), graph.train_batch(ep))
+    return eager, graph
+
+
+def assert_same_state(eager, graph):
+    oe, og = eager.optimizer, graph.optimizer
+    assert torch.equal(oe.flat_params, og.flat_params)
+    assert torch.equal(oe.flat_square_avg, og.flat_square_avg)
+    assert torch.equal(oe.flat_grads, og.flat_grads)
+    assert oe.steps == og.steps == K
+
+
+IC = dict(model="rnn", commnet=False, hard_attn=False, recurrent=True, rnn_type="MLP", policy_impl="tc_tanh",
+          comm_passes=1, share_weights=False)
+FF = dict(grad_impl="kernels_ff", ic3net=False, recurrent=False, rnn_type="MLP", policy_impl="tc_ff", ff_chunk=7,
+          entr=0.01)
+CASES = {
+    "ic3net_full": dict(),
+    "ic3net_windows": dict(windows=True),
+    "ic3net_passes2_shared": dict(comm_passes=2, share_weights=True),
+    "ic3net_no_cuts": dict(detach_gap=10000),
+    "ic_tanh_full": dict(IC),
+    "ic_tanh_windows": dict(IC, windows=True),
+    "mlp_ff": dict(FF, model="mlp", commnet=False, hard_attn=False),
+    "ic3net_ff_passes2": dict(FF, model="commnet", commnet=1, hard_attn=1, comm_passes=2, share_weights=False),
+}
+
+
+@pytest.mark.parametrize("case", sorted(CASES))
+def test_graph_update_is_bit_identical(case):
+    over = dict(CASES[case])
+    eager, graph = train_both(PP, 37, **over)                 # 37 x 10 agent rows: a ragged last 128-row tile
+    assert_same_state(eager, graph)
+    assert graph.update_captures == 1
+    if eager.grad_kernels:
+        assert eager.record_mode == graph.record_mode == ("window" if over.get("windows") else "full")
+
+
+def test_traffic_junction_curriculum_recaptures_exactly_on_a_step():
+    # add_rate moves at epochs 1 and 2 (curr_start 0, curr_end 4, step 0.05): spawn_thr changes, the graph re-captures;
+    # the repeated epochs move nothing and must replay the graph they have
+    over = dict(normalize_rewards=True, add_rate_min=0.1, add_rate_max=0.3, curr_start=0, curr_end=4)
+    eager = make_trainer(TJ, 24, False, **over)
+    graph = make_trainer(TJ, 24, True, **over)
+    captures, thr = [], []
+    for ep in (0, 0, 1, 1, 2):
+        same_stat(eager.train_batch(ep), graph.train_batch(ep))
+        captures.append(graph.update_captures)
+        thr.append(int(graph.env.env.cfg.spawn_thr))
+    changes = [i == 0 or thr[i] != thr[i - 1] for i in range(len(thr))]
+    assert sum(changes) >= 2
+    assert captures == list(np.cumsum(changes))
+    for a, b in ((eager.optimizer.flat_params, graph.optimizer.flat_params),
+                 (eager.optimizer.flat_square_avg, graph.optimizer.flat_square_avg),
+                 (eager.optimizer.flat_grads, graph.optimizer.flat_grads)):
+        assert torch.equal(a, b)
+
+
+def test_packed_weights_stay_current_after_a_replay():
+    tr = make_trainer(PP, 8, True)
+    tr.train_batch(0)
+    net = tr.policy_net
+    key = net._packed_key
+    net.packed()
+    assert net._packed_key == key                            # nothing to re-pack: the replay packed the new weights
+    before = {k: v.clone() for k, v in net._bufs.items()}
+    net.packed(force=True)
+    for k, v in net._bufs.items():
+        assert torch.equal(before[k], v), k
+
+
+def test_fp16_range_flag_raises_after_the_replay():
+    """Weights outside the fp16 split range: the same RuntimeError as the eager update, from the statistics vector read
+    after the replay (an error word, not a device fault), and the update leaves the parameters as they were."""
+    for graph in (False, True):
+        tr = make_trainer(PP, 4, graph)
+        with torch.no_grad():
+            tr.policy_net.f_module.weight_hh.mul_(4000.0)
+        before = tr.optimizer.flat_params.clone()
+        with pytest.raises(RuntimeError, match="0x200"):
+            tr.train_batch(0)
+        assert torch.equal(before, tr.optimizer.flat_params)
+
+
+def test_refusals():
+    from ic3net_b200 import data, models
+    from ic3net_b200.trainer import Trainer
+    with pytest.raises(NotImplementedError, match="autograd"):
+        make_trainer(PP, 4, True, grad_impl="autograd")
+    with pytest.raises(NotImplementedError, match="forward_grad"):
+        make_trainer(PP, 4, True, forward_grad="kernels")
+    meta, _ = load_golden(PP)
+    args = ns(meta["args"], nenvs=4, seed=1, env_id0=0, obs_mode="index", use_graph=False, recurrent=False,
+              random=True, graph_update=True, lrate=1e-3)
+    env = data.init(args.env_name, args)
+    finish_args(args, env)
+    args.recurrent = False
+    with pytest.raises(NotImplementedError, match="Random"):
+        Trainer(args, models.Random(args, args.num_inputs), env)
+
+
+def test_cli_epoch_and_save_load_round_trip(tmp_path):
+    """One epoch end to end with --graph_update, saved, re-loaded and continued: every checkpoint equals the eager
+    run's bit for bit (parameters, RMSprop state, log)."""
+    from ic3net_b200 import main as m
+    base = ["--env_name", "predator_prey", "--nagents", "3", "--dim", "5", "--vision", "1", "--max_steps", "20",
+            "--hid_size", "128", "--ic3net", "--recurrent", "--nenvs", "16", "--num_epochs", "1", "--epoch_size", "2",
+            "--batch_size", "30", "--seed", "4", "--detach_gap", "10", "--lrate", "0.001"]
+    ck = {}
+    for mode, extra in (("eager", []), ("graph", ["--graph_update"])):
+        a, b = str(tmp_path / (mode + "_a.pt")), str(tmp_path / (mode + "_b.pt"))
+        assert m.main(base + extra + ["--save", a]) == 0
+        assert m.main(base + extra + ["--load", a, "--save", b]) == 0
+        with m._utils_alias():
+            ck[mode] = [torch.load(p, weights_only=False) for p in (a, b)]
+    for de, dg in zip(ck["eager"], ck["graph"]):
+        for k in de["policy_net"]:
+            assert torch.equal(de["policy_net"][k], dg["policy_net"][k]), k
+        se, sg = de["trainer"]["state"], dg["trainer"]["state"]
+        assert sorted(se) == sorted(sg) and len(se) > 0
+        for i in se:
+            assert torch.equal(se[i]["square_avg"], sg[i]["square_avg"]) and float(se[i]["step"]) == float(sg[i]["step"])
+        for k in ("reward", "action_loss", "value_loss", "num_steps"):
+            if k in de["log"]:
+                assert np.array_equal(np.asarray(de["log"][k].data), np.asarray(dg["log"][k].data)), k
+    assert float(ck["graph"][1]["trainer"]["state"][0]["step"]) == 4.0
+
+
+@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs two GPUs")
+def test_two_ranks_stay_identical_and_equal_eager(tmp_path):
+    worker = os.path.join(os.path.dirname(os.path.abspath(__file__)), "graph_update_nccl_worker.py")
+    outs = {}
+    for mode in ("eager", "graph"):
+        out = tmp_path / mode
+        out.mkdir()
+        cmd = [sys.executable, "-m", "torch.distributed.run", "--nproc-per-node", "2", "--master-port",
+               str(29611 if mode == "eager" else 29612), worker, mode, str(out)]
+        subprocess.run(cmd, check=True, cwd=ROOT, timeout=900)
+        outs[mode] = [torch.load(str(out / ("rank%d.pt" % r)), weights_only=False) for r in range(2)]
+    for mode in outs:
+        assert torch.equal(outs[mode][0]["params"], outs[mode][1]["params"])
+    for r in range(2):
+        for key in ("params", "square_avg", "grads"):
+            assert torch.equal(outs["eager"][r][key], outs["graph"][r][key]), key
+        assert outs["eager"][r]["stats"] == outs["graph"][r]["stats"]
