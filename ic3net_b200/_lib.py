@@ -54,7 +54,7 @@ class RolloutIO(C.Structure):
                 ("comm_next", _p), ("alive_next", _p), ("rec_reward", _p), ("rec_episode_mask", _p),
                 ("rec_mini_mask", _p), ("rec_alive", _p), ("stat_reward", _p), ("stat_comm", _p),
                 ("stat_success", _p), ("stat_episodes", _p), ("stat_steps", _p), ("batch_size", C.c_int32),
-                ("reserved0", C.c_int32), ("halted", _p), ("rec_valid", _p), ("snap_T", C.c_int32),
+                ("episodes", C.c_int32), ("halted", _p), ("rec_valid", _p), ("snap_T", C.c_int32),
                 ("reserved1", C.c_int32), ("snap_fresh", _p), ("snap_comm", _p), ("snap_alive", _p), ("snap_tep", _p),
                 ("snap_pp_loc", _p), ("snap_tj_loc", _p), ("snap_tj_alive", _p), ("snap_tj_last_act", _p),
                 ("snap_tj_route_id", _p)]
@@ -81,7 +81,7 @@ class PolicyCfg(C.Structure):
                 ("head_dim", C.c_int32 * MAX_HEADS), ("hard_attn", C.c_int32), ("comm_avg", C.c_int32),
                 ("comm_mask_zero", C.c_int32), ("env_id0", C.c_uint32), ("seed", C.c_uint64),
                 ("obs_off", C.c_int32), ("obs_vocab", C.c_int32), ("obs_ncount", C.c_int32), ("cell", C.c_int32),
-                ("passes", C.c_int32), ("x_tanh", C.c_int32), ("h_from_x", C.c_int32), ("reserved0", C.c_int32)]
+                ("passes", C.c_int32), ("x_tanh", C.c_int32), ("h_from_x", C.c_int32), ("greedy", C.c_int32)]
 
 
 class PolicyParams(C.Structure):

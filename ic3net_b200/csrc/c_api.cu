@@ -13,6 +13,7 @@ extern "C" const char* ic3_strerror(int code) {
     case IC3_E_NULL: return "required pointer is NULL";
     case IC3_E_RANGE: return "argument out of the supported range";
     case IC3_E_UNSUPPORTED: return "configuration not implemented by the kernels";
+    case IC3_E_ARG: return "arguments contradict each other";
     default: break;
   }
   if (code > 0) return cudaGetErrorString((cudaError_t)code);

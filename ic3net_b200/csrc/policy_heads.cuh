@@ -6,8 +6,9 @@
 #include "ic3_common.cuh"
 
 // log-softmax + inverse-CDF sampling of one head; logits live one per lane
-// (lane off+a holds logit a).  Every lane of the warp executes this.
-__device__ __forceinline__ void head_logp_sample(float mylogit, int off, int na, float u, bool do_sample,
+// (lane off+a holds logit a).  Every lane of the warp executes this.  greedy: the action is the lowest index of
+// the largest logit (torch.argmax) instead of the draw u.
+__device__ __forceinline__ void head_logp_sample(float mylogit, int off, int na, float u, bool do_sample, bool greedy,
                                                  float& mylogp, int& action) {
   float m = -INFINITY;
   for (int a = 0; a < na; ++a) m = fmaxf(m, __shfl_sync(IC3_FULL_MASK, mylogit, off + a));
@@ -16,7 +17,10 @@ __device__ __forceinline__ void head_logp_sample(float mylogit, int off, int na,
   const float lse = m + logf(s);
   mylogp = mylogit - lse;
   action = na - 1;
-  if (do_sample) {
+  if (do_sample && greedy) {
+    for (int a = na - 1; a >= 0; --a)
+      if (__shfl_sync(IC3_FULL_MASK, mylogit, off + a) == m) action = a;
+  } else if (do_sample) {
     float cdf = 0.f;
     bool found = false;
     for (int a = 0; a < na; ++a) {
@@ -51,16 +55,17 @@ __device__ __forceinline__ void heads_for_row(const ic3_policy_cfg& cfg, const f
   if (lane == 0) value[grow] = mylogit;
   uint4 w = make_uint4(0, 0, 0, 0);
   const bool do_sample = action != nullptr;
-  if (do_sample && !draws)
+  const bool greedy = cfg.greedy != 0;    // argmax: neither the action stream nor draws is read
+  if (do_sample && !greedy && !draws)
     w = ic3_draw24(cfg.seed, cfg.env_id0 + (uint32_t)e, tick ? tick[e] : 0u, IC3_STREAM_ACTION, (uint32_t)i);
   int off = 1;
   for (int k = 0; k < cfg.nheads; ++k) {
     const int na = cfg.head_dim[k];
     uint32_t u24 = 0;
-    if (do_sample) u24 = draws ? draws[grow * cfg.nheads + k] : ic3_word(w, k);
+    if (do_sample && !greedy) u24 = draws ? draws[grow * cfg.nheads + k] : ic3_word(w, k);
     float mylogp;
     int act;
-    head_logp_sample(mylogit, off, na, (float)u24 * 5.9604644775390625e-08f, do_sample, mylogp, act);
+    head_logp_sample(mylogit, off, na, (float)u24 * 5.9604644775390625e-08f, do_sample, greedy, mylogp, act);
     if (lane >= off && lane < off + na) logp[grow * atot + (off - 1) + (lane - off)] = mylogp;
     if (do_sample && lane == 0) action[grow * cfg.nheads + k] = act;
     off += na;
@@ -87,19 +92,21 @@ struct HeadsFinish {
   float* value;           // [R]
   float* logp;            // [R, sum(na)]
   int32_t* action;        // [R, nheads] or NULL (no sampling)
+  int greedy;             // argmax instead of sampling (ic3_policy_cfg.greedy)
 };
 
 // Log-softmax per head and inverse-CDF sampling of ONE agent row by ONE thread (action_utils.py:32-36): logit[1 + j] is
 // action logit j, heads concatenated (logit[0], the value, is not read), 1 + atot <= IC3_HEAD_PAD.  Head k samples with
 // word k of the action stream (env_id0 + e, tick[e], IC3_STREAM_ACTION, i) or draws[row, k]; action == NULL: no
-// sampling.  Shared by the tensor-core heads (heads_finish_row) and the Random policy step (random_policy.cu).
+// sampling; greedy: the lowest index of the head's largest logit (torch.argmax), no stream or draws read.  Shared by
+// the tensor-core heads (heads_finish_row) and the Random policy step (random_policy.cu).
 __device__ __forceinline__ void heads_logp_sample_row(const float (&logit)[IC3_HEAD_PAD], int nheads,
                                                       const int* head_dim, int atot, uint64_t seed, uint32_t env_id0,
                                                       const uint32_t* tick, const uint32_t* draws, long row, int e,
-                                                      int i, float* logp, int32_t* action) {
+                                                      int i, float* logp, int32_t* action, bool greedy) {
   const bool do_sample = action != nullptr;
   uint4 d24 = make_uint4(0, 0, 0, 0);
-  if (do_sample && !draws)
+  if (do_sample && !greedy && !draws)
     d24 = ic3_draw24(seed, env_id0 + (uint32_t)e, tick ? tick[e] : 0u, IC3_STREAM_ACTION, (uint32_t)i);
   int off = 1;
   for (int k = 0; k < nheads; ++k) {
@@ -114,7 +121,7 @@ __device__ __forceinline__ void heads_logp_sample_row(const float (&logit)[IC3_H
       if (o >= off && o < off + na) ssum += expf(logit[o] - m);
     const float lse = m + logf(ssum);
     uint32_t u24 = 0;
-    if (do_sample) u24 = draws ? draws[(size_t)row * nheads + k] : ic3_word(d24, k);
+    if (do_sample && !greedy) u24 = draws ? draws[(size_t)row * nheads + k] : ic3_word(d24, k);
     const float u = (float)u24 * 5.9604644775390625e-08f;
     float cdf = 0.f;
     int act = na - 1;
@@ -124,6 +131,13 @@ __device__ __forceinline__ void heads_logp_sample_row(const float (&logit)[IC3_H
       if (o >= off && o < off + na) {
         const float lp = logit[o] - lse;
         logp[(size_t)row * atot + (o - 1)] = lp;
+        if (greedy) {
+          if (!found && logit[o] == m) {
+            act = o - off;
+            found = true;
+          }
+          continue;
+        }
         cdf += expf(lp);
         if (!found && cdf > u) {
           act = o - off;
@@ -156,5 +170,5 @@ __device__ __forceinline__ void heads_finish_row(const HeadsFinish& f, long row,
   for (int o = 0; o < IC3_HEAD_PAD; ++o) logit[o] += (o < 1 + atot) ? __ldg(f.head_b + o) : 0.f;
   f.value[row] = logit[0];
   heads_logp_sample_row(logit, f.nheads, f.head_dim, atot, f.seed, f.env_id0, f.tick, f.draws, row, e, i, f.logp,
-                        f.action);
+                        f.action, f.greedy != 0);
 }

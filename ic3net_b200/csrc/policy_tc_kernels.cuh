@@ -715,9 +715,10 @@ __global__ void __launch_bounds__(256) heads_kernel(ic3_policy_cfg cfg, ic3_poli
   }
   if (live && o == 0) io.value[row] = logit;
   const bool do_sample = io.action != nullptr;
+  const bool greedy = cfg.greedy != 0;    // argmax: neither the action stream nor draws is read
   const int e = live ? (int)(row / cfg.N) : 0, i = live ? (int)(row - (long)e * cfg.N) : 0;
   uint32_t w0 = 0, w1 = 0, w2 = 0, w3 = 0;
-  if (do_sample && !io.draws) {
+  if (do_sample && !greedy && !io.draws) {
     if (o == 0 && live) {
       const uint4 d = ic3_draw24(cfg.seed, cfg.env_id0 + (uint32_t)e, io.tick ? io.tick[e] : 0u, IC3_STREAM_ACTION, (uint32_t)i);
       w0 = d.x; w1 = d.y; w2 = d.z; w3 = d.w;
@@ -734,13 +735,16 @@ __global__ void __launch_bounds__(256) heads_kernel(ic3_policy_cfg cfg, ic3_poli
     for (int a = 0; a < na; ++a) s += expf(__shfl_sync(IC3_FULL_MASK, logit, off + a, P) - m);
     const float mylogp = logit - (m + logf(s));
     uint32_t u24 = 0;
-    if (do_sample) {
+    if (do_sample && !greedy) {
       if (io.draws) u24 = live ? io.draws[(size_t)row * cfg.nheads + k] : 0u;
       else u24 = k == 0 ? w0 : (k == 1 ? w1 : (k == 2 ? w2 : w3));
     }
     const float u = (float)u24 * 5.9604644775390625e-08f;
     int act = na - 1;
-    if (do_sample) {
+    if (do_sample && greedy) {
+      for (int a = na - 1; a >= 0; --a)
+        if (__shfl_sync(IC3_FULL_MASK, logit, off + a, P) == m) act = a;
+    } else if (do_sample) {
       float cdf = 0.f;
       bool found = false;
       for (int a = 0; a < na; ++a) {
@@ -768,7 +772,7 @@ __global__ void __launch_bounds__(128) heads_finish_kernel(ic3_policy_cfg cfg, i
 #pragma unroll
   for (int k = 0; k < IC3_MAX_HEADS; ++k) f.head_dim[k] = cfg.head_dim[k];
   f.seed = cfg.seed; f.env_id0 = cfg.env_id0; f.tick = io.tick; f.draws = io.draws;
-  f.value = io.value; f.logp = io.logp; f.action = io.action;
+  f.value = io.value; f.logp = io.logp; f.action = io.action; f.greedy = cfg.greedy;
   const int e = (int)(row / cfg.N), i = (int)(row - (long)e * cfg.N);
   heads_finish_row(f, row, e, i);
 }

@@ -56,7 +56,7 @@ __global__ void __launch_bounds__(128) random_policy_kernel(const __grid_constan
     logit[1 + j] = z;
   }
   heads_logp_sample_row(logit, cfg.nheads, cfg.head_dim, atot, cfg.seed, cfg.env_id0, tick, draws, row, e, i, logp,
-                        action);
+                        action, false);
 }
 
 }  // namespace
@@ -64,6 +64,7 @@ __global__ void __launch_bounds__(128) random_policy_kernel(const __grid_constan
 extern "C" int ic3_random_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_io* io, const uint32_t* random_draws,
                                       void* stream) {
   if (!cfg || !io) return IC3_E_NULL;
+  if (cfg->greedy) return IC3_E_ARG;                 // an argmax over the uniform policy's logits means nothing
   if (cfg->B <= 0 || cfg->N <= 0 || cfg->N > IC3_MAX_AGENTS) return IC3_E_RANGE;
   if (cfg->nheads < 1 || cfg->nheads > IC3_MAX_HEADS) return IC3_E_RANGE;
   int tot = 1;

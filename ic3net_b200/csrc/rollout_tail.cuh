@@ -16,12 +16,21 @@ static inline RolloutOpt make_rollout_opt(const ic3_rollout_io* r) {
   return o;
 }
 
+// Host-side rules of the two halting modes (ic3_rollout_io.batch_size / episodes); r may be NULL.
+static inline int ic3_rollout_quota_check(const ic3_rollout_io* r) {
+  if (!r) return IC3_OK;
+  if (r->episodes < 0) return IC3_E_RANGE;
+  if (r->episodes > 0 && (r->batch_size > 0 || !r->halted || !r->stat_episodes)) return IC3_E_ARG;
+  return IC3_OK;
+}
+
 // Reference batch boundary (trainer.py:231-237): a worker plays whole episodes until it holds >= batch_size steps,
 // so its last episode overshoots.  With r.batch_size > 0 a slot HALTS at the first episode end at which its step
 // count has reached batch_size; from then on the lock-step iterations skip it: no env step, no statistics, null
-// records (rec_valid = 0, alive = 0, reward = 0, episode_mask = 0).  Returns true for a halted slot.
+// records (rec_valid = 0, alive = 0, reward = 0, episode_mask = 0).  With r.episodes > 0 (evaluation) a slot halts
+// the same way at the episode end at which it has completed `episodes` episodes.  Returns true for a halted slot.
 __device__ __forceinline__ bool ic3_rollout_halted(const ic3_rollout_io& r, int e, int B, int N, int lane) {
-  if (r.batch_size <= 0 || !r.halted || !r.halted[e]) return false;
+  if ((r.batch_size <= 0 && r.episodes <= 0) || !r.halted || !r.halted[e]) return false;
   if (lane < N) {
     const size_t idx = ((size_t)r.t * B + e) * N + lane;
     if (r.rec_reward) r.rec_reward[idx] = 0.f;
@@ -67,7 +76,10 @@ __device__ __forceinline__ bool ic3_rollout_tail(const ic3_rollout_io& r, int e,
     if (r.stat_steps) nsteps = (r.stat_steps[e] += 1);                             // :109
     if (done_t) {
       if (r.batch_size > 0 && r.halted && nsteps >= r.batch_size) r.halted[e] = 1; // trainer.py:231 loop condition
-      if (r.stat_episodes) r.stat_episodes[e] += 1;                                // :235
+      if (r.stat_episodes) {
+        const int neps = (r.stat_episodes[e] += 1);                                // :235
+        if (r.episodes > 0 && r.halted && neps >= r.episodes) r.halted[e] = 1;     // episode quota
+      }
       if (r.stat_success && success > 0) r.stat_success[e] += success;             // :124-125
     }
   }

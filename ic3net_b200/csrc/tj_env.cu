@@ -416,6 +416,8 @@ extern "C" int ic3_tj_step(const ic3_tj_cfg* cfg, const ic3_tj_state* st, const 
   if (!act || !reward || !err || act_stride < 1) return IC3_E_NULL;
   if (r && (!r->t_ep || !r->fresh || !r->alive_next || (r->hard_attn && (!r->comm_next || !r->action))))
     return IC3_E_NULL;
+  rc = ic3_rollout_quota_check(r);
+  if (rc) return rc;
   return tj_launch(cfg, st, act, act_stride, draws, reward, obs, err, r, 1, (cudaStream_t)stream);
 }
 

@@ -6,7 +6,9 @@
 Every reference flag is accepted with its meaning; flags of subsystems outside the accelerated
 path (``--plot``/visdom, ``--display``/curses) are
 parsed and rejected with a clear message.  New flags: ``--nenvs`` (environment slots per GPU),
-``--obs_mode`` (index | dense), ``--policy_impl`` (tc | simt | tc_tanh | tc_ff), ``--use_graph``, ``--graph_update``.
+``--obs_mode`` (index | dense), ``--policy_impl`` (tc | simt | tc_tanh | tc_ff), ``--use_graph``, ``--graph_update``,
+and evaluation of whole episodes every K epochs (``--eval_every``, ``--eval_episodes``, ``--eval_nenvs``,
+``--eval_greedy``; Trainer.evaluate).
 Multi-GPU: launch with ``python -m torch.distributed.run --nproc-per-node N -m ic3net_b200.main ...``.
 """
 import argparse
@@ -98,6 +100,12 @@ def build_parser():
                              'CUDA graphs with one host read per update; needs grad_impl kernels or kernels_ff')
     parser.add_argument('--rollout_only', action='store_true', default=False,
                         help='collect batches and statistics without the optimizer step')
+    parser.add_argument('--eval_every', type=int, default=0,
+                        help='evaluate the policy every K epochs on whole episodes (0: never)')
+    parser.add_argument('--eval_episodes', type=int, default=1, help='episodes per evaluation slot')
+    parser.add_argument('--eval_nenvs', type=int, default=None, help='evaluation slots per GPU (default: --nenvs)')
+    parser.add_argument('--eval_greedy', action='store_true', default=False,
+                        help='evaluate with the argmax action of every head instead of sampled actions')
     return parser
 
 
@@ -177,6 +185,19 @@ def epoch_lines(epoch, stat, epoch_time):
     return [head] + [fmt.format(stat[key]) for key, fmt in _EPOCH_LINES if key in stat]
 
 
+def eval_line(stat, greedy, episodes, slots):
+    """The line printed for an evaluation: its stat dict (raw sums, Trainer.evaluate) normalised field by field as
+    update_log normalises an epoch's, without touching the log."""
+    np.set_printoptions(precision=2)
+    div = dict(LOG_FIELDS)
+    v = {k: (stat[k] / stat[div[k]] if div.get(k) and stat[div[k]] > 0 else stat[k]) for k in stat}
+    parts = [fmt.format(v[k]) for k, fmt in (('success', 'Success {:.2f}'), ('reward', 'Reward {}'),
+                                             ('steps_taken', 'Steps-taken {:.2f}'), ('comm_action', 'Comm-Action {}'))
+             if k in v]
+    return 'Eval ({}, {} episodes \u00d7 {} slots): '.format('greedy' if greedy else 'sampled', episodes, slots) + \
+        '  '.join(parts)
+
+
 class _utils_alias(object):
     """Checkpoints interchange with the reference (main.py:260-272): its ``log`` is pickled as ``utils.LogField``.
     Inside this context the name ``utils`` resolves to ic3net_b200.utils and our LogField class pickles under that name, so files written here load in the reference and
@@ -199,20 +220,23 @@ class _utils_alias(object):
         return False
 
 
-def save_checkpoint(path, policy_net, log, trainer):
-    """main.py:260-265."""
+def save_checkpoint(path, policy_net, log, trainer, evals=None):
+    """main.py:260-265; evals: the evaluation results [(epoch, stat dict)], stored under 'eval' unless None."""
     d = dict(policy_net=policy_net.state_dict(), log=log, trainer=trainer.state_dict())
+    if evals is not None:
+        d['eval'] = list(evals)
     with _utils_alias():
         torch.save(d, path)
 
 
 def load_checkpoint(path, policy_net, log, trainer):
-    """main.py:267-272."""
+    """main.py:267-272.  Returns the checkpoint's evaluation results [(epoch, stat dict)] ([] without 'eval')."""
     with _utils_alias():
         d = torch.load(path, weights_only=False)
     policy_net.load_state_dict(d['policy_net'])
     log.update({k: LogField(*v) for k, v in d['log'].items()})
     trainer.load_state_dict(d['trainer'])
+    return list(d.get('eval', []))
 
 
 def main(argv=None):
@@ -260,8 +284,10 @@ def main(argv=None):
     trainer = MultiGPUTrainer(args, lambda: Trainer(args, policy_net, env))
 
     log = make_log()
+    evals = []
     if args.load:
-        load_checkpoint(args.load, policy_net, log, trainer)
+        evals = load_checkpoint(args.load, policy_net, log, trainer)
+    eval_slots = world * (args.eval_nenvs or args.nenvs)
 
     for ep in range(args.num_epochs):
         epoch_begin = time.time()
@@ -279,10 +305,16 @@ def main(argv=None):
             for ln in epoch_lines(epoch, stat, epoch_time):
                 print(ln)
             print('steps/s {:.0f}'.format(nsteps / max(epoch_time, 1e-9)))
+        if args.eval_every and epoch % args.eval_every == 0:    # every rank plays its slots; the sum is reduced
+            es = trainer.evaluate(args.eval_episodes, args.eval_greedy)
+            evals.append((epoch, es))
+            if rank == 0:
+                print(eval_line(es, args.eval_greedy, args.eval_episodes, eval_slots))
+        ck = evals if (evals or args.eval_every) else None     # without evaluation the checkpoint stays as it was
         if args.save_every and ep and args.save != '' and ep % args.save_every == 0 and rank == 0:
-            save_checkpoint(args.save + '_' + str(ep), policy_net, log, trainer)
+            save_checkpoint(args.save + '_' + str(ep), policy_net, log, trainer, ck)
         if args.save != '' and rank == 0:                # main.py:257-258: every epoch
-            save_checkpoint(args.save, policy_net, log, trainer)
+            save_checkpoint(args.save, policy_net, log, trainer, ck)
     if world > 1:
         torch.distributed.destroy_process_group()
     return 0

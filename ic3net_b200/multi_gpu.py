@@ -213,6 +213,15 @@ class MultiGPUTrainer(object):
             tr.optimizer.step()                                  # multi_processing.py:97
         return stat
 
+    def evaluate(self, episodes=1, greedy=False, epoch=None):
+        """Trainer.evaluate on every rank's evaluation slots; the statistics vector is summed over ranks with one
+        all-reduce, so every rank returns the stat dict of all ranks' episodes."""
+        tr = self.trainer
+        vec, e = tr.evaluate_vector(episodes, greedy, epoch)
+        if _dist_on():
+            dist.all_reduce(vec, op=dist.ReduceOp.SUM)
+        return tr.stat_from_vector(vec.cpu().numpy(), e)
+
     def state_dict(self):
         return self.trainer.state_dict()
 

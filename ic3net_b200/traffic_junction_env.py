@@ -173,6 +173,22 @@ class TrafficJunctionEnv(object):
             self.add_rate = step_size * (self.exact_rate // step_size)
             self.cfg.spawn_thr = self._spawn_thr()
 
+    def curriculum_until(self, epoch):
+        """add_rate as training reaches it at `epoch`: the curriculum replayed from add_rate_min through reset(1) ..
+        reset(epoch) (the final epoch gives the target add_rate)."""
+        self.exact_rate = self.add_rate = self.add_rate_min
+        self.epoch_last_update = 0
+        self.cfg.spawn_thr = self._spawn_thr()
+        if self.curr_end - self.curr_start > 0 and self.add_rate_max - self.add_rate_min > 0:
+            for ep in range(1, epoch + 1):
+                self.curriculum(ep)
+                self.epoch_last_update = ep
+
+    def set_add_rate(self, other):
+        """Take the curriculum state (add_rate and its progress) of another env of the same configuration."""
+        self.exact_rate, self.add_rate, self.epoch_last_update = other.exact_rate, other.add_rate, other.epoch_last_update
+        self.cfg.spawn_thr = self._spawn_thr()
+
     def _get_obs(self):
         obs = self._new_obs()
         _lib.check(_lib.load().ic3_tj_obs(C.byref(self.cfg), C.byref(self.state), obs.data_ptr(), _lib.stream()))

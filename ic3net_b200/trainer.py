@@ -48,6 +48,7 @@ hidden-state record or checkpoint at all; the backward re-runs the forward from 
 consecutive lock-steps (K*B env slots at once, K from the memory the device has left, ``FF_CHUNK_STEPS``), with the
 products of the backward on the tensor cores (csrc/ff_grad_tc.cu).
 """
+import argparse
 import ctypes as C
 import math
 from collections import namedtuple
@@ -55,7 +56,7 @@ from collections import namedtuple
 import torch
 import torch.nn.functional as F
 
-from . import _lib
+from . import _lib, data
 from .models import Random
 from .optim import FlatRMSprop
 from .utils import merge_stat
@@ -196,9 +197,10 @@ class Trainer(object):
                                           "<= 7 action logits, a vision window of <= 5 x 5 cells and an observation "
                                           "pattern of <= 512 columns" % (self.grad_impl, _lib.MAX_PASSES))
 
-    def _policy_cfg(self):
-        """ic3_policy_cfg of the policy step over this GPU's slots, with the env's Philox key and env ids."""
-        e = self.env.env
+    def _policy_cfg(self, e=None):
+        """ic3_policy_cfg of the policy step over this GPU's slots of env e (default: the training env), with the env's
+        Philox key and env ids."""
+        e = self.env.env if e is None else e
         cfg = self.policy_net.policy_cfg(e.nenvs)
         cfg.seed, cfg.env_id0 = e.cfg.seed, e.cfg.env_id0
         return cfg
@@ -213,34 +215,43 @@ class Trainer(object):
         """ic3_bptt_workspace_bytes of the policy configuration cfg on this environment (0: not covered)."""
         return int(_lib.load().ic3_bptt_workspace_bytes(C.byref(self._bptt_plan(cfg))))
 
-    def _encoder_table(self, cfg=None, w=None):
-        """The policy's per-position encoder table for this environment (CommNetMLP.encoder_table), built from its
-        current packed weights; cfg and w are accepted for callers that hold them and are not needed."""
-        return self.policy_net.encoder_table(self.env.env)
+    def _encoder_table(self, cfg=None, w=None, e=None):
+        """The policy's per-position encoder table for env e (default: the training env; CommNetMLP.encoder_table),
+        built from its current packed weights; cfg and w are accepted for callers that hold them and are not needed."""
+        return self.policy_net.encoder_table(self.env.env if e is None else e)
 
     # ------------------------------------------------------------------ buffers
+    def _slot_buffers(self, B, T, dev):
+        """What every run of the lock-step loop over B slots needs: episode state, statistics, T steps of action /
+        log-prob / value and, for a policy with weights, h, c and x."""
+        N, H = self.args.nagents, self.args.hid_size
+        nh = len(self.args.naction_heads)
+        A = sum(self.args.naction_heads)
+        z = lambda *s, dtype=torch.float32: torch.zeros(*s, dtype=dtype, device=dev)
+        b = dict(T=T, comm=z(B, N, dtype=torch.uint8), alive=torch.ones(B, N, dtype=torch.uint8, device=dev),
+                 fresh=torch.ones(B, dtype=torch.uint8, device=dev), t_ep=z(B, dtype=torch.int32),
+                 action=z(T, B, N, nh, dtype=torch.int32), logp=z(T, B, N, A), value=z(T, B * N), step_reward=z(B, N),
+                 stat_reward=z(B, N), stat_comm=z(B, N), stat_success=z(B, dtype=torch.int32),
+                 stat_episodes=z(B, dtype=torch.int32), stat_steps=z(B, dtype=torch.int32),
+                 err=z(1, dtype=torch.int32), halted=z(B, dtype=torch.uint8), statvec=z(4 + 2 * N, dtype=torch.float64))
+        if not self.random_policy:            # models.Random has no encoder or recurrent state
+            b.update(h=z(B * N, H), c=z(B * N, H), x=z(B * N, H))
+        return b
+
     def _alloc(self, T):
         # the previous buffers go back to the allocator before the records are sized
         self._buf = self._graph = self._ugraphs = None
         e = self.env.env
         B, N, H = e.nenvs, self.args.nagents, self.args.hid_size
         dev = e.device
-        nh = len(self.args.naction_heads)
         A = sum(self.args.naction_heads)
         z = lambda *s, dtype=torch.float32: torch.zeros(*s, dtype=dtype, device=dev)
-        b = dict(T=T, comm=z(B, N, dtype=torch.uint8), alive=torch.ones(B, N, dtype=torch.uint8, device=dev),
-                 fresh=torch.ones(B, dtype=torch.uint8, device=dev), t_ep=z(B, dtype=torch.int32),
-                 action=z(T, B, N, nh, dtype=torch.int32), logp=z(T, B, N, A), value=z(T, B * N),
-                 reward=z(T, B, N), emask=z(T, B, dtype=torch.uint8), mini=z(T, B, N, dtype=torch.uint8),
-                 ralive=z(T, B, N, dtype=torch.uint8), step_reward=z(B, N),
-                 stat_reward=z(B, N), stat_comm=z(B, N), stat_success=z(B, dtype=torch.int32),
-                 stat_episodes=z(B, dtype=torch.int32), stat_steps=z(B, dtype=torch.int32),
-                 err=z(1, dtype=torch.int32), halted=z(B, dtype=torch.uint8), valid=z(T, B, dtype=torch.uint8),
-                 statvec=z(4 + 2 * N, dtype=torch.float64))
-        if self.random_policy:                # no encoder, observation or recurrent state
+        b = self._slot_buffers(B, T, dev)
+        b.update(reward=z(T, B, N), emask=z(T, B, dtype=torch.uint8), mini=z(T, B, N, dtype=torch.uint8),
+                 ralive=z(T, B, N, dtype=torch.uint8), valid=z(T, B, dtype=torch.uint8))
+        if self.random_policy:                # no observation or recurrent state
             self._buf = b
             return b
-        b.update(h=z(B * N, H), c=z(B * N, H), x=z(B * N, H))
         if self.obs_mode == 'dense':
             b['obs'] = torch.empty(B, N, self.env.observation_dim, dtype=torch.float32, device=dev)
         if self.record_for_grad:
@@ -359,43 +370,50 @@ class Trainer(object):
     # medium, 20 MB, 1 % faster; predator-prey hard, 1.19 GB, 9 % faster).
     OVERLAP_MIN_OBS_BYTES = 8 << 20
 
-    def _overlap_obs(self):
+    def _overlap_obs(self, e=None):
         """Dense observations on the tensor-core policy path: the policy step computes x from the env state (the fused
         index encoder; without the per-position table, which measured no faster beside the writer, so dense mode never
         builds it) and the observation block is written concurrently on a side stream.  Not for blocks smaller than
         OVERLAP_MIN_OBS_BYTES."""
         if self.obs_mode != 'dense':
             return False
-        e = self.env.env
+        e = self.env.env if e is None else e
         if e.nenvs * self.args.nagents * self.env.observation_dim * 4 < self.OVERLAP_MIN_OBS_BYTES:
             return False
         return self.policy_net.fuses_encoder(e)
 
-    def _enqueue(self, T, quota=0):
+    def _enqueue(self, T, quota=0, b=None, e=None, episodes=0, greedy=False):
         """Enqueue T lock-step iterations on the current stream (no host sync).  quota > 0: reference batch
         boundary -- a slot halts at the first episode end with >= quota steps (ic3_rollout_io.batch_size);
-        quota = 0: episodes still open at iteration T-1 are cut there."""
+        quota = 0: episodes still open at iteration T-1 are cut there.  b, e: buffers and env (default: the training
+        rollout's; evaluate passes its own, which hold no records and one lock-step of action / log-prob / value
+        scratch, and no observation block: x comes from the env state); episodes > 0: episode quota
+        (ic3_rollout_io.episodes); greedy: argmax actions (ic3_policy_cfg.greedy)."""
+        b = self._buf if b is None else b
+        e = self.env.env if e is None else e
         if self.random_policy:
-            return self._enqueue_random(T, quota)
-        b, e, net = self._buf, self.env.env, self.policy_net
+            return self._enqueue_random(T, quota, b, e, episodes)
+        net = self.policy_net
         lib = _lib.load()
         B = e.nenvs
-        cfg = self._policy_cfg()
+        cfg = self._policy_cfg(e)
+        cfg.greedy = int(greedy)
         w = net.packed()
         s = _lib.stream()
         ws, _ = net.workspace(B)          # tensor-core path scratch (None for the fp32 SIMT kernel)
-        rec = self.record_for_grad
+        rec = self.record_for_grad and 's_fresh' in b
         full = rec and self._record_mode == 'full'    # the policy step writes (h, c) straight into the records
         window = rec and self._record_mode == 'window'    # (h, c) checkpoints + max |c| per step (_alloc)
         hc = not self._h_only_records()               # the tanh RNN's kernel records: h alone
-        dense = self.obs_mode == 'dense'
+        dense = 'obs' in b                            # _alloc makes the block for obs_mode 'dense'
         # dense observations written on a side stream while the policy step runs (see _overlap_obs)
-        overlap = self._overlap_obs()
+        overlap = dense and self._overlap_obs(e)
         # tensor-core path: the index encoder is fused into the policy step (x never leaves the operand image)
-        fused_x = self._fused_x() or overlap
+        fused_x = (not dense and net.fuses_encoder(e)) or overlap
         src = {}
         if fused_x:
-            src = dict(_lib.env_source(e.cfg, e.state), x_table=None if overlap else _lib.ptr(self._encoder_table()))
+            src = dict(_lib.env_source(e.cfg, e.state),
+                       x_table=None if overlap else _lib.ptr(self._encoder_table(e=e)))
         if overlap:
             main = torch.cuda.current_stream()
             if self._side is None or self._side.device != main.device:
@@ -441,11 +459,12 @@ class Trainer(object):
                                                     b['x'].data_ptr(), s))
             hin, hout = (b['rec_h'][t], b['rec_h'][t + 1]) if full else (b['h'], b['h'])
             cin, cout = (b['rec_c'][t], b['rec_c'][t + 1]) if full and hc else (b['c'], b['c'])
+            r = t % b['T']                    # record row: t, or 0 in evaluate's one-step scratch
             io = _lib.PolicyIO(x=None if fused_x else b['x'].data_ptr(), h=hin.data_ptr(), c=cin.data_ptr(),
                                comm_action=b['comm'].data_ptr() if self.hard else None, alive=b['alive'].data_ptr(),
                                fresh=b['fresh'].data_ptr(), tick=e.tick.data_ptr(), draws=None,
-                               h_out=hout.data_ptr(), c_out=cout.data_ptr(), value=b['value'][t].data_ptr(),
-                               logp=b['logp'][t].data_ptr(), action=b['action'][t].data_ptr(),
+                               h_out=hout.data_ptr(), c_out=cout.data_ptr(), value=b['value'][r].data_ptr(),
+                               logp=b['logp'][r].data_ptr(), action=b['action'][r].data_ptr(),
                                workspace=_lib.ptr(ws), err=b['err'].data_ptr(), **src)
             _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
             if window and hc:
@@ -454,54 +473,60 @@ class Trainer(object):
                 torch.linalg.vector_norm(b['c'], math.inf, out=b['c_abs'][t])
             if overlap:
                 main.wait_stream(side)
-            self._env_step(t, T, quota, snap, s)
+            self._env_step(t, T, quota, snap, s, b, e, episodes)
 
-    def _env_step(self, t, T, quota, snap, s):
+    def _env_step(self, t, T, quota, snap, s, b=None, e=None, episodes=0):
         """Env step of lock-step iteration t on the actions the policy step wrote to the records, with the
-        Trainer.get_episode bookkeeping and auto-reset (ic3_rollout_io; ``snap``: its snap_* fields)."""
-        b, e, args = self._buf, self.env.env, self.args
+        Trainer.get_episode bookkeeping and auto-reset (ic3_rollout_io; ``snap``: its snap_* fields).  b, e, episodes:
+        see _enqueue; a record evaluate's buffers do not hold is passed as NULL."""
+        b = self._buf if b is None else b
+        e = self.env.env if e is None else e
+        args = self.args
         lib = _lib.load()
         nh = len(args.naction_heads)
+        act = b['action'][t % b['T']]
+        rec = lambda k: _lib.ptr(b.get(k))
         r = _lib.RolloutIO(t=t, max_steps=args.max_steps, nheads=nh, hard_attn=int(self.hard),
                            comm_action_one=int(bool(args.comm_action_one)),
-                           last=int(t == T - 1 and quota <= 0), batch_size=int(quota),
-                           halted=b['halted'].data_ptr(), rec_valid=b['valid'].data_ptr(), **snap,
-                           action=b['action'][t].data_ptr(), t_ep=b['t_ep'].data_ptr(),
+                           last=int(t == T - 1 and quota <= 0 and episodes <= 0), batch_size=int(quota),
+                           episodes=int(episodes), halted=b['halted'].data_ptr(), rec_valid=rec('valid'), **snap,
+                           action=act.data_ptr(), t_ep=b['t_ep'].data_ptr(),
                            fresh=b['fresh'].data_ptr(), comm_next=b['comm'].data_ptr(),
-                           alive_next=b['alive'].data_ptr(), rec_reward=b['reward'].data_ptr(),
-                           rec_episode_mask=b['emask'].data_ptr(), rec_mini_mask=b['mini'].data_ptr(),
-                           rec_alive=b['ralive'].data_ptr(), stat_reward=b['stat_reward'].data_ptr(),
+                           alive_next=b['alive'].data_ptr(), rec_reward=rec('reward'),
+                           rec_episode_mask=rec('emask'), rec_mini_mask=rec('mini'),
+                           rec_alive=rec('ralive'), stat_reward=b['stat_reward'].data_ptr(),
                            stat_comm=b['stat_comm'].data_ptr(), stat_success=b['stat_success'].data_ptr(),
                            stat_episodes=b['stat_episodes'].data_ptr(), stat_steps=b['stat_steps'].data_ptr())
         if self.is_tj:
-            _lib.check(lib.ic3_tj_step(C.byref(e.cfg), C.byref(e.state), b['action'][t].data_ptr(), nh, None,
+            _lib.check(lib.ic3_tj_step(C.byref(e.cfg), C.byref(e.state), act.data_ptr(), nh, None,
                                        b['step_reward'].data_ptr(), None, b['err'].data_ptr(), C.byref(r), s))
         else:
-            _lib.check(lib.ic3_pp_step(C.byref(e.cfg), C.byref(e.state), b['action'][t].data_ptr(), nh,
+            _lib.check(lib.ic3_pp_step(C.byref(e.cfg), C.byref(e.state), act.data_ptr(), nh,
                                        b['step_reward'].data_ptr(), None, b['err'].data_ptr(), C.byref(r), s))
 
-    def random_cfg(self):
+    def random_cfg(self, e=None):
         """ic3_policy_cfg of the Random policy step: the fields ic3_random_policy_step reads (B, N, heads, Philox key
-        and env ids of this GPU's slots)."""
-        e, heads = self.env.env, list(self.args.naction_heads)
+        and env ids of this GPU's slots of env e, default the training env)."""
+        e, heads = self.env.env if e is None else e, list(self.args.naction_heads)
         return _lib.PolicyCfg(B=e.nenvs, N=self.args.nagents, nheads=len(heads),
                               head_dim=(C.c_int32 * _lib.MAX_HEADS)(*heads), env_id0=e.cfg.env_id0, seed=e.cfg.seed)
 
-    def _enqueue_random(self, T, quota):
+    def _enqueue_random(self, T, quota, b, e, episodes=0):
         """_enqueue for models.Random: per lock-step iteration one ic3_random_policy_step (value, log-probs and actions
         into the records, from the env's action tick) and the env step."""
-        b, e = self._buf, self.env.env
         lib = _lib.load()
-        cfg = self.random_cfg()
+        cfg = self.random_cfg(e)
         s = _lib.stream()
         for t in range(T):
-            io = _lib.PolicyIO(tick=e.tick.data_ptr(), value=b['value'][t].data_ptr(), logp=b['logp'][t].data_ptr(),
-                               action=b['action'][t].data_ptr())
+            r = t % b['T']
+            io = _lib.PolicyIO(tick=e.tick.data_ptr(), value=b['value'][r].data_ptr(), logp=b['logp'][r].data_ptr(),
+                               action=b['action'][r].data_ptr())
             _lib.check(lib.ic3_random_policy_step(C.byref(cfg), C.byref(io), None, s))
-            self._env_step(t, T, quota, {}, s)
+            self._env_step(t, T, quota, {}, s, b, e, episodes)
 
-    def _episode_boundary(self, epoch):
-        e, b = self.env.env, self._buf
+    def _episode_boundary(self, epoch, b=None, e=None):
+        b = self._buf if b is None else b
+        e = self.env.env if e is None else e
         if self.is_tj:
             e.reset(epoch, want_obs=False)
         else:
@@ -529,22 +554,8 @@ class Trainer(object):
             # 196-200,620-626; a re-seeded env changes cfg.seed) and a stale graph is re-captured
             key = (T, int(quota), int(getattr(e.cfg, 'spawn_thr', 0)), int(e.cfg.seed), int(e.cfg.env_id0))
             if self._graph is None or self._graph_key != key:
-                # warm-up pass (lazy function attributes, allocator) on a snapshot of the env state, rewound afterwards:
-                # the captured pass then starts from exactly the state an eager rollout would start from (same RNG ticks)
-                snap = e.snapshot()
-                keys = ('fresh', 'comm', 'alive', 't_ep', 'h', 'c', 'halted', 'stat_reward', 'stat_comm', 'stat_success',
-                        'stat_episodes', 'stat_steps')
-                saved = {k: b[k].clone() for k in keys if k in b}
-                self._enqueue(T, quota)
-                torch.cuda.synchronize()
-                e.restore(snap)                   # env state, RNG ticks ...
-                for k, v in saved.items():        # ... and the trainer-side episode state, as the boundary above left them
-                    b[k].copy_(v)
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    self._enqueue(T, quota)
-                self._graph, self._graph_key = g, key
-                g.replay()
+                self._graph, self._graph_key = self._capture(b, e, lambda: self._enqueue(T, quota)), key
+                self._graph.replay()
             else:
                 self._graph.replay()
         else:
@@ -553,10 +564,30 @@ class Trainer(object):
                             reward=b['reward'], episode_mask=b['emask'], episode_mini_mask=b['mini'],
                             alive_mask=b['ralive'], valid=b['valid'])
 
-    def stat_vector(self):
+    def _capture(self, b, e, enqueue):
+        """CUDA graph of enqueue() on buffers b and env e, not yet replayed.  A warm-up pass (lazy function attributes,
+        allocator) runs first on a snapshot of the env state and is rewound: the captured pass then starts from exactly
+        the state an eager run would start from (same RNG ticks)."""
+        snap = e.snapshot()
+        keys = ('fresh', 'comm', 'alive', 't_ep', 'h', 'c', 'halted', 'stat_reward', 'stat_comm', 'stat_success',
+                'stat_episodes', 'stat_steps')
+        saved = {k: b[k].clone() for k in keys if k in b}
+        enqueue()
+        torch.cuda.synchronize()
+        e.restore(snap)                   # env state, RNG ticks ...
+        for k, v in saved.items():        # ... and the trainer-side episode state, as the boundary left them
+            b[k].copy_(v)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            enqueue()
+        return g
+
+    def stat_vector(self, b=None, e=None):
         """Device float64 vector [num_episodes, num_steps, success, err flags, reward[N], comm_action[N]] of this
-        GPU's slots (one kernel, csrc/returns.cu ic3_stat_reduce); no host synchronisation."""
-        b, e = self._buf, self.env.env
+        GPU's slots (one kernel, csrc/returns.cu ic3_stat_reduce); no host synchronisation.  b, e: buffers and env
+        (default: the training rollout's)."""
+        b = self._buf if b is None else b
+        e = self.env.env if e is None else e
         _lib.check(_lib.load().ic3_stat_reduce(e.nenvs, self.args.nagents, b['stat_episodes'].data_ptr(),
                                                b['stat_steps'].data_ptr(), b['stat_success'].data_ptr(),
                                                b['err'].data_ptr(), b['stat_reward'].data_ptr(),
@@ -564,9 +595,10 @@ class Trainer(object):
                                                b['statvec'].data_ptr(), _lib.stream()))
         return b['statvec']
 
-    def stat_from_vector(self, v):
+    def stat_from_vector(self, v, e=None):
         """Host-side stat dict with the reference's keys (trainer.py:73-75,86-88,109-110,124-125,235) from a
-        stat_vector() (of this GPU, or summed over ranks) that has been copied to the host."""
+        stat_vector() (of this GPU, or summed over ranks) that has been copied to the host; e: the env it was collected
+        on (default: the training env)."""
         args, N = self.args, self.args.nagents
         flags = int(v[3])
         if flags:
@@ -589,7 +621,7 @@ class Trainer(object):
         if self.is_tj:
             # every episode of the batch reports the same env.stat['add_rate'] (traffic_junction_env.py:249-250),
             # merged by + over episodes and workers (trainer.py:124-125, utils.py:15-29)
-            stat['add_rate'] = self.env.env.add_rate * stat['num_episodes']
+            stat['add_rate'] = (self.env.env if e is None else e).add_rate * stat['num_episodes']
         return stat
 
     def collect_stat(self):
@@ -615,6 +647,70 @@ class Trainer(object):
         if getattr(self.args, 'batch_boundary', 'reference') == 'cut':
             return full, 0
         return (bs + ms - 1 if self.episodes_end_early() else full), bs
+
+    # ------------------------------------------------------------------ evaluation
+    def _eval_state(self):
+        """The evaluation environment (args.eval_nenvs slots, default nenvs, built once with data.init) and its buffers.
+        Its global env ids follow every rank's training ids: training's are id0 + rank * nenvs + [0, nenvs) with id0 the
+        job's first training id (this rank's env_id0 - rank * nenvs), evaluation's id0 + world * nenvs +
+        rank * eval_nenvs + [0, eval_nenvs), so its Philox streams never meet training's."""
+        if getattr(self, '_eval', None) is not None:
+            return self._eval
+        tr_env, args = self.env.env, self.args
+        ne = int(getattr(args, 'eval_nenvs', None) or tr_env.nenvs)
+        dist = torch.distributed
+        on = dist.is_available() and dist.is_initialized()
+        world, rank = (dist.get_world_size(), dist.get_rank()) if on else (1, 0)
+        ea = argparse.Namespace(**vars(args))
+        ea.nenvs = ne
+        ea.env_id0 = int(tr_env.cfg.env_id0) - rank * tr_env.nenvs + world * tr_env.nenvs + rank * ne
+        e = data.init(args.env_name, ea).env
+        e.cfg.seed = tr_env.cfg.seed
+        self._eval = dict(env=e, buf=self._slot_buffers(ne, 1, e.device), graph=None, key=None)
+        return self._eval
+
+    def evaluate_vector(self, episodes=1, greedy=False, epoch=None):
+        """evaluate without the host read: the device float64 statistics vector (stat_vector's layout) of the episodes,
+        and the evaluation env they were played on."""
+        episodes = int(episodes)
+        if episodes < 1:
+            raise ValueError("evaluate plays at least one episode per slot, not %d" % episodes)
+        if greedy and self.random_policy:
+            raise ValueError("models.Random has no greedy action: its logits do not depend on the observation")
+        ev = self._eval_state()
+        e, b = ev['env'], ev['buf']
+        if self.is_tj:
+            if epoch is None:
+                e.set_add_rate(self.env.env)
+            else:
+                e.curriculum_until(int(epoch))
+        self._episode_boundary(None, b, e)
+        b['err'].zero_()
+        T = episodes * int(self.args.max_steps)
+        if not self.random_policy:
+            self.policy_net.packed()
+            # always rebuilt: a replayed training update re-builds the training env's table only, yet marks every
+            # table current (CommNetMLP.mark_packed_current)
+            self.policy_net.encoder_table(e, force=True)
+        run = lambda: self._enqueue(T, 0, b, e, episodes, greedy)
+        if self.use_graph:
+            key = (T, episodes, bool(greedy), int(getattr(e.cfg, 'spawn_thr', 0)), int(e.cfg.seed), int(e.cfg.env_id0))
+            if ev['graph'] is None or ev['key'] != key:
+                ev['graph'], ev['key'] = self._capture(b, e, run), key
+            ev['graph'].replay()
+        else:
+            run()
+        return self.stat_vector(b, e), e
+
+    def evaluate(self, episodes=1, greedy=False, epoch=None):
+        """Play exactly ``episodes`` whole episodes in every slot of the evaluation env (see _eval_state), each slot
+        from a fresh reset, with sampled actions or, ``greedy``, the argmax of every head.  Returns the collect_stat
+        dict of those episodes (raw sums; num_episodes = episodes * eval_nenvs).  Traffic junction: ``epoch`` sets
+        add_rate through the env's curriculum as training reaches it at that epoch; None takes the training env's
+        current add_rate.  Training state (env, ticks, buffers, records, graphs) is not touched; the policy is only
+        read.  Successive calls continue the evaluation env's random streams."""
+        vec, e = self.evaluate_vector(episodes, greedy, epoch)
+        return self.stat_from_vector(vec.cpu().numpy(), e)
 
     def steps_per_batch(self):
         return self.batch_plan()[0]

@@ -43,7 +43,8 @@ enum {
   IC3_OK = 0,
   IC3_E_NULL = -1,        /* required pointer missing */
   IC3_E_RANGE = -2,       /* size / enum out of the supported range */
-  IC3_E_UNSUPPORTED = -3  /* configuration the kernels do not implement */
+  IC3_E_UNSUPPORTED = -3, /* configuration the kernels do not implement */
+  IC3_E_ARG = -4          /* arguments that contradict each other */
 };
 
 enum {
@@ -123,7 +124,12 @@ typedef struct {
    * stat_steps[slot] >= batch_size and is skipped by every later lock-step (null records).  With
    * T >= batch_size + max_steps - 1 lock-steps every slot halts by itself and `last` stays 0.  0 / NULL: off. */
   int32_t batch_size;
-  int32_t reserved0;
+  /* Episode quota (evaluation): episodes > 0 with halted != NULL: a slot halts at the episode end at which
+   * stat_episodes[slot] reaches `episodes` and is skipped by every later lock-step like a slot past batch_size.
+   * With T >= episodes * max_steps lock-steps every slot halts by itself and `last` stays 0.  Needs stat_episodes;
+   * batch_size > 0 together with episodes > 0, or episodes > 0 without halted / stat_episodes, is IC3_E_ARG, and
+   * episodes < 0 is IC3_E_RANGE.  0: off. */
+  int32_t episodes;
   uint8_t* halted;         /* [B] in/out: slot has completed its batch */
   uint8_t* rec_valid;      /* [T, B] 1 = a real step of this slot, 0 = slot already halted (may be NULL) */
   /* Inputs of the NEXT policy step, recorded for Trainer.compute_grad (all optional; written at index t + 1 when
@@ -250,7 +256,10 @@ typedef struct {
    *   h_from_x  the hidden state entering the first pass is x itself instead of io->h (comm.py:129)
    * Variants run on the fp32 SIMT kernel (the tensor-core path implements the all-zero configuration). */
   int32_t cell, passes, x_tanh, h_from_x;
-  int32_t reserved0;
+  /* 1: with io->action != NULL each head takes the lowest index of its largest fp32 logit (torch.argmax) instead of
+   * the inverse-CDF draw; value and log-probs are written as in sampled mode, and neither the action stream nor
+   * io->draws is read.  0: sampled actions.  ic3_random_policy_step refuses 1 (IC3_E_ARG). */
+  int32_t greedy;
 } ic3_policy_cfg;
 
 enum { IC3_CELL_LSTM = 0, IC3_CELL_TANH = 1 };
