@@ -288,13 +288,13 @@ class CommNetMLP(nn.Module):
         self._packed_key = key
         return self._packed
 
-    def mark_packed_current(self):
-        """A replayed CUDA graph has just re-packed the current parameters (and re-built the encoder tables) on the
-        device: take the parameters' present version counters as the key, so packed() does not pack them again."""
+    def mark_packed_current(self, envs=()):
+        """A replayed CUDA graph has just re-packed the current parameters and re-built the encoder tables of envs: take
+        the parameters' present version counters as the key of those, so packed() and encoder_table() keep them."""
         key = tuple((p.data_ptr(), p._version) for p in self._param_list())
-        for env, (k, table) in list(self._enc_tables.items()):
-            if k == self._packed_key:
-                self._enc_tables[env] = (key, table)
+        for env in envs:
+            if env in self._enc_tables:          # none where the layout has no separate class terms (encoder_table)
+                self._enc_tables[env] = (key, self._enc_tables[env][1])
         self._packed_key = key
 
     def policy_params(self, get):

@@ -74,6 +74,11 @@ TJ_RECORDS = (('s_tjloc', 'car_loc', 'loc', 'snap_tj_loc'), ('s_tjalive', 'alive
               ('s_tjlast', 'car_last_act', 'last_act', 'snap_tj_last_act'),
               ('s_tjroute', 'route_id', 'route_id', 'snap_tj_route_id'))
 
+# What a lock-step writes in every slot's buffers (models.Random has no h or c): the state a warm-up pass before a CUDA
+# graph capture rewinds (_capture)
+SLOT_STATE = ('fresh', 'comm', 'alive', 't_ep', 'h', 'c', 'halted', 'stat_reward', 'stat_comm', 'stat_success',
+              'stat_episodes', 'stat_steps', 'err')
+
 
 def policy_forward_torch(net, x, h, c, g, n_alive):
     """Differentiable torch restatement of the policy step the kernels run (comm.py:134-244 for every variant of
@@ -146,13 +151,10 @@ class Trainer(object):
         self._buf = None
         self._record_mode = None             # 'full' | 'window' per allocation (record_mode)
         self._ff_K = None                    # graph_update: kernels_ff chunk length frozen into the captured update
-        self._graph = None
-        self._graph_key = None
+        self._graphs = {}                    # 'rollout' | 'evaluate' | 'update' -> (key, graphs, result) (_replay)
         self._side = None                    # stream of the dense observation writer (_overlap_obs)
         # graph_update: train_batch replays the whole update from CUDA graphs (train_batch_graph)
         self.graph_update = bool(getattr(args, 'graph_update', False))
-        self._ugraphs = None
-        self._ugraph_key = None
         self.update_captures = 0             # graph_update: how often the update was captured
         if self.random_policy and self.graph_update:
             raise NotImplementedError("graph_update replays a gradient update; models.Random has neither gradient nor "
@@ -239,8 +241,10 @@ class Trainer(object):
         return b
 
     def _alloc(self, T):
-        # the previous buffers go back to the allocator before the records are sized
-        self._buf = self._graph = self._ugraphs = None
+        # the previous buffers, and the graphs that run on them, go back to the allocator before the records are sized
+        self._buf = None
+        for name in ('rollout', 'update'):
+            self._graphs.pop(name, None)
         e = self.env.env
         B, N, H = e.nenvs, self.args.nagents, self.args.hid_size
         dev = e.device
@@ -287,7 +291,6 @@ class Trainer(object):
                 if hc:
                     b.update(c_abs=z(T), win_c=[e_(L, B * N, H) for _ in range(nb)])
         self._buf = b
-        self._graph = None
         return b
 
     # The BPTT kernels' (h, c) records.  What the device has for them is measured when the rollout buffers have been
@@ -535,52 +538,93 @@ class Trainer(object):
             b[k].zero_()
         b['fresh'].fill_(1)
 
+    def _begin(self, T, epoch, b=None, e=None):
+        """Start a run of T lock-step iterations on buffers b and env e (default: the training rollout's, allocated
+        anew when T changes): fresh episodes in every slot (trainer.py:28-32, 45-51; the TJ curriculum may move
+        cfg.spawn_thr), the error word zeroed, and the packed weights and e's encoder table brought up to date outside
+        any graph capture (_refresh_weights).  Returns (b, e)."""
+        if b is None:
+            if self._buf is None or self._buf['T'] != T:
+                self._alloc(T)
+            b = self._buf
+        e = self.env.env if e is None else e
+        self._episode_boundary(epoch, b, e)
+        b['err'].zero_()
+        self._refresh_weights(b, e)
+        return b, e
+
+    def _refresh_weights(self, b, e, force=False):
+        """Re-pack the weights and re-build the encoder table a run on buffers b and env e reads (none with a dense
+        observation block) if the parameters changed since they were built; with force always."""
+        if not self.random_policy:
+            self.policy_net.packed(force=force)
+            if 'obs' not in b:
+                self.policy_net.encoder_table(e, force=force)
+
     def rollout(self, T, epoch=0, quota=0):
         """T lock-step iterations from fresh episodes in every slot (``quota``: see _enqueue).  Returns a
         RolloutBatch of stacked [T, B, ...] device tensors (views of the trainer's record buffers)."""
-        e = self.env.env
-        if self._buf is None or self._buf['T'] != T:
-            self._alloc(T)
-        b = self._buf
-        self._episode_boundary(epoch)             # trainer.py:28-32, 45-51
-        b['err'].zero_()
-        if not self.random_policy:
-            self.policy_net.packed()              # (re)pack weights outside any graph capture
-            if self._fused_x():
-                self._encoder_table()             # ... and the encoder table with them
+        b, e = self._begin(T, epoch)
+        run = lambda: self._enqueue(T, quota)
         if self.use_graph:
-            # kernel arguments passed BY VALUE are frozen into a captured graph: everything of that kind that can
-            # change between rollouts is part of the key (the TJ curriculum moves cfg.spawn_thr, traffic_junction_env.py:
-            # 196-200,620-626; a re-seeded env changes cfg.seed) and a stale graph is re-captured
-            key = (T, int(quota), int(getattr(e.cfg, 'spawn_thr', 0)), int(e.cfg.seed), int(e.cfg.env_id0))
-            if self._graph is None or self._graph_key != key:
-                self._graph, self._graph_key = self._capture(b, e, lambda: self._enqueue(T, quota)), key
-                self._graph.replay()
-            else:
-                self._graph.replay()
+            self._replay('rollout', self._graph_key(T, e, int(quota)), b, e, [run])
         else:
-            self._enqueue(T, quota)
+            run()
         return RolloutBatch(action=b['action'], logp=b['logp'], value=b['value'].view(T, e.nenvs, -1),
                             reward=b['reward'], episode_mask=b['emask'], episode_mini_mask=b['mini'],
                             alive_mask=b['ralive'], valid=b['valid'])
 
-    def _capture(self, b, e, enqueue):
-        """CUDA graph of enqueue() on buffers b and env e, not yet replayed.  A warm-up pass (lazy function attributes,
-        allocator) runs first on a snapshot of the env state and is rewound: the captured pass then starts from exactly
-        the state an eager run would start from (same RNG ticks)."""
+    def _graph_key(self, T, e, *extras):
+        """Key of a run of T lock-steps on env e captured into CUDA graphs: kernel arguments passed BY VALUE are frozen
+        into a graph, so everything of that kind that can change between runs is part of the key (the TJ curriculum
+        moves cfg.spawn_thr, traffic_junction_env.py:196-200,620-626; a re-seeded env changes cfg.seed), with the
+        caller's own such values in extras."""
+        return (T, int(getattr(e.cfg, 'spawn_thr', 0)), int(e.cfg.seed), int(e.cfg.env_id0), e.nenvs) + extras
+
+    def _replay(self, name, key, b, e, phases, between=None, restore=()):
+        """Run phases on buffers b and env e by replaying the CUDA graphs cached under name, captured first (_capture)
+        when the cache holds none for this key.  Returns (what phases[0] returned, whether they were captured now)."""
+        entry = self._graphs.get(name)
+        captured = entry is None or entry[0] != key
+        if captured:
+            entry = self._graphs[name] = (key,) + self._capture(b, e, phases, between, restore)
+        _, graphs, out = entry
+        graphs[0].replay()
+        for g in graphs[1:]:
+            between(out)
+            g.replay()
+        return out, captured
+
+    def _capture(self, b, e, phases, between=None, restore=()):
+        """CUDA graphs of phases on buffers b and env e, not yet replayed: phases[0]() returns r (or None), each later
+        phase is called with r.  A warm-up pass (lazy library state, allocator, workspaces) runs first and is rewound --
+        env state and RNG ticks, b's SLOT_STATE, the tensors in restore -- and the weights are re-packed (the warm-up may
+        have packed updated ones, and restored parameters keep their version counters), so the capture starts where an
+        eager run would.  One graph holds all phases; with between(r), an eager step between phases (MultiGPUTrainer's
+        all-reduces), each phase is a graph of its own in the first one's memory pool.  Returns (graphs, r)."""
         snap = e.snapshot()
-        keys = ('fresh', 'comm', 'alive', 't_ep', 'h', 'c', 'halted', 'stat_reward', 'stat_comm', 'stat_success',
-                'stat_episodes', 'stat_steps')
-        saved = {k: b[k].clone() for k in keys if k in b}
-        enqueue()
+        saved = [(t, t.clone()) for t in [b[k] for k in SLOT_STATE if k in b] + list(restore)]
+        out = phases[0]()
+        for phase in phases[1:]:
+            if between is not None:
+                between(out)
+            phase(out)
         torch.cuda.synchronize()
-        e.restore(snap)                   # env state, RNG ticks ...
-        for k, v in saved.items():        # ... and the trainer-side episode state, as the boundary left them
-            b[k].copy_(v)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            enqueue()
-        return g
+        e.restore(snap)
+        for t, v in saved:
+            t.copy_(v)
+        self._refresh_weights(b, e, force=True)
+        graphs = [torch.cuda.CUDAGraph()]
+        with torch.cuda.graph(graphs[0]):
+            out = phases[0]()
+            if between is None:
+                for phase in phases[1:]:
+                    phase(out)
+        for phase in phases[1:] if between is not None else ():
+            graphs.append(torch.cuda.CUDAGraph())
+            with torch.cuda.graph(graphs[-1], pool=graphs[0].pool()):
+                phase(out)
+        return graphs, out
 
     def stat_vector(self, b=None, e=None):
         """Device float64 vector [num_episodes, num_steps, success, err flags, reward[N], comm_action[N]] of this
@@ -666,7 +710,7 @@ class Trainer(object):
         ea.env_id0 = int(tr_env.cfg.env_id0) - rank * tr_env.nenvs + world * tr_env.nenvs + rank * ne
         e = data.init(args.env_name, ea).env
         e.cfg.seed = tr_env.cfg.seed
-        self._eval = dict(env=e, buf=self._slot_buffers(ne, 1, e.device), graph=None, key=None)
+        self._eval = dict(env=e, buf=self._slot_buffers(ne, 1, e.device))
         return self._eval
 
     def evaluate_vector(self, episodes=1, greedy=False, epoch=None):
@@ -684,20 +728,11 @@ class Trainer(object):
                 e.set_add_rate(self.env.env)
             else:
                 e.curriculum_until(int(epoch))
-        self._episode_boundary(None, b, e)
-        b['err'].zero_()
         T = episodes * int(self.args.max_steps)
-        if not self.random_policy:
-            self.policy_net.packed()
-            # always rebuilt: a replayed training update re-builds the training env's table only, yet marks every
-            # table current (CommNetMLP.mark_packed_current)
-            self.policy_net.encoder_table(e, force=True)
+        self._begin(T, None, b, e)
         run = lambda: self._enqueue(T, 0, b, e, episodes, greedy)
         if self.use_graph:
-            key = (T, episodes, bool(greedy), int(getattr(e.cfg, 'spawn_thr', 0)), int(e.cfg.seed), int(e.cfg.env_id0))
-            if ev['graph'] is None or ev['key'] != key:
-                ev['graph'], ev['key'] = self._capture(b, e, run), key
-            ev['graph'].replay()
+            self._replay('evaluate', self._graph_key(T, e, episodes, bool(greedy)), b, e, [run])
         else:
             run()
         return self.stat_vector(b, e), e
@@ -1154,55 +1189,7 @@ class Trainer(object):
         b = self._buf
         self.optimizer.step_dev(out, b['opt_err'])
         out[-1:].copy_(b['opt_err'])
-        self.policy_net.packed(force=True)
-        if self._fused_x():
-            self.policy_net.encoder_table(self.env.env, force=True)
-
-    def _update_key(self, T, quota):
-        """Everything a captured update freezes by value that can change between updates: a change re-captures."""
-        e, opt = self.env.env, self.optimizer
-        return (T, int(quota), int(getattr(e.cfg, 'spawn_thr', 0)), int(e.cfg.seed), int(e.cfg.env_id0), e.nenvs,
-                self._record_mode, self._ff_K, opt.lr, opt.alpha, opt.eps)
-
-    def _capture_update(self, T, quota, reduce):
-        """Warm-up pass (lazy library state, allocator, the gradient kernels' workspaces), rewound so that it leaves no
-        trace (env state and RNG ticks, episode state, parameters, gradients, second moments, packed weights), then the
-        capture.  Nothing runs in the capture: the caller replays it."""
-        b, e, opt, net = self._buf, self.env.env, self.optimizer, self.policy_net
-        if self.grad_ff:
-            self._ff_K = self._ff_chunk_steps(T, self._policy_cfg())
-        snap = e.snapshot()
-        keys = ('fresh', 'comm', 'alive', 't_ep', 'h', 'c', 'halted', 'stat_reward', 'stat_comm', 'stat_success',
-                'stat_episodes', 'stat_steps', 'err')
-        saved = {k: b[k].clone() for k in keys if k in b}
-        flat = [opt.flat_params, opt.flat_grads, opt.flat_square_avg]
-        saved_flat = [t.clone() for t in flat]
-        out = self._update_head(T, quota)
-        if reduce is not None:
-            reduce(out)
-        self._update_tail(out)
-        torch.cuda.synchronize()
-        e.restore(snap)
-        for k, v in saved.items():
-            b[k].copy_(v)
-        for t, v in zip(flat, saved_flat):
-            t.copy_(v)
-        net.packed(force=True)                # the weights the warm-up packed were the updated ones
-        if self._fused_x():
-            net.encoder_table(e, force=True)
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            out = self._update_head(T, quota)
-            if reduce is None:
-                self._update_tail(out)
-        graphs = [g]
-        if reduce is not None:
-            g2 = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g2, pool=g.pool()):
-                self._update_tail(out)
-            graphs.append(g2)
-        self._ugraphs, self._uout = graphs, out
-        self.update_captures += 1
+        self._refresh_weights(b, self.env.env, force=True)
 
     def train_batch_graph(self, epoch, reduce=None):
         """train_batch replayed from CUDA graphs (graph_update); one host read per update.  reduce(out), if given, runs
@@ -1210,28 +1197,19 @@ class Trainer(object):
         in place).  Returns the stat dict train_batch returns."""
         if not self.record_for_grad:
             raise RuntimeError("set args.record_for_grad = True before the rollout to use compute_grad")
-        e, net, opt = self.env.env, self.policy_net, self.optimizer
+        net, opt = self.policy_net, self.optimizer
         T, quota = self.batch_plan()
-        if self._buf is None or self._buf['T'] != T:
-            self._alloc(T)
-            self._ff_K = None
-        b = self._buf
+        b, e = self._begin(T, epoch)
         if 'opt_err' not in b:
             b['opt_err'] = torch.zeros(1, dtype=torch.int32, device=e.device)
-        self._episode_boundary(epoch)             # trainer.py:28-32, 45-51 (TJ curriculum: may move spawn_thr)
-        b['err'].zero_()
-        net.packed()                              # no-ops when the last replay left the pack current
-        if self._fused_x():
-            self._encoder_table()
-        if self._ugraphs is None or self._update_key(T, quota) != self._ugraph_key:
-            self._ff_K = None
-            self._capture_update(T, quota, reduce)
-            self._ugraph_key = self._update_key(T, quota)
-        self._ugraphs[0].replay()
-        if reduce is not None:
-            reduce(self._uout)
-            self._ugraphs[1].replay()
-        host = self._uout.cpu().numpy()
+        key = lambda: self._graph_key(T, e, int(quota), self._record_mode, self._ff_K, opt.lr, opt.alpha, opt.eps)
+        if self.grad_ff and self._graphs.get('update', (None,))[0] != key():
+            self._ff_K = self._ff_chunk_steps(T, self._policy_cfg())     # measured anew for each capture
+        # the warm-up before the capture also rewinds the parameters, gradients and second moments
+        out, captured = self._replay('update', key(), b, e, (lambda: self._update_head(T, quota), self._update_tail),
+                                     reduce, (opt.flat_params, opt.flat_grads, opt.flat_square_avg))
+        self.update_captures += captured
+        host = out.cpu().numpy()
         nstat = host.size - 4
         stat = self.stat_from_vector(host[:nstat])    # raises on the rollout's flags; the update then changed nothing
         if int(host[-1]):
@@ -1239,7 +1217,7 @@ class Trainer(object):
                                                                                                 host[1]))
         opt.steps += 1
         opt.mark_params_changed()
-        net.mark_packed_current()
+        net.mark_packed_current([] if 'obs' in b else [e])      # the tables _update_tail re-built (_refresh_weights)
         if self.grad_ff:
             self.ff_chunk_steps = self._ff_K
         merge_stat({k: float(host[nstat + i]) for i, k in enumerate(self.LOSS_KEYS)}, stat)

@@ -319,6 +319,20 @@ def test_evaluation_leaves_training_untouched(case):
     assert torch.equal(plain.env.env.tick, evald.env.env.tick)
 
 
+def test_evaluation_reads_the_weights_of_replayed_updates():
+    """Evaluations between updates, sampled and greedy, eager and replayed (use_graph), of a trainer whose updates are
+    replayed (graph_update) equal those of an eager trainer bit for bit: the evaluation env's encoder table follows the
+    weights every update leaves."""
+    eager, graph = make_trainer(PP, 256, False), make_trainer(PP, 256, True)
+    for ep in range(K + 1):
+        for use_graph, greedy in ((False, False), (True, True), (True, False), (False, True)):
+            eager.use_graph = graph.use_graph = use_graph
+            same_stat(eager.evaluate(1, greedy), graph.evaluate(1, greedy))
+        eager.use_graph = graph.use_graph = False
+        if ep < K:
+            same_stat(eager.train_batch(ep), graph.train_batch(ep))
+
+
 @pytest.mark.parametrize("name", [PP, TJ])
 def test_graph_replay_equals_eager(name):
     eager, graph = make_trainer(name, 512, False), make_trainer(name, 512, False, use_graph=True)
@@ -329,10 +343,10 @@ def test_graph_replay_equals_eager(name):
 def test_traffic_junction_epoch_sets_add_rate_and_recaptures():
     tr = make_trainer(TJ, 256, False, use_graph=True, curr_start=1, curr_end=10, add_rate_min=0.05, add_rate_max=0.2)
     s0 = tr.evaluate(1)
-    k0 = tr._eval["key"]
+    k0 = tr._graphs["evaluate"][0]
     assert s0["add_rate"] == pytest.approx(0.05 * 256)
     s1 = tr.evaluate(1, epoch=20)
-    assert tr._eval["key"] != k0
+    assert tr._graphs["evaluate"][0] != k0
     assert s1["add_rate"] / s1["num_episodes"] == pytest.approx(tr._eval["env"].add_rate)
     assert tr._eval["env"].add_rate == pytest.approx(0.2, abs=0.011)
     assert tr.env.env.add_rate == pytest.approx(0.05)               # the training env keeps its curriculum
