@@ -124,7 +124,7 @@ class MultiGPUTrainer(object):
     # ------------------------------------------------------------------ reductions
     def reduce(self, stat):
         """Sum gradients and additive stats (a HOST dict) over ranks; returns the merged stat.  Generic path
-        (any trainer with ``params`` / ``optimizer``); the device path of train_batch avoids the host dict."""
+        (any trainer with ``params`` / ``optimizer``); Trainer.update avoids the host dict."""
         params = self.trainer.params
         opt = self.trainer.optimizer
         if hasattr(opt, 'flat_grads'):
@@ -171,10 +171,11 @@ class MultiGPUTrainer(object):
         return stat
 
     def _reduce_in_place(self, vec):
-        """graph_update: all-reduce(sum) the flat gradient buffer and the device vector [statistics | loss sums | ...]
-        in place (multi_processing.py:86-94)."""
-        dist.all_reduce(self.trainer.optimizer.flat_grads, op=dist.ReduceOp.SUM)
-        self.collectives += 1
+        """Trainer.update's reduce: all-reduce(sum) the flat gradient buffer (not for models.Random, which has no
+        gradient) and the device vector [statistics | loss sums | ...] in place (multi_processing.py:86-94)."""
+        if not self.trainer.random_policy:
+            dist.all_reduce(self.trainer.optimizer.flat_grads, op=dist.ReduceOp.SUM)
+            self.collectives += 1
         dist.all_reduce(vec, op=dist.ReduceOp.SUM)
 
     def run_batch(self, epoch):
@@ -186,22 +187,10 @@ class MultiGPUTrainer(object):
 
     def train_batch(self, epoch):
         tr = self.trainer
-        if getattr(tr, 'graph_update', False):
-            # the update replayed from CUDA graphs; with several ranks the two all-reduces run eagerly between the head
-            # graph (rollout .. gradients) and the tail graph (optimizer step, weight pack): NCCL calls stay outside
-            # any capture
-            return tr.train_batch_graph(epoch, self._reduce_in_place if _dist_on() else None)
-        if hasattr(tr, 'stat_vector') and hasattr(tr.optimizer, 'flat_grads'):
-            learns = not getattr(tr, 'random_policy', False)     # models.Random: no gradient, no optimizer step
-            T, quota = tr.batch_plan()
-            batch = tr.rollout(T, epoch, quota=quota)            # statistics stay on the device up to reduce_device
-            if learns:
-                tr.optimizer.zero_grad(set_to_none=False)
-            loss_vec = tr.compute_grad_device(batch)
-            stat = self.reduce_device(loss_vec, with_grads=learns)
-            if learns:
-                tr.optimizer.step(grad_div=stat['num_steps'])    # multi_processing.py:95-97 in one kernel
-            return stat
+        if hasattr(tr, 'update'):
+            # the reduce runs between the head (rollout .. gradients) and the tail (optimizer step, weight pack), eagerly
+            # also when graph_update replays both: NCCL calls stay outside any capture
+            return tr.update(epoch, self._reduce_in_place if _dist_on() else None)
         batch, stat = tr.run_batch(epoch)
         tr.optimizer.zero_grad(set_to_none=False)
         s = tr.compute_grad(batch)

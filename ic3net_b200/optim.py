@@ -60,8 +60,8 @@ class FlatRMSprop(object):
             if p.grad is None or p.grad.data_ptr() != g.data_ptr():
                 p.grad = g                                      # someone dropped / replaced .grad: re-attach
 
-    def step(self, grad_div=1.0):
-        """One update with ``grad / grad_div`` (the trainer passes the global number of env steps)."""
+    def _fold_grads(self):
+        """Bring every parameter's gradient into the flat buffer the update kernels read."""
         self._check_attached()
         for p, g in zip(self.params, self._views(self.flat_grads)):
             if p.grad is None:
@@ -69,6 +69,10 @@ class FlatRMSprop(object):
             if p.grad.data_ptr() != g.data_ptr():               # autograd replaced the tensor: fold it back in
                 g.copy_(p.grad)
                 p.grad = g
+
+    def step(self, grad_div=1.0):
+        """One update with ``grad / grad_div`` (the trainer passes the global number of env steps)."""
+        self._fold_grads()
         _lib.check(_lib.load().ic3_rmsprop_step(self.numel, self.lr, self.alpha, self.eps, float(grad_div),
                                                 self.flat_grads.data_ptr(), self.flat_params.data_ptr(),
                                                 self.flat_square_avg.data_ptr(), _lib.stream()))
@@ -80,7 +84,7 @@ class FlatRMSprop(object):
         stat (ic3_rmsprop_step_dev; nothing happens when stat[3] holds error flags, IC3_ERR_GRAD_DIV goes to the int32
         device word err when the count is not positive).  No host read, so a CUDA graph can hold it; the caller advances
         ``steps`` and calls mark_params_changed() once the update has run."""
-        self._check_attached()
+        self._fold_grads()
         _lib.check(_lib.load().ic3_rmsprop_step_dev(self.numel, self.lr, self.alpha, self.eps, stat.data_ptr(),
                                                     self.flat_grads.data_ptr(), self.flat_params.data_ptr(),
                                                     self.flat_square_avg.data_ptr(), err.data_ptr(), _lib.stream()))

@@ -47,6 +47,11 @@ next.  With ``grad_impl = 'kernels_ff'`` their gradient comes from the kernels o
 hidden-state record or checkpoint at all; the backward re-runs the forward from the env-state records over chunks of K
 consecutive lock-steps (K*B env slots at once, K from the memory the device has left, ``FF_CHUNK_STEPS``), with the
 products of the backward on the tensor cores (csrc/ff_grad_tc.cu).
+
+Update (``train_batch`` -> ``update``, trainer.py:245-256): gradient zeroing, rollout, gradient, statistics vector,
+RMSprop with the step count read on the device and the weight re-pack, with one host read at the end, which raises on a
+device error flag of the rollout or the gradient (the step is then skipped).  ``graph_update`` replays the same phases
+from CUDA graphs instead of running them; MultiGPUTrainer runs its all-reduces between them.
 """
 import argparse
 import ctypes as C
@@ -147,13 +152,14 @@ class Trainer(object):
         if self.grad_impl not in ('auto', 'kernels', 'kernels_ff', 'autograd'):
             raise ValueError("grad_impl must be 'auto', 'kernels', 'kernels_ff' or 'autograd', not %r" % (self.grad_impl,))
         self.grad_kernels = False
+        self.grad_ff = False
         self._bptt = None
         self._buf = None
         self._record_mode = None             # 'full' | 'window' per allocation (record_mode)
         self._ff_K = None                    # graph_update: kernels_ff chunk length frozen into the captured update
         self._graphs = {}                    # 'rollout' | 'evaluate' | 'update' -> (key, graphs, result) (_replay)
         self._side = None                    # stream of the dense observation writer (_overlap_obs)
-        # graph_update: train_batch replays the whole update from CUDA graphs (train_batch_graph)
+        # graph_update: train_batch replays the whole update from CUDA graphs (update)
         self.graph_update = bool(getattr(args, 'graph_update', False))
         self.update_captures = 0             # graph_update: how often the update was captured
         if self.random_policy and self.graph_update:
@@ -565,14 +571,18 @@ class Trainer(object):
         """T lock-step iterations from fresh episodes in every slot (``quota``: see _enqueue).  Returns a
         RolloutBatch of stacked [T, B, ...] device tensors (views of the trainer's record buffers)."""
         b, e = self._begin(T, epoch)
+        self._run_rollout(T, quota, b, e)
+        return RolloutBatch(action=b['action'], logp=b['logp'], value=b['value'].view(T, e.nenvs, -1),
+                            reward=b['reward'], episode_mask=b['emask'], episode_mini_mask=b['mini'],
+                            alive_mask=b['ralive'], valid=b['valid'])
+
+    def _run_rollout(self, T, quota, b, e):
+        """Enqueue the training rollout on buffers b and env e, replayed from the 'rollout' CUDA graph with use_graph."""
         run = lambda: self._enqueue(T, quota)
         if self.use_graph:
             self._replay('rollout', self._graph_key(T, e, int(quota)), b, e, [run])
         else:
             run()
-        return RolloutBatch(action=b['action'], logp=b['logp'], value=b['value'].view(T, e.nenvs, -1),
-                            reward=b['reward'], episode_mask=b['emask'], episode_mini_mask=b['mini'],
-                            alive_mask=b['ralive'], valid=b['valid'])
 
     def _graph_key(self, T, e, *extras):
         """Key of a run of T lock-steps on env e captured into CUDA graphs: kernel arguments passed BY VALUE are frozen
@@ -872,10 +882,9 @@ class Trainer(object):
             raise RuntimeError("set args.record_for_grad = True before the rollout to use compute_grad")
         return self._losses_device()
 
-    def _losses_device(self, graph=False):
-        """compute_grad_device after its check.  graph: the form a CUDA graph can hold (graph_update): the BPTT kernels
-        take max |c| from the device (ic3_bptt_begin_dev) and kernels_ff runs with the chunk length frozen at capture
-        (self._ff_K); the gradient is the same bit for bit."""
+    def _losses_device(self, K=None):
+        """compute_grad_device after its check, with no host read, so a CUDA graph can hold it (update).  K: the
+        kernels_ff chunk length (None: _ff_chunk_steps measures it now)."""
         b, args = self._buf, self.args
         e = self.env.env
         T, B, N = b['T'], e.nenvs, args.nagents
@@ -893,9 +902,9 @@ class Trainer(object):
         if self.random_policy:
             return self._random_losses(adv, ret)
         if self.grad_kernels:
-            return self._compute_grad_kernels(adv, ret, dev_cmax=graph)
+            return self._compute_grad_kernels(adv, ret)
         if self.grad_ff:
-            return self._compute_grad_ff(adv, ret, K=self._ff_K if graph else None)
+            return self._compute_grad_ff(adv, ret, K)
         W = self.grad_window
         nw = (T + W - 1) // W
         dh = dc = None
@@ -930,12 +939,12 @@ class Trainer(object):
         ent = -(logp * logp.exp() * b['valid'].double().view(T, B, 1, 1)).sum()      # :213-217, real steps only
         return torch.stack([a_loss, v_loss, ent])
 
-    def _compute_grad_kernels(self, adv, ret, dev_cmax=False):
-        """Hand-written BPTT (csrc/bptt_tc.cu): one ic3_bptt_step per lock-step iteration, last to first (one host read
-        up front: max |c| of the record, the bound behind the operand scale; dev_cmax: none, ic3_bptt_begin_dev reduces
-        it on the device).  In window mode (record_mode) the policy
-        step re-runs each window from its checkpoint just ahead of the backward (_recompute_window); the gradient is
-        bit-identical to full records'.  Returns the device float64 vector of the three loss sums."""
+    def _compute_grad_kernels(self, adv, ret):
+        """Hand-written BPTT (csrc/bptt_tc.cu): one ic3_bptt_step per lock-step iteration, last to first, after
+        ic3_bptt_begin_dev has reduced max |c| of the record, the bound behind the operand scale, on the device.  In
+        window mode (record_mode) the policy step re-runs each window from its checkpoint just ahead of the backward
+        (_recompute_window); the gradient is bit-identical to full records'.  Returns the device float64 vector of the
+        three loss sums."""
         b, net, args, e = self._buf, self.policy_net, self.args, self.env.env
         lib = _lib.load()
         T, B, N, H = b['T'], e.nenvs, args.nagents, args.hid_size
@@ -960,16 +969,9 @@ class Trainer(object):
             cut = (((b['s_tep'] + 1) % args.detach_gap) == 0).to(torch.uint8).contiguous()
         window = self._record_mode == 'window'
         W, nb = self.grad_window, self._window_buffers()
-        if dev_cmax:
-            cmax = None                         # from the device: the same values as below (ic3_bptt_begin_dev)
-            csrc = None if not hc else b['c_abs'] if window else b['rec_c'][1:]
-        elif not hc:
-            cmax = 0.0                          # no cell state: the operand scale bounds |dh| alone
-        elif window:
-            cmax = float(b['c_abs'].max().item())                              # tracked per step by the rollout
-        else:
-            lo, hi = torch.aminmax(b['rec_c'][1:])                              # bound of |c| for the operand scale
-            cmax = max(abs(float(lo.item())), abs(float(hi.item())))
+        # max |c| over every step's c, from the full record or from the per-step maxima the rollout kept in window mode;
+        # the tanh RNN has no cell state, and its operand scale bounds |dh| alone
+        csrc = None if not hc else b['c_abs'] if window else b['rec_c'][1:]
 
         def state(t):                          # (h, c) entering step t and h' leaving it (c: None for the tanh RNN)
             if not window:
@@ -980,7 +982,7 @@ class Trainer(object):
                 return b['ck_h'][k], b['ck_c'][k] if hc else None, wh[0]
             return wh[j - 1], b['win_c'][k % nb][j - 1] if hc else None, wh[j]
         # window mode: window k, steps [t0, t1), is re-run on this stream right before ic3_bptt_step(t1 + 1) is issued
-        # (before ic3_bptt_begin when there is no such step).  The look-ahead ic3_bptt_prepare(t) on the library's side
+        # (before ic3_bptt_begin_dev when there is no such step).  The look-ahead ic3_bptt_prepare(t) on the library's side
         # stream waits for this stream's work up to ic3_bptt_step(t + 2), so it sees every window it reads; and the
         # buffer window k overwrites (that of window k + nb, all of whose steps are >= t1 + 2) has no reader left.
         todo = list(reversed(range((T + W - 1) // W))) if window else []
@@ -993,10 +995,7 @@ class Trainer(object):
         st['dh'].zero_()
         if hc:
             st['dc'].zero_()
-        if dev_cmax:
-            _lib.check(lib.ic3_bptt_begin_dev(C.byref(plan), _lib.ptr(csrc), 0 if csrc is None else csrc.numel(), s))
-        else:
-            _lib.check(lib.ic3_bptt_begin(C.byref(plan), cmax, s))
+        _lib.check(lib.ic3_bptt_begin_dev(C.byref(plan), _lib.ptr(csrc), 0 if csrc is None else csrc.numel(), s))
         value = b['value']
 
         def step_io(t):
@@ -1154,35 +1153,24 @@ class Trainer(object):
 
     # only used when there is a single process (trainer.py:245-256)
     def train_batch(self, epoch):
-        if self.graph_update:
-            return self.train_batch_graph(epoch)
-        batch, stat = self.run_batch(epoch)
-        if self.random_policy:
-            # no gradient: the reference's step skips a parameter whose .grad is None (trainer.py:251-254), so the
-            # parameter and the optimizer state (state == {}) stay as they are
-            merge_stat(self.compute_grad(batch), stat)
-            return stat
-        self.optimizer.zero_grad(set_to_none=False)
-        s = self.compute_grad(batch)
-        merge_stat(s, stat)
-        self.optimizer.step(grad_div=stat['num_steps'])      # grad /= num_steps, then the update (trainer.py:251-254)
-        return stat
+        return self.update(epoch)
 
-    # ------------------------------------------------------------------ graph_update
-    # The update as CUDA graphs: head = gradient zeroing, rollout, ic3_stat_reduce, returns, advantages, gradient kernels
-    # and their finish, all into the float64 vector out = [statistics | loss sums | optimizer flags]; tail = RMSprop with
-    # the divisor read from out (ic3_rmsprop_step_dev), then the weight pack and encoder table of the updated parameters,
-    # which the next update's rollout uses.  One graph holds both; with a reduce between them (MultiGPUTrainer: the
-    # all-reduces of the gradients and of out stay eager) each is a graph of its own.  The episode boundary (env reset,
-    # TJ curriculum) runs eagerly before the replay, and the host reads out once after it.
+    # ------------------------------------------------------------------ the update
+    # head: gradient zeroing, rollout, returns, advantages, gradient kernels and their finish, then ic3_stat_reduce (after
+    # the gradient, so its flag word also holds what the gradient kernels set), into the float64 vector out = [statistics
+    # | loss sums | optimizer flags].  tail: RMSprop with the divisor read from out (ic3_rmsprop_step_dev skips it on
+    # error flags), then the weight pack and encoder table the next rollout reads.  Neither reads back to the host, so
+    # graph_update can replay them: one graph, or one each around a reduce.  models.Random has no gradient to zero and no
+    # tail: its .grad stays None and the optimizer state empty, as the reference's step skips it (trainer.py:251-254).
 
-    def _update_head(self, T, quota):
-        b, opt = self._buf, self.optimizer
-        opt.flat_grads.zero_()
-        self._enqueue(T, quota)
+    def _update_head(self, rollout, K):
+        b = self._buf
+        if not self.random_policy:
+            self.optimizer.zero_grad(set_to_none=False)
+            b['opt_err'].zero_()
+        rollout()
+        losses = self._losses_device(K)
         vec = self.stat_vector()
-        losses = self._losses_device(graph=True)
-        b['opt_err'].zero_()
         return torch.cat([vec, losses.to(vec.dtype), torch.zeros(1, dtype=vec.dtype, device=vec.device)])
 
     def _update_tail(self, out):
@@ -1191,35 +1179,51 @@ class Trainer(object):
         out[-1:].copy_(b['opt_err'])
         self._refresh_weights(b, self.env.env, force=True)
 
-    def train_batch_graph(self, epoch, reduce=None):
-        """train_batch replayed from CUDA graphs (graph_update); one host read per update.  reduce(out), if given, runs
-        eagerly between the head and the tail graph (the data-parallel all-reduces of the flat gradients and of out,
-        in place).  Returns the stat dict train_batch returns."""
-        if not self.record_for_grad:
+    def update(self, epoch, reduce=None):
+        """One training update (trainer.py:245-256): rollout, gradient and RMSprop step, with one host read.  reduce(out),
+        if given, runs eagerly between the head and the tail (the data-parallel all-reduces of the flat gradients and of
+        out, in place).  graph_update: head and tail are replayed from CUDA graphs; otherwise they run eagerly, the
+        rollout replayed from its own graph with use_graph (as run_batch does).  Raises on a device error flag of the
+        rollout or the gradient, in which case the parameters and the optimizer state are as they were.  Returns the
+        stat dict."""
+        if not self.record_for_grad and not self.random_policy:
             raise RuntimeError("set args.record_for_grad = True before the rollout to use compute_grad")
         net, opt = self.policy_net, self.optimizer
+        learns = not self.random_policy
         T, quota = self.batch_plan()
         b, e = self._begin(T, epoch)
-        if 'opt_err' not in b:
+        if learns and 'opt_err' not in b:
             b['opt_err'] = torch.zeros(1, dtype=torch.int32, device=e.device)
         key = lambda: self._graph_key(T, e, int(quota), self._record_mode, self._ff_K, opt.lr, opt.alpha, opt.eps)
-        if self.grad_ff and self._graphs.get('update', (None,))[0] != key():
-            self._ff_K = self._ff_chunk_steps(T, self._policy_cfg())     # measured anew for each capture
-        # the warm-up before the capture also rewinds the parameters, gradients and second moments
-        out, captured = self._replay('update', key(), b, e, (lambda: self._update_head(T, quota), self._update_tail),
-                                     reduce, (opt.flat_params, opt.flat_grads, opt.flat_square_avg))
-        self.update_captures += captured
+        K = None                             # kernels_ff chunk length: measured for each update and each capture
+        if self.grad_ff:
+            held = self.graph_update and self._graphs.get('update', (None,))[0] == key()
+            K = self._ff_K if held else self._ff_chunk_steps(T, self._policy_cfg())
+        if self.graph_update:
+            self._ff_K = K                   # part of the key: a captured update keeps the K it holds
+            # the warm-up before the capture also rewinds the parameters, gradients and second moments
+            head = lambda: self._update_head(lambda: self._enqueue(T, quota), K)
+            out, captured = self._replay('update', key(), b, e, (head, self._update_tail), reduce,
+                                         (opt.flat_params, opt.flat_grads, opt.flat_square_avg))
+            self.update_captures += captured
+        else:
+            out = self._update_head(lambda: self._run_rollout(T, quota, b, e), K)
+            if reduce is not None:
+                reduce(out)
+            if learns:
+                self._update_tail(out)
         host = out.cpu().numpy()
         nstat = host.size - 4
-        stat = self.stat_from_vector(host[:nstat])    # raises on the rollout's flags; the update then changed nothing
+        stat = self.stat_from_vector(host[:nstat])    # raises on the flags; the tail then changed nothing
         if int(host[-1]):
             raise RuntimeError("device-side error flag %#x in the optimizer step (step count %r)" % (int(host[-1]),
                                                                                                 host[1]))
-        opt.steps += 1
-        opt.mark_params_changed()
-        net.mark_packed_current([] if 'obs' in b else [e])      # the tables _update_tail re-built (_refresh_weights)
+        if learns:
+            opt.steps += 1
+            opt.mark_params_changed()
+            net.mark_packed_current([] if 'obs' in b else [e])      # the tables _update_tail re-built (_refresh_weights)
         if self.grad_ff:
-            self.ff_chunk_steps = self._ff_K
+            self.ff_chunk_steps = K
         merge_stat({k: float(host[nstat + i]) for i, k in enumerate(self.LOSS_KEYS)}, stat)
         self.stats = stat
         return stat

@@ -464,7 +464,8 @@ int ic3_stat_reduce(int32_t B, int32_t N, const int32_t* stat_episodes, const in
  * (cfg->obs_vocab > 0), a window of at most 5 x 5 cells and an observation pattern of at most 512 columns.  Every other
  * configuration gets a workspace of 0 bytes.
  * The host walks the lock-step iterations t = T-1 .. 0:
- *     ic3_bptt_begin(plan, max |c| of the record, stream)
+ *     ic3_bptt_begin(plan, max |c| of the record, stream), or ic3_bptt_begin_dev(plan, record, n, stream), which
+ *     reduces that maximum on the device (no host read; the form the Trainer uses)
  *     for t in reversed(range(T)): ic3_bptt_step(plan, &io_t, stream)
  *     ic3_bptt_finish(plan, params, grads, losses, stream)
  * The backward unit is one (step t, comm pass p); ic3_bptt_step runs the units (t, P-1) .. (t, 0), after re-running

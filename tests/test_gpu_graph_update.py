@@ -1,8 +1,11 @@
-"""graph_update: the whole training update (rollout, statistics, returns, advantages, gradient kernels, RMSprop, weight
-pack) replayed from CUDA graphs (Trainer.train_batch_graph).  Each case trains the same seed and initial weights for K
+"""Trainer.update, the training update (rollout, returns, advantages, gradient kernels, statistics, RMSprop, weight pack),
+run eagerly or, with graph_update, replayed from CUDA graphs.  Each case trains the same seed and initial weights for K
 updates eagerly and with graph_update and asserts bit-identical flat parameters, second moments, the last update's
-gradients and the stat dicts; plus the fp16-range flag after a replay, the refusals, the CLI with --save / --load, and
-the re-capture rule of the traffic-junction curriculum."""
+gradients and the stat dicts, and both equal the reference's call sequence (run_batch, zero_grad, compute_grad,
+step(grad_div)); plus the device max |c| of ic3_bptt_begin_dev against ic3_bptt_begin, error flags of the rollout and
+of the gradient, the refusals, the CLI with --save / --load, and the re-capture rule of the traffic-junction
+curriculum."""
+import ctypes as C
 import os
 import subprocess
 import sys
@@ -63,6 +66,19 @@ def assert_same_state(eager, graph):
     assert oe.steps == og.steps == K
 
 
+def reference_update(tr, epoch):
+    """The reference's Trainer.train_batch (trainer.py:245-256) spelled out on the Trainer's public calls, the divisor
+    taken on the host.  models.Random has no gradient: no zero_grad and no step (its parameter keeps .grad None)."""
+    from ic3net_b200.utils import merge_stat
+    batch, stat = tr.run_batch(epoch)
+    if not tr.random_policy:
+        tr.optimizer.zero_grad()
+    merge_stat(tr.compute_grad(batch), stat)
+    if not tr.random_policy:
+        tr.optimizer.step(grad_div=stat["num_steps"])
+    return stat
+
+
 IC = dict(model="rnn", commnet=False, hard_attn=False, recurrent=True, rnn_type="MLP", policy_impl="tc_tanh",
           comm_passes=1, share_weights=False)
 FF = dict(grad_impl="kernels_ff", ic3net=False, recurrent=False, rnn_type="MLP", policy_impl="tc_ff", ff_chunk=7,
@@ -87,6 +103,88 @@ def test_graph_update_is_bit_identical(case):
     assert graph.update_captures == 1
     if eager.grad_kernels:
         assert eager.record_mode == graph.record_mode == ("window" if over.get("windows") else "full")
+
+
+@pytest.mark.parametrize("case", sorted(CASES) + ["autograd"])
+def test_update_equals_the_reference_sequence(case):
+    """K updates of train_batch, eager and (where it is allowed) with graph_update, equal K updates of the reference's
+    call sequence bit for bit: parameters, second moments, gradients and stat dicts."""
+    over = dict(CASES.get(case, dict(grad_impl="autograd")))
+    ref = make_trainer(PP, 37, False, **over)
+    want = [reference_update(ref, ep) for ep in range(K)]
+    for graph in (False, True) if case in CASES else (False,):
+        tr = make_trainer(PP, 37, graph, **over)
+        for ep in range(K):
+            same_stat(want[ep], tr.train_batch(ep))
+        assert_same_state(ref, tr)
+
+
+def test_random_update_equals_the_reference_sequence():
+    from test_gpu_random import make_trainer as make_random, random_args
+    ref, tr = (make_random(random_args("c2", nenvs=64, batch_size=100))[1] for _ in range(2))
+    p0 = tr.optimizer.flat_params.clone()
+    for ep in range(K):
+        same_stat(reference_update(ref, ep), tr.train_batch(ep))
+    for t in (ref, tr):
+        assert torch.equal(t.optimizer.flat_params, p0)
+        assert t.policy_net.parameter.grad is None
+        assert t.state_dict()["state"] == {}
+
+
+def test_use_graph_update_replays_the_rollout_graph():
+    """use_graph without graph_update: the update's rollout is replayed from the 'rollout' CUDA graph -- its kernels are
+    enqueued only by the warm-up and the capture of the first update -- and every update equals that of a trainer
+    without use_graph bit for bit; BPTT kernels and models.Random."""
+    from test_gpu_random import make_trainer as make_random, random_args
+    pairs = [(make_trainer(PP, 37, False), make_trainer(PP, 37, False, use_graph=True)),
+             tuple(make_random(random_args("c2", nenvs=64, batch_size=100, use_graph=g))[1] for g in (False, True))]
+    for plain, replayed in pairs:
+        enqueue, calls = replayed._enqueue, []
+
+        def counted(*args, enqueue=enqueue, calls=calls):
+            calls.append(args)
+            return enqueue(*args)
+
+        replayed._enqueue = counted
+        for ep in range(K):
+            same_stat(plain.train_batch(ep), replayed.train_batch(ep))
+        assert len(calls) == 2 and "rollout" in replayed._graphs
+        for key in ("action", "logp", "value", "reward"):
+            assert torch.equal(plain._buf[key], replayed._buf[key]), key
+        for a, b in ((plain.optimizer.flat_params, replayed.optimizer.flat_params),
+                     (plain.optimizer.flat_square_avg, replayed.optimizer.flat_square_avg),
+                     (plain.optimizer.flat_grads, replayed.optimizer.flat_grads)):
+            assert torch.equal(a, b)
+
+
+BEGIN_CASES = {"full": dict(), "windows": dict(windows=True), "passes3": dict(comm_passes=3), "tanh": dict(IC)}
+
+
+@pytest.mark.parametrize("case", sorted(BEGIN_CASES))
+def test_device_begin_leaves_the_workspace_of_the_host_begin(case):
+    """ic3_bptt_begin_dev reduces max |c| on the device; ic3_bptt_begin, which takes it from the host, is its reference
+    form.  On one plan, from a zeroed workspace each, the two leave the same bytes: full records (rec_c[1:]), window
+    records (the rollout's per-step maxima), three comm passes (the bound grows by P - 1) and the tanh RNN (no c)."""
+    from ic3net_b200 import _lib
+    tr = make_trainer(PP, 37, False, **BEGIN_CASES[case])
+    tr.run_batch(0)
+    b, lib, s = tr._buf, _lib.load(), _lib.stream()
+    hc = not tr._h_only_records()
+    plan = tr._bptt_plan(tr._policy_cfg(), tr.policy_net.packed(), _lib.ptr(tr._encoder_table()) if hc else None)
+    ws = torch.zeros(int(lib.ic3_bptt_workspace_bytes(C.byref(plan))), dtype=torch.uint8, device=b["h"].device)
+    plan.workspace = ws.data_ptr()
+    c = None
+    if hc:
+        c = b["c_abs"] if tr.record_mode == "window" else b["rec_c"][1:]
+    assert tr.record_mode == ("window" if case == "windows" else "full")
+    cmax = 0.0 if c is None else float(c.abs().max())
+    _lib.check(lib.ic3_bptt_begin(C.byref(plan), cmax, s))
+    torch.cuda.synchronize()
+    host = ws.clone()
+    ws.zero_()
+    _lib.check(lib.ic3_bptt_begin_dev(C.byref(plan), _lib.ptr(c), 0 if c is None else c.numel(), s))
+    torch.cuda.synchronize()
+    assert torch.equal(host, ws)
 
 
 def test_traffic_junction_curriculum_recaptures_exactly_on_a_step():
@@ -133,6 +231,28 @@ def test_fp16_range_flag_raises_after_the_replay():
         with pytest.raises(RuntimeError, match="0x200"):
             tr.train_batch(0)
         assert torch.equal(before, tr.optimizer.flat_params)
+
+
+def test_flag_set_during_the_gradient_raises():
+    """A flag the gradient kernels set (here: ERR_FP16_RANGE or-ed into the error word right after them, a plain torch
+    op the capture holds) stops the step and raises, eager and replayed; the parameters and second moments stay."""
+    from ic3net_b200 import _lib
+    for graph in (False, True):
+        tr = make_trainer(PP, 4, graph)
+        losses = tr._losses_device
+
+        def flagged(*args, tr=tr, losses=losses):
+            out = losses(*args)
+            tr._buf["err"].bitwise_or_(_lib.ERR_FP16_RANGE)
+            return out
+
+        tr._losses_device = flagged
+        before = (tr.optimizer.flat_params.clone(), tr.optimizer.flat_square_avg.clone())
+        with pytest.raises(RuntimeError, match="0x200"):
+            tr.train_batch(0)
+        assert torch.equal(before[0], tr.optimizer.flat_params)
+        assert torch.equal(before[1], tr.optimizer.flat_square_avg)
+        assert tr.optimizer.steps == 0
 
 
 def test_refusals():
