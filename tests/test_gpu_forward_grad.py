@@ -92,9 +92,11 @@ def encode64(tr, roles, w):
     return (w["enc_w"].t()[idx] * val.double().unsqueeze(-1)).sum(1) + w["enc_b"]
 
 
-def one_step(tr, t, seed=0):
-    """forward + backward of step t of the trainer's records (env state, (h, c), masks) under random upstream gradients;
-    returns (kernel gradients by name + 'h' / 'c', float64 gradients, |terms| sums of the action heads)."""
+def one_step(tr, t, seed=0, scale=1.0, spike=None):
+    """forward + backward of step t of the trainer's records (env state, (h, c), masks) under random upstream gradients
+    times ``scale``; ``spike = (key, v)`` sets the last entry (last row, last column) of upstream gradient ``key``
+    ('dh', 'dc', 'dvalue' or 'dlogp') to v.  Returns (kernel gradients by name + 'h' / 'c', float64 gradients, |terms|
+    sums of the action heads)."""
     from ic3net_b200.trainer import policy_forward_torch
     net, args, e, b = tr.policy_net, tr.args, tr.env.env, tr._buf
     B, N, H = e.nenvs, args.nagents, args.hid_size
@@ -115,7 +117,10 @@ def one_step(tr, t, seed=0):
     h2, c2 = hid if lstm else (hid, None)
     assert value.grad_fn is not None and h2.grad_fn is not None and all(a.grad_fn is not None for a in action)
     logp = torch.cat(action, -1).reshape(R, -1)
-    up = dict(dlogp=rnd(R, logp.shape[1]), dvalue=rnd(R), dh=rnd(R, H) * 0.1, dc=rnd(R, H) * 0.1)
+    up = dict(dlogp=rnd(R, logp.shape[1]) * scale, dvalue=rnd(R) * scale, dh=rnd(R, H) * (0.1 * scale),
+              dc=rnd(R, H) * (0.1 * scale))
+    if spike is not None:
+        up[spike[0]].view(-1)[-1] = spike[1]
     loss = (logp * up["dlogp"]).sum() + (value.reshape(R) * up["dvalue"]).sum() + (h2 * up["dh"]).sum()
     if lstm:
         loss = loss + (c2 * up["dc"]).sum()
