@@ -13,7 +13,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def build(B, env_id0):
-    from test_gpu_random import make_trainer, random_args
+    from gpu_harness import random_args, random_trainer as make_trainer
     args = random_args("c5", nenvs=B, eval_nenvs=B, env_id0=env_id0, max_steps=30)
     return args, make_trainer(args)[1]
 

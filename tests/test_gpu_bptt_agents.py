@@ -10,7 +10,7 @@ below reach N = 1, a full warp of 32 agents (traffic junction with 32 cars; pred
 communicating prey), and N that straddle both row blocks; each asserts the geometry and the record events it is there
 for, so a later change of B or of the episode lengths cannot silently lose an edge.
 
-Bars: the BPTT bar (test_gpu_bptt_kernels.assert_within_bar and its tanh-RNN and forward_grad twins): per tensor 1e-4 of
+Bars: the gradient bar of tests/gpu_harness.py: per tensor 1e-4 of
 its largest entry, the encoder weight also per column, the action heads also 2^-20 of their sum of |terms|.  Returns:
 2.5e-7 max(1, |ref|), two float32 ulps (the kernel sums in float64 and rounds once; the order of its sum over agents can
 move that rounding by one ulp).  Statistics: counts and the err word exact, sums within 1e-12 of their sum of |terms|."""
@@ -18,15 +18,12 @@ import numpy as np
 import pytest
 import torch
 
-import test_gpu_bptt_passes as passes
-import test_gpu_bptt_rnn as rnn
 from bptt_ref import heads_abs_sums, trainer_reference
+from gpu_harness import (OPT_IN, TOL, assert_within_bar as within_bar, bar_errors, events, grads_of,
+                         lstm_trainer as make_trainer, one_step, passes_trainer, pattern_columns,
+                         rnn_records_reference, rnn_trainer, sweep_batch, trainer_within_bar, window_vs_full)
 from helpers import load_golden
 from passes_oracle import records_reference
-from test_gpu_bptt_kernels import (TOL, _sweep_batch, assert_within_bar, compare, events, kernel_grad, make_trainer,
-                                   pattern_columns)
-from test_gpu_bptt_windows import window_vs_full
-from test_gpu_forward_grad import OPT_IN, one_step, within_bar
 
 pytestmark = pytest.mark.gpu
 
@@ -90,7 +87,8 @@ def assert_drop_last_fails(tr, got, gloss, ref, rloss, label):
     Bn = tr.env.env.nenvs
     last, _ = trainer_reference(tr, slots=(Bn - 1, Bn))
     dropped = {k: ref[k] - last[k] for k in ref}
-    derrs = compare(got, gloss, dropped, rloss, label + " without the last slot", heads_abs_sums(tr))
+    derrs = bar_errors(got, dropped, heads_abs_sums(tr))
+    print("%s without the last slot: %s" % (label, " ".join("%s %.1e" % kv for kv in derrs.items())))
     assert any(v > TOL for v in derrs.values()), derrs
 
 
@@ -116,15 +114,15 @@ SENSITIVE = ("pp-1", "tj-32")
 @pytest.mark.parametrize("case", list(ONE_PASS))
 def test_one_pass(case):
     name, N, split, over = ONE_PASS[case]
-    tr, _, _ = make_trainer(name, B, seed=77, id0=3, **dict(agents(name, N), **SHORT, **over))
+    tr = make_trainer(name, B, seed=77, id0=3, **dict(agents(name, N), **SHORT, **over))
     assert tr.grad_kernels
     g = assert_geometry(tr, N, split)
     tr.run_batch(0)
     ev = assert_events(tr)
-    got, gloss = kernel_grad(tr)
+    got, gloss = grads_of(tr)
     ref, rloss = trainer_reference(tr)
     label = "%s %s %s" % (case, g, ev)
-    assert_within_bar(tr, got, gloss, ref, rloss, label)
+    trainer_within_bar(tr, got, gloss, ref, rloss, label)
     if case in SENSITIVE:
         assert_drop_last_fails(tr, got, gloss, ref, rloss, label)
 
@@ -134,16 +132,16 @@ def test_one_agent_row_thresholds(case):
     """N = 1: the most tiles and prep CTAs per env of any geometry.  Fewer rows than one prep CTA, and more tiles than
     SMs (dgrad CTAs with two tiles: about 128 SMs + 1 one-agent envs)."""
     sms = torch.cuda.get_device_properties(0).multi_processor_count
-    probe, _, _ = make_trainer(PP, 1, **agents(PP, 1))
-    Bn = _sweep_batch(case, sms, 1, pattern_columns(probe))
-    tr, _, _ = make_trainer(PP, Bn, seed=77, id0=3, **dict(agents(PP, 1), **SHORT))
+    probe = make_trainer(PP, 1, **agents(PP, 1))
+    Bn = sweep_batch(case, sms, 1, pattern_columns(probe))
+    tr = make_trainer(PP, Bn, seed=77, id0=3, **dict(agents(PP, 1), **SHORT))
     g = assert_geometry(tr, 1, False)
     assert (g["R"] < 64) if case == "R<64" else (g["tiles"] > sms and g["R"] == 128 * sms + 1), (g, sms)
     tr.run_batch(0)
     ev = assert_events(tr)
-    got, gloss = kernel_grad(tr)
+    got, gloss = grads_of(tr)
     ref, rloss = trainer_reference(tr)
-    assert_within_bar(tr, got, gloss, ref, rloss, "%s B=%d SMs=%d %s %s" % (case, Bn, sms, g, ev))
+    trainer_within_bar(tr, got, gloss, ref, rloss, "%s B=%d SMs=%d %s %s" % (case, Bn, sms, g, ev))
 
 
 # ---------------------------------------------------------------------------------------------------- comm passes
@@ -162,14 +160,15 @@ MULTI_PASS = {
 def test_comm_passes(case):
     """IC3Net with 2 passes, and CommNet with 3 passes of one shared C module summing the messages (comm_mode sum)."""
     name, N, split, P, share, over = MULTI_PASS[case]
-    tr = passes.make_trainer(name, B, P, share, seed=77, id0=3, **dict(agents(name, N), **SHORT, **over))
+    tr = passes_trainer(name, B, seed=77, id0=3, comm_passes=P, share_weights=share,
+                        **dict(agents(name, N), **SHORT, **over))
     assert tr.grad_kernels
     g = assert_geometry(tr, N, split)
     tr.run_batch(0)
     ev = assert_events(tr)
-    got, gloss = passes.grads_of(tr)
+    got, gloss = grads_of(tr)
     ref, rloss = records_reference(tr)
-    assert_within_bar(tr, got, gloss, ref, rloss, "%s %s %s" % (case, g, ev))
+    trainer_within_bar(tr, got, gloss, ref, rloss, "%s %s %s" % (case, g, ev))
 
 
 # ---------------------------------------------------------------------------------------------------- IC / IRIC
@@ -184,14 +183,14 @@ RNN_CASES = {
 @pytest.mark.parametrize("case", list(RNN_CASES))
 def test_tanh_rnn(case):
     name, N, split = RNN_CASES[case]
-    tr = rnn.make_trainer(name, B, seed=77, id0=3, **dict(agents(name, N), **SHORT))
+    tr = rnn_trainer(name, B, seed=77, id0=3, **dict(agents(name, N), **SHORT))
     assert tr.grad_kernels and tr.grad_impl == "kernels"
     g = assert_geometry(tr, N, split)
     tr.run_batch(0)
     ev = assert_events(tr)
-    got, gloss = rnn.grads_of(tr)
-    ref, rloss = rnn.records_reference(tr)
-    rnn.assert_within_bar(tr, got, gloss, ref, rloss, "%s %s %s" % (case, g, ev))
+    got, gloss = grads_of(tr)
+    ref, rloss = rnn_records_reference(tr)
+    trainer_within_bar(tr, got, gloss, ref, rloss, "%s %s %s" % (case, g, ev))
 
 
 # ---------------------------------------------------------------------------------------------------- forward_grad
@@ -209,7 +208,7 @@ def test_forward_grad_one_step(case):
     """ic3_policy_step_backward (CommNetMLP.forward with forward_grad='kernels'): the gradients of the weights and of
     (h, c) under random upstream gradients against float64 autograd of the step."""
     name, N, P, over = FORWARD_GRAD[case]
-    tr = passes.make_trainer(name, B, P, False, seed=5, id0=0, **dict(OPT_IN, **agents(name, N), **SHORT, **over))
+    tr = passes_trainer(name, B, seed=5, id0=0, comm_passes=P, **dict(OPT_IN, **agents(name, N), **SHORT, **over))
     assert tr.args.nagents == N
     tr.rollout(tr.args.max_steps + 4, 0)
     b = tr._buf

@@ -11,7 +11,7 @@ with the rollout's own kernels (ic3_policy_pass_states).  Covered:
   - bit-identical gradients run to run, between the two-stream and the one-stream schedule, between full and
     windowed records; the refusal of the tanh-cell families.
 
-Bar against the float64 yardsticks: that of tests/test_gpu_bptt_kernels.py (assert_within_bar).  Against autograd: per
+Bar against the float64 yardsticks: the gradient bar of tests/gpu_harness.py (trainer_within_bar).  Against autograd: per
 tensor, max |kernels - autograd| <= 1e-4 of the autograd tensor's largest entry, the action heads' entries also 2^-20
 of their sum of |terms| (the heads' gradient reads the recorded log-probs, autograd re-evaluates them in fp32); loss
 sums rtol 2e-4.  comm_mode 'sum' is cross-checked against autograd on short episodes only: summed messages over
@@ -19,86 +19,21 @@ several passes make the recurrence ill-conditioned enough that the two fp32 forw
 (the heads' gradients, which do not depend on the backward recursion at all, then differ too); the float64 anchors
 are not affected, since they read the same records as the kernels."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-from bptt_ref import heads_abs_sums, max_rel_err, oracle_grad_sum
-from helpers import finish_args, golden_names, load_golden, ns
+from bptt_ref import max_rel_err, oracle_grad_sum
+from gpu_harness import (assert_same_grads, grads_of, kernels_vs_autograd, one_stream_schedule, passes_trainer,
+                         trainer_within_bar)
+from helpers import golden_names, load_golden
 from passes_oracle import make_weights, passes_oracle, records_reference
 from policy_ref import params_f64, step_f64
-from test_gpu_bptt_kernels import assert_within_bar
-
-TOL = 1e-4
-LOSS_KEYS = ("action_loss", "value_loss", "entropy")
-TESTS = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(TESTS)
 
 
-def make_trainer(name, B, passes, share=False, seed=808, id0=30, grad_impl="kernels", windows=False, **over):
-    """Trainer on the arguments of fixture ``name`` with ``passes`` comm passes (overridden by ``over``); the module's
-    own initialisation under the fixture's weight seed, so two trainers of the same arguments hold the same weights."""
-    from ic3net_b200 import data
-    from ic3net_b200.comm import CommNetMLP
-    from ic3net_b200.trainer import Trainer
-    meta, _ = load_golden(name)
-    kw = dict(nenvs=B, seed=seed, env_id0=id0, obs_mode="index", use_graph=False, policy_impl="tc", record_for_grad=True,
-              grad_impl=grad_impl, comm_passes=passes, share_weights=share)
-    kw.update(over)
-    args = ns(meta["args"], **kw)
-    env = data.init(args.env_name, args)
-    finish_args(args, env)
-    torch.manual_seed(meta["weights_seed"])
-    net = CommNetMLP(args, args.num_inputs)
-    tr = Trainer(args, net, env)
-    if windows:
-        tr.RECORD_BYTES_LIMIT = 0
-    return tr
-
-
-def grads_of(tr):
-    """compute_grad of the recorded batch from zeroed gradients: ({name: float64 grad}, loss dict)."""
-    tr.optimizer.zero_grad(set_to_none=False)
-    s = tr.compute_grad(None)
-    return {k: p.grad.detach().to(torch.float64).clone() for k, p in tr.policy_net.named_parameters()}, s
-
-
-def kernels_vs_autograd(name, B, passes, share=False, **over):
-    """The same seeded batch differentiated by the kernels and by autograd: {tensor: error / max |autograd|}."""
-    tk = make_trainer(name, B, passes, share, **over)
-    ta = make_trainer(name, B, passes, share, grad_impl="autograd", **over)
-    assert tk.grad_kernels and not ta.grad_kernels
-    tk.run_batch(0)
-    ta.run_batch(0)
-    assert torch.equal(tk._buf["action"], ta._buf["action"])          # one rollout, two backward passes
-    gk, sk = grads_of(tk)
-    ga, sa = grads_of(ta)
-    sums = heads_abs_sums(tk)
-    errs = {}
-    for k, a in ga.items():
-        m = float(a.abs().max())
-        if m == 0.0:                                   # hidd_encoder: not part of the forward
-            assert float(gk[k].abs().max()) == 0.0, k
-            continue
-        if k in sums:
-            errs[k] = float(((gk[k] - a).abs() / (TOL * m + 2.0 ** -20 * sums[k])).max()) * TOL
-        else:
-            errs[k] = float((gk[k] - a).abs().max()) / m
-    label = "%s B=%d passes=%d share=%s %s" % (name, B, passes, share, over)
-    print("%s: %s | losses %s" % (label, " ".join("%s %.1e" % kv for kv in errs.items()),
-                                  " ".join("%s %.6g/%.6g" % (q, sk[q], sa[q]) for q in LOSS_KEYS)))
-    bad = {k: v for k, v in errs.items() if not v <= TOL}
-    assert not bad, (label, bad)
-    for q in LOSS_KEYS:
-        assert np.isclose(sk[q], sa[q], rtol=2e-4, atol=1e-3), (label, q, sk[q], sa[q])
-    if share:                                          # one C module: one gradient, added by every pass
-        names = [n for n, _ in tk.policy_net.named_parameters()]
-        assert not any(n.startswith("C_modules.1") for n in names), names
-    return tk
+def make_trainer(name, B, passes, share=False, **over):
+    return passes_trainer(name, B, comm_passes=passes, share_weights=share, **over)
 
 
 # ---------------------------------------------------------------------------------------------------- the re-run
@@ -168,7 +103,12 @@ def test_pass_states_rerun(name, passes, share):
     ("grad_pp_hard_ic3net_h128", 3, True, dict(max_steps=6)),
 ])
 def test_gradient_matches_autograd(name, passes, share, over):
-    tk = kernels_vs_autograd(name, 64, passes, share, **over)
+    tk = make_trainer(name, 64, passes, share, **over)
+    ta = make_trainer(name, 64, passes, share, grad_impl="autograd", **over)
+    kernels_vs_autograd(tk, ta, "%s B=64 passes=%d share=%s %s" % (name, passes, share, over))
+    if share:                                          # one C module: one gradient, added by every pass
+        names = [n for n, _ in tk.policy_net.named_parameters()]
+        assert not any(n.startswith("C_modules.1") for n in names), names
     b, args = tk._buf, tk.args
     assert int(b["s_fresh"][1:].sum()) > 0
     if args.detach_gap <= args.max_steps:
@@ -186,23 +126,15 @@ def test_kernels_match_reference_pinned_oracle(name, B):
     the float64 oracle replaying every slot teacher-forced (tests/passes_oracle.py; pinned to the unmodified reference
     by tests/test_oracle_passes.py), and against the float64 backward over the kernel trainer's own records.  B * N is
     never a multiple of 128: a ragged last tile (13 slots of 10 agents: 130 rows, two rows in the second tile)."""
-    from ic3net_b200 import data
-    from ic3net_b200.comm import CommNetMLP
-    from ic3net_b200.trainer import Trainer
     from oracle import policy as opolicy
     meta, z = load_golden(name)
     seed, id0 = 808, 30
-    args = ns(meta["args"], nenvs=B, seed=seed, env_id0=id0, obs_mode="index", use_graph=False, policy_impl="tc",
-              record_for_grad=True, grad_impl="kernels")
-    passes, share = int(args.comm_passes), bool(args.share_weights)
-    assert (B * args.nagents) % 128 != 0
-    env = data.init(args.env_name, args)
-    finish_args(args, env)
-    net = CommNetMLP(args, args.num_inputs)
-    sd = make_weights(meta["weights_seed"], args.num_inputs, args.hid_size, args.naction_heads, args.comm_init, passes,
-                      share)
-    net.load_state_dict({k: torch.from_numpy(v).float() for k, v in sd.items()})
-    tr = Trainer(args, net, env)
+    a = meta["args"]
+    passes, share = int(a["comm_passes"]), bool(a["share_weights"])
+    assert (B * a["nagents"]) % 128 != 0
+    sd = make_weights(meta["weights_seed"], meta["obs_dim"], a["hid_size"], meta["heads"], a["comm_init"], passes, share)
+    tr = passes_trainer(name, B, seed, id0, init_seed=None, weights=sd, comm_passes=passes, share_weights=share)
+    args = tr.args
     assert tr.grad_kernels
     batch, stat = tr.run_batch(0)
     T, quota = tr.batch_plan()
@@ -216,8 +148,8 @@ def test_kernels_match_reference_pinned_oracle(name, B):
     for k, r in ref.items():                   # the two float64 yardsticks agree (fp32 records vs float64 rollout)
         assert max_rel_err(r.cpu().numpy(), want[k]) < 1e-5, (name, k)
     label = "%s B=%d" % (name, B)
-    assert_within_bar(tr, got, gloss, oracle, wstat, label + " vs oracle")
-    assert_within_bar(tr, got, gloss, ref, rloss, label + " vs float64 records")
+    trainer_within_bar(tr, got, gloss, oracle, wstat, label + " vs oracle")
+    trainer_within_bar(tr, got, gloss, ref, rloss, label + " vs float64 records")
 
 
 @pytest.mark.gpu
@@ -230,52 +162,22 @@ def test_full_size_gradient_matches_float64(name, B, passes, share):
     tr.run_batch(0)
     got, gloss = grads_of(tr)
     ref, rloss = records_reference(tr)
-    assert_within_bar(tr, got, gloss, ref, rloss, "%s B=%d passes=%d share=%s" % (name, B, passes, share))
+    trainer_within_bar(tr, got, gloss, ref, rloss, "%s B=%d passes=%d share=%s" % (name, B, passes, share))
 
 
 # ---------------------------------------------------------------------------------------------------- determinism
-
-SCHEDULE_T = (1, 2, 5)
-
-
-def schedule_grads(out_dir):
-    """Gradients and losses after cut rollouts of T = 1, 2, 5 steps with 3 comm passes (odd unit counts), as .npy files
-    under out_dir.  Run in this process and in a child with IC3_BPTT_OVERLAP=0."""
-    tr = make_trainer("grad_pp_hard_ic3net_h128", 400, 3, seed=13, id0=2)
-    for T in SCHEDULE_T:
-        tr.rollout(T, 0, quota=0)
-        got, s = grads_of(tr)
-        for k, v in got.items():
-            np.save(os.path.join(out_dir, "T%d_%s.npy" % (T, k)), v.cpu().numpy())
-        np.save(os.path.join(out_dir, "T%d_losses.npy" % T), np.array([s[q] for q in LOSS_KEYS]))
-
 
 @pytest.mark.gpu
 def test_repeated_compute_grad_is_bit_identical():
     tr = make_trainer("grad_tj_hard_ic3net_h128", 300, 2, True)
     tr.run_batch(0)
-    g1, s1 = grads_of(tr)
-    g2, s2 = grads_of(tr)
-    assert all(torch.equal(g1[k], g2[k]) for k in g1), [k for k in g1 if not torch.equal(g1[k], g2[k])]
-    assert s1 == s2
+    assert_same_grads(grads_of(tr), grads_of(tr))
 
 
 @pytest.mark.gpu
 def test_one_stream_schedule_is_bit_identical(tmp_path):
-    mine, child = tmp_path / "overlap", tmp_path / "serial"
-    mine.mkdir()
-    child.mkdir()
-    schedule_grads(str(mine))
-    env = dict(os.environ, IC3_BPTT_OVERLAP="0")
-    code = ("import sys; sys.path[:0] = [%r, %r]; import test_gpu_bptt_passes as m; m.schedule_grads(%r)"
-            % (ROOT, TESTS, str(child)))
-    r = subprocess.run([sys.executable, "-c", code], env=env, cwd=ROOT, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-4000:]
-    files = sorted(os.listdir(mine))
-    assert files == sorted(os.listdir(child)) and len(files) > len(SCHEDULE_T)
-    for f in files:
-        a, b = np.load(mine / f), np.load(child / f)
-        assert np.array_equal(a, b), (f, np.abs(a - b).max())
+    """Cut rollouts of T = 1, 2, 5 steps with 3 comm passes (odd unit counts)."""
+    one_stream_schedule(tmp_path, "gpu_harness", "schedule_passes", more_than=3)
 
 
 @pytest.mark.gpu
@@ -289,9 +191,7 @@ def test_windowed_records_are_bit_identical(name, passes, share):
         tr.run_batch(0)
         out[tr.record_mode] = grads_of(tr)
     assert tf.record_mode == "full" and tw.record_mode == "window"
-    (gf, sf), (gw, sw) = out["full"], out["window"]
-    assert all(torch.equal(gf[k], gw[k]) for k in gf), [k for k in gf if not torch.equal(gf[k], gw[k])]
-    assert sf == sw
+    assert_same_grads(out["full"], out["window"])
 
 
 # ---------------------------------------------------------------------------------------------------- refusals

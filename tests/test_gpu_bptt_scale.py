@@ -26,73 +26,25 @@ reduction that misses rows, stays within the bar; the cases here make such fault
 
 Perturbations enter the records or the weights between the rollout and compute_grad (rewards: the returns are computed
 from them; head weights: the heads' backward starts from the recorded log-probs and values), so the kernels and the
-float64 yardstick read the same inputs.  Bar: that of the other BPTT tests (assert_within_bar), every gradient entry
+float64 yardstick read the same inputs.  Bar: the gradient bar of tests/gpu_harness.py, every gradient entry
 finite, the error word 0.  Each case asserts its own precondition in float64 so that it cannot pass vacuously."""
 import ctypes as C
-import os
-import subprocess
-import sys
 
-import numpy as np
 import pytest
 import torch
 
-import test_gpu_bptt_rnn as rnn
 from bptt_ref import returns_and_advantages, trainer_reference
+from gpu_harness import (GAMMA0, OPT_IN, PP, SMALL, TJ, assert_within_bar, finite_and_clean, grads_of,
+                         lstm_trainer as make_trainer, one_step, one_stream_schedule, passes_trainer,
+                         rnn_records_reference, rnn_trainer, swing, trainer_within_bar)
 from passes_oracle import records_reference as passes_reference
-from test_gpu_bptt_kernels import assert_within_bar, kernel_grad, make_trainer
-from test_gpu_bptt_passes import make_trainer as passes_trainer
-from test_gpu_forward_grad import one_step, within_bar
 
 pytestmark = pytest.mark.gpu
 
-TESTS = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(TESTS)
-PP, TJ = "grad_pp_hard_ic3net_h128", "grad_tj_hard_ic3net_h128"
-SMALL = {PP: 37, TJ: 24}               # 370 / 480 rows: ragged last tiles
 FULL = {PP: 8192, TJ: 4096}
-SWING = 1e4
-GAMMA0 = dict(gamma=0.0, mean_ratio=0.0, normalize_rewards=False)    # advantage of step t from the reward of step t
 
 
 # ---------------------------------------------------------------------------------------------------- helpers
-
-def step_adv(tr):
-    """np [T]: max over rows of |advantage * alive| per step, float64 -- what the heads' d outputs scale with."""
-    b = tr._buf
-    T = b["T"]
-    _, adv = returns_and_advantages(tr)
-    a = adv.to(torch.float64).reshape(T, -1) * b["ralive"][:T].reshape(T, -1).to(torch.float64)
-    return a.abs().amax(1).cpu().numpy()
-
-
-def swing(tr, pattern, factor=SWING):
-    """Scale the recorded rewards by step: 'even' / 'odd' steps x factor, 'block' the first half / factor and the
-    second half x factor.  Asserts the swing of the per-step advantage maxima it was made for."""
-    r, T = tr._buf["reward"], tr._buf["T"]
-    with torch.no_grad():
-        if pattern == "even":
-            r[0:T:2] *= factor
-        elif pattern == "odd":
-            r[1:T:2] *= factor
-        else:
-            r[:T // 2] /= factor
-            r[T // 2:T] *= factor
-    # Steps after every slot has halted have no live row (a = 0) and are left out.  Steps whose reward is zero on
-    # every row (traffic junction's first step of an episode) keep their advantage, -value, whatever the factor: at
-    # least 80% of the neighbouring live pairs (of the second half's live steps) must swing.
-    a = step_adv(tr)
-    if pattern == "block":
-        hi = a[T // 2:]
-        ratios = hi[hi > 0] / a[:T // 2].max()
-    else:
-        lo, hi = np.minimum(a[1:], a[:-1]), np.maximum(a[1:], a[:-1])
-        ratios = hi[lo > 0] / lo[lo > 0]
-    assert len(ratios) >= T // 4, (pattern, a)
-    ratio = np.quantile(ratios, 0.2)
-    assert ratio >= 1e3, (pattern, ratio, a)
-    return ratio
-
 
 def dominate(tr, k, factor=1e6):
     """Scale the rewards of env slot k on odd steps: there its heads dominate every other slot's, and on even steps
@@ -107,27 +59,20 @@ def dominate(tr, k, factor=1e6):
     assert mine >= 1e4 * others, (k, mine, others)
 
 
-def finite_and_clean(tr, got, label):
-    bad = [k for k, v in got.items() if not torch.isfinite(v).all()]
-    assert not bad, (label, "non-finite gradient", bad)
-    err = int(tr._buf["err"].item())
-    assert err == 0, (label, "error word", hex(err))
-
-
 def check_lstm(tr, label, reference=trainer_reference):
-    got, gloss = kernel_grad(tr)
+    got, gloss = grads_of(tr)
     finite_and_clean(tr, got, label)
     ref, rloss = reference(tr)
-    errs = assert_within_bar(tr, got, gloss, ref, rloss, label)
+    errs = trainer_within_bar(tr, got, gloss, ref, rloss, label)
     print("%s: worst error %.2e (bar 1e-4)" % (label, max(errs.values())))
     return got, gloss
 
 
 def check_rnn(tr, label):
-    got, gloss = rnn.grads_of(tr)
+    got, gloss = grads_of(tr)
     finite_and_clean(tr, got, label)
-    ref, rloss = rnn.records_reference(tr)
-    rnn.assert_within_bar(tr, got, gloss, ref, rloss, label)
+    ref, rloss = rnn_records_reference(tr)
+    trainer_within_bar(tr, got, gloss, ref, rloss, label)
 
 
 def scale_heads(tr, factor):
@@ -152,42 +97,16 @@ def test_step_swings(name, gap, pattern):
     """Neighbouring steps' bounds differ by 1e4: a unit reading the other parity's head bound, scale or inverse scale
     overflows in one of the two mirrored patterns.  detach_gap 1: every step's incoming d(h, c) is dropped."""
     over = dict(GAMMA0, **({"detach_gap": 1} if gap == "1" else {}))
-    tr, _, _ = make_trainer(name, SMALL[name], seed=41, id0=5, **over)
+    tr = make_trainer(name, SMALL[name], seed=41, id0=5, **over)
     tr.run_batch(0)
     ratio = swing(tr, pattern)
     check_lstm(tr, "%s B=%d detach_gap=%d %s (80%% of step ratios >= %.1e)" % (name, SMALL[name], tr.args.detach_gap,
                                                                               pattern, ratio))
 
 
-def swing_grads(out_dir):
-    """Kernel gradients and losses of two swing batches (even steps of predator-prey, odd steps of traffic junction),
-    saved under out_dir.  Run in this process and in a child with IC3_BPTT_OVERLAP=0."""
-    for name, pattern in ((PP, "even"), (TJ, "odd")):
-        tr, _, _ = make_trainer(name, SMALL[name], seed=41, id0=5, **GAMMA0)
-        tr.run_batch(0)
-        swing(tr, pattern)
-        got, s = kernel_grad(tr)
-        finite_and_clean(tr, got, name)
-        for k, v in got.items():
-            np.save(os.path.join(out_dir, "%s_%s.npy" % (pattern, k)), v.cpu().numpy())
-        np.save(os.path.join(out_dir, "%s_losses.npy" % pattern), np.array([s[q] for q in sorted(s)]))
-
-
 def test_swings_one_stream_schedule_is_bit_identical(tmp_path):
-    mine, child = tmp_path / "overlap", tmp_path / "serial"
-    mine.mkdir()
-    child.mkdir()
-    swing_grads(str(mine))
-    env = dict(os.environ, IC3_BPTT_OVERLAP="0")
-    code = ("import sys; sys.path[:0] = [%r, %r]; import test_gpu_bptt_scale as m; m.swing_grads(%r)"
-            % (ROOT, TESTS, str(child)))
-    r = subprocess.run([sys.executable, "-c", code], env=env, cwd=ROOT, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    files = sorted(os.listdir(mine))
-    assert files == sorted(os.listdir(child)) and len(files) > 2
-    for f in files:
-        a, b = np.load(mine / f), np.load(child / f)
-        assert np.array_equal(a, b), (f, np.abs(a - b).max())
+    """Kernel gradients and losses of two swing batches (even steps of predator-prey, odd steps of traffic junction)."""
+    one_stream_schedule(tmp_path, "gpu_harness", "swing_grads", more_than=2, timeout=900)
 
 
 @pytest.mark.parametrize("name,pattern", [(PP, "odd"), (TJ, "even")])
@@ -196,12 +115,10 @@ def test_swings_window_records_are_bit_identical(name, pattern):
     maxima give the same gradient bit for bit."""
     out = []
     for windows in (False, True):
-        tr, _, _ = make_trainer(name, SMALL[name], seed=41, id0=5, **GAMMA0)
-        if windows:
-            tr.RECORD_BYTES_LIMIT = 0
+        tr = make_trainer(name, SMALL[name], seed=41, id0=5, windows=windows, **GAMMA0)
         tr.run_batch(0)
         swing(tr, pattern)
-        got, s = kernel_grad(tr)
+        got, s = grads_of(tr)
         finite_and_clean(tr, got, name)
         out.append((tr.record_mode, got, s))
     (m0, g0, s0), (m1, g1, s1) = out
@@ -219,7 +136,8 @@ def test_swings_window_records_are_bit_identical(name, pattern):
 def test_swings_comm_passes(name, passes, share, over, pattern):
     """comm_passes > 1: the units (t, P-1) .. (t, 0) alternate the parity inside a step and nothing is launched ahead;
     the heads (last pass) and the recursion-only passes get bounds from different terms."""
-    tr = passes_trainer(name, SMALL[name], passes, share, seed=41, id0=5, **dict(GAMMA0, **over))
+    tr = passes_trainer(name, SMALL[name], seed=41, id0=5, comm_passes=passes, share_weights=share,
+                        **dict(GAMMA0, **over))
     tr.run_batch(0)
     swing(tr, pattern)
     check_lstm(tr, "%s passes=%d share=%s %s %s" % (name, passes, share, over, pattern), passes_reference)
@@ -230,7 +148,7 @@ def test_swings_comm_passes(name, passes, share, over, pattern):
 @pytest.mark.parametrize("name", [PP, TJ])
 def test_swings_tanh_rnn(name, impl, pattern):
     """The IC tanh RNN: the dz operand takes the scale of its unit."""
-    tr = rnn.make_trainer(name, SMALL[name], seed=41, id0=5, policy_impl=impl, **GAMMA0)
+    tr = rnn_trainer(name, SMALL[name], seed=41, id0=5, policy_impl=impl, **GAMMA0)
     tr.run_batch(0)
     swing(tr, pattern)
     check_rnn(tr, "IC %s B=%d %s %s" % (name, SMALL[name], impl, pattern))
@@ -238,7 +156,7 @@ def test_swings_tanh_rnn(name, impl, pattern):
 
 @pytest.mark.parametrize("name,pattern", [(PP, "even"), (TJ, "odd")])
 def test_swings_full_size(name, pattern):
-    tr, _, _ = make_trainer(name, FULL[name], seed=5, id0=0, **GAMMA0)
+    tr = make_trainer(name, FULL[name], seed=5, id0=0, **GAMMA0)
     tr.run_batch(0)
     swing(tr, pattern)
     check_lstm(tr, "%s B=%d %s" % (name, FULL[name], pattern))
@@ -259,7 +177,7 @@ def test_one_slot_dominates(where, forget):
     360..369 of the ragged last tile (370 rows)."""
     B = SMALL[PP]
     k = {"first": 0, "straddles-tile": 12, "last": B - 1}[where]
-    tr, _, _ = make_trainer(PP, B, seed=41, id0=5, **GAMMA0)
+    tr = make_trainer(PP, B, seed=41, id0=5, **GAMMA0)
     N = tr.args.nagents
     assert where != "straddles-tile" or (k * N) // 128 != (k * N + N - 1) // 128
     if forget == "closed":
@@ -273,7 +191,7 @@ def test_one_slot_dominates(where, forget):
 @pytest.mark.parametrize("name", [PP, TJ])
 def test_last_slot_dominates_full_size(name, forget):
     B = FULL[name]
-    tr, _, _ = make_trainer(name, B, seed=5, id0=0, **GAMMA0)
+    tr = make_trainer(name, B, seed=5, id0=0, **GAMMA0)
     if forget == "closed":
         close_forget_gate(tr)
     tr.run_batch(0)
@@ -288,7 +206,7 @@ def test_last_slot_dominates_full_size(name, forget):
 def test_head_weight_extremes(name, case):
     """After the rollout: every head weight scaled (both ends of the operand range), or one entry of hidden unit 127
     made 1e3 times the largest weight of its head (the heads' bound takes its maximum over every unit)."""
-    tr, _, _ = make_trainer(name, SMALL[name], seed=41, id0=5)
+    tr = make_trainer(name, SMALL[name], seed=41, id0=5)
     tr.run_batch(0)
     net = tr.policy_net
     if case.startswith("x"):
@@ -319,7 +237,7 @@ def test_saturated_cells(name, pattern):
     """i, f, g saturated before the rollout: c grows by about 1 per step (|c| past 20), the bound's max(1, cmax / 4)
     factor is large and d c is carried through f ~ 1."""
     from ic3net_b200 import _lib
-    tr, _, _ = make_trainer(name, SMALL[name], seed=41, id0=5, max_steps=40, **GAMMA0)
+    tr = make_trainer(name, SMALL[name], seed=41, id0=5, max_steps=40, **GAMMA0)
     set_gate_bias(tr, i=6.0, f=6.0, g=3.0)
     tr.run_batch(0)
     assert int(tr._buf["err"].item()) & _lib.ERR_FP16_RANGE == 0
@@ -334,7 +252,7 @@ def test_saturated_cells(name, pattern):
 def test_cell_gradient_dominates(name):
     """f ~ 1 carries d c back undamped while the recurrent and comm weights (x1e-3) leave d h small: after a large step,
     the next unit's bound is almost all dcmax."""
-    tr, _, _ = make_trainer(name, SMALL[name], seed=41, id0=5, **GAMMA0)
+    tr = make_trainer(name, SMALL[name], seed=41, id0=5, **GAMMA0)
     net = tr.policy_net
     with torch.no_grad():
         net.f_module.weight_hh.mul_(1e-3)
@@ -369,7 +287,7 @@ def begin_workspaces(plan, c, n):
 
 def lstm_plan(passes):
     from ic3net_b200 import _lib
-    tr = passes_trainer(PP, 5, passes, seed=41, id0=5)
+    tr = passes_trainer(PP, 5, seed=41, id0=5, comm_passes=passes)
     tr.run_batch(0)
     plan = tr._bptt_plan(tr._policy_cfg(), tr.policy_net.packed(), _lib.ptr(tr._encoder_table()))
     return tr, plan
@@ -441,11 +359,10 @@ def test_device_cmax_past_2_31_floats():
 def test_upstream_extremes(scale, spike):
     """ic3_policy_step_backward reduces the maxima of the caller's d h', d c' (and the heads' bound of d value) on the
     device; a spike of 1e5 in the last row and column of one of them must reach the bound."""
-    from test_gpu_bptt_passes import make_trainer as lstm_trainer
-    tr = lstm_trainer(PP, SMALL[PP], 1, False, seed=5, id0=0, obs_api="handle", forward_grad="kernels")
+    tr = passes_trainer(PP, SMALL[PP], seed=5, id0=0, **OPT_IN)
     tr.rollout(tr.args.max_steps + 4, 0)
     got, ref, sums = one_step(tr, tr.args.max_steps - 2, scale=scale, spike=None if spike is None else (spike, 1e5))
     bad = [k for k, v in got.items() if not torch.isfinite(v).all()]
     assert not bad, bad
-    errs = within_bar(got, ref, sums, "upstream x%g spike %s" % (scale, spike))
+    errs = assert_within_bar(got, ref, sums, "upstream x%g spike %s" % (scale, spike))
     print("upstream x%g spike %s: worst error %.2e (bar 1e-4)" % (scale, spike, max(errs.values())))

@@ -7,92 +7,17 @@ gradient and loss sums bit-identical to full records (full batch sizes, ragged /
 starts and detach_gap cuts on window starts, enemy_comm, hard attention off, dense and index observations, eager and
 CUDA-graph rollouts, the one-stream schedule), every recomputed window equal to the full record bit for bit, the
 reference fixtures against the float64 oracle, a batch whose full records do not fit on the card, and the selection."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
 
 from bptt_ref import LOSS_KEYS, max_rel_err, oracle_grad_sum, returns_and_advantages, trainer_reference
-from helpers import finish_args, golden_names, load_golden, ns
+from gpu_harness import (LOSS_ATOL, LOSS_RTOL, SUM_FLOOR, TOL, flat_grad, lstm_fixture_weights,
+                         lstm_trainer as make_trainer, one_stream_schedule, window_vs_full)
+from helpers import golden_names, load_golden
 from oracle import policy as opolicy
-from oracle.gen_golden import make_weights
 
 pytestmark = pytest.mark.gpu
-
-TESTS = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(TESTS)
-TOL = 1e-4
-
-
-def make_trainer(name, B, seed=808, id0=30, windows=False, **over):
-    """Kernel-gradient Trainer on the arguments of fixture ``name`` (overridden by ``over``), weights from the
-    fixture's seed; ``windows``: full records never fit, so the records are windows."""
-    from ic3net_b200 import data
-    from ic3net_b200.comm import CommNetMLP
-    from ic3net_b200.trainer import Trainer
-    meta, z = load_golden(name)
-    kw = dict(nenvs=B, seed=seed, env_id0=id0, obs_mode="index", use_graph=False, policy_impl="tc",
-              record_for_grad=True, grad_impl="kernels")
-    kw.update(over)
-    args = ns(meta["args"], **kw)
-    env = data.init(args.env_name, args)
-    finish_args(args, env)
-    net = CommNetMLP(args, args.num_inputs)
-    sd = make_weights(meta["weights_seed"], args.num_inputs, args.hid_size, args.naction_heads, args.comm_init)
-    net.load_state_dict({k: torch.from_numpy(v).float() for k, v in sd.items()})
-    tr = Trainer(args, net, env)
-    if windows:
-        tr.RECORD_BYTES_LIMIT = 0
-    return tr, sd, z
-
-
-def flat_grad(tr):
-    """compute_grad of the last rollout from zeroed gradients: (flat gradient buffer, float64 loss sums), copies."""
-    tr.optimizer.zero_grad(set_to_none=False)
-    losses = tr.compute_grad_device(None).clone()
-    g = tr.optimizer.flat_grads.clone()
-    assert int(tr._buf["err"].item()) == 0
-    return g, losses
-
-
-def row_mask(tr, t):
-    """[B*N] rows of the env slots that were still playing at step t."""
-    return tr._buf["valid"][t].bool().repeat_interleave(tr.args.nagents)
-
-
-def window_vs_full(name, B, W, **over):
-    """Full-record and window-record trainers on the same seeded batch: asserts bit-identical rollouts, gradients and
-    loss sums, and every recomputed window equal to the full record on the rows of slots still playing.  Returns
-    {mode: (flat gradient, losses)} as numpy arrays and the full trainer."""
-    tf, _, _ = make_trainer(name, B, grad_window=W, **over)
-    tw, _, _ = make_trainer(name, B, grad_window=W, windows=True, **over)
-    out = {}
-    for tr in (tf, tw):
-        tr.run_batch(0)
-        g, s = flat_grad(tr)
-        out[tr.record_mode] = (g.cpu().numpy(), s.cpu().numpy())
-    assert tf.record_mode == "full" and tw.record_mode == "window" and "rec_h" not in tw._buf
-    for k in ("action", "valid", "logp", "value", "s_fresh", "s_tep"):
-        assert torch.equal(tf._buf[k], tw._buf[k]), k
-    T = tw._buf["T"]
-    for k in range((T + W - 1) // W):
-        wh, wc = tw._recompute_window(k)
-        for j in range(wh.shape[0]):
-            t = k * W + j
-            m = row_mask(tw, t)
-            assert torch.equal(wh[j][m], tf._buf["rec_h"][t + 1][m]), (k, j)
-            assert torch.equal(wc[j][m], tf._buf["rec_c"][t + 1][m]), (k, j)
-        if k + 1 < (T + W - 1) // W:     # the checkpoints are the rollout's state at the window starts
-            m = row_mask(tw, (k + 1) * W - 1)
-            assert torch.equal(tw._buf["ck_h"][k + 1][m], tf._buf["rec_h"][(k + 1) * W][m]), k
-    (gf, sf), (gw, sw) = out["full"], out["window"]
-    assert np.array_equal(gf, gw), np.abs(gf - gw).max()
-    assert np.array_equal(sf, sw), (sf, sw)
-    assert np.isfinite(gf).all() and np.abs(gf).max() > 0
-    return out, tf
 
 
 def boundary_events(tr, W):
@@ -145,32 +70,11 @@ def test_windows_are_bit_identical(case):
         assert tf._buf["T"] <= W
 
 
-def one_stream_case(out_dir):
-    """window_vs_full at one-step and ragged windows; saves the window-mode gradients and losses under out_dir.  Run
-    in this process and in a child with IC3_BPTT_OVERLAP=0."""
-    for W in (1, 5):
-        out, _ = window_vs_full("grad_pp_hard_ic3net_h128", 400, W, seed=13, id0=2)
-        g, s = out["window"]
-        np.save(os.path.join(out_dir, "W%d_grad.npy" % W), g)
-        np.save(os.path.join(out_dir, "W%d_losses.npy" % W), s)
-
-
 def test_one_stream_schedule(tmp_path):
     """IC3_BPTT_OVERLAP=0 (read once per process: a child) runs the look-ahead kernels on the caller's stream, behind
     the recompute of every window: still bit-identical to full records, and to the two-stream schedule."""
-    mine, child = tmp_path / "overlap", tmp_path / "serial"
-    mine.mkdir()
-    child.mkdir()
-    one_stream_case(str(mine))
-    env = dict(os.environ, IC3_BPTT_OVERLAP="0")
-    code = ("import sys; sys.path[:0] = [%r, %r]; import test_gpu_bptt_windows as m; m.one_stream_case(%r)"
-            % (ROOT, TESTS, str(child)))
-    r = subprocess.run([sys.executable, "-c", code], env=env, cwd=ROOT, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stderr[-4000:]
-    files = sorted(os.listdir(mine))
-    assert files == sorted(os.listdir(child)) and len(files) == 4
-    for f in files:
-        assert np.array_equal(np.load(mine / f), np.load(child / f)), f
+    files = one_stream_schedule(tmp_path, "gpu_harness", "schedule_windows", more_than=3)
+    assert len(files) == 4
 
 
 # ---------------------------------------------------------------------------------------------------- reference
@@ -183,7 +87,9 @@ def test_windows_match_oracle(name):
     """Every hid_size-128 gradient fixture in window mode (4-step windows) against the float64 oracle's sum over the
     slots, at the bar of the full-record kernels (test_gpu_grad.py)."""
     B, seed, id0 = 5, 808, 30
-    tr, sd, z = make_trainer(name, B, seed, id0, windows=True, grad_window=4)
+    tr = make_trainer(name, B, seed, id0, windows=True, grad_window=4)
+    meta, z = load_golden(name)
+    sd = lstm_fixture_weights(meta, tr.args)
     batch, stat = tr.run_batch(0)
     assert tr.record_mode == "window"
     T, quota = tr.batch_plan()
@@ -193,7 +99,7 @@ def test_windows_match_oracle(name):
                                           batch.valid.cpu().numpy(), seed, id0, quota, T)
     assert stat["num_steps"] == nsteps
     for q in LOSS_KEYS:
-        assert np.isclose(s[q], wstat[q], rtol=2e-4, atol=1e-3), (q, s[q], wstat[q])
+        assert np.isclose(s[q], wstat[q], rtol=LOSS_RTOL, atol=LOSS_ATOL), (q, s[q], wstat[q])
     worst = 0.0
     for key, prm in tr.policy_net.named_parameters():
         if want[key] is None or not np.any(want[key]):
@@ -281,7 +187,7 @@ def test_batch_beyond_full_records_trains():
     gradients and statistics under PEAK_BOUND; then, on the next batch, the kernels' gradient of 5 sampled slots and
     the last slot (the other slots' learning signal masked out) matches the float64 reference over those slots."""
     B = 8192
-    tr, _, _ = make_trainer("grad_pp_hard_ic3net_h128", B, seed=5, id0=0, batch_size=1000, max_steps=80)
+    tr = make_trainer("grad_pp_hard_ic3net_h128", B, seed=5, id0=0, batch_size=1000, max_steps=80)
     T, _ = tr.batch_plan()
     assert T == 1079 and tr._record_bytes(T)["full"] > torch.cuda.get_device_properties(0).total_memory
     assert tr.record_mode == "window"
@@ -317,12 +223,12 @@ def test_batch_beyond_full_records_trains():
     abs_sums = slot_heads_abs_sums(tr, rec_h, slots)
     worst = {}
     for k, r in ref.items():
-        allowed = TOL * r.abs().max() + (2.0 ** -20 * abs_sums[k] if k in abs_sums else 0.0)
+        allowed = TOL * r.abs().max() + (SUM_FLOOR * abs_sums[k] if k in abs_sums else 0.0)
         worst[k] = float(((got[k] - r).abs() / allowed).max()) * TOL
     print("slots %s: %s" % (slots, " ".join("%s %.1e" % kv for kv in worst.items())))
     assert all(v <= TOL for v in worst.values()), worst
     for q in LOSS_KEYS:
-        assert np.isclose(s[q], rloss[q], rtol=2e-4, atol=1e-3), (q, s[q], rloss[q])
+        assert np.isclose(s[q], rloss[q], rtol=LOSS_RTOL, atol=LOSS_ATOL), (q, s[q], rloss[q])
 
 
 # ---------------------------------------------------------------------------------------------------- selection
@@ -332,7 +238,7 @@ def test_selection():
     the full records picks windows; a device too small even for the windows raises an error that names the bytes,
     before anything is allocated for the records, and the trainer stays usable."""
     from ic3net_b200.trainer import Trainer
-    tr, _, _ = make_trainer("grad_pp_hard_ic3net_h128", 400)
+    tr = make_trainer("grad_pp_hard_ic3net_h128", 400)
     assert tr.record_mode == "full"
     tr.run_batch(0)
     assert tr.record_mode == "full" and "rec_h" in tr._buf

@@ -15,39 +15,20 @@ import numpy as np
 import pytest
 import torch
 
+from gpu_harness import (PP, TJ, UPDATE_FF, UPDATE_IC, UPDATES, argmax_check, close, cpu, episode_trainer,
+                         head_logits_f64, lstm_direct_step, lstm_outputs, make_lstm_net, same_stat, synthetic,
+                         update_trainer)
 from helpers import golden_names, load_golden, make_oracle_env
 from oracle.rollout import run_episode
 from policy_ref import params_f64, step_f64
-from test_gpu_rollout import build, close, cpu
-from test_gpu_graph_update import FF, IC, K, make_trainer, same_stat
-from test_gpu_policy_rows import direct_step, make_net, outputs, synthetic
 
 pytestmark = pytest.mark.gpu
 
-PP, TJ = "grad_pp_hard_ic3net_h128", "grad_tj_hard_ic3net_h128"
-TIE = 1e-5
 SIMT = dict(policy_impl="simt", grad_impl="autograd")
-POLICIES = {"tc": dict(), "simt": SIMT, "tc_ff": dict(FF, model="mlp", commnet=False, hard_attn=False),
-            "tc_tanh": dict(IC)}
+POLICIES = {"tc": dict(), "simt": SIMT, "tc_ff": dict(UPDATE_FF, model="mlp", commnet=False, hard_attn=False),
+            "tc_tanh": dict(UPDATE_IC)}
 STATE = ("fresh", "comm", "alive", "t_ep", "h", "c", "halted", "stat_reward", "stat_comm", "stat_success",
          "stat_episodes", "stat_steps")
-
-
-def argmax_check(logits, act, heads, label):
-    """act [R, nheads] against the argmax of float64 logits [R, sum(heads)]; rows whose top two logits are within
-    TIE * max(1, |logit|) are exempt.  Returns the number of exempt rows."""
-    off, exempt = 0, 0
-    for k, na in enumerate(heads):
-        lg = logits[:, off:off + na]
-        want = lg.argmax(1)
-        top2 = np.sort(lg, 1)[:, -2:] if na > 1 else np.concatenate([lg - 1, lg], 1)
-        near = (top2[:, 1] - top2[:, 0]) < TIE * np.maximum(1.0, np.abs(top2[:, 1]))
-        bad = np.nonzero(~near & (want != act[:, k]))[0]
-        assert bad.size == 0, "%s head %d: greedy action differs from the float64 argmax at rows %s" % (label, k, bad[:10])
-        assert act[:, k].min() >= 0 and act[:, k].max() < na
-        exempt += int(near.sum())
-        off += na
-    return exempt
 
 
 class F64Weights(object):
@@ -79,18 +60,11 @@ def tanh_step_f64(tr, net, obs, h0, comm, alive, fresh):
     return torch.cat(logps, 1)
 
 
-def head_logits_f64(net, h):
-    """Float64 action logits of the heads on hidden state h [R, H] (value head dropped)."""
-    w = net._kernel_weights()
-    return torch.cat([h.detach().double() @ hw.detach().double().t() + hb.detach().double()
-                      for hw, hb in zip(w["head_w"], w["head_b"])], 1)
-
-
 @pytest.mark.parametrize("impl", sorted(POLICIES))
 @pytest.mark.parametrize("name,B", [(PP, 8192), (TJ, 4096)])
 def test_greedy_every_row(name, B, impl):
     over = dict(POLICIES[impl], record_for_grad=False, grad_impl="auto")
-    tr = make_trainer(name, B, False, max_steps=6, eval_nenvs=B, **over)
+    tr = update_trainer(name, B, False, max_steps=6, eval_nenvs=B, **over)
     assert tr.policy_net.policy_impl == impl
     ev = tr._eval_state()
     e, b = ev["env"], ev["buf"]
@@ -138,16 +112,16 @@ def test_greedy_heads_paths(heads):
     explicit draws from the same inputs, log-probs and value bit-identical, actions the argmax of the float64 heads."""
     N, O, B = 7, 61, 300
     R = B * N
-    net, a = make_net(N, O, heads, wseed=sum(heads))
+    net, a = make_lstm_net(N, O, heads, wseed=sum(heads))
     inputs = synthetic(B, N, O, seed=len(heads) + sum(heads))
     draws = torch.randint(0, 1 << 24, (R, len(heads)), dtype=torch.int32, device="cuda")
-    sampled = outputs(R, heads)
-    assert direct_step(net, *inputs, sampled, draws=draws) == 0
+    sampled = lstm_outputs(R, heads)
+    assert lstm_direct_step(net, *inputs, sampled, draws=draws) == 0
     proto = net.policy_cfg
     net.policy_cfg = lambda Bn: _greedy(proto(Bn))
     try:
-        greedy = outputs(R, heads)
-        assert direct_step(net, *inputs, greedy, draws=draws) == 0
+        greedy = lstm_outputs(R, heads)
+        assert lstm_direct_step(net, *inputs, greedy, draws=draws) == 0
     finally:
         net.policy_cfg = proto
     for k in ("value", "logp", "h", "c"):
@@ -160,8 +134,8 @@ def test_greedy_heads_paths(heads):
             hb.fill_(0.25)
     net.policy_cfg = lambda Bn: _greedy(proto(Bn))
     try:
-        tied = outputs(R, heads)
-        assert direct_step(net, *inputs, tied, draws=draws) == 0
+        tied = lstm_outputs(R, heads)
+        assert lstm_direct_step(net, *inputs, tied, draws=draws) == 0
     finally:
         net.policy_cfg = proto
     assert bool((tied["action"] == 0).all()), heads
@@ -171,7 +145,7 @@ def test_greedy_heads_paths(heads):
 def test_ties_take_the_lowest_index(impl):
     """Zero action-head weights and equal biases make every logit of a head equal: greedy evaluation picks action 0 in
     every head on every row, on every policy path."""
-    tr = make_trainer(PP, 256, False, max_steps=5, eval_nenvs=256, **dict(POLICIES[impl], record_for_grad=False,
+    tr = update_trainer(PP, 256, False, max_steps=5, eval_nenvs=256, **dict(POLICIES[impl], record_for_grad=False,
                                                                            grad_impl="auto"))
     w = tr.policy_net._kernel_weights()
     with torch.no_grad():
@@ -190,7 +164,7 @@ def test_one_slot_plays_the_reference_greedy_episode(name, impl):
     log-probs are close enough for fp32 to flip the argmax."""
     meta, z = load_golden(name)
     ids = meta["env_ids"]
-    args, env, net, tr, p = build(meta, max(ids) + 1, "index", impl=impl)
+    args, env, net, tr, p = episode_trainer(meta, max(ids) + 1, impl=impl)
     T = args.max_steps
     tr._alloc(T)
     tr._episode_boundary(meta["epoch"])
@@ -230,7 +204,7 @@ def test_sampled_evaluation_equals_the_oracle_replay(B):
     CDF edge (fp32 may flip it) is skipped."""
     E = 2
     meta, _ = load_golden("ep_pp_hard_ic3net")
-    args, env, net, tr, p = build(meta, B, "index", impl="tc", eval_nenvs=B, max_steps=30)
+    args, env, net, tr, p = episode_trainer(meta, B, impl="tc", eval_nenvs=B, max_steps=30)
     st = tr.evaluate(E)
     ev = tr._eval
     e, b = ev["env"], ev["buf"]
@@ -283,7 +257,7 @@ def _greedy(cfg):
 @pytest.mark.parametrize("B", [5, 13, 8192])
 @pytest.mark.parametrize("E", [1, 3])
 def test_every_slot_plays_its_quota(B, E):
-    tr = make_trainer(PP, B, False, max_steps=20, eval_nenvs=B)
+    tr = update_trainer(PP, B, False, max_steps=20, eval_nenvs=B)
     for greedy in (False, True):
         st = tr.evaluate(E, greedy)
         b = tr._eval["buf"]
@@ -293,7 +267,7 @@ def test_every_slot_plays_its_quota(B, E):
 
 
 def test_sampled_evaluation_is_reproducible_and_continues_its_streams():
-    a, b = make_trainer(PP, 13, False, eval_nenvs=13), make_trainer(PP, 13, False, eval_nenvs=13)
+    a, b = update_trainer(PP, 13, False, eval_nenvs=13), update_trainer(PP, 13, False, eval_nenvs=13)
     s1, s2 = a.evaluate(2), b.evaluate(2)
     same_stat(s1, s2)
     s3 = a.evaluate(2)
@@ -301,7 +275,7 @@ def test_sampled_evaluation_is_reproducible_and_continues_its_streams():
 
 
 ISOLATION = {"ic3net_full": dict(), "ic3net_windows": dict(windows=True),
-             "mlp_ff": dict(FF, model="mlp", commnet=False, hard_attn=False), "ic_tanh": dict(IC),
+             "mlp_ff": dict(UPDATE_FF, model="mlp", commnet=False, hard_attn=False), "ic_tanh": dict(UPDATE_IC),
              "ic3net_graph_update": dict(graph=True), "ic3net_use_graph": dict(use_graph=True)}
 
 
@@ -309,8 +283,8 @@ ISOLATION = {"ic3net_full": dict(), "ic3net_windows": dict(windows=True),
 def test_evaluation_leaves_training_untouched(case):
     over = dict(ISOLATION[case])
     graph = over.pop("graph", False)
-    plain, evald = make_trainer(PP, 1024, graph, **over), make_trainer(PP, 1024, graph, **over)
-    for ep in range(K):
+    plain, evald = update_trainer(PP, 1024, graph, **over), update_trainer(PP, 1024, graph, **over)
+    for ep in range(UPDATES):
         evald.evaluate(1, greedy=bool(ep % 2))
         same_stat(plain.train_batch(ep), evald.train_batch(ep))
     for x, y in ((plain.optimizer.flat_params, evald.optimizer.flat_params),
@@ -323,25 +297,25 @@ def test_evaluation_reads_the_weights_of_replayed_updates():
     """Evaluations between updates, sampled and greedy, eager and replayed (use_graph), of a trainer whose updates are
     replayed (graph_update) equal those of an eager trainer bit for bit: the evaluation env's encoder table follows the
     weights every update leaves."""
-    eager, graph = make_trainer(PP, 256, False), make_trainer(PP, 256, True)
-    for ep in range(K + 1):
+    eager, graph = update_trainer(PP, 256, False), update_trainer(PP, 256, True)
+    for ep in range(UPDATES + 1):
         for use_graph, greedy in ((False, False), (True, True), (True, False), (False, True)):
             eager.use_graph = graph.use_graph = use_graph
             same_stat(eager.evaluate(1, greedy), graph.evaluate(1, greedy))
         eager.use_graph = graph.use_graph = False
-        if ep < K:
+        if ep < UPDATES:
             same_stat(eager.train_batch(ep), graph.train_batch(ep))
 
 
 @pytest.mark.parametrize("name", [PP, TJ])
 def test_graph_replay_equals_eager(name):
-    eager, graph = make_trainer(name, 512, False), make_trainer(name, 512, False, use_graph=True)
+    eager, graph = update_trainer(name, 512, False), update_trainer(name, 512, False, use_graph=True)
     for greedy in (False, True, False):
         same_stat(eager.evaluate(2, greedy), graph.evaluate(2, greedy))
 
 
 def test_traffic_junction_epoch_sets_add_rate_and_recaptures():
-    tr = make_trainer(TJ, 256, False, use_graph=True, curr_start=1, curr_end=10, add_rate_min=0.05, add_rate_max=0.2)
+    tr = update_trainer(TJ, 256, False, use_graph=True, curr_start=1, curr_end=10, add_rate_min=0.05, add_rate_max=0.2)
     s0 = tr.evaluate(1)
     k0 = tr._graphs["evaluate"][0]
     assert s0["add_rate"] == pytest.approx(0.05 * 256)
@@ -350,13 +324,13 @@ def test_traffic_junction_epoch_sets_add_rate_and_recaptures():
     assert s1["add_rate"] / s1["num_episodes"] == pytest.approx(tr._eval["env"].add_rate)
     assert tr._eval["env"].add_rate == pytest.approx(0.2, abs=0.011)
     assert tr.env.env.add_rate == pytest.approx(0.05)               # the training env keeps its curriculum
-    eager = make_trainer(TJ, 256, False, curr_start=1, curr_end=10, add_rate_min=0.05, add_rate_max=0.2)
+    eager = update_trainer(TJ, 256, False, curr_start=1, curr_end=10, add_rate_min=0.05, add_rate_max=0.2)
     eager.evaluate(1)
     same_stat(s1, eager.evaluate(1, epoch=20))
 
 
 def test_random_policy_evaluates_sampled_and_refuses_greedy():
-    from test_gpu_random import make_trainer as random_trainer, random_args
+    from gpu_harness import random_args, random_trainer
     _, tr = random_trainer(random_args("c2", nenvs=64, max_steps=20))
     st = tr.evaluate(2)
     assert st["num_episodes"] == 2 * 64
@@ -366,6 +340,6 @@ def test_random_policy_evaluates_sampled_and_refuses_greedy():
 
 def test_multi_gpu_trainer_single_process_equals_trainer():
     from ic3net_b200.multi_gpu import MultiGPUTrainer
-    a = make_trainer(PP, 64, False)
-    m = MultiGPUTrainer(a.args, lambda: make_trainer(PP, 64, False))
+    a = update_trainer(PP, 64, False)
+    m = MultiGPUTrainer(a.args, lambda: update_trainer(PP, 64, False))
     same_stat(a.evaluate(2, True), m.evaluate(2, True))

@@ -21,106 +21,30 @@ import numpy as np
 import pytest
 import torch
 
-import test_gpu_grad_ff as gf
+from gpu_harness import (MARGIN, PP, ROW_TOL, TJ, assert_close, close, compare_rows, ff_chunk_sizes_and_determinism,
+                         ff_direct_step, ff_full_size, ff_gradient_arrays, ff_halted_slots_contribute_nothing, ff_net,
+                         ff_pinned_oracle, ff_step_f64, ff_trainer, gated_mean, gates_f64, rollout_and_grad, sum_tol,
+                         variant_net)
 from helpers import golden_names, load_golden
 from policy_ref import inverse_cdf
 
 pytestmark = pytest.mark.gpu
 
-TOL, MARGIN, TILE = 1e-5, 1e-5, 64
-
-
-def sum_tol(N):
-    return max(TOL, 3e-6 * (N - 1))
-PP, TJ = gf.PP, gf.TJ
+TILE = 64                   # rows per CTA tile of ff_tc_kernel
 
 
 def make_trainer(name, B, family, **kw):
     kw.setdefault("policy_impl", "tc_ff")
-    tr = gf.make_trainer(name, B, family, **kw)
+    tr = ff_trainer(name, B, family, **kw)
     assert tr.policy_net.policy_impl == kw["policy_impl"]
     return tr
 
 
-@pytest.fixture
-def tc_ff_trainers(monkeypatch):
-    """Every trainer tests/test_gpu_grad_ff.py builds (its make_trainer and fixture_trainer) gets policy_impl 'tc_ff':
-    its checks then run on this forward, at the bars the SIMT forward meets."""
-    orig = gf.ns
-    monkeypatch.setattr(gf, "ns", lambda a, **kw: orig(a, **dict(kw, policy_impl="tc_ff")))
-
-
-def rel_err(got, ref):
-    got, ref = got.to(torch.float64), ref.to(torch.float64)
-    return ((got - ref).abs() / ref.abs().clamp_min(1.0)).reshape(ref.shape[0], -1)
-
-
-def compare(label, got, ref, worst=None, tol=TOL):
-    msgs = []
-    R = ref["value"].shape[0]
-    for k in got:
-        e = rel_err(got[k].reshape(R, -1), ref[k].reshape(R, -1))
-        m = float(e.max())
-        if worst is not None:
-            worst[k] = max(worst.get(k, 0.0), m)
-        if not m <= tol:
-            r, col = divmod(int(e.argmax()), e.shape[1])
-            msgs.append("%s: %s max %.3e at row %d col %d; %d rows over the bar" % (
-                label, k, m, r, col, int((e > tol).any(1).sum())))
-    assert not msgs, "\n".join(msgs)
-
-
-def gates_f64(B, N, comm, alive, fresh, hard, avg):
-    """(g [B, N, 1], den [B, 1, 1]) of the gated mean (comm.py:102-107,171-175,194-196; trainer.py:45-51)."""
-    dev = "cuda"
-    fr = (fresh.bool() if fresh is not None else torch.zeros(B, dtype=torch.bool, device=dev)).unsqueeze(1)
-    al = alive.double() if alive is not None else torch.ones(B, N, dtype=torch.float64, device=dev)
-    al = torch.where(fr, torch.ones_like(al), (al != 0).double())
-    n_alive = al.sum(1, keepdim=True)
-    g = al * (torch.where(fr, torch.zeros_like(al), (comm != 0).double()) if hard else 1.0)
-    one = torch.ones_like(n_alive)
-    den = torch.where(n_alive > 1, n_alive - 1, one) if avg else one
-    return g.unsqueeze(-1), den.unsqueeze(-1)
-
-
-def gated_mean(h, g, den):
-    """S[k] = g[k] sum_{j != k} g[j] h[j] / den, h [B, N, H]."""
-    return g * ((g * h).sum(1, keepdim=True) - g * h) / den
-
-
-def step_f64(net, x, B, comm=None, alive=None, fresh=None, passes=None):
-    """x~ = tanh(x); per pass h = tanh(x~ + C_p(S_p) + f_p(h)); value and log-probs, in float64 (comm.py:127-129,179-239,
-    models.py:23-36).  Returns h' of every pass too."""
-    w = net._kernel_weights()
-    d = lambda t: t.detach().to("cuda", torch.float64)
-    cfg = net.policy_cfg(B)
-    N, P = net.nagents, passes or max(1, int(cfg.passes))
-    xt = torch.tanh(x.double())
-    h, hs = xt, []
-    g, den = gates_f64(B, N, comm, alive, fresh, bool(cfg.hard_attn), bool(cfg.comm_avg))
-    for p in range(P):
-        cw, cb = d(w["c_w"][min(p, len(w["c_w"]) - 1)]), d(w["c_b"][min(p, len(w["c_b"]) - 1)])
-        z = xt + cb + h @ d(w["f_w"][p]).t() + d(w["f_b"][p])
-        if not cfg.comm_mask_zero:
-            z = z + (gated_mean(h.view(B, N, -1), g, den).reshape(B * N, -1) @ cw.t())
-        h = torch.tanh(z)
-        hs.append(h)
-    logp = torch.cat([torch.log_softmax(h @ d(hw).t() + d(hb), -1) for hw, hb in zip(w["head_w"], w["head_b"])], -1)
-    return dict(h=h, value=(h @ d(w["value_w"]).t() + d(w["value_b"]))[:, 0], logp=logp), hs
+def compare(label, got, ref, worst=None, tol=ROW_TOL):
+    compare_rows(label, got, ref, worst, tol)
 
 
 # ---------------------------------------------------------------------------------------------------- direct steps
-
-def ff_net(N, heads, impl, family="ic3net", passes=1, share=False, mode="avg", wseed=3, H=128, O=61):
-    from ic3net_b200 import models
-    from ic3net_b200.comm import CommNetMLP
-    a = argparse.Namespace(nagents=N, hid_size=H, comm_passes=passes, recurrent=False, rnn_type="MLP", continuous=False,
-                           naction_heads=list(heads), comm_mask_zero=False, comm_mode=mode,
-                           hard_attn=family == "ic3net", comm_init="uniform", share_weights=share, seed=0, env_id0=0,
-                           commnet=family != "mlp", policy_impl=impl)
-    torch.manual_seed(wseed)
-    return (models.MLP if family == "mlp" else CommNetMLP)(a, O)
-
 
 def twin_nets(N, heads, family="ic3net", wseed=3, **kw):
     tc, simt = ff_net(N, heads, "tc_ff", family, wseed=wseed, **kw), ff_net(N, heads, "simt", family, wseed=wseed, **kw)
@@ -141,25 +65,6 @@ def outputs(R, heads, extra=0):
     nan = lambda *s: torch.full(s, 0x7FC0DEAD, dtype=torch.int32, device="cuda").view(torch.float32)
     return dict(h=nan(R + extra, 128), value=nan(R + extra), logp=nan(R + extra, sum(heads)),
                 action=torch.full((R + extra, len(heads)), -7, dtype=torch.int32, device="cuda"))
-
-
-def direct_step(net, x, B, out, comm=None, alive=None, fresh=None, draws=None, passes=None):
-    """ic3_policy_step as the trainer calls it (the policy's packed weights and workspace), into the caller's buffers;
-    returns the device flag word."""
-    from ic3net_b200 import _lib
-    lib = _lib.load()
-    cfg, w = net.policy_cfg(B), net.packed()
-    if passes is not None:
-        cfg.passes = passes
-    ws, _ = net.workspace(B)
-    err = torch.zeros(1, dtype=torch.int32, device="cuda")
-    io = _lib.PolicyIO(x=x.data_ptr(), h=None, c=None, comm_action=_lib.ptr(comm), alive=_lib.ptr(alive),
-                       fresh=_lib.ptr(fresh), tick=None, draws=_lib.ptr(draws), h_out=out["h"].data_ptr(), c_out=None,
-                       value=out["value"].data_ptr(), logp=out["logp"].data_ptr(), action=_lib.ptr(out.get("action")),
-                       workspace=_lib.ptr(ws), err=err.data_ptr())
-    _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), _lib.stream()))
-    torch.cuda.synchronize()
-    return int(err.item())
 
 
 def record_inputs(tr, t):
@@ -197,13 +102,13 @@ def test_full_size_every_row_matches_float64(name, B, family, over):
     assert int(tr._buf["err"].item()) == 0
     b, net = tr._buf, tr.policy_net
     heads = tr.args.naction_heads
-    tol = sum_tol(N) if over.get("comm_mode") == "sum" else TOL
+    tol = sum_tol(N) if over.get("comm_mode") == "sum" else ROW_TOL
     worst, nfresh, ndead = {}, 0, 0
     for t in range(T):
         inp = record_inputs(tr, t)
-        ref, _ = step_f64(net, inp["x"], B, inp["comm"], inp["alive"], inp["fresh"])
+        ref, _ = ff_step_f64(net, inp["x"], B, inp["comm"], inp["alive"], inp["fresh"])
         out = outputs(R, heads)
-        assert direct_step(net, inp["x"], B, out, inp["comm"], inp["alive"], inp["fresh"]) == 0
+        assert ff_direct_step(net, inp["x"], B, out, inp["comm"], inp["alive"], inp["fresh"]) == 0
         compare("%s %s step %d (direct)" % (name, family, t), {k: out[k] for k in ("h", "value", "logp")}, ref, worst, tol)
         compare("%s %s step %d (rollout)" % (name, family, t),
                 dict(value=b["value"][t].reshape(R), logp=b["logp"][t].reshape(R, -1)), ref, worst, tol)
@@ -219,9 +124,8 @@ def test_full_size_every_row_matches_float64(name, B, family, over):
 @pytest.mark.parametrize("name", ["var_mlp", "var_commnet_nonrec2"])
 def test_forward_fixtures_of_the_reference(name):
     """The unmodified reference's forward (its state_dict, inputs, outputs) through policy_impl 'tc_ff'."""
-    from test_gpu_variants import build, close
     meta, z = load_golden(name)
-    a, net = build(meta, z, "tc_ff")
+    a, net = variant_net(meta, z, "tc_ff")
     assert net.policy_impl == "tc_ff"
     B, n = z["obs"].shape[0], a.nagents
     obs = torch.tensor(z["obs"], dtype=torch.float32, device="cuda")
@@ -241,20 +145,19 @@ def test_forward_fixtures_of_the_reference(name):
 def test_hid_size_32_fixture_is_refused():
     """var_commnet_nonrec_share is a hid_size 32 policy: outside the kernel, so 'tc_ff' refuses it (its forward stays on
     'simt', tests/test_gpu_variants.py)."""
-    from test_gpu_variants import build
     meta, z = load_golden("var_commnet_nonrec_share")
     assert meta["args"]["hid_size"] != 128
     with pytest.raises(NotImplementedError):
-        build(meta, z, "tc_ff")
+        variant_net(meta, z, "tc_ff")
 
 
 @pytest.mark.parametrize("name", golden_names("gradff_"))
-def test_gradient_fixtures_of_the_reference(name, tc_ff_trainers):
+def test_gradient_fixtures_of_the_reference(name):
     """kernels_ff with the tc_ff forward: the pinned float64 oracle on 5 and 13 slots, and one slot against the
     reference's stored gradient arrays."""
-    gf.test_kernels_match_reference_pinned_oracle(name, 5)
-    gf.test_kernels_match_reference_pinned_oracle(name, 13)
-    gf.test_kernels_match_reference_gradient_arrays(name)
+    ff_pinned_oracle(name, 5, "tc_ff")
+    ff_pinned_oracle(name, 13, "tc_ff")
+    ff_gradient_arrays(name, "tc_ff")
 
 
 # ---------------------------------------------------------------------------------------------------- 3. re-run
@@ -283,7 +186,7 @@ def test_rerun_equals_rollout_step(name, family, over):
                                         _lib.stream()))
     for p in range(1, P + 1):
         out = outputs(R, tr.args.naction_heads)
-        assert direct_step(net, inp["x"], B, out, inp["comm"], inp["alive"], inp["fresh"], passes=p) == 0
+        assert ff_direct_step(net, inp["x"], B, out, inp["comm"], inp["alive"], inp["fresh"], passes=p) == 0
         assert torch.equal(st_h[p], out["h"]), p
     assert torch.allclose(st_h[0], torch.tanh(inp["x"]), rtol=0, atol=1e-6)
     g, den = gates_f64(B, N, inp["comm"], inp["alive"], inp["fresh"], bool(cfg.hard_attn), bool(cfg.comm_avg))
@@ -304,18 +207,18 @@ GRAD_FULL = [(n, fam, dict(comm_passes=p, share_weights=s)) for n in (PP, TJ)
 
 
 @pytest.mark.parametrize("name,family,over", GRAD_FULL + [(PP, "mlp", {})])
-def test_full_size_gradient_matches_float64(name, family, over, tc_ff_trainers):
-    gf.test_full_size_gradient_matches_float64(name, family, over)
+def test_full_size_gradient_matches_float64(name, family, over):
+    ff_full_size(name, family, over, "tc_ff")
 
 
-def test_gradient_is_bit_identical_run_to_run(tc_ff_trainers):
-    gf.test_chunk_sizes_and_determinism("ic3net", dict(comm_passes=2))
-    gf.test_chunk_sizes_and_determinism("mlp", {})
+def test_gradient_is_bit_identical_run_to_run():
+    ff_chunk_sizes_and_determinism("ic3net", dict(comm_passes=2), "tc_ff")
+    ff_chunk_sizes_and_determinism("mlp", {}, "tc_ff")
 
 
 @pytest.mark.parametrize("name,family,over", [(PP, "ic3net", dict(comm_passes=2)), (TJ, "commnet", dict(comm_passes=2))])
-def test_halted_slots_contribute_nothing(name, family, over, tc_ff_trainers):
-    gf.test_halted_slots_contribute_nothing(name, family, over)
+def test_halted_slots_contribute_nothing(name, family, over):
+    ff_halted_slots_contribute_nothing(name, family, over, "tc_ff")
 
 
 # ---------------------------------------------------------------------------------------------------- 5. row counts
@@ -337,13 +240,13 @@ def test_row_counts_and_rows_past_R(case, family, per_sm):
     before = [t.clone() for t in (x, comm, alive, fresh)]
     out = outputs(R, heads, extra)
     pristine = {k: v.clone() for k, v in out.items()}
-    assert direct_step(net, x, R, out, comm, alive, fresh, draws=torch.zeros(R, 2, dtype=torch.int32, device="cuda")) == 0
+    assert ff_direct_step(net, x, R, out, comm, alive, fresh, draws=torch.zeros(R, 2, dtype=torch.int32, device="cuda")) == 0
     bits = lambda t: t.view(torch.int32) if t.dtype == torch.float32 else t
     for k, v in out.items():
         assert torch.equal(bits(v[R:]), bits(pristine[k][R:])), (case, k)
     for a, b in zip((x, comm, alive, fresh), before):
         assert torch.equal(a, b)
-    ref, _ = step_f64(net, x, R, comm, alive, fresh)
+    ref, _ = ff_step_f64(net, x, R, comm, alive, fresh)
     compare("%s %s R=%d" % (family, case, R), {k: out[k][:R] for k in ("h", "value", "logp")}, ref)
 
 
@@ -357,12 +260,12 @@ def test_agents_per_env(N, family, passes, mode):
     net = ff_net(N, heads, "tc_ff", family, passes=passes, mode=mode, wseed=N)
     x, comm, alive, fresh = inputs(B, N, seed=N)
     out = outputs(R, heads, extra)
-    assert direct_step(net, x, B, out, comm, alive, fresh) == 0
+    assert ff_direct_step(net, x, B, out, comm, alive, fresh) == 0
     assert torch.isnan(out["h"][R:]).all() and bool((out["action"][R:] == -7).all())
-    ref, _ = step_f64(net, x, B, comm, alive, fresh)
+    ref, _ = ff_step_f64(net, x, B, comm, alive, fresh)
     worst = {}
     compare("%s N=%d" % (family, N), {k: out[k][:R] for k in ("h", "value", "logp")}, ref, worst,
-            sum_tol(N) if mode == "sum" else TOL)
+            sum_tol(N) if mode == "sum" else ROW_TOL)
     print("%s %d passes %s N=%d: %s" % (family, passes, mode, N, " ".join("%s %.2e" % kv for kv in worst.items())))
 
 
@@ -383,7 +286,7 @@ def test_sampling_with_explicit_draws(heads, family):
     rows = np.arange(R)
     u24[rows % 8 == 0] = 0
     u24[rows % 8 == 1] = (1 << 24) - 1
-    ref, _ = step_f64(tc, x, B, comm, alive, fresh)
+    ref, _ = ff_step_f64(tc, x, B, comm, alive, fresh)
     off = 0
     for k, na in enumerate(heads):
         cdf = np.cumsum(np.exp(ref["logp"][:, off:off + na].cpu().numpy()), -1)
@@ -393,8 +296,8 @@ def test_sampling_with_explicit_draws(heads, family):
         off += na
     draws = torch.as_tensor(u24.astype(np.int32), device="cuda").contiguous()
     o_tc, o_simt = outputs(R, heads), outputs(R, heads)
-    assert direct_step(tc, x, B, o_tc, comm, alive, fresh, draws=draws) == 0
-    assert direct_step(simt, x, B, o_simt, comm, alive, fresh, draws=draws) == 0
+    assert ff_direct_step(tc, x, B, o_tc, comm, alive, fresh, draws=draws) == 0
+    assert ff_direct_step(simt, x, B, o_simt, comm, alive, fresh, draws=draws) == 0
     compare("heads %s" % (heads,), {k: o_tc[k] for k in ("h", "value", "logp")}, ref)
     a_tc, a_simt = o_tc["action"].cpu().numpy(), o_simt["action"].cpu().numpy()
     off = 0
@@ -422,10 +325,10 @@ def test_weight_limit_of_the_fp16_split(which):
         with torch.no_grad():
             (net.f_modules[1] if which == "f" else net.C_modules[1]).weight[3, 7] = entry
         out = outputs(B * N, heads)
-        flags = direct_step(net, x, B, out, comm, alive, fresh)
+        flags = ff_direct_step(net, x, B, out, comm, alive, fresh)
         if ok:
             assert flags == 0
-            ref, _ = step_f64(net, x, B, comm, alive, fresh)
+            ref, _ = ff_step_f64(net, x, B, comm, alive, fresh)
             compare("|w| 255", {k: out[k] for k in ("h", "value", "logp")}, ref)
         else:
             assert flags == 0x200
@@ -441,9 +344,9 @@ def test_largest_sum_mode_communication_stays_in_range():
             m.weight.mul_(0.01)
     x = torch.full((B * N, 128), 6.0, device="cuda")
     out = outputs(B * N, heads)
-    assert direct_step(net, x, B, out) == 0
+    assert ff_direct_step(net, x, B, out) == 0
     assert float(torch.tanh(x.double()).min()) * (N - 1) > 30.9
-    ref, _ = step_f64(net, x, B)
+    ref, _ = ff_step_f64(net, x, B)
     compare("sum S = 31", {k: out[k] for k in ("h", "value", "logp")}, ref, tol=sum_tol(N))
 
 
@@ -469,9 +372,9 @@ def test_autograd_gradient_with_tc_ff_rollout(family):
     with kernels_ff on the same rollout."""
     ka = make_trainer(PP, 48, family, comm_passes=2 if family != "mlp" else 1)
     au = make_trainer(PP, 48, family, grad_impl="autograd", comm_passes=2 if family != "mlp" else 1)
-    gk, sk = gf.rollout_and_grad(ka)
-    ga, sa = gf.rollout_and_grad(au)
-    gf.assert_close(gk, sk, ga, sa)
+    gk, sk = rollout_and_grad(ka)
+    ga, sa = rollout_and_grad(au)
+    assert_close(gk, sk, ga, sa)
     assert int(ka._buf["err"].item()) == 0 and int(au._buf["err"].item()) == 0
 
 

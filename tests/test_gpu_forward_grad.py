@@ -19,153 +19,11 @@ import pytest
 import torch
 
 from bptt_ref import heads_abs_sums, returns_and_advantages
-from test_gpu_bptt_passes import make_trainer as lstm_trainer
-from test_gpu_bptt_rnn import make_trainer as rnn_trainer
-
-TOL = 1e-4
-COL_FLOOR = 1e-6
-SUM_FLOOR = 2.0 ** -20
-OPT_IN = dict(obs_api="handle", forward_grad="kernels")
+from gpu_harness import OPT_IN, assert_within_bar as within_bar, handle, one_step, passes_trainer, rnn_trainer, set_state
 
 
-def handle(tr):
-    from ic3net_b200.lazy_obs import LazyObs
-    e = tr.env.env
-    return LazyObs(e, (e.nenvs, tr.args.nagents, tr.env.observation_dim))
-
-
-def set_state(tr, t):
-    """Put the env state the records hold for step t back into the live env (a handle then describes step t)."""
-    e, b = tr.env.env, tr._buf
-    for key, attr, _, _ in tr._records:
-        getattr(e, attr).copy_(b[key][t])
-    e.obs_version += 1
-
-
-def within_bar(got, ref, sums, label):
-    """{name: error on the 1e-4 scale}; asserts every entry <= 1e-4."""
-    errs = {}
-    for k, r in ref.items():
-        g = got[k].double()
-        m = float(r.abs().max())
-        if m == 0.0:
-            assert float(g.abs().max()) == 0.0, (label, k)
-            continue
-        allowed = TOL * m + (SUM_FLOOR * sums[k] if k in sums else 0.0)
-        errs[k] = float(((g - r).abs() / allowed).max()) * TOL
-        if r.dim() == 2 and k.endswith(("encoder.weight", "affine1.weight")):
-            allowed = TOL * r.abs().amax(0) + COL_FLOOR * m
-            errs[k + "[cols]"] = float(((g - r).abs().amax(0) / allowed).max()) * TOL
-    worst = max(errs, key=errs.get)
-    print("%s: worst %s %.2e | %s" % (label, worst, errs[worst], " ".join("%s %.1e" % kv for kv in errs.items())))
-    bad = {k: v for k, v in errs.items() if not v <= TOL}
-    assert not bad, (label, bad)
-    return errs
-
-
-class _Roles(object):
-    """Stand-in module for trainer.policy_forward_torch: the policy's kernel-side weights as float64 leaves."""
-
-    def __init__(self, net):
-        self._cfg_proto = net._cfg_proto
-        self.leaf = {}
-        self.w = {k: ([self._conv(t) for t in v] if isinstance(v, list) else self._conv(v))
-                  for k, v in net._kernel_weights().items()}
-
-    def _conv(self, t):
-        if id(t) not in self.leaf:
-            self.leaf[id(t)] = t.detach().double().requires_grad_(isinstance(t, torch.nn.Parameter))
-        return self.leaf[id(t)]
-
-    def _kernel_weights(self):
-        return self.w
-
-
-def encode64(tr, roles, w):
-    """x = encoder(obs) in float64 from the live env state."""
-    e = tr.env.env
-    R = e.nenvs * tr.args.nagents
-    if tr.is_tj:
-        obs = e._get_obs().reshape(R, -1).double()
-        return obs @ w["enc_w"].t() + w["enc_b"]
-    idx, val = tr._pp_sparse_obs(e.loc)
-    return (w["enc_w"].t()[idx] * val.double().unsqueeze(-1)).sum(1) + w["enc_b"]
-
-
-def one_step(tr, t, seed=0, scale=1.0, spike=None):
-    """forward + backward of step t of the trainer's records (env state, (h, c), masks) under random upstream gradients
-    times ``scale``; ``spike = (key, v)`` sets the last entry (last row, last column) of upstream gradient ``key``
-    ('dh', 'dc', 'dvalue' or 'dlogp') to v.  Returns (kernel gradients by name + 'h' / 'c', float64 gradients, |terms|
-    sums of the action heads)."""
-    from ic3net_b200.trainer import policy_forward_torch
-    net, args, e, b = tr.policy_net, tr.args, tr.env.env, tr._buf
-    B, N, H = e.nenvs, args.nagents, args.hid_size
-    R = B * N
-    lstm = net._cfg_proto["cell"] == 0
-    hard = bool(args.hard_attn) and bool(args.commnet)
-    set_state(tr, t)
-    h = b["rec_h"][t].clone().requires_grad_(True)
-    c = b["rec_c"][t].clone().requires_grad_(True) if lstm else None
-    comm, alive = b["s_comm"][t].clone(), b["s_alive"][t].clone()
-    info = dict(alive_mask=alive)
-    if hard:
-        info["comm_action"] = comm
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    rnd = lambda *s: torch.randn(*s, device="cuda", generator=g)
-    net.zero_grad(set_to_none=True)
-    action, value, hid = net([handle(tr), (h, c) if lstm else h], info)
-    h2, c2 = hid if lstm else (hid, None)
-    assert value.grad_fn is not None and h2.grad_fn is not None and all(a.grad_fn is not None for a in action)
-    logp = torch.cat(action, -1).reshape(R, -1)
-    up = dict(dlogp=rnd(R, logp.shape[1]) * scale, dvalue=rnd(R) * scale, dh=rnd(R, H) * (0.1 * scale),
-              dc=rnd(R, H) * (0.1 * scale))
-    if spike is not None:
-        up[spike[0]].view(-1)[-1] = spike[1]
-    loss = (logp * up["dlogp"]).sum() + (value.reshape(R) * up["dvalue"]).sum() + (h2 * up["dh"]).sum()
-    if lstm:
-        loss = loss + (c2 * up["dc"]).sum()
-    loss.backward()
-    got = {n: p.grad.detach().clone() for n, p in net.named_parameters() if p.grad is not None}
-    got["h"] = h.grad.detach().clone()
-    if lstm:
-        got["c"] = c.grad.detach().clone()
-    # float64 autograd of the same step
-    roles = _Roles(net)
-    w = roles.w
-    h64 = b["rec_h"][t].double().requires_grad_(True)
-    c64 = b["rec_c"][t].double().requires_grad_(True) if lstm else None
-    x = encode64(tr, roles, w)
-    a64 = alive.double()
-    n_alive = a64.sum(1, keepdim=True)
-    gate = a64 * comm.double() if hard else a64
-    hh, cc, v64, lps = policy_forward_torch(roles, x, h64, c64, gate, n_alive)
-    lp64 = torch.cat(lps, -1)
-    L = ((lp64 * up["dlogp"].double()).sum() + (v64.reshape(R) * up["dvalue"].double()).sum()
-         + (hh * up["dh"].double()).sum())
-    if lstm:
-        L = L + (cc * up["dc"].double()).sum()
-    names = {id(p): n for n, p in net.named_parameters()}
-    leaves = [(names[i], t) for i, t in roles.leaf.items() if i in names]
-    inputs = [h64] + ([c64] if lstm else []) + [t for _, t in leaves]
-    out = torch.autograd.grad(L, inputs)
-    ref = {"h": out[0]}
-    if lstm:
-        ref["c"] = out[1]
-    for (n, _), gr in zip(leaves, out[len(inputs) - len(leaves):]):
-        ref[n] = gr
-    # |terms| of the action heads' gradients: |d logit|^T |h'|
-    sums, off = {}, 0
-    dl = up["dlogp"].double()
-    for m, na in enumerate(args.naction_heads):
-        lpm = lp64[:, off:off + na].detach()
-        d = dl[:, off:off + na]
-        dlogit = (d - lpm.exp() * d.sum(1, keepdim=True)).abs()
-        pre = [k for k in ref if k.endswith("heads.%d.weight" % m)][0][:-len("weight")]
-        sums[pre + "weight"] = dlogit.t() @ hh.detach().abs()
-        sums[pre + "bias"] = dlogit.sum(0)
-        off += na
-    assert int(b["err"].item()) == 0
-    return got, ref, sums
+def lstm_trainer(name, B, passes, share, **over):
+    return passes_trainer(name, B, comm_passes=passes, share_weights=share, **over)
 
 
 LSTM_STEP = [

@@ -14,46 +14,19 @@ import numpy as np
 import pytest
 import torch
 
+from gpu_harness import UPDATE_FF, UPDATE_IC, UPDATES, same_stat, update_trainer
 from helpers import finish_args, load_golden, ns
 
 pytestmark = pytest.mark.gpu
 
 PP, TJ = "grad_pp_hard_ic3net_h128", "grad_tj_hard_ic3net_h128"
-K = 3
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def make_trainer(name, B, graph, model="commnet", windows=False, ff_chunk=None, **over):
-    from ic3net_b200 import data, models
-    from ic3net_b200.comm import CommNetMLP
-    from ic3net_b200.trainer import Trainer
-    meta, _ = load_golden(name)
-    kw = dict(nenvs=B, seed=808, env_id0=30, obs_mode="index", use_graph=False, policy_impl="tc",
-              record_for_grad=True, grad_impl="kernels", graph_update=graph, lrate=1e-3)
-    kw.update(over)
-    args = ns(meta["args"], **kw)
-    env = data.init(args.env_name, args)
-    finish_args(args, env)
-    torch.manual_seed(meta["weights_seed"])
-    net = {"rnn": models.RNN, "mlp": models.MLP, "commnet": CommNetMLP}[model](args, args.num_inputs)
-    tr = Trainer(args, net, env)
-    if windows:
-        tr.RECORD_BYTES_LIMIT = 0
-    if ff_chunk is not None:
-        tr.FF_CHUNK_STEPS = ff_chunk
-    return tr
-
-
-def same_stat(a, b):
-    assert sorted(a) == sorted(b)
-    for k in a:
-        assert np.array_equal(np.asarray(a[k]), np.asarray(b[k])), k
-
-
 def train_both(name, B, epochs=None, **over):
-    """(eager trainer, graph trainer) after K updates each, asserting identical stat dicts along the way."""
-    eager, graph = make_trainer(name, B, False, **over), make_trainer(name, B, True, **over)
-    for ep in (epochs or range(K)):
+    """(eager trainer, graph trainer) after UPDATES updates each, asserting identical stat dicts along the way."""
+    eager, graph = update_trainer(name, B, False, **over), update_trainer(name, B, True, **over)
+    for ep in (epochs or range(UPDATES)):
         same_stat(eager.train_batch(ep), graph.train_batch(ep))
     return eager, graph
 
@@ -63,7 +36,7 @@ def assert_same_state(eager, graph):
     assert torch.equal(oe.flat_params, og.flat_params)
     assert torch.equal(oe.flat_square_avg, og.flat_square_avg)
     assert torch.equal(oe.flat_grads, og.flat_grads)
-    assert oe.steps == og.steps == K
+    assert oe.steps == og.steps == UPDATES
 
 
 def reference_update(tr, epoch):
@@ -79,19 +52,15 @@ def reference_update(tr, epoch):
     return stat
 
 
-IC = dict(model="rnn", commnet=False, hard_attn=False, recurrent=True, rnn_type="MLP", policy_impl="tc_tanh",
-          comm_passes=1, share_weights=False)
-FF = dict(grad_impl="kernels_ff", ic3net=False, recurrent=False, rnn_type="MLP", policy_impl="tc_ff", ff_chunk=7,
-          entr=0.01)
 CASES = {
     "ic3net_full": dict(),
     "ic3net_windows": dict(windows=True),
     "ic3net_passes2_shared": dict(comm_passes=2, share_weights=True),
     "ic3net_no_cuts": dict(detach_gap=10000),
-    "ic_tanh_full": dict(IC),
-    "ic_tanh_windows": dict(IC, windows=True),
-    "mlp_ff": dict(FF, model="mlp", commnet=False, hard_attn=False),
-    "ic3net_ff_passes2": dict(FF, model="commnet", commnet=1, hard_attn=1, comm_passes=2, share_weights=False),
+    "ic_tanh_full": dict(UPDATE_IC),
+    "ic_tanh_windows": dict(UPDATE_IC, windows=True),
+    "mlp_ff": dict(UPDATE_FF, model="mlp", commnet=False, hard_attn=False),
+    "ic3net_ff_passes2": dict(UPDATE_FF, model="commnet", commnet=1, hard_attn=1, comm_passes=2, share_weights=False),
 }
 
 
@@ -107,23 +76,23 @@ def test_graph_update_is_bit_identical(case):
 
 @pytest.mark.parametrize("case", sorted(CASES) + ["autograd"])
 def test_update_equals_the_reference_sequence(case):
-    """K updates of train_batch, eager and (where it is allowed) with graph_update, equal K updates of the reference's
-    call sequence bit for bit: parameters, second moments, gradients and stat dicts."""
+    """UPDATES updates of train_batch, eager and (where it is allowed) with graph_update, equal as many updates of the
+    reference's call sequence bit for bit: parameters, second moments, gradients and stat dicts."""
     over = dict(CASES.get(case, dict(grad_impl="autograd")))
-    ref = make_trainer(PP, 37, False, **over)
-    want = [reference_update(ref, ep) for ep in range(K)]
+    ref = update_trainer(PP, 37, False, **over)
+    want = [reference_update(ref, ep) for ep in range(UPDATES)]
     for graph in (False, True) if case in CASES else (False,):
-        tr = make_trainer(PP, 37, graph, **over)
-        for ep in range(K):
+        tr = update_trainer(PP, 37, graph, **over)
+        for ep in range(UPDATES):
             same_stat(want[ep], tr.train_batch(ep))
         assert_same_state(ref, tr)
 
 
 def test_random_update_equals_the_reference_sequence():
-    from test_gpu_random import make_trainer as make_random, random_args
+    from gpu_harness import random_args, random_trainer as make_random
     ref, tr = (make_random(random_args("c2", nenvs=64, batch_size=100))[1] for _ in range(2))
     p0 = tr.optimizer.flat_params.clone()
-    for ep in range(K):
+    for ep in range(UPDATES):
         same_stat(reference_update(ref, ep), tr.train_batch(ep))
     for t in (ref, tr):
         assert torch.equal(t.optimizer.flat_params, p0)
@@ -135,8 +104,8 @@ def test_use_graph_update_replays_the_rollout_graph():
     """use_graph without graph_update: the update's rollout is replayed from the 'rollout' CUDA graph -- its kernels are
     enqueued only by the warm-up and the capture of the first update -- and every update equals that of a trainer
     without use_graph bit for bit; BPTT kernels and models.Random."""
-    from test_gpu_random import make_trainer as make_random, random_args
-    pairs = [(make_trainer(PP, 37, False), make_trainer(PP, 37, False, use_graph=True)),
+    from gpu_harness import random_args, random_trainer as make_random
+    pairs = [(update_trainer(PP, 37, False), update_trainer(PP, 37, False, use_graph=True)),
              tuple(make_random(random_args("c2", nenvs=64, batch_size=100, use_graph=g))[1] for g in (False, True))]
     for plain, replayed in pairs:
         enqueue, calls = replayed._enqueue, []
@@ -146,7 +115,7 @@ def test_use_graph_update_replays_the_rollout_graph():
             return enqueue(*args)
 
         replayed._enqueue = counted
-        for ep in range(K):
+        for ep in range(UPDATES):
             same_stat(plain.train_batch(ep), replayed.train_batch(ep))
         assert len(calls) == 2 and "rollout" in replayed._graphs
         for key in ("action", "logp", "value", "reward"):
@@ -157,7 +126,7 @@ def test_use_graph_update_replays_the_rollout_graph():
             assert torch.equal(a, b)
 
 
-BEGIN_CASES = {"full": dict(), "windows": dict(windows=True), "passes3": dict(comm_passes=3), "tanh": dict(IC)}
+BEGIN_CASES = {"full": dict(), "windows": dict(windows=True), "passes3": dict(comm_passes=3), "tanh": dict(UPDATE_IC)}
 
 
 @pytest.mark.parametrize("case", sorted(BEGIN_CASES))
@@ -166,7 +135,7 @@ def test_device_begin_leaves_the_workspace_of_the_host_begin(case):
     form.  On one plan, from a zeroed workspace each, the two leave the same bytes: full records (rec_c[1:]), window
     records (the rollout's per-step maxima), three comm passes (the bound grows by P - 1) and the tanh RNN (no c)."""
     from ic3net_b200 import _lib
-    tr = make_trainer(PP, 37, False, **BEGIN_CASES[case])
+    tr = update_trainer(PP, 37, False, **BEGIN_CASES[case])
     tr.run_batch(0)
     b, lib, s = tr._buf, _lib.load(), _lib.stream()
     hc = not tr._h_only_records()
@@ -191,8 +160,8 @@ def test_traffic_junction_curriculum_recaptures_exactly_on_a_step():
     # add_rate moves at epochs 1 and 2 (curr_start 0, curr_end 4, step 0.05): spawn_thr changes, the graph re-captures;
     # the repeated epochs move nothing and must replay the graph they have
     over = dict(normalize_rewards=True, add_rate_min=0.1, add_rate_max=0.3, curr_start=0, curr_end=4)
-    eager = make_trainer(TJ, 24, False, **over)
-    graph = make_trainer(TJ, 24, True, **over)
+    eager = update_trainer(TJ, 24, False, **over)
+    graph = update_trainer(TJ, 24, True, **over)
     captures, thr = [], []
     for ep in (0, 0, 1, 1, 2):
         same_stat(eager.train_batch(ep), graph.train_batch(ep))
@@ -208,7 +177,7 @@ def test_traffic_junction_curriculum_recaptures_exactly_on_a_step():
 
 
 def test_packed_weights_stay_current_after_a_replay():
-    tr = make_trainer(PP, 8, True)
+    tr = update_trainer(PP, 8, True)
     tr.train_batch(0)
     net = tr.policy_net
     key = net._packed_key
@@ -224,7 +193,7 @@ def test_fp16_range_flag_raises_after_the_replay():
     """Weights outside the fp16 split range: the same RuntimeError as the eager update, from the statistics vector read
     after the replay (an error word, not a device fault), and the update leaves the parameters as they were."""
     for graph in (False, True):
-        tr = make_trainer(PP, 4, graph)
+        tr = update_trainer(PP, 4, graph)
         with torch.no_grad():
             tr.policy_net.f_module.weight_hh.mul_(4000.0)
         before = tr.optimizer.flat_params.clone()
@@ -238,7 +207,7 @@ def test_flag_set_during_the_gradient_raises():
     op the capture holds) stops the step and raises, eager and replayed; the parameters and second moments stay."""
     from ic3net_b200 import _lib
     for graph in (False, True):
-        tr = make_trainer(PP, 4, graph)
+        tr = update_trainer(PP, 4, graph)
         losses = tr._losses_device
 
         def flagged(*args, tr=tr, losses=losses):
@@ -259,9 +228,9 @@ def test_refusals():
     from ic3net_b200 import data, models
     from ic3net_b200.trainer import Trainer
     with pytest.raises(NotImplementedError, match="autograd"):
-        make_trainer(PP, 4, True, grad_impl="autograd")
+        update_trainer(PP, 4, True, grad_impl="autograd")
     with pytest.raises(NotImplementedError, match="forward_grad"):
-        make_trainer(PP, 4, True, forward_grad="kernels")
+        update_trainer(PP, 4, True, forward_grad="kernels")
     meta, _ = load_golden(PP)
     args = ns(meta["args"], nenvs=4, seed=1, env_id0=0, obs_mode="index", use_graph=False, recurrent=False,
               random=True, graph_update=True, lrate=1e-3)

@@ -9,8 +9,7 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import finish_args, load_golden, ns
-from oracle.gen_golden import make_weights
+from gpu_harness import fixture_trainer
 
 pytestmark = pytest.mark.gpu
 
@@ -18,19 +17,11 @@ BIG_QUOTA = 1 << 30          # no slot halts: every call of _enqueue(1) is one m
 
 
 def build(name, B, seed=13, **over):
-    from ic3net_b200 import data
-    from ic3net_b200.comm import CommNetMLP
-    from ic3net_b200.trainer import Trainer
-    meta, _ = load_golden(name)
-    args = ns(meta["args"], nenvs=B, seed=seed, env_id0=0, obs_mode="dense", policy_impl=None, **over)
-    env = data.init(args.env_name, args)
-    finish_args(args, env)
-    net = CommNetMLP(args, args.num_inputs)
-    sd = make_weights(meta["weights_seed"], args.num_inputs, args.hid_size, args.naction_heads, args.comm_init)
-    net.load_state_dict({k: torch.from_numpy(v).float() for k, v in sd.items()})
-    tr = Trainer(args, net, env)
+    """(args, env, Trainer) on dense observations, the fixture's weights, the two-stream path at any size."""
+    tr = fixture_trainer(name, B, seed, 0, obs_mode="dense", policy_impl=None, record_for_grad=False,
+                         weights="fixture", **over)
     tr.OVERLAP_MIN_OBS_BYTES = 0             # the small fixtures take the two-stream path too
-    return args, env, tr
+    return tr.args, tr.env, tr
 
 
 CASES = [pytest.param("ep_pp_hard_ic3net", 24, 6, id="pp_hard"),

@@ -7,23 +7,12 @@ import numpy as np
 import pytest
 import torch
 
+from gpu_harness import close, cpu
 from helpers import finish_args, golden_names, load_golden, make_oracle_env, ns, tj_tables
 from oracle import policy as opolicy
 from oracle.gen_golden import make_weights
 
 pytestmark = pytest.mark.gpu
-
-TOL = 1e-5
-
-
-def close(a, b, tol=TOL):
-    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
-    return np.all(np.abs(a - b) <= tol * np.maximum(1.0, np.abs(b)))
-
-
-def cpu(t):
-    return t.detach().cpu().numpy()
-
 
 IMPLS = ["tc", "simt"]
 

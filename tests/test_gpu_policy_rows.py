@@ -10,121 +10,26 @@ explicit draws; the rows past R; and both sides of the fp16 operand-split limits
 
 Bar: |gpu - ref| <= 1e-5 * max(1, |ref|) on h', c', value and log-probs (DESIGN.md section 2).  A failure names the worst
 element's row, 128-row tile, warpgroup, column half, work item and CTA of lstm_tc_kernel."""
-import argparse
-import ctypes as C
-
 import numpy as np
 import pytest
 import torch
 
-from bptt_ref import tj_record_obs
-from helpers import finish_args, load_golden, ns
-from oracle import philox
-from oracle.gen_golden import make_weights
-from policy_ref import inverse_cdf, params_f64, philox_u24, step_f64
+from gpu_harness import (MARGIN, TC_TILE, TC_TILE_PAD, compare_rows, lstm_direct_step, lstm_outputs, make_lstm_net,
+                         params_f64, ref_dict, rows_trainer, sms, step_f64, synthetic, tc_geometry, tc_where,
+                         trainer_rows)
+from helpers import load_golden
+from policy_ref import inverse_cdf
 
 pytestmark = pytest.mark.gpu
 
-TOL = 1e-5
-MARGIN = 1e-5               # draws closer than this to a CDF edge may flip between fp32 and float64
-TILE, TILE_PAD = 128, 8     # rows per tile; tiles are padded to a multiple of 8 (csrc/policy_tc.cu)
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def geometry(R):
-    """(tiles, padded tiles, work items, CTAs) of lstm_tc_kernel for R rows: one item per (tile, 64-unit column half),
-    a persistent grid of min(items, SMs) CTAs (one resident CTA per SM)."""
-    nt = -(-R // TILE)
-    ntp = -(-nt // TILE_PAD) * TILE_PAD
-    return nt, ntp, 2 * ntp, min(2 * ntp, sms())
-
-
-def rel_err(got, ref):
-    got, ref = got.to(torch.float64), ref.to(torch.float64)
-    return ((got - ref).abs() / ref.abs().clamp_min(1.0)).reshape(ref.shape[0], -1)
-
-
-def where(err, R, unit_cols):
-    """Where the worst element of err [R, W] sits in the kernel's work decomposition."""
-    r, col = divmod(int(err.argmax()), err.shape[1])
-    _, _, items, grid = geometry(R)
-    tile, wg = r // TILE, (r % TILE) // 64
-    if unit_cols:            # h', c': hidden unit `col` belongs to the column half col // 64
-        half = col // 64
-        item = 2 * tile + half
-        return "row %d col %d: tile %d, warpgroup %d, column half %d, item %d, CTA %d (of %d, %d items)" % (
-            r, col, tile, wg, half, item, item % grid, grid, items)
-    return "row %d col %d: tile %d, warpgroup %d, items %d/%d, CTAs %d/%d (of %d)" % (
-        r, col, tile, wg, 2 * tile, 2 * tile + 1, (2 * tile) % grid, (2 * tile + 1) % grid, grid)
-
 
 def compare(label, got, ref, worst=None):
-    """got / ref: dicts of h, c [R, H], value [R], logp [R, A] (h, c may be absent from got).  Asserts the bar;
-    returns {output: max error}."""
-    errs, msgs = {}, []
-    R = ref["value"].shape[0]
-    for k in ("h", "c", "value", "logp"):
-        if k not in got:
-            continue
-        e = rel_err(got[k].reshape(R, -1), ref[k].reshape(R, -1))
-        errs[k] = float(e.max())
-        if worst is not None:
-            worst[k] = max(worst.get(k, 0.0), errs[k])
-        if not errs[k] <= TOL:
-            nbad = int((e > TOL).any(1).sum())
-            msgs.append("%s: %s max %.3e at %s; %d rows over the bar" % (label, k, errs[k], where(e, R, k in "hc"),
-                                                                      nbad))
-    assert not msgs, "\n".join(msgs)
-    return errs
+    """Every row of got against ref at the bar, a failure named in lstm_tc_kernel's work decomposition."""
+    return compare_rows(label, got, ref, worst, where=tc_where(ref["value"].shape[0]))
 
-
-def ref_dict(h, c, value, logps):
-    return dict(h=h, c=c, value=value, logp=torch.cat(logps, -1))
 
 
 # ---------------------------------------------------------------------------------------------------- policies
-
-def policy_args(N, heads, hard_attn=True, comm_mode="avg", comm_mask_zero=False, passes=1, share=False, impl="tc"):
-    return argparse.Namespace(nagents=N, hid_size=128, comm_passes=passes, recurrent=True, rnn_type="LSTM",
-                              continuous=False, naction_heads=list(heads), comm_mask_zero=comm_mask_zero,
-                              comm_mode=comm_mode, hard_attn=hard_attn, comm_init="uniform", share_weights=share,
-                              seed=0, env_id0=0, commnet=True, policy_impl=impl)
-
-
-def make_net(N, O, heads, wseed=3, **kw):
-    """CommNetMLP with the weights of make_weights (one comm pass) or, with comm_passes > 1, its own seeded init."""
-    from ic3net_b200.comm import CommNetMLP
-    a = policy_args(N, heads, **kw)
-    torch.manual_seed(wseed)
-    net = CommNetMLP(a, O)
-    if a.comm_passes == 1:
-        sd = make_weights(wseed, O, 128, heads)
-        net.load_state_dict({k: torch.from_numpy(v).float() for k, v in sd.items()})
-    return net, a
-
-
-def synthetic(B, N, O, seed, h_scale=1.0, c_scale=3.0):
-    """Sparse integer observations, h in [-1, 1], c in [-3, 3], random comm / alive masks; env b % 4 == 0 has nobody
-    alive, b % 4 == 1 exactly one agent, b % 4 == 2 everybody."""
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    dev = "cuda"
-    obs = ((torch.rand(B, N, O, generator=g, device=dev) < 0.1) *
-           torch.randint(1, 4, (B, N, O), generator=g, device=dev)).float()
-    h = (torch.rand(B * N, 128, generator=g, device=dev) * 2 - 1) * h_scale
-    c = (torch.rand(B * N, 128, generator=g, device=dev) * 2 - 1) * c_scale
-    comm = torch.randint(0, 2, (B, N), generator=g, device=dev, dtype=torch.uint8)
-    alive = torch.randint(0, 2, (B, N), generator=g, device=dev, dtype=torch.uint8)
-    kind = torch.arange(B, device=dev) % 4
-    alive[kind == 0] = 0
-    one = torch.zeros(N, dtype=torch.uint8, device=dev)
-    one[N // 2] = 1
-    alive[kind == 1] = one
-    alive[kind == 2] = 1
-    return obs, h, c, comm, alive
-
 
 def reference(net, a, obs, h, c, comm, alive):
     B, N, O = obs.shape
@@ -147,113 +52,11 @@ def forward(net, a, obs, h, c, comm, alive):
 
 # ---------------------------------------------------------------------------------------------------- a. full size
 
-def make_trainer(name, B, seed=5, id0=0, **over):
-    """Trainer (tensor-core policy, index observations, records for the gradient) on fixture ``name``'s arguments and
-    weights.  With the BPTT kernels the records hold every step's (h, c) (rec_h / rec_c); otherwise grad_window = 1
-    checkpoints (h, c) before every step (ck_h / ck_c)."""
-    from ic3net_b200 import data
-    from ic3net_b200.comm import CommNetMLP
-    from ic3net_b200.trainer import Trainer
-    meta, _ = load_golden(name)
-    args = ns(meta["args"], nenvs=B, seed=seed, env_id0=id0, obs_mode="index", use_graph=False, policy_impl="tc",
-              record_for_grad=True, grad_window=1, **over)
-    env = data.init(args.env_name, args)
-    finish_args(args, env)
-    torch.manual_seed(meta["weights_seed"])
-    net = CommNetMLP(args, args.num_inputs)
-    if int(args.comm_passes) == 1:
-        sd = make_weights(meta["weights_seed"], args.num_inputs, args.hid_size, args.naction_heads, args.comm_init)
-        net.load_state_dict({k: torch.from_numpy(v).float() for k, v in sd.items()})
-    return Trainer(args, net, env)
-
-
-def trainer_rows(tr, T, label, sensitivity=False):
-    """One rollout of T lock-steps, then every row of every step against step_f64 from the recorded state entering the
-    step, the recorded observation state and masks.  Recorded actions are recomputed from the reference's log-probs
-    with the trainer's own Philox draws.  Returns {output: worst error}."""
-    e, args = tr.env.env, tr.args
-    B, N = e.nenvs, args.nagents
-    R = B * N
-    tick0 = e.tick.clone().to(torch.int64).cpu().numpy()
-    tr.rollout(T, 0)
-    tr.collect_stat()                                    # raises on a device-side flag
-    b = tr._buf
-    gk = tr.grad_kernels
-    hs, cs = (b["rec_h"], b["rec_c"]) if gk else (b["ck_h"], b["ck_c"])
-    passes = int(args.comm_passes)
-    P = params_f64(tr.policy_net.state_dict(), passes, device="cuda")
-    kw = dict(nagents=N, passes=passes, hard_attn=bool(args.hard_attn) and bool(args.commnet),
-              comm_mode=getattr(args, "comm_mode", "avg"), comm_mask_zero=bool(args.comm_mask_zero))
-    seed, id0 = int(e.cfg.seed), int(e.cfg.env_id0)
-    heads = list(args.naction_heads)
-
-    def obs(t):
-        if tr.is_tj:
-            return tj_record_obs(tr, t, 0, B).reshape(R, -1).double()
-        idx, val = tr._pp_sparse_obs(b["s_loc"][t])
-        return idx, val.double()
-
-    worst, flips, draws, nfresh = {}, 0, 0, 0
-    for t in range(T):
-        ref = ref_dict(*step_f64(P, obs(t), hs[t], cs[t], b["s_comm"][t], b["s_alive"][t], b["s_fresh"][t], **kw))
-        nfresh += int(b["s_fresh"][t].sum())
-        got = dict(value=b["value"][t], logp=b["logp"][t].reshape(R, -1))
-        if gk or t + 1 < T:                              # checkpoints (ck_h) hold the state entering steps 0 .. T-1
-            got.update(h=hs[t + 1], c=cs[t + 1])
-        compare("%s step %d" % (label, t), got, ref, worst)
-        # actions: the draws of (seed, env_id0 + b, tick, agent), inverse CDF on the float64 log-probs
-        u24 = philox_u24(seed, id0 + np.arange(B)[:, None], (tick0 + t)[:, None], philox.STREAM_ACTION,
-                         np.arange(N)[None, :]).reshape(R, 4)
-        act = b["action"][t].reshape(R, -1).cpu().numpy()
-        off = 0
-        for k, na in enumerate(heads):
-            want, margin = inverse_cdf(ref["logp"][:, off:off + na], u24[:, k])
-            safe = margin > MARGIN
-            bad = np.nonzero(safe & (want != act[:, k]))[0]
-            assert bad.size == 0, "%s step %d head %d: action differs at rows %s" % (label, t, k, bad[:10])
-            flips += int((want != act[:, k]).sum())
-            draws += R
-            off += na
-    assert flips <= 1e-3 * draws, (flips, draws)
-    assert nfresh > B, "every slot must start an episode again inside the rollout"
-    print("%s: %d rows x %d steps, worst |gpu - ref| / max(1, |ref|): %s; action flips at CDF edges %d of %d" % (
-        label, R, T, " ".join("%s %.2e" % kv for kv in worst.items()), flips, draws))
-    if sensitivity:
-        show_sensitivity(tr, P, obs, hs, cs, kw, label)
-    return worst
-
-
-def show_sensitivity(tr, P, obs, hs, cs, kw, label):
-    """The comparison notices a one-env mix-up and a dropped episode reset: both modified references break the bar."""
-    b, N = tr._buf, kw["nagents"]
-    fr = b["s_fresh"]
-    got = lambda t: dict(h=hs[t + 1], c=cs[t + 1], value=b["value"][t], logp=b["logp"][t].reshape(hs[t].shape[0], -1))
-    # in the middle of an episode, env's h taken from its neighbour env + 1 (the pair whose states differ most: traffic-
-    # junction envs whose cars have not entered yet hold identical states)
-    best = (-1.0, 0, 0)
-    for t in range(1, fr.shape[0] - 1):
-        hv = hs[t].view(fr.shape[1], N, -1)
-        d = (hv[:-1] - hv[1:]).abs().amax((1, 2)).masked_fill((fr[t, :-1] != 0) | (fr[t, 1:] != 0), -1.0)
-        best = max(best, (float(d.max()), t, int(d.argmax())))
-    _, t, env = best
-    h = hs[t].clone()
-    h[env * N:(env + 1) * N] = hs[t][(env + 1) * N:(env + 2) * N]
-    swapped = ref_dict(*step_f64(P, obs(t), h, cs[t], b["s_comm"][t], b["s_alive"][t], fr[t], **kw))
-    # a step that starts new episodes, with the resets ignored: the state the last episode left enters the step
-    tr_ = next(t for t in range(1, fr.shape[0] - 1) if bool(fr[t].any()))
-    unreset = ref_dict(*step_f64(P, obs(tr_), hs[tr_], cs[tr_], b["s_comm"][tr_], b["s_alive"][tr_], None, **kw))
-    for what, ts, ref in (("h of env %d + 1 in env %d at step %d" % (env, env, t), t, swapped),
-                          ("%d resets of step %d ignored" % (int(fr[tr_].sum()), tr_), tr_, unreset)):
-        with pytest.raises(AssertionError) as exc:
-            compare("%s, reference with the %s" % (label, what), got(ts), ref)
-        print(str(exc.value).splitlines()[0][:300])
-
-
 @pytest.mark.parametrize("name,B", [("grad_pp_hard_ic3net_h128", 8192), ("grad_tj_hard_ic3net_h128", 4096)])
 def test_full_size_every_row_matches_float64(name, B):
     """81 920 rows: 640 tiles, 1280 work items, nine or ten items per CTA.  max_steps 6 over 14 lock-steps: every slot
     starts three episodes, so the fresh branches of the operand preparation and of the epilogue run at full size."""
-    tr = make_trainer(name, B, max_steps=6)
+    tr = rows_trainer(name, B, max_steps=6)
     assert tr.grad_kernels
     trainer_rows(tr, 14, "%s B=%d" % (name, B), sensitivity=True)
 
@@ -263,13 +66,13 @@ def test_full_size_every_row_matches_float64(name, B):
 def sweep_batch(case, N, nsm):
     """Env slots B (N agents each) giving the row / tile / work-item count the case is about."""
     def with_tiles(nt):                                  # R just past nt - 1 tiles: the last tile holds 1..N rows
-        return ((nt - 1) * TILE) // N + 1
+        return ((nt - 1) * TC_TILE) // N + 1
     if case == "R<64":
         return 63 // N
     if case == "64<R<128":
         return 127 // N
     if case == "R=128k+1":
-        return next(b for b in range(1, 1 << 16) if (b * N) % TILE == 1 and b * N > 2 * TILE)
+        return next(b for b in range(1, 1 << 16) if (b * N) % TC_TILE == 1 and b * N > 2 * TC_TILE)
     if case == "no-padding-tiles":
         return 1024                                      # R = 1024 N: 8 N tiles
     if case == "7-padding-tiles":
@@ -288,10 +91,10 @@ def sweep_batch(case, N, nsm):
 
 def sweep_checks(case, B, N, nsm):
     R = B * N
-    nt, ntp, items, grid = geometry(R)
-    ok = {"R<64": R < 64, "64<R<128": 64 < R < 128, "R=128k+1": R % TILE == 1 and nt >= 3,
-          "no-padding-tiles": R % TILE == 0 and nt % TILE_PAD == 0,
-          "7-padding-tiles": nt % TILE_PAD == 1,
+    nt, ntp, items, grid = tc_geometry(R)
+    ok = {"R<64": R < 64, "64<R<128": 64 < R < 128, "R=128k+1": R % TC_TILE == 1 and nt >= 3,
+          "no-padding-tiles": R % TC_TILE == 0 and nt % TC_TILE_PAD == 0,
+          "7-padding-tiles": nt % TC_TILE_PAD == 1,
           "items<SMs": items < nsm, "items>SMs": nsm < items < 2 * nsm,
           "items>=3SMs": items >= 3 * nsm and items % nsm != 0}[case]
     assert ok, (case, B, N, R, nt, ntp, items, nsm)
@@ -315,7 +118,7 @@ def test_row_and_work_item_sweep(case, N, impl):
     B = sweep_batch(case, N, nsm)
     label = sweep_checks(case, B, N, nsm) + " " + impl
     O = 61
-    net, a = make_net(N, O, (5, 2), wseed=N, impl=impl)
+    net, a = make_lstm_net(N, O, (5, 2), wseed=N, impl=impl)
     inputs = synthetic(B, N, O, seed=1000 * N + len(case))
     errs = compare(label, forward(net, a, *inputs), reference(net, a, *inputs))
     print(label, " ".join("%s %.2e" % kv for kv in errs.items()))
@@ -335,7 +138,7 @@ def test_variants_beyond_one_tile(kw):
     nsm = sms()
     B = sweep_batch("items>=3SMs", N, nsm)
     label = sweep_checks("items>=3SMs", B, N, nsm) + " " + str(kw)
-    net, a = make_net(N, O, (5, 2), wseed=7, **kw)
+    net, a = make_lstm_net(N, O, (5, 2), wseed=7, **kw)
     assert net.policy_impl == "tc"
     inputs = synthetic(B, N, O, seed=77)
     errs = compare(label, forward(net, a, *inputs), reference(net, a, *inputs))
@@ -349,7 +152,7 @@ def test_enemy_comm_rollout_beyond_one_tile():
     nsm = sms()
     B = sweep_batch("items>=3SMs", N, nsm)
     label = sweep_checks("items>=3SMs", B, N, nsm) + " enemy_comm"
-    tr = make_trainer(name, B, seed=9, id0=4, max_steps=5)
+    tr = rows_trainer(name, B, seed=9, id0=4, max_steps=5)
     trainer_rows(tr, 12, label)
 
 
@@ -357,40 +160,12 @@ def test_two_pass_rollout_with_resets():
     """comm_passes = 2 in a trainer rollout with episode resets: the recorded values / log-probs and the state entering
     every next step against float64 replayed over the trainer's own (h, c) checkpoints."""
     name = "grad_pp_hard_ic3net_h128"
-    tr = make_trainer(name, 1024, seed=21, id0=2, comm_passes=2, max_steps=5, grad_impl="autograd")
+    tr = rows_trainer(name, 1024, seed=21, id0=2, comm_passes=2, max_steps=5, grad_impl="autograd")
     assert tr.policy_net.policy_impl == "tc" and tr.policy_net.is_variant and not tr.grad_kernels
     trainer_rows(tr, 12, "pp hard comm_passes=2 B=1024")
 
 
 # ---------------------------------------------------------------------------------------------------- d. heads
-
-def direct_step(net, obs, h, c, comm, alive, out, draws=None):
-    """ic3_policy_step through the C ABI as CommNetMLP.forward calls it, into the caller's buffers out[h, c, value,
-    logp, action] (explicit draws [R, nheads] when given).  Returns the device flag word of the step."""
-    from ic3net_b200 import _lib
-    lib = _lib.load()
-    B = obs.shape[0]
-    cfg = net.policy_cfg(B)
-    w = net.packed()
-    x = torch.empty(B * net.nagents, net.hid_size, device="cuda")
-    _lib.check(lib.ic3_encoder_dense(C.byref(cfg), C.byref(w), obs.data_ptr(), x.data_ptr(), _lib.stream()))
-    ws, _ = net.workspace(B)
-    err = torch.zeros(1, dtype=torch.int32, device="cuda")
-    io = _lib.PolicyIO(x=x.data_ptr(), h=h.data_ptr(), c=c.data_ptr(), comm_action=_lib.ptr(comm),
-                       alive=_lib.ptr(alive), fresh=None, tick=None, draws=_lib.ptr(draws), h_out=out["h"].data_ptr(),
-                       c_out=out["c"].data_ptr(), value=out["value"].data_ptr(), logp=out["logp"].data_ptr(),
-                       action=_lib.ptr(out.get("action")), workspace=_lib.ptr(ws), err=err.data_ptr())
-    _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), _lib.stream()))
-    torch.cuda.synchronize()
-    return int(err.item())
-
-
-def outputs(R, heads, extra=0):
-    """Output buffers with `extra` rows past R, every element a NaN bit pattern (actions: -7)."""
-    nan = lambda *s: torch.full(s, 0x7FC0DEAD, dtype=torch.int32, device="cuda").view(torch.float32)
-    return dict(h=nan(R + extra, 128), c=nan(R + extra, 128), value=nan(R + extra), logp=nan(R + extra, sum(heads)),
-                action=torch.full((R + extra, len(heads)), -7, dtype=torch.int32, device="cuda"))
-
 
 HEADS = [(5, 2), (2, 2, 2, 1), (9, 2), (5, 5, 5), (3, 4, 2, 5), (9, 8), (16, 15), (8, 8, 8, 7)]
 
@@ -403,7 +178,7 @@ def test_heads_with_explicit_draws(heads):
     N, O, B = 7, 61, 300
     R = B * N
     nout = 1 + sum(heads)
-    net, a = make_net(N, O, heads, wseed=sum(heads))
+    net, a = make_lstm_net(N, O, heads, wseed=sum(heads))
     inputs = synthetic(B, N, O, seed=nout)
     ref = reference(net, a, *inputs)
     rs = np.random.RandomState(nout)
@@ -419,8 +194,8 @@ def test_heads_with_explicit_draws(heads):
         u24[on, k] = np.clip(np.where(rows[on] % 8 == 2, np.floor(edge[on]), np.ceil(edge[on])), 0, (1 << 24) - 1)
         off += na
     draws = torch.as_tensor(u24.astype(np.int32), device="cuda").contiguous()
-    out = outputs(R, heads)
-    assert direct_step(net, *inputs, out, draws=draws) == 0
+    out = lstm_outputs(R, heads)
+    assert lstm_direct_step(net, *inputs, out, draws=draws) == 0
     label = "heads %s (%d outputs)" % (heads, nout)
     errs = compare(label, out, ref)
     act = out["action"].cpu().numpy()
@@ -449,12 +224,12 @@ def test_writes_stay_inside_the_rows(case, heads, passes):
     B = sweep_batch(case, N, nsm)
     label = sweep_checks(case, B, N, nsm) + " heads %s passes %d" % (heads, passes)
     R = B * N
-    net, a = make_net(N, O, heads, wseed=11, passes=passes)
+    net, a = make_lstm_net(N, O, heads, wseed=11, passes=passes)
     obs, h, c, comm, alive = synthetic(B, N, O, seed=5)
     before = [t.clone() for t in (obs, h, c, comm, alive)]
-    out = outputs(R, heads, extra)
+    out = lstm_outputs(R, heads, extra)
     pristine = {k: v.clone() for k, v in out.items()}
-    assert direct_step(net, obs, h, c, comm, alive, out,
+    assert lstm_direct_step(net, obs, h, c, comm, alive, out,
                        draws=torch.zeros(R, len(heads), dtype=torch.int32, device="cuda")) == 0
     for k, v in out.items():
         bits = lambda t: t.view(torch.int32) if t.dtype == torch.float32 else t
@@ -471,7 +246,7 @@ def limit_case(enc_bias=None, c_entry=None, small=False):
     (device flag word, got, ref)."""
     N, O = 10, 61
     B = sweep_batch("items>SMs", N, sms())
-    net, a = make_net(N, O, (5, 2), wseed=13)
+    net, a = make_lstm_net(N, O, (5, 2), wseed=13)
     obs, h, c, comm, alive = synthetic(B, N, O, seed=13, h_scale=1e-4 if small else 1.0, c_scale=1e-4 if small else 3.0)
     with torch.no_grad():
         if enc_bias is not None:
@@ -490,8 +265,8 @@ def limit_case(enc_bias=None, c_entry=None, small=False):
             net.encoder.weight.mul_(1e-4)
             net.encoder.bias.mul_(1e-4)
     R = B * N
-    out = outputs(R, (5, 2))
-    flags = direct_step(net, obs, h, c, comm, alive, out, draws=torch.zeros(R, 2, dtype=torch.int32, device="cuda"))
+    out = lstm_outputs(R, (5, 2))
+    flags = lstm_direct_step(net, obs, h, c, comm, alive, out, draws=torch.zeros(R, 2, dtype=torch.int32, device="cuda"))
     return flags, out, reference(net, a, obs, h, c, comm, alive), net, obs
 
 

@@ -4,7 +4,7 @@ default forward of every tanh-cell policy (models.MLP, the non-recurrent CommNet
 baselines), and comm_passes > 1 / share_weights of the LSTM CommNet / IC3Net below hid_size 128.
 
 Covered:
-  1. the tanh yardsticks (test_gpu_ff_tc.step_f64, test_gpu_rnn_tc.step_f64) against the reference's own forward
+  1. the tanh yardsticks (gpu_harness.ff_step_f64 and rnn_step_f64) against the reference's own forward
      fixtures var_mlp, var_commnet_nonrec2, var_commnet_nonrec_share (hid_size 32) and var_rnn_tanh, to 1e-10, so
      that the bars below rest on the reference (the LSTM yardstick policy_ref.step_f64 is pinned by
      tests/test_policy_ref.py);
@@ -25,7 +25,7 @@ Covered:
      actions against the float64 argmax, and exact ties taking the lowest index.
 
 Bar: |gpu - ref| <= 1e-5 * max(1, |ref|) on h', c', value and log-probs (DESIGN.md section 2), except comm_mode sum with
-several passes, which takes test_gpu_ff_tc.sum_tol: S is up to N - 1 times an h, so each pass multiplies the error of
+several passes, which takes gpu_harness.sum_tol: S is up to N - 1 times an h, so each pass multiplies the error of
 h by up to N - 1 through the next S.  On this kernel too that is what the error follows: 3 shared sum-mode passes with
 the 20 traffic-junction agents measured 5.9e-6 (H 128) and 8.2e-6 (H 64) on h', against <= 1.4e-7 for every
 avg-mode family.  A failure names the row, env, CTA and its position in the CTA's 64-row tile.  A neighbour env's
@@ -49,23 +49,17 @@ import numpy as np
 import pytest
 import torch
 
-import test_gpu_bptt_rnn as rnn_trainers
-import test_gpu_ff_tc as ff
-import test_gpu_grad_ff as gf
-import test_gpu_policy_rows as pr
-import test_gpu_rnn_tc as rt
 from bptt_ref import tj_record_obs
+from gpu_harness import (MARGIN, PP, ROW_TOL, TJ, argmax_check, compare_rows, ff_direct_step, ff_net, ff_step_f64,
+                         ff_trainer, head_logits_f64, policy_args, ref_dict, rnn_net, rnn_step_f64, rnn_trainer,
+                         sum_tol, synthetic, trainer_rows, variant_net)
 from helpers import load_golden
 from oracle import philox
 from policy_ref import inverse_cdf, params_f64, philox_u24, step_f64
-from test_gpu_evaluate import argmax_check, head_logits_f64
-from test_gpu_variants import build
 
 pytestmark = pytest.mark.gpu
 
-TOL, MARGIN = pr.TOL, pr.MARGIN
 ROWS = 64                   # agent rows per CTA tile of policy_step_kernel
-PP, TJ = gf.PP, gf.TJ
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -100,24 +94,15 @@ def where(r, B, N):
         r, env, r - env * N, cta, ctas, r - cta * epb * N, filled, ROWS - filled)
 
 
-def compare(label, got, ref, B, N, worst=None, tol=TOL):
+def at(B, N):
+    """compare_rows' ``where`` for policy_step_kernel: the worst element's env, CTA and place in the CTA's tile."""
+    return lambda r, col, k: "%s, col %d" % (where(r, B, N), col)
+
+
+def compare(label, got, ref, B, N, worst=None, tol=ROW_TOL):
     """got / ref: dicts of h, c [R, H], value [R], logp [R, A] (any of them may be absent from got).  Asserts the bar;
     returns {output: max error}."""
-    R = B * N
-    errs, msgs = {}, []
-    for k in ("h", "c", "value", "logp"):
-        if k not in got:
-            continue
-        e = pr.rel_err(got[k].reshape(R, -1), ref[k].reshape(R, -1))
-        errs[k] = float(e.max())
-        if worst is not None:
-            worst[k] = max(worst.get(k, 0.0), errs[k])
-        if not errs[k] <= tol:
-            r, col = divmod(int(e.nan_to_num(float("inf")).argmax()), e.shape[1])
-            msgs.append("%s: %s max %.3e at %s, col %d; %d rows over the bar" % (
-                label, k, errs[k], where(r, B, N), col, int((~(e <= tol)).any(1).sum())))
-    assert not msgs, "\n".join(msgs)
-    return errs
+    return compare_rows(label, got, ref, worst, tol, where=at(B, N))
 
 
 def fmt(worst):
@@ -127,21 +112,21 @@ def fmt(worst):
 # ---------------------------------------------------------------------------------------------------- yardsticks
 
 def reference(net, obs, B, h, c, comm, alive, fresh):
-    """Float64 step of net by its family: policy_ref.step_f64 (LSTM cell), test_gpu_rnn_tc.step_f64 (tanh RNN),
-    test_gpu_ff_tc.step_f64 (non-recurrent tanh).  obs: dense [R, O] or sparse (index, value), float64."""
+    """Float64 step of net by its family: policy_ref.step_f64 (LSTM cell), rnn_step_f64 (tanh RNN),
+    ff_step_f64 (non-recurrent tanh).  obs: dense [R, O] or sparse (index, value), float64."""
     from ic3net_b200 import _lib, bptt
     p, N = net._cfg_proto, net.nagents
     hard = bool(p["hard_attn"])
     if p["cell"] == _lib.CELL_LSTM:
         P = params_f64(net.state_dict(), p["passes"], device="cuda")
-        return pr.ref_dict(*step_f64(P, obs, h, c, comm if hard else None, alive, fresh, nagents=N, passes=p["passes"],
+        return ref_dict(*step_f64(P, obs, h, c, comm if hard else None, alive, fresh, nagents=N, passes=p["passes"],
                                      hard_attn=hard, comm_mode="avg" if p["comm_avg"] else "sum",
                                      comm_mask_zero=bool(p["comm_mask_zero"])))
     if not p["h_from_x"]:
-        return rt.step_f64(net.state_dict(), obs, h, fresh, N)
+        return rnn_step_f64(net.state_dict(), obs, h, fresh, N)
     w = net._kernel_weights()
     x = bptt.encode({"encoder.weight": w["enc_w"].detach().double(), "encoder.bias": w["enc_b"].detach().double()}, obs)
-    return ff.step_f64(net, x, B, comm if hard else None, alive, fresh)[0]
+    return ff_step_f64(net, x, B, comm if hard else None, alive, fresh)[0]
 
 
 def sum_mode(net):
@@ -161,16 +146,16 @@ def test_tanh_yardsticks_match_the_reference_fixtures(name):
     sd = {k[3:]: t(z[k]) for k in z.files if k.startswith("sd_")}
     obs = t(z["obs"]).reshape(R, O)
     if meta["model"] == "rnn":
-        ref = rt.step_f64(sd, obs, t(z["h"]).reshape(R, -1), None, N)
+        ref = rnn_step_f64(sd, obs, t(z["h"]).reshape(R, -1), None, N)
         want = dict(h=t(z["h2"]).reshape(R, -1))
     else:
-        _, net = build(meta, z, "simt")
+        _, net = variant_net(meta, z, "simt")
         net.double()
         net.load_state_dict(sd)                           # the fixture's float64 weights, not their float32 rounding
         assert net._kernel_weights()["enc_w"].dtype == torch.float64
         w = net._kernel_weights()
         x = obs @ w["enc_w"].detach().t() + w["enc_b"].detach()
-        ref, _ = ff.step_f64(net, x, K, t(z["comm"]) if meta["hard_attn"] else None,
+        ref, _ = ff_step_f64(net, x, K, t(z["comm"]) if meta["hard_attn"] else None,
                              t(z["alive"]) if meta["use_alive"] else None, None)
         want = {}
     want.update(value=t(z["value"]).reshape(R),
@@ -246,7 +231,7 @@ def tanh_rows(tr, T, label, negative=False):
     heads = list(args.naction_heads)
     assert net.policy_impl == "simt" and not tr.grad_kernels and tr.grad_window == 1
     rnn = not net._cfg_proto["h_from_x"]
-    tol = ff.sum_tol(N) if sum_mode(net) else TOL
+    tol = sum_tol(N) if sum_mode(net) else ROW_TOL
     tick0 = e.tick.clone().to(torch.int64).cpu().numpy()
     tr.rollout(T, 0)
     tr.collect_stat()                                    # raises on a device-side flag
@@ -263,7 +248,7 @@ def tanh_rows(tr, T, label, negative=False):
             got["h"] = b["ck_h"][t + 1]
         elif not rnn:
             out = outputs(R, H, heads, False)
-            assert ff.direct_step(net, record_x(tr, t), B, out, comm if tr.hard else None, alive, fresh) == 0
+            assert ff_direct_step(net, record_x(tr, t), B, out, comm if tr.hard else None, alive, fresh) == 0
             assert torch.equal(out["value"], got["value"]) and torch.equal(out["logp"], got["logp"]), (label, t)
             got["h"] = out["h"]
         compare("%s step %d" % (label, t), got, ref, B, N, worst, tol)
@@ -294,17 +279,8 @@ def tanh_rows(tr, T, label, negative=False):
     return worst
 
 
-def simt_where(monkeypatch, N):
-    """test_gpu_policy_rows.trainer_rows names the worst element in the tensor-core kernel's tiles; here in the SIMT
-    kernel's (N agents per env)."""
-    def at(err, R, unit_cols):
-        r, col = divmod(int(err.argmax()), err.shape[1])
-        return "%s, col %d" % (where(r, R // N, N), col)
-    monkeypatch.setattr(pr, "where", at)
-
-
 def lstm_trainer(name, B, H, **over):
-    tr = gf.make_trainer(name, B, "ic3net", grad_impl="autograd", policy_impl="simt", hid_size=H, recurrent=True,
+    tr = ff_trainer(name, B, "ic3net", grad_impl="autograd", policy_impl="simt", hid_size=H, recurrent=True,
                          rnn_type="LSTM", grad_window=1, **over)
     assert tr.policy_net.policy_impl == "simt" and tr.policy_net.recurrent and not tr.grad_kernels
     return tr
@@ -313,20 +289,20 @@ def lstm_trainer(name, B, H, **over):
 def tanh_trainer(name, B, family, H, **over):
     kw = dict(grad_impl="autograd", policy_impl="simt", hid_size=H, grad_window=1)
     if family == "rnn":
-        return rnn_trainers.make_trainer(name, B, **dict(kw, **over))
-    return gf.make_trainer(name, B, family, **dict(kw, **over))
+        return rnn_trainer(name, B, **dict(kw, **over))
+    return ff_trainer(name, B, family, **dict(kw, **over))
 
 
 LSTM_FULL = [(PP, 8192, 64), (TJ, 4096, 64), (PP, 8192, 128), (PP, 8192, 32)]
 
 
 @pytest.mark.parametrize("name,B,H", LSTM_FULL)
-def test_full_size_lstm_every_row_matches_float64(name, B, H, monkeypatch):
+def test_full_size_lstm_every_row_matches_float64(name, B, H):
     """81 920 rows per step, 14 lock-steps with max_steps 6: every slot starts three episodes.  H 64 on both envs also
     shows that a neighbour env's state and an ignored reset break the bar."""
     tr = lstm_trainer(name, B, H, seed=5, id0=0, max_steps=6)
-    simt_where(monkeypatch, tr.args.nagents)
-    pr.trainer_rows(tr, 14, "simt LSTM IC3Net H=%d %s B=%d" % (H, name, B), sensitivity=H == 64)
+    trainer_rows(tr, 14, "simt LSTM IC3Net H=%d %s B=%d" % (H, name, B), sensitivity=H == 64,
+                 where=at(B, tr.args.nagents))
 
 
 TANH_FULL = [(PP, 8192, fam, H, over) for H in (128, 64)
@@ -339,7 +315,7 @@ TANH_FULL = [(PP, 8192, fam, H, over) for H in (128, 64)
 def test_full_size_tanh_every_row_matches_float64(name, B, family, H, over):
     """81 920 rows per step, 14 lock-steps with max_steps 6.  H 64 also shows that a neighbour env's observation
     (non-recurrent IC3Net) and ignored resets (tanh RNN) break the bar."""
-    tr =tanh_trainer(name, B, family, H, seed=5, id0=0, max_steps=6, **over)
+    tr = tanh_trainer(name, B, family, H, seed=5, id0=0, max_steps=6, **over)
     tanh_rows(tr, 14, "simt %s H=%d %s B=%d %s" % (family, H, name, B, over), negative=H == 64 and
               family in ("ic3net", "rnn"))
 
@@ -350,7 +326,7 @@ def lstm_net(N, O, heads, H, wseed=3, comm_init="uniform", **kw):
     """CommNetMLP with the LSTM cell on the SIMT kernel (test_gpu_policy_rows.policy_args at any hid_size), the module's
     own seeded initialisation."""
     from ic3net_b200.comm import CommNetMLP
-    a = pr.policy_args(N, heads, impl="simt", **kw)
+    a = policy_args(N, heads, impl="simt", **kw)
     a.hid_size, a.comm_init = H, comm_init
     torch.manual_seed(wseed)
     return CommNetMLP(a, O)
@@ -358,8 +334,8 @@ def lstm_net(N, O, heads, H, wseed=3, comm_init="uniform", **kw):
 
 def tanh_net(family, N, O, heads, H, wseed=3, passes=1, share=False, mode="avg"):
     if family == "rnn":
-        return rt.rnn_net(N, O, heads, "simt", wseed=wseed, H=H)
-    return ff.ff_net(N, heads, "simt", family, passes=passes, share=share, mode=mode, wseed=wseed, H=H, O=O)
+        return rnn_net(N, O, heads, "simt", wseed=wseed, H=H)
+    return ff_net(N, heads, "simt", family, passes=passes, share=share, mode=mode, wseed=wseed, H=H, O=O)
 
 
 def direct_step(net, obs, h, c, comm, alive, fresh, out, draws=None, greedy=False):
@@ -382,7 +358,7 @@ def direct_step(net, obs, h, c, comm, alive, fresh, out, draws=None, greedy=Fals
 
 def inputs(net, B, O, seed):
     """test_gpu_policy_rows.synthetic at the net's hid_size (its h, c cut to H columns), and the fresh envs b % 5 == 3."""
-    obs, h, c, comm, alive = pr.synthetic(B, net.nagents, O, seed)
+    obs, h, c, comm, alive = synthetic(B, net.nagents, O, seed)
     H = net.hid_size
     fresh = (torch.arange(B, device="cuda") % 5 == 3).to(torch.uint8)
     return obs, h[:, :H].contiguous(), c[:, :H].contiguous(), comm, alive, fresh
@@ -398,7 +374,7 @@ def run_case(net, B, O, seed, label, worst=None):
     from ic3net_b200 import _lib
     carries = not net._cfg_proto["h_from_x"]
     lstm = net._cfg_proto["cell"] == _lib.CELL_LSTM
-    tol = ff.sum_tol(N) if sum_mode(net) else TOL
+    tol = sum_tol(N) if sum_mode(net) else ROW_TOL
     obs, h, c, comm, alive, fresh = inputs(net, B, O, seed)
     obs64 = obs.reshape(R, -1).double()
     info = {"alive_mask": alive, "comm_action": comm} if net._cfg_proto["hard_attn"] else {"alive_mask": alive}
@@ -544,7 +520,7 @@ def test_mlp_and_tanh_rnn_direct_beyond_one_cta(H, family):
 
 @pytest.mark.parametrize("family", ["mlp", "rnn", "enemy_comm"])
 @pytest.mark.parametrize("H", [32, 64])
-def test_trainer_rollout_beyond_one_cta(H, family, monkeypatch):
+def test_trainer_rollout_beyond_one_cta(H, family):
     """models.MLP, the tanh RNN (IC) and the LSTM IC3Net with --enemy_comm (the prey is agent row N - 1 of every env)
     in a trainer rollout of 12 lock-steps over 301 slots with episode resets, every row against float64."""
     B, T = 301, 12
@@ -553,8 +529,7 @@ def test_trainer_rollout_beyond_one_cta(H, family, monkeypatch):
         tr = lstm_trainer(name, B, H, seed=9, id0=4, max_steps=5)
         N = tr.args.nagents
         assert N == load_golden(name)[0]["args"]["nfriendly"] + 1 and tr.env.env.nagent_rows == N
-        simt_where(monkeypatch, N)
-        pr.trainer_rows(tr, T, "simt enemy_comm H=%d %s" % (H, sweep_checks("many-CTAs", B, N)))
+        trainer_rows(tr, T, "simt enemy_comm H=%d %s" % (H, sweep_checks("many-CTAs", B, N)), where=at(B, N))
     else:
         tr = tanh_trainer(PP, B, family, H, seed=9, id0=4, max_steps=5)
         tanh_rows(tr, T, "simt %s H=%d %s" % (family, H, sweep_checks("many-CTAs", B, tr.args.nagents)))

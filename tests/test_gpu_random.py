@@ -13,7 +13,6 @@ Covered:
   - CUDA-graph replay bit-identical to eager;
   - no parameter moves, the optimizer state stays empty, checkpoints interchange with the reference's Random +
     torch.optim.RMSprop; two ranks reduce to what one process holding both shards computes; the CLI trains."""
-import argparse
 import ctypes as C
 import os
 import subprocess
@@ -24,43 +23,12 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import finish_args, golden_names, load_golden, ns
+from gpu_harness import random_args, random_trainer as make_trainer
+from helpers import golden_names, load_golden, ns
 import random_oracle as ro
 
 pytestmark = pytest.mark.gpu
 HERE = os.path.dirname(os.path.abspath(__file__))
-
-# BASELINE.json configs[1] and configs[4] (bench.py WORKLOADS pp_hard_ic3net / tj_hard_ic3net), with --random
-GEOMETRY = {
-    "c2": dict(env_name="predator_prey", nagents=10, dim=20, vision=1, max_steps=80, nenvs=8192, mode="mixed"),
-    "c5": dict(env_name="traffic_junction", nagents=20, dim=18, vision=0, max_steps=80, nenvs=4096,
-               difficulty="hard", add_rate_min=0.02, add_rate_max=0.05, curr_start=250, curr_end=1250),
-}
-
-
-def random_args(geometry, **over):
-    d = dict(hid_size=128, recurrent=False, rnn_type="MLP", commnet=False, ic3net=False, random=True, hard_attn=False,
-             comm_action_one=False, comm_mode="avg", comm_passes=1, comm_mask_zero=False, share_weights=False,
-             batch_size=500, lrate=1e-3, gamma=1.0, mean_ratio=1.0, normalize_rewards=False, value_coeff=0.01, entr=0.0,
-             nenemies=1, no_stay=False, moving_prey=False, enemy_comm=False, mode="mixed", vocab_type="bool",
-             add_rate_min=0.05, add_rate_max=0.2, curr_start=0, curr_end=0, difficulty="easy", seed=11, env_id0=0,
-             obs_mode="index", use_graph=False, detach_gap=10000, advantages_per_action=False)
-    d.update(GEOMETRY[geometry] if geometry else {})
-    d.update(over)
-    a = argparse.Namespace(**d)
-    a.nfriendly = a.nagents
-    return a
-
-
-def make_trainer(args):
-    from ic3net_b200 import data, models
-    from ic3net_b200.trainer import Trainer
-    env = data.init(args.env_name, args)
-    finish_args(args, env)
-    torch.manual_seed(args.seed)
-    net = models.Random(args, args.num_inputs)
-    return net, Trainer(args, net, env)
-
 
 def records(tr):
     b = tr._buf

@@ -9,83 +9,35 @@ with this forward (float64 records at both full sizes, run-to-run, full / window
 bit); CUDA-graph rollouts; the refusals; the command line.
 
 Bar of the forward: |gpu - ref| <= 1e-5 * max(1, |ref|) on h', value and log-probs (DESIGN.md section 2)."""
-import argparse
 import ctypes as C
-import functools
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-import test_gpu_bptt_rnn as grad_tests
 from bptt_ref import tj_record_obs
+from gpu_harness import (MARGIN, PP, TJ, close, compare_rows, one_stream_schedule, rnn_full_size, rnn_gradient_arrays,
+                         rnn_net, rnn_pinned_oracle, rnn_run_to_run, rnn_step_f64, rnn_trainer, rnn_windows, variant_net)
 from helpers import golden_names, load_golden
 from oracle import philox
 from policy_ref import inverse_cdf, philox_u24
 
 pytestmark = pytest.mark.gpu
 
-TOL, MARGIN, TILE = 1e-5, 1e-5, 64
-TESTS = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(TESTS)
-PP, TJ = grad_tests.PP, grad_tests.TJ
-
-
-_ic_trainer = grad_tests.make_trainer
+TILE = 64                   # rows per CTA tile of the tc_tanh step (ff_tc_kernel)
 
 
 def make_trainer(*a, **kw):
     kw.setdefault("policy_impl", "tc_tanh")
-    tr = _ic_trainer(*a, **kw)
+    tr = rnn_trainer(*a, **kw)
     assert tr.policy_net.policy_impl == kw["policy_impl"]
     return tr
 
 
-@pytest.fixture
-def tc_tanh_trainers(monkeypatch):
-    """The IC trainers of tests/test_gpu_bptt_rnn.py built with policy_impl 'tc_tanh': its checks then run on this
-    forward, at the bars the SIMT path meets."""
-    monkeypatch.setattr(grad_tests, "make_trainer", functools.partial(make_trainer, policy_impl="tc_tanh"))
-
-
-def rel_err(got, ref):
-    got, ref = got.to(torch.float64), ref.to(torch.float64)
-    return ((got - ref).abs() / ref.abs().clamp_min(1.0)).reshape(ref.shape[0], -1)
-
-
 def compare(label, got, ref, worst=None):
-    msgs = []
-    R = ref["value"].shape[0]
-    for k in got:
-        e = rel_err(got[k].reshape(R, -1), ref[k].reshape(R, -1))
-        m = float(e.max())
-        if worst is not None:
-            worst[k] = max(worst.get(k, 0.0), m)
-        if not m <= TOL:
-            r, col = divmod(int(e.argmax()), e.shape[1])
-            msgs.append("%s: %s max %.3e at row %d col %d (tile %d, warp %d); %d rows over the bar" % (
-                label, k, m, r, col, r // TILE, (r % TILE) // 16, int((e > TOL).any(1).sum())))
-    assert not msgs, "\n".join(msgs)
-
-
-def step_f64(sd, x_or_obs, h, fresh, N, encoded=False):
-    """h' = tanh(affine1(obs) + affine2(h)), value, log-probs in float64 (models.py:83-91); fresh slots enter with h = 0."""
-    from ic3net_b200 import bptt
-    f64 = torch.float64
-    P = {k: v.detach().to("cuda", f64) for k, v in sd.items()}
-    h = h.to(f64)
-    if fresh is not None:
-        h = h.masked_fill(fresh.bool().repeat_interleave(N).unsqueeze(1), 0.0)
-    x = x_or_obs.to(f64) if encoded else bptt.encode({"encoder.weight": P["affine1.weight"],
-                                                      "encoder.bias": P["affine1.bias"]}, x_or_obs)
-    h2 = torch.tanh(x + h @ P["affine2.weight"].t() + P["affine2.bias"])
-    nh = sum(1 for k in P if k.startswith("heads.") and k.endswith(".weight"))
-    logp = torch.cat([torch.log_softmax(h2 @ P["heads.%d.weight" % m].t() + P["heads.%d.bias" % m], -1)
-                      for m in range(nh)], -1)
-    return dict(h=h2, value=(h2 @ P["value_head.weight"].t() + P["value_head.bias"])[:, 0], logp=logp)
+    """Every row of got against ref at the bar, a failure named by its 64-row tile and 16-row warp."""
+    compare_rows(label, got, ref, worst, where=lambda r, col, k: "row %d col %d (tile %d, warp %d)" % (
+        r, col, r // TILE, (r % TILE) // 16))
 
 
 # ---------------------------------------------------------------------------------------------------- 1. full size
@@ -110,7 +62,7 @@ def test_full_size_every_row_matches_float64(name, B):
         else:
             idx, val = tr._pp_sparse_obs(b["s_loc"][t])
             obs = (idx, val.double())
-        ref = step_f64(sd, obs, b["rec_h"][t], b["s_fresh"][t], N)
+        ref = rnn_step_f64(sd, obs, b["rec_h"][t], b["s_fresh"][t], N)
         nfresh += int(b["s_fresh"][t].sum())
         compare("%s step %d" % (name, t), dict(h=b["rec_h"][t + 1], value=b["value"][t], logp=b["logp"][t].reshape(R, -1)),
                 ref, worst)
@@ -133,9 +85,8 @@ def test_full_size_every_row_matches_float64(name, B):
 
 def test_forward_fixture_of_the_reference():
     """var_rnn_tanh (the unmodified reference's models.RNN: its state_dict, inputs, outputs) through models.RNN.forward."""
-    from test_gpu_variants import build, close
     meta, z = load_golden("var_rnn_tanh")
-    a, net = build(meta, z, "tc_tanh")
+    a, net = variant_net(meta, z, "tc_tanh")
     assert net.policy_impl == "tc_tanh"
     B, n, H = z["obs"].shape[0], a.nagents, a.hid_size
     obs = torch.tensor(z["obs"], dtype=torch.float32, device="cuda")
@@ -150,24 +101,15 @@ def test_forward_fixture_of_the_reference():
 
 
 @pytest.mark.parametrize("name", golden_names("gradrnn_"))
-def test_gradient_fixtures_of_the_reference(name, tc_tanh_trainers):
+def test_gradient_fixtures_of_the_reference(name):
     """One slot replays the reference's own batch (same episodes and actions as the fixture, asserted by the step and
     episode counts and the loss sums): gradient within 1e-4 of the largest entry of the stored arrays; then B = 5 against
     the float64 oracle and the float64 backward over the records."""
-    grad_tests.test_kernels_match_reference_gradient_arrays(name)
-    grad_tests.test_kernels_match_reference_pinned_oracle(name, 5)
+    rnn_gradient_arrays(name, "tc_tanh")
+    rnn_pinned_oracle(name, 5, "tc_tanh")
 
 
 # ---------------------------------------------------------------------------------------------------- direct steps
-
-def rnn_net(N, O, heads, impl, wseed=3, H=128):
-    from ic3net_b200 import models
-    a = argparse.Namespace(nagents=N, hid_size=H, comm_passes=1, recurrent=True, rnn_type="MLP", continuous=False,
-                           naction_heads=list(heads), comm_mask_zero=False, comm_mode="avg", hard_attn=False,
-                           comm_init="uniform", share_weights=False, seed=0, env_id0=0, commnet=False, policy_impl=impl)
-    torch.manual_seed(wseed)
-    return models.RNN(a, O)
-
 
 def twin_nets(N, O, heads, wseed=3):
     tc, simt = rnn_net(N, O, heads, "tc_tanh", wseed), rnn_net(N, O, heads, "simt", wseed)
@@ -225,7 +167,7 @@ def test_sampling_with_explicit_draws(heads):
     rows = np.arange(R)
     u24[rows % 8 == 0] = 0
     u24[rows % 8 == 1] = (1 << 24) - 1
-    ref = step_f64(tc.state_dict(), obs.reshape(R, O).double(), h, None, N)
+    ref = rnn_step_f64(tc.state_dict(), obs.reshape(R, O).double(), h, None, N)
     off = 0
     for k, na in enumerate(heads):
         cdf = np.cumsum(np.exp(ref["logp"][:, off:off + na].cpu().numpy()), -1)
@@ -284,7 +226,7 @@ def test_row_counts_and_rows_past_R(case):
         assert torch.equal(x, y)
     worst = {}
     compare("%s R=%d tiles=%d CTAs=%d" % (case, R, -(-R // TILE), 2 * nsm),
-            {k: out[k][:R] for k in ("h", "value", "logp")}, step_f64(net.state_dict(), obs.reshape(R, O).double(), h, fresh, 1),
+            {k: out[k][:R] for k in ("h", "value", "logp")}, rnn_step_f64(net.state_dict(), obs.reshape(R, O).double(), h, fresh, 1),
             worst)
     print(case, R, " ".join("%s %.2e" % kv for kv in worst.items()))
 
@@ -304,7 +246,7 @@ def test_fresh_slots_start_from_zero_and_dead_cars_are_stepped_like_simt():
     draws = torch.full((R, 1), 1 << 23, dtype=torch.int32, device="cuda")
     assert direct_step(tc, obs, h, o_tc, alive=alive, fresh=fresh, draws=draws)[0] == 0
     assert direct_step(simt, obs, h, o_simt, alive=alive, fresh=fresh, draws=draws)[0] == 0
-    ref = step_f64(tc.state_dict(), obs.reshape(R, O).double(), h, fresh, N)
+    ref = rnn_step_f64(tc.state_dict(), obs.reshape(R, O).double(), h, fresh, N)
     for o in (o_tc, o_simt):
         compare("fresh / dead", {k: o[k] for k in ("h", "value", "logp")}, ref)
     assert int((alive == 0).sum()) > R // 4
@@ -326,7 +268,7 @@ def test_weight_limit_of_the_fp16_split():
             act, val, h2 = net([obs, h], {})
             torch.cuda.synchronize()
             net.check_errors()
-            ref = step_f64(net.state_dict(), obs.reshape(B * N, O).double(), h, None, N)
+            ref = rnn_step_f64(net.state_dict(), obs.reshape(B * N, O).double(), h, None, N)
             compare("|w| 255", dict(h=h2, value=val.reshape(-1), logp=torch.cat(act, -1).reshape(B * N, -1)), ref)
         else:
             net([obs, h], {})
@@ -336,39 +278,23 @@ def test_weight_limit_of_the_fp16_split():
 
 # ---------------------------------------------------------------------------------------------------- 7. gradient
 
-def test_full_size_gradient_matches_float64(tc_tanh_trainers):
+def test_full_size_gradient_matches_float64():
     for name, B in ((PP, 8192), (TJ, 4096)):
-        grad_tests.test_full_size_gradient_matches_float64(name, B)
+        rnn_full_size(name, B, "tc_tanh")
 
 
-def test_gradient_is_bit_identical_run_to_run(tc_tanh_trainers):
-    grad_tests.test_repeated_compute_grad_is_bit_identical()
+def test_gradient_is_bit_identical_run_to_run():
+    rnn_run_to_run("tc_tanh")
 
 
 @pytest.mark.parametrize("name,window", [(PP, 4), (TJ, 1)])
-def test_windowed_records_are_bit_identical(name, window, tc_tanh_trainers):
+def test_windowed_records_are_bit_identical(name, window):
     """Window mode re-runs the index encoder and the tc_tanh step: the same h' as the rollout bit for bit."""
-    grad_tests.test_windowed_records_are_bit_identical(name, window)
-
-
-def schedule_grads(out_dir):
-    grad_tests.make_trainer = functools.partial(make_trainer, policy_impl="tc_tanh")
-    grad_tests.schedule_grads(out_dir)
+    rnn_windows(name, window, "tc_tanh")
 
 
 def test_one_stream_schedule_is_bit_identical(tmp_path):
-    mine, child = tmp_path / "overlap", tmp_path / "serial"
-    mine.mkdir()
-    child.mkdir()
-    code = ("import sys; sys.path[:0] = [%r, %r]; import test_gpu_rnn_tc as m; m.schedule_grads(%%r)" % (ROOT, TESTS))
-    for d, over in ((mine, {}), (child, dict(IC3_BPTT_OVERLAP="0"))):
-        r = subprocess.run([sys.executable, "-c", code % str(d)], env=dict(os.environ, **over), cwd=ROOT,
-                           capture_output=True, text=True, timeout=600)
-        assert r.returncode == 0, r.stderr[-4000:]
-    files = sorted(os.listdir(mine))
-    assert files == sorted(os.listdir(child)) and len(files) > 3
-    for f in files:
-        assert np.array_equal(np.load(mine / f), np.load(child / f)), f
+    one_stream_schedule(tmp_path, "gpu_harness", "schedule_rnn_tc_tanh", more_than=3)
 
 
 # ---------------------------------------------------------------------------------------------------- 8. graph

@@ -7,38 +7,12 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import finish_args, golden_names, load_golden, make_oracle_env, ns, tj_tables
+from gpu_harness import close, cpu, episode_trainer
+from helpers import golden_names, load_golden, make_oracle_env, tj_tables
 from oracle import policy as opolicy
-from oracle.gen_golden import make_weights
 from oracle.rollout import run_episode
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
-
-
-def close(a, b, tol=TOL):
-    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
-    return np.all(np.abs(a - b) <= tol * np.maximum(1.0, np.abs(b)))
-
-
-def cpu(t):
-    return t.detach().cpu().numpy()
-
-
-def build(meta, B, obs_mode="index", use_graph=False, seed=None, env_id0=0, impl=None, **over):
-    from ic3net_b200 import data
-    from ic3net_b200.comm import CommNetMLP
-    from ic3net_b200.trainer import Trainer
-    args = ns(meta["args"], nenvs=B, seed=meta["seed"] if seed is None else seed, env_id0=env_id0,
-              obs_mode=obs_mode, use_graph=use_graph, policy_impl=impl, **over)
-    env = data.init(args.env_name, args)
-    finish_args(args, env)
-    if impl == "tc" and args.hid_size != 128:
-        pytest.skip("tensor-core path is specialised for hid_size 128")
-    net = CommNetMLP(args, args.num_inputs)
-    sd = make_weights(meta["weights_seed"], args.num_inputs, args.hid_size, args.naction_heads, args.comm_init)
-    net.load_state_dict({k: torch.from_numpy(v).float() for k, v in sd.items()})
-    return args, env, net, Trainer(args, net, env), opolicy.params_to_f64(sd)
 
 
 @pytest.mark.parametrize("name", golden_names("ep_"))
@@ -48,7 +22,7 @@ def test_first_episode_matches_reference_golden(name, obs_mode, impl):
     meta, z = load_golden(name)
     ids = meta["env_ids"]
     B = max(ids) + 1
-    args, env, net, tr, p = build(meta, B, obs_mode, impl=impl)
+    args, env, net, tr, p = episode_trainer(meta, B, obs_mode, impl=impl)
     T = args.max_steps
     batch = tr.rollout(T, meta["epoch"])
     torch.cuda.synchronize()
@@ -77,7 +51,7 @@ def test_lockstep_rollout_matches_oracle(name, B, T, impl):
     """Every slot, every episode (auto-reset, cut at the batch end), teacher-forced with
     the GPU's own actions so both sides stay on one trajectory; plus the stat sums."""
     meta, z = load_golden(name)
-    args, env, net, tr, p = build(meta, B, "index", seed=321, env_id0=50, impl=impl)
+    args, env, net, tr, p = episode_trainer(meta, B, seed=321, env_id0=50, impl=impl)
     is_tj = args.env_name == "traffic_junction"
     batch = tr.rollout(T, 0)
     stat = tr.collect_stat()
@@ -134,7 +108,7 @@ def test_graph_replay_equals_eager():
     meta, z = load_golden("ep_tj_medium_ic3net")
     res = {}
     for use_graph in (True, False):
-        args, env, net, tr, p = build(meta, 16, "index", use_graph=use_graph, seed=5)
+        args, env, net, tr, p = episode_trainer(meta, 16, use_graph=use_graph, seed=5)
         out = []
         for k in range(3):
             b = tr.rollout(40, 0)
@@ -156,7 +130,7 @@ def test_encoder_forms_give_identical_rollouts(name):
         pytest.skip("fused encoder is part of the tensor-core path (hid_size 128)")
     res = []
     for mode, overlap in (("index", False), ("dense", True), ("dense", False)):
-        args, env, net, tr, p = build(meta, 24, mode, seed=77)
+        args, env, net, tr, p = episode_trainer(meta, 24, mode, seed=77)
         if overlap:
             tr.OVERLAP_MIN_OBS_BYTES = 0             # the small fixtures take the two-stream path too
         assert tr._overlap_obs() == overlap
@@ -173,7 +147,7 @@ def test_pp_hard_full_size_rollout_properties():
     """BASELINE c2 at full size (8192 envs): invariants of a 20-step lock-step rollout."""
     meta, z = load_golden("ep_pp_hard_ic3net")
     B, T = 8192, 20
-    args, env, net, tr, p = build(meta, B, "index", seed=9)
+    args, env, net, tr, p = episode_trainer(meta, B, seed=9)
     b = tr.rollout(T, 0)
     stat = tr.collect_stat()
     assert stat["num_steps"] == B * T
@@ -230,7 +204,7 @@ def test_full_size_rollout_sampled_slots_match_oracle(name, B):
     step by step through the float64 oracle (bit-exact integers / rewards, 1e-5 on values and log-probs)."""
     meta, z = load_golden(name)
     T, seed, id0 = 24, 4242, 1000
-    args, env, net, tr, p = build(meta, B, "index", seed=seed, env_id0=id0)
+    args, env, net, tr, p = episode_trainer(meta, B, seed=seed, env_id0=id0)
     batch = tr.rollout(T, 0)
     stat = tr.collect_stat()
     assert stat["num_steps"] == B * T
@@ -252,7 +226,7 @@ def test_observation_handle_api_is_bit_identical_to_the_dense_tensor_api(name, i
     meta, z = load_golden(name)
     out = {}
     for api in ("dense", "handle"):
-        args, env, net, tr, p = build(meta, 9, "index", seed=77, impl=impl, obs_api=api)
+        args, env, net, tr, p = episode_trainer(meta, 9, seed=77, impl=impl, obs_api=api)
         B, N = 9, args.nagents
         obs = env.reset(0)
         assert isinstance(obs, LazyObs) == (api == "handle")
@@ -295,7 +269,7 @@ def test_graph_is_recaptured_when_the_curriculum_moves_the_spawn_rate():
     over = dict(add_rate_min=0.05, add_rate_max=0.5, curr_start=0, curr_end=4)
     res = {}
     for use_graph in (False, True):
-        args, env, net, tr, p = build(meta, 16, "index", use_graph=use_graph, seed=5, **over)
+        args, env, net, tr, p = episode_trainer(meta, 16, use_graph=use_graph, seed=5, **over)
         out = []
         for epoch in (0, 1, 2, 3, 3, 6):
             b = tr.rollout(20, epoch)

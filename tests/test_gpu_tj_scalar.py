@@ -11,18 +11,14 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import finish_args, load_golden, ns, tj_tables
-from oracle.gen_golden import make_weights
+from gpu_harness import LOSS_ATOL, LOSS_RTOL, close, cpu, episode_trainer, trainer_rows
+from helpers import load_golden, ns, tj_tables
 from tj_scalar_oracle import make_env as make_oracle
 
 pytestmark = pytest.mark.gpu
 ENV_CASES = ["tj_scalar_env_easy", "tj_scalar_env_medium_v1", "tj_scalar_env_hard"]
 EP = "tj_scalar_ep_medium_ic3net"
 GRAD = "tj_scalar_grad_hard_ic3net_h128"
-
-
-def cpu(t):
-    return t.detach().cpu().numpy()
 
 
 def lib():
@@ -138,26 +134,6 @@ def test_index_and_fused_encoders_equal_the_dense_encoder(H):
     assert torch.equal(x_dense[dead], net.encoder.bias.detach().expand(int(dead.sum()), H))
 
 
-def build(meta, B, obs_mode="index", impl=None, seed=None, env_id0=0, use_graph=False, weights=True, **over):
-    from ic3net_b200 import data
-    from ic3net_b200.comm import CommNetMLP
-    from ic3net_b200.trainer import Trainer
-    args = ns(meta["args"], nenvs=B, seed=meta["seed"] if seed is None else seed, env_id0=env_id0, obs_mode=obs_mode,
-              use_graph=use_graph, policy_impl=impl, **over)
-    env = data.init(args.env_name, args)
-    finish_args(args, env)
-    net = CommNetMLP(args, args.num_inputs)
-    if weights:                 # make_weights draws the recurrent CommNet's state_dict
-        sd = make_weights(meta["weights_seed"], args.num_inputs, args.hid_size, args.naction_heads, args.comm_init)
-        net.load_state_dict({k: torch.from_numpy(v).float() for k, v in sd.items()})
-    return args, env, net, Trainer(args, net, env)
-
-
-def close(a, b, tol=1e-5):
-    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
-    return np.all(np.abs(a - b) <= tol * np.maximum(1.0, np.abs(b)))
-
-
 @pytest.mark.parametrize("obs_mode", ["index", "dense"])
 @pytest.mark.parametrize("impl", ["tc", "simt"])
 def test_episode_matches_reference_fixture(obs_mode, impl):
@@ -165,7 +141,7 @@ def test_episode_matches_reference_fixture(obs_mode, impl):
     masks, values and log-probabilities."""
     meta, z = load_golden(EP)
     ids = meta["env_ids"]
-    args, env, net, tr = build(meta, max(ids) + 1, obs_mode, impl)
+    args, env, net, tr, _ = episode_trainer(meta, max(ids) + 1, obs_mode, impl=impl)
     assert not net.fuses_encoder(env.env) and net.encoder_table(env.env) is None
     assert not tr._overlap_obs()
     batch = tr.rollout(args.max_steps, meta["epoch"])
@@ -193,9 +169,8 @@ def test_full_size_every_row_matches_float64(impl):
     """Traffic-junction hard, 4096 slots x 20 cars: a 14-step rollout with max_steps 6 (every slot resets twice, cars
     spawn, crash, leave and sit dead at (0,0)); every row of every step against the float64 step on the observation
     rebuilt from the recorded env state (Trainer._record_state: loc, alive, last_act, route_id)."""
-    from test_gpu_policy_rows import trainer_rows
     meta, _ = load_golden(GRAD)
-    args, env, net, tr = build(meta, 4096, "index", impl, seed=5, record_for_grad=True, grad_window=1, max_steps=6)
+    args, env, net, tr, _ = episode_trainer(meta, 4096, impl=impl, seed=5, record_for_grad=True, grad_window=1, max_steps=6)
     assert not tr.grad_kernels
     trainer_rows(tr, 14, "tj scalar hard %s" % impl)
     alive = cpu(tr._buf["s_alive"])
@@ -207,8 +182,8 @@ def test_autograd_gradient_matches_the_reference(impl):
     """One slot on the fixture's streams stops at the reference's batch boundary and the autograd recompute (observations
     rebuilt from the records by ic3_tj_obs) gives the reference's compute_grad gradient."""
     meta, z = load_golden(GRAD)
-    args, env, net, tr = build(meta, 1, "index", impl, env_id0=meta["env_id"], record_for_grad=True, grad_window=16,
-                               grad_impl="auto")
+    args, env, net, tr, _ = episode_trainer(meta, 1, impl=impl, env_id0=meta["env_id"], record_for_grad=True,
+                                            grad_window=16, grad_impl="auto")
     assert tr.grad_impl == "autograd" and not tr.grad_kernels
     batch, stat = tr.run_batch(0)
     if stat["num_steps"] != meta["num_steps"]:
@@ -217,7 +192,7 @@ def test_autograd_gradient_matches_the_reference(impl):
     tr.optimizer.zero_grad(set_to_none=False)
     s = tr.compute_grad(batch)
     for q in ("action_loss", "value_loss", "entropy"):
-        assert np.isclose(s[q], meta[q], rtol=2e-4, atol=1e-3), (q, s[q], meta[q])
+        assert np.isclose(s[q], meta[q], rtol=LOSS_RTOL, atol=LOSS_ATOL), (q, s[q], meta[q])
     checked = 0
     for key, prm in net.named_parameters():
         if "g_" + key in z.files:
@@ -240,8 +215,8 @@ def test_gradient_kernels_refuse_the_scalar_vocabulary(grad_impl):
         if grad_impl == "kernels_ff" else {}
     m = dict(meta, args=dict(meta["args"], **kw))
     with pytest.raises(NotImplementedError):
-        build(m, 4, "index", "tc" if grad_impl == "kernels" else "simt", weights=False, record_for_grad=True,
-              grad_window=16, grad_impl=grad_impl)
+        episode_trainer(m, 4, impl="tc" if grad_impl == "kernels" else "simt", weights=False, record_for_grad=True,
+                        grad_window=16, grad_impl=grad_impl)
 
 
 @pytest.mark.parametrize("obs_mode", ["index", "dense"])
@@ -249,7 +224,7 @@ def test_graph_replay_equals_eager(obs_mode):
     meta, _ = load_golden(EP)
     res = {}
     for use_graph in (True, False):
-        args, env, net, tr = build(meta, 16, obs_mode, "tc", seed=5, use_graph=use_graph)
+        args, env, net, tr, _ = episode_trainer(meta, 16, obs_mode, impl="tc", seed=5, use_graph=use_graph)
         out = []
         for _ in range(3):
             b = tr.rollout(40, 0)

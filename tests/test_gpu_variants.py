@@ -8,29 +8,10 @@ import numpy as np
 import pytest
 import torch
 
+from gpu_harness import close, variant_net
 from helpers import golden_names, load_golden
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-5
-
-
-def close(a, b, tol=TOL):
-    a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
-    return np.all(np.abs(a - b) <= tol * np.maximum(1.0, np.abs(b)))
-
-
-def build(meta, z, policy_impl=None):
-    from ic3net_b200 import models
-    from ic3net_b200.comm import CommNetMLP
-    a = argparse.Namespace(**meta["args"])
-    a.naction_heads, a.continuous = list(meta["heads"]), False
-    a.policy_impl = policy_impl
-    cls = {"commnet": CommNetMLP, "mlp": models.MLP, "rnn": models.RNN}[meta["model"]]
-    net = cls(a, meta["obs_dim"])
-    sd = {k[3:]: torch.from_numpy(z[k]).float() for k in z.files if k.startswith("sd_")}
-    assert set(net.state_dict().keys()) == set(sd.keys()), (sorted(net.state_dict().keys()), sorted(sd.keys()))
-    net.load_state_dict(sd)                               # reference checkpoints load key for key
-    return a, net
 
 
 @pytest.mark.parametrize("impl", [None, "simt"])
@@ -39,7 +20,7 @@ def test_variant_forward_matches_reference(name, impl):
     """impl None = the implementation the module picks (wgmma for the LSTM-cell variants at hid_size 128, whatever the
     number of comm passes); 'simt' = the fp32 kernel forced on those same cases."""
     meta, z = load_golden(name)
-    a, net = build(meta, z, impl)
+    a, net = variant_net(meta, z, impl)
     if impl == "simt" and not (net.tc_capable and a.hid_size == 128):
         pytest.skip("the module picks the SIMT kernel for this case anyway")
     n, H = a.nagents, a.hid_size
@@ -79,7 +60,7 @@ def test_tanh_cell_variant_on_tensor_core_path_is_refused():
     for name in ("var_commnet_nonrec2", "var_mlp", "var_rnn_tanh"):
         meta, z = load_golden(name)
         with pytest.raises(NotImplementedError):
-            build(meta, z, policy_impl="tc")
+            variant_net(meta, z, policy_impl="tc")
 
 
 @pytest.mark.parametrize("model,extra", [("rnn", dict(rnn_type="MLP")), ("rnn", dict(rnn_type="LSTM")), ("mlp", {}),

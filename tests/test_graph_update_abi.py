@@ -5,7 +5,7 @@ import ctypes as C
 
 import pytest
 
-from test_bptt_args import FAKE, _setup
+from bptt_plan import FAKE, _setup
 
 E_NULL, E_RANGE = -1, -2
 
