@@ -32,6 +32,7 @@ ERR_BAD_ACTION = 4
 ERR_PIPELINE = 0x100
 ERR_FP16_RANGE = 0x200
 ERR_GRAD_DIV = 0x400
+ERR_TRACE_SLOT = 0x800
 
 PP_MODES = {"mixed": 0, "cooperative": 1, "competitive": 2}
 
@@ -57,7 +58,7 @@ class RolloutIO(C.Structure):
                 ("episodes", C.c_int32), ("halted", _p), ("rec_valid", _p), ("snap_T", C.c_int32),
                 ("reserved1", C.c_int32), ("snap_fresh", _p), ("snap_comm", _p), ("snap_alive", _p), ("snap_tep", _p),
                 ("snap_pp_loc", _p), ("snap_tj_loc", _p), ("snap_tj_alive", _p), ("snap_tj_last_act", _p),
-                ("snap_tj_route_id", _p)]
+                ("snap_tj_route_id", _p), ("out_loc", _p), ("out_success", _p)]
 
 
 class TJCfg(C.Structure):
@@ -146,6 +147,20 @@ class FfGradIO(C.Structure):
                 ("valid", _p)]
 
 
+class EvalStepIO(C.Structure):
+    _fields_ = [("pp_env", C.POINTER(PPCfg)), ("pp_state", C.POINTER(PPState)), ("tj_env", C.POINTER(TJCfg)),
+                ("tj_state", C.POINTER(TJState)), ("nheads", C.c_int32), ("logp_cols", C.c_int32),
+                ("comm_col", C.c_int32), ("max_steps", C.c_int32), ("t_ep", _p), ("halted", _p), ("action", _p),
+                ("value", _p), ("logp", _p), ("reward", _p), ("fresh", _p), ("out_loc", _p), ("out_success", _p),
+                ("err", _p)]
+
+
+class EvalTrace(C.Structure):
+    _fields_ = [("T", C.c_int32), ("K", C.c_int32), ("slots", _p), ("loc", _p), ("loc_next", _p), ("alive", _p),
+                ("action", _p), ("value", _p), ("reward", _p), ("t_ep", _p), ("done", _p), ("success", _p),
+                ("valid", _p), ("comm_prob", _p), ("route_id", _p)]
+
+
 # every symbol include/ic3net_b200.h declares: name -> (restype, argtypes)
 _PTR = C.c_void_p
 SYMBOLS = {
@@ -184,6 +199,8 @@ SYMBOLS = {
                                        _PTR]),
     "ic3_sample_actions": (C.c_int, [C.POINTER(PolicyCfg), _PTR, _PTR, _PTR, _PTR, _PTR]),
     "ic3_random_policy_step": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyIO), _PTR, _PTR]),
+    "ic3_trace_step": (C.c_int, [C.POINTER(EvalStepIO), C.POINTER(EvalTrace), C.c_int32, _PTR]),
+    "ic3_comm_map_step": (C.c_int, [C.POINTER(EvalStepIO), _PTR, _PTR]),
     "ic3_returns_scan": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, _PTR, _PTR, _PTR, _PTR,
                                    _PTR]),
     "ic3_bptt_workspace_bytes": (C.c_uint64, [C.POINTER(BpttPlan)]),

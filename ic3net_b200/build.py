@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libic3net_b200.so")
 SOURCES = ["c_api.cu", "pp_env.cu", "tj_env.cu", "policy.cu", "policy_tc.cu", "ff_tc.cu", "ff_grad_tc.cu", "bptt_tc.cu",
-           "returns.cu", "optim.cu", "random_policy.cu"]
+           "returns.cu", "optim.cu", "random_policy.cu", "eval_trace.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [ "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]

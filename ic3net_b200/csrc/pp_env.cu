@@ -177,6 +177,11 @@ __global__ void pp_step_kernel(PPArgs a, const int32_t* __restrict__ act, int ac
           a.st.tick[e] += 1;
         }
         if (r.has) {
+          if (r.io.out_loc && lane <= N) {             // before the auto-reset (ic3_trace_step)
+            int* d = r.io.out_loc + ((size_t)e * (N + 1) + lane) * 2;
+            d[0] = rr;
+            d[1] = cc;
+          }
           const bool done_t = ic3_rollout_tail(r.io, e, a.cfg.B, NA, lane, (float)rew, done, 1, 0, success);
           if (done_t) {
             __syncwarp();

@@ -72,6 +72,7 @@ __device__ __forceinline__ bool ic3_rollout_tail(const ic3_rollout_io& r, int e,
     if (r.rec_valid) r.rec_valid[(size_t)r.t * B + e] = 1;
     r.fresh[e] = done_t ? 1 : 0;
     r.t_ep[e] = done_t ? 0 : tep + 1;
+    if (r.out_success) r.out_success[e] = (done_t && success > 0) ? 1 : 0;
     int nsteps = 0;
     if (r.stat_steps) nsteps = (r.stat_steps[e] += 1);                             // :109
     if (done_t) {

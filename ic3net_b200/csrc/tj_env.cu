@@ -211,6 +211,10 @@ __global__ void tj_step_kernel(TJArgs a, const int32_t* __restrict__ act, int ac
         a.st.tick[e] = tick + 1;
       }
       if (r.has) {
+        if (r.io.out_loc && lane < N) {                // before the auto-reset (ic3_trace_step)
+          r.io.out_loc[i * 2] = rr;
+          r.io.out_loc[i * 2 + 1] = cc;
+        }
         // episode_over is never set by the reference env (:219,252): episodes end on max_steps
         const bool done_t = ic3_rollout_tail(r.io, e, cfg.B, N, lane, (float)rew, false, (uint8_t)alive,
                                              (uint8_t)completed, 1 - failed);

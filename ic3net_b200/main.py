@@ -106,6 +106,10 @@ def build_parser():
     parser.add_argument('--eval_nenvs', type=int, default=None, help='evaluation slots per GPU (default: --nenvs)')
     parser.add_argument('--eval_greedy', action='store_true', default=False,
                         help='evaluate with the argmax action of every head instead of sampled actions')
+    parser.add_argument('--eval_trace', type=str, default='',
+                        help='with --eval_every: record every evaluation and write PREFIX_epoch<E>.npz (rank 0\'s slots: '
+                             'per-step trajectories and the map of where agents open their gate)')
+    parser.add_argument('--eval_trace_slots', type=int, default=8, help='evaluation slots recorded by --eval_trace')
     return parser
 
 
@@ -229,6 +233,21 @@ def save_checkpoint(path, policy_net, log, trainer, evals=None):
         torch.save(d, path)
 
 
+def save_eval_trace(prefix, epoch, args, grid_shape, trace, cmap):
+    """PREFIX_epoch<E>.npz: the trace's arrays, the comm map's under 'map_<key>', and what it takes to read them."""
+    d = dict(trace.arrays())
+    for k, v in (cmap or {}).items():
+        d['map_' + k] = v
+    pp = args.env_name == 'predator_prey'
+    d.update(env_name=np.array(args.env_name), grid_shape=np.asarray(grid_shape, dtype=np.int64),
+             nagents=np.int64(args.nagents),
+             nfriendly=np.int64(getattr(args, 'nfriendly', args.nagents) if pp else args.nagents),
+             naction_heads=np.asarray(args.naction_heads, dtype=np.int64), max_steps=np.int64(args.max_steps),
+             episodes=np.int64(args.eval_episodes), greedy=np.int64(bool(args.eval_greedy)),
+             hard_attn=np.int64(bool(args.hard_attn and args.commnet)))
+    np.savez(prefix + '_epoch%d.npz' % epoch, **d)
+
+
 def load_checkpoint(path, policy_net, log, trainer):
     """main.py:267-272.  Returns the checkpoint's evaluation results [(epoch, stat dict)] ([] without 'eval')."""
     with _utils_alias():
@@ -306,7 +325,15 @@ def main(argv=None):
                 print(ln)
             print('steps/s {:.0f}'.format(nsteps / max(epoch_time, 1e-9)))
         if args.eval_every and epoch % args.eval_every == 0:    # every rank plays its slots; the sum is reduced
-            es = trainer.evaluate(args.eval_episodes, args.eval_greedy)
+            if args.eval_trace:
+                cfg, tj = env.env.cfg, args.env_name == 'traffic_junction'
+                es, trace, cmap = trainer.evaluate_trace(args.eval_episodes, args.eval_greedy,
+                                                         slots=min(args.eval_trace_slots, args.eval_nenvs or args.nenvs))
+                if rank == 0:
+                    save_eval_trace(args.eval_trace, epoch, args, (cfg.h, cfg.w) if tj else (cfg.dim, cfg.dim),
+                                    trace, cmap)
+            else:
+                es = trainer.evaluate(args.eval_episodes, args.eval_greedy)
             evals.append((epoch, es))
             if rank == 0:
                 print(eval_line(es, args.eval_greedy, args.eval_episodes, eval_slots))

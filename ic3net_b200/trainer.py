@@ -61,7 +61,7 @@ from collections import namedtuple
 import torch
 import torch.nn.functional as F
 
-from . import _lib, data
+from . import _lib, data, eval_trace
 from .models import Random
 from .optim import FlatRMSprop
 from .utils import merge_stat
@@ -391,17 +391,18 @@ class Trainer(object):
             return False
         return self.policy_net.fuses_encoder(e)
 
-    def _enqueue(self, T, quota=0, b=None, e=None, episodes=0, greedy=False):
+    def _enqueue(self, T, quota=0, b=None, e=None, episodes=0, greedy=False, recorder=None):
         """Enqueue T lock-step iterations on the current stream (no host sync).  quota > 0: reference batch
         boundary -- a slot halts at the first episode end with >= quota steps (ic3_rollout_io.batch_size);
         quota = 0: episodes still open at iteration T-1 are cut there.  b, e: buffers and env (default: the training
         rollout's; evaluate passes its own, which hold no records and one lock-step of action / log-prob / value
         scratch, and no observation block: x comes from the env state); episodes > 0: episode quota
-        (ic3_rollout_io.episodes); greedy: argmax actions (ic3_policy_cfg.greedy)."""
+        (ic3_rollout_io.episodes); greedy: argmax actions (ic3_policy_cfg.greedy); recorder: an eval_trace.Recorder
+        that keeps every lock-step between its policy step and its env step (evaluate_trace)."""
         b = self._buf if b is None else b
         e = self.env.env if e is None else e
         if self.random_policy:
-            return self._enqueue_random(T, quota, b, e, episodes)
+            return self._enqueue_random(T, quota, b, e, episodes, recorder)
         net = self.policy_net
         lib = _lib.load()
         B = e.nenvs
@@ -482,12 +483,16 @@ class Trainer(object):
                 torch.linalg.vector_norm(b['c'], math.inf, out=b['c_abs'][t])
             if overlap:
                 main.wait_stream(side)
-            self._env_step(t, T, quota, snap, s, b, e, episodes)
+            if recorder is not None:
+                recorder.step(t, s)
+            self._env_step(t, T, quota, snap, s, b, e, episodes, recorder)
+        if recorder is not None:
+            recorder.finish(T, s)
 
-    def _env_step(self, t, T, quota, snap, s, b=None, e=None, episodes=0):
+    def _env_step(self, t, T, quota, snap, s, b=None, e=None, episodes=0, recorder=None):
         """Env step of lock-step iteration t on the actions the policy step wrote to the records, with the
-        Trainer.get_episode bookkeeping and auto-reset (ic3_rollout_io; ``snap``: its snap_* fields).  b, e, episodes:
-        see _enqueue; a record evaluate's buffers do not hold is passed as NULL."""
+        Trainer.get_episode bookkeeping and auto-reset (ic3_rollout_io; ``snap``: its snap_* fields).  b, e, episodes,
+        recorder: see _enqueue; a record evaluate's buffers do not hold is passed as NULL."""
         b = self._buf if b is None else b
         e = self.env.env if e is None else e
         args = self.args
@@ -505,7 +510,8 @@ class Trainer(object):
                            rec_episode_mask=rec('emask'), rec_mini_mask=rec('mini'),
                            rec_alive=rec('ralive'), stat_reward=b['stat_reward'].data_ptr(),
                            stat_comm=b['stat_comm'].data_ptr(), stat_success=b['stat_success'].data_ptr(),
-                           stat_episodes=b['stat_episodes'].data_ptr(), stat_steps=b['stat_steps'].data_ptr())
+                           stat_episodes=b['stat_episodes'].data_ptr(), stat_steps=b['stat_steps'].data_ptr(),
+                           **(recorder.rollout_fields() if recorder is not None else {}))
         if self.is_tj:
             _lib.check(lib.ic3_tj_step(C.byref(e.cfg), C.byref(e.state), act.data_ptr(), nh, None,
                                        b['step_reward'].data_ptr(), None, b['err'].data_ptr(), C.byref(r), s))
@@ -520,7 +526,7 @@ class Trainer(object):
         return _lib.PolicyCfg(B=e.nenvs, N=self.args.nagents, nheads=len(heads),
                               head_dim=(C.c_int32 * _lib.MAX_HEADS)(*heads), env_id0=e.cfg.env_id0, seed=e.cfg.seed)
 
-    def _enqueue_random(self, T, quota, b, e, episodes=0):
+    def _enqueue_random(self, T, quota, b, e, episodes=0, recorder=None):
         """_enqueue for models.Random: per lock-step iteration one ic3_random_policy_step (value, log-probs and actions
         into the records, from the env's action tick) and the env step."""
         lib = _lib.load()
@@ -531,7 +537,11 @@ class Trainer(object):
             io = _lib.PolicyIO(tick=e.tick.data_ptr(), value=b['value'][r].data_ptr(), logp=b['logp'][r].data_ptr(),
                                action=b['action'][r].data_ptr())
             _lib.check(lib.ic3_random_policy_step(C.byref(cfg), C.byref(io), None, s))
-            self._env_step(t, T, quota, {}, s, b, e, episodes)
+            if recorder is not None:
+                recorder.step(t, s)
+            self._env_step(t, T, quota, {}, s, b, e, episodes, recorder)
+        if recorder is not None:
+            recorder.finish(T, s)
 
     def _episode_boundary(self, epoch, b=None, e=None):
         b = self._buf if b is None else b
@@ -723,9 +733,8 @@ class Trainer(object):
         self._eval = dict(env=e, buf=self._slot_buffers(ne, 1, e.device))
         return self._eval
 
-    def evaluate_vector(self, episodes=1, greedy=False, epoch=None):
-        """evaluate without the host read: the device float64 statistics vector (stat_vector's layout) of the episodes,
-        and the evaluation env they were played on."""
+    def _eval_prepare(self, episodes, greedy, epoch):
+        """Argument checks and the evaluation env's add_rate for an evaluation; returns (env, buffers, lock-steps)."""
         episodes = int(episodes)
         if episodes < 1:
             raise ValueError("evaluate plays at least one episode per slot, not %d" % episodes)
@@ -738,7 +747,13 @@ class Trainer(object):
                 e.set_add_rate(self.env.env)
             else:
                 e.curriculum_until(int(epoch))
-        T = episodes * int(self.args.max_steps)
+        return e, b, episodes * int(self.args.max_steps)
+
+    def evaluate_vector(self, episodes=1, greedy=False, epoch=None):
+        """evaluate without the host read: the device float64 statistics vector (stat_vector's layout) of the episodes,
+        and the evaluation env they were played on."""
+        e, b, T = self._eval_prepare(episodes, greedy, epoch)
+        episodes = int(episodes)
         self._begin(T, None, b, e)
         run = lambda: self._enqueue(T, 0, b, e, episodes, greedy)
         if self.use_graph:
@@ -756,6 +771,42 @@ class Trainer(object):
         read.  Successive calls continue the evaluation env's random streams."""
         vec, e = self.evaluate_vector(episodes, greedy, epoch)
         return self.stat_from_vector(vec.cpu().numpy(), e)
+
+    def evaluate_trace_vector(self, episodes=1, greedy=False, epoch=None, slots=8, comm_map=True):
+        """evaluate_trace without the host read: (device statistics vector, evaluation env, eval_trace.Recorder holding
+        the trajectories and the comm map on the device)."""
+        e, b, T = self._eval_prepare(episodes, greedy, epoch)
+        episodes = int(episodes)
+        slots = eval_trace.parse_slots(slots, e.nenvs)
+        key = (T, slots, bool(comm_map))
+        rec = self._eval.get('trace')
+        if rec is None or rec.key != key:
+            self._graphs.pop('evaluate_trace', None)       # its graph writes into the recorder it replaces
+            self._eval['trace'] = None
+            rec = self._eval['trace'] = eval_trace.Recorder(self, e, b, T, slots, bool(comm_map))
+            rec.key = key
+        self._begin(T, None, b, e)
+
+        def run():
+            rec.begin()
+            self._enqueue(T, 0, b, e, episodes, greedy, recorder=rec)
+        if self.use_graph:
+            self._replay('evaluate_trace', self._graph_key(T, e, episodes, bool(greedy)) + key[1:], b, e, [run])
+        else:
+            run()
+        return self.stat_vector(b, e), e, rec
+
+    def evaluate_trace(self, episodes=1, greedy=False, epoch=None, slots=8, comm_map=True):
+        """evaluate, recording what the agents do: returns (stat, trace, cmap).  stat is what evaluate returns for the
+        same call (the same loop, env, buffers and random streams).  trace (eval_trace.EvalTraceResult) holds every
+        lock-step of the recorded slots -- ``slots``: the first K evaluation slots, or a sequence of distinct local slot
+        numbers -- as [T, K, ...] numpy arrays, T = episodes * max_steps.  cmap (comm_map; else None): integer counts
+        over every slot of visits to each cell and each episode step and, with --hard_attn, of gate openings there
+        (ic3_comm_map_step).  The trace and the map come back in one device->host copy."""
+        vec, e, rec = self.evaluate_trace_vector(episodes, greedy, epoch, slots, comm_map)
+        stat = self.stat_from_vector(vec.cpu().numpy(), e)
+        trace, cmap = rec.to_host()
+        return stat, trace, cmap
 
     def steps_per_batch(self):
         return self.batch_plan()[0]

@@ -55,8 +55,9 @@ enum {
   IC3_ERR_FP16_RANGE = 0x200, /* tensor-core path: an activation (|a| >= 4094) or folded weight (|w| >= 255) left the range of
                                the fp16 hi/lo operand split; results of that step are not trustworthy -> use the
                                fp32 SIMT kernels (policy_impl = 'simt') for such a model */
-  IC3_ERR_GRAD_DIV = 0x400  /* ic3_rmsprop_step_dev: the step count it divides by was not a positive finite number; the
+  IC3_ERR_GRAD_DIV = 0x400, /* ic3_rmsprop_step_dev: the step count it divides by was not a positive finite number; the
                                parameters, gradients and second moments were left unchanged */
+  IC3_ERR_TRACE_SLOT = 0x800 /* ic3_trace_step: a recorded slot index lies outside [0, B); nothing was written for it */
 };
 
 enum { IC3_PP_MIXED = 0, IC3_PP_COOPERATIVE = 1, IC3_PP_COMPETITIVE = 2 };
@@ -146,6 +147,11 @@ typedef struct {
   uint8_t* snap_tj_alive;  /* [T, B, N] */
   uint8_t* snap_tj_last_act; /* [T, B, N] */
   int32_t* snap_tj_route_id; /* [T, B, N] */
+  /* Outcome of this step as it stands before the auto-reset overwrites it, for the evaluation recorder
+   * (ic3_trace_step); both optional, written for every slot that steps: */
+  int32_t* out_loc;        /* [B, rows, 2] positions after the move (predator_prey: N+1 rows, predators then prey;
+                              traffic_junction: N cars, dead ones at (0, 0)) */
+  uint8_t* out_success;    /* [B] 1 = the step ended the slot's episode with env.stat['success'] > 0, else 0 */
 } ic3_rollout_io;
 
 /* reset(): predator_prey_env.py:146-168.  Draws N+1 distinct cells per env from
@@ -436,6 +442,72 @@ int ic3_sample_actions(const ic3_policy_cfg* cfg, const float* logp, const uint3
 #define IC3_RANDOM_WORDS 16
 int ic3_random_policy_step(const ic3_policy_cfg* cfg, const ic3_policy_io* io, const uint32_t* random_draws,
                            void* stream);
+
+/* ------------------------------------------------------------------------
+ * Evaluation recorder (Trainer.evaluate_trace): what the lock-step loop of an evaluation holds for one step only --
+ * the state entering step t, the policy step's outputs, the env step's outcome -- kept before the next step overwrites
+ * it.  Both calls are launched between policy step t and env step t; they never read the host and allocate nothing,
+ * so they can be captured into a CUDA graph.  Bad arguments return IC3_E_* before any device work.
+ * ---------------------------------------------------------------------- */
+typedef struct {
+  /* the evaluation environment: exactly one pair (HOST pointers to the structs of device pointers) */
+  const ic3_pp_cfg* pp_env;
+  const ic3_pp_state* pp_state;
+  const ic3_tj_cfg* tj_env;
+  const ic3_tj_state* tj_state;
+  int32_t nheads;          /* columns of action, 1 .. IC3_MAX_HEADS */
+  int32_t logp_cols;       /* columns of logp: the sum of the head sizes */
+  int32_t comm_col;        /* column of logp holding log p(open) of the gate head (--hard_attn), -1 without a gate */
+  int32_t max_steps;       /* args.max_steps, 1 .. 32767 */
+  /* the lock-step's scratch (device): state entering step t and the outputs of policy step t */
+  const int32_t* t_ep;     /* [B] step index inside the episode */
+  const uint8_t* halted;   /* [B] 1 = the slot has played its quota (ic3_rollout_io.halted) */
+  const int32_t* action;   /* [B, NA, nheads] */
+  const float* value;      /* [B*NA] */
+  const float* logp;       /* [B, NA, logp_cols] */
+  /* what env step t - 1 left (ic3_rollout_io of that step) */
+  const float* reward;     /* [B, NA] the step's reward */
+  const uint8_t* fresh;    /* [B] 1 = that step ended the slot's episode */
+  const int32_t* out_loc;  /* [B, rows, 2] ic3_rollout_io.out_loc */
+  const uint8_t* out_success; /* [B] ic3_rollout_io.out_success */
+  int32_t* err;            /* device flag word (IC3_ERR_TRACE_SLOT) */
+} ic3_eval_step_io;
+
+/* Trajectories of K slots over T = episodes * max_steps lock-steps, arrays [T, K, ...] (device).  NA = agent rows of
+ * the policy (predator_prey: N, + 1 with enemy_comm; traffic_junction: N), rows = positions per slot (predator_prey:
+ * N+1, predators then prey; traffic_junction: N).  Row t of a slot that had already played its quota entering step t
+ * is padding: valid = 0 and every other field 0. */
+typedef struct {
+  int32_t T, K;
+  const int32_t* slots;    /* [K] local slot numbers, each in [0, B) */
+  int16_t* loc;            /* [T, K, rows, 2] positions entering step t */
+  int16_t* loc_next;       /* [T, K, rows, 2] positions after step t's move, before the auto-reset */
+  uint8_t* alive;          /* [T, K, NA] the agent is in the environment entering step t (predator_prey: 1) */
+  int8_t* action;          /* [T, K, NA, nheads] */
+  float* value;            /* [T, K, NA] */
+  float* reward;           /* [T, K, NA] */
+  int16_t* t_ep;           /* [T, K] */
+  uint8_t* done;           /* [T, K] step t ended the slot's episode */
+  uint8_t* success;        /* [T, K] step t ended an episode with env.stat['success'] > 0 */
+  uint8_t* valid;          /* [T, K] */
+  float* comm_prob;        /* [T, K, NA] exp(log p(open)) of the gate action of step t; NULL without a gate */
+  int16_t* route_id;       /* [T, K, N] traffic_junction only (route of each car entering step t, -1 before its
+                              first spawn); NULL for predator_prey */
+} ic3_eval_trace;
+
+/* Call t (0 <= t < T, between policy step t and env step t) writes row t's state and policy outputs and row t - 1's
+ * outcome (loc_next, reward, done, success); one closing call with t == T after the last env step writes row T - 1's
+ * outcome alone.  A slot index outside [0, B) raises IC3_ERR_TRACE_SLOT. */
+int ic3_trace_step(const ic3_eval_step_io* io, const ic3_eval_trace* tr, int32_t t, void* stream);
+
+/* Adds this lock-step's counts over every agent row of the environment into counts (device uint64), keyed by the
+ * state entering step t.  Counted: rows of slots that have not played their quota, of friendly agents (the prey row
+ * under enemy_comm is not), alive (traffic_junction: in the environment); "open" = the gate action of step t is 1.
+ * Layout, npos = dim*dim (predator_prey) or h*w (traffic_junction), cell = row * width + col:
+ *   visits[npos], open[npos], visits_t[max_steps], open_t[max_steps], and for predator_prey
+ *   visits_reached[2], open_reached[2] (index 1: the predator stands on the prey);
+ * without a gate (comm_col < 0) the open* blocks are absent.  Integer sums: the counts do not depend on the order. */
+int ic3_comm_map_step(const ic3_eval_step_io* io, uint64_t* counts, void* stream);
 
 /* ------------------------------------------------------------------------
  * REINFORCE returns  (trainer.py:160-173), the first step of Trainer.compute_grad
