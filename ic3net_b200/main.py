@@ -8,11 +8,13 @@ path (``--plot``/visdom, ``--display``/curses) are
 parsed and rejected with a clear message.  New flags: ``--nenvs`` (environment slots per GPU),
 ``--obs_mode`` (index | dense), ``--policy_impl`` (tc | simt | tc_tanh | tc_ff), ``--use_graph``, ``--graph_update``,
 and evaluation of whole episodes every K epochs (``--eval_every``, ``--eval_episodes``, ``--eval_nenvs``,
-``--eval_greedy``; Trainer.evaluate).
+``--eval_greedy``; Trainer.evaluate), and resuming an interrupted run exactly where it stopped (``--resumable``,
+``--resume``: a run-state sidecar beside every checkpoint; SIGTERM / SIGINT save and exit after the update in flight).
 Multi-GPU: launch with ``python -m torch.distributed.run --nproc-per-node N -m ic3net_b200.main ...``.
 """
 import argparse
 import os
+import signal
 import sys
 import time
 
@@ -110,6 +112,13 @@ def build_parser():
                         help='with --eval_every: record every evaluation and write PREFIX_epoch<E>.npz (rank 0\'s slots: '
                              'per-step trajectories and the map of where agents open their gate)')
     parser.add_argument('--eval_trace_slots', type=int, default=8, help='evaluation slots recorded by --eval_trace')
+    parser.add_argument('--resumable', action='store_true', default=False,
+                        help='with --save: every checkpoint write also writes the run state to <checkpoint>.run, and '
+                             'SIGTERM / SIGINT save both and exit after the update in flight, so --resume can continue '
+                             'the run bit for bit')
+    parser.add_argument('--resume', default='', type=str,
+                        help='continue the run saved with --resumable at checkpoint PATH (and PATH.run) at the epoch '
+                             'and update where it stopped; --num_epochs stays the total of the whole run')
     return parser
 
 
@@ -224,13 +233,64 @@ class _utils_alias(object):
         return False
 
 
-def save_checkpoint(path, policy_net, log, trainer, evals=None):
-    """main.py:260-265; evals: the evaluation results [(epoch, stat dict)], stored under 'eval' unless None."""
+def write_atomic(writers):
+    """writers: [(path, write(tmp_path))].  Every file is written under a temporary name beside its path first, then
+    all are moved into place with os.replace.  If a writer fails, its temporaries are removed and the files already
+    at the paths stay as they were."""
+    tmps = []
+    try:
+        for path, write in writers:
+            tmps.append('%s.tmp%d' % (path, os.getpid()))
+            write(tmps[-1])
+    except BaseException:
+        for t in tmps:
+            if os.path.exists(t):
+                os.remove(t)
+        raise
+    for (path, _), t in zip(writers, tmps):
+        os.replace(t, path)
+
+
+def checkpoint_position(d):
+    """(optimizer steps, logged epochs) of a checkpoint dict: a run-state sidecar records both, so a sidecar that
+    does not belong to its checkpoint (a kill between the two renames of a save) is recognised."""
+    steps = [int(float(st.get('step', 0))) for st in d['trainer']['state'].values()]
+    return max(steps, default=0), len(d['log']['epoch'].data)
+
+
+def save_checkpoint(path, policy_net, log, trainer, evals=None, run=None):
+    """main.py:260-265; evals: the evaluation results [(epoch, stat dict)], stored under 'eval' unless None.
+    run: with --resumable, {'ep', 'update', 'stat', 'state'} -- the loop position (the 0-based epoch, the updates of
+    it done, their merged stat) and the trainer's run_state() -- written to path + '.run' beside the checkpoint, with
+    the checkpoint's optimizer steps and epochs.  Both files are replaced atomically (write_atomic)."""
     d = dict(policy_net=policy_net.state_dict(), log=log, trainer=trainer.state_dict())
     if evals is not None:
         d['eval'] = list(evals)
-    with _utils_alias():
-        torch.save(d, path)
+
+    def write(p):
+        with _utils_alias():
+            torch.save(d, p)
+    writers = [(path, write)]
+    if run is not None:
+        steps, epochs = checkpoint_position(d)
+        side = dict(run, version=RUN_FILE_VERSION, steps=steps, epochs=epochs)
+        writers.append((path + '.run', lambda p: torch.save(side, p)))
+    write_atomic(writers)
+
+
+RUN_FILE_VERSION = 1
+
+
+def read_run_file(path):
+    """The run-state sidecar of checkpoint path (save_checkpoint's ``run``, plus 'version', 'steps', 'epochs')."""
+    if not os.path.exists(path + '.run'):
+        raise FileNotFoundError("no run state %s.run beside the checkpoint %s: --resume continues a run saved with "
+                                "--resumable (--load restores the policy and log of any checkpoint)" % (path, path))
+    run = torch.load(path + '.run', weights_only=False)
+    if run.get('version') != RUN_FILE_VERSION:
+        raise ValueError("%s.run has version %r; this program reads version %d" % (path, run.get('version'),
+                                                                                  RUN_FILE_VERSION))
+    return run
 
 
 def save_eval_trace(prefix, epoch, args, grid_shape, trace, cmap):
@@ -252,10 +312,54 @@ def load_checkpoint(path, policy_net, log, trainer):
     """main.py:267-272.  Returns the checkpoint's evaluation results [(epoch, stat dict)] ([] without 'eval')."""
     with _utils_alias():
         d = torch.load(path, weights_only=False)
+    return _apply_checkpoint(d, policy_net, log, trainer)
+
+
+def _apply_checkpoint(d, policy_net, log, trainer):
     policy_net.load_state_dict(d['policy_net'])
     log.update({k: LogField(*v) for k, v in d['log'].items()})
     trainer.load_state_dict(d['trainer'])
     return list(d.get('eval', []))
+
+
+def resume_checkpoint(path, run, policy_net, log, trainer):
+    """--resume: load_checkpoint after checking that run (read_run_file) belongs to the checkpoint and loading its run
+    state into the trainer (which refuses another configuration).  Returns the checkpoint's evaluation results."""
+    with _utils_alias():
+        d = torch.load(path, weights_only=False)
+    have = checkpoint_position(d)
+    if have != (run['steps'], run['epochs']):
+        raise ValueError("%s.run does not belong to %s: it was written after %d optimizer steps and %d epochs, the "
+                         "checkpoint after %d and %d (a save was interrupted between its two files)"
+                         % (path, path, run['steps'], run['epochs'], have[0], have[1]))
+    trainer.load_run_state(run['state'])
+    return _apply_checkpoint(d, policy_net, log, trainer)
+
+
+class StopOnSignal(object):
+    """--resumable: SIGTERM and SIGINT only raise a flag; the training loop saves and exits after the update in flight.
+    restore() puts the previous handlers back."""
+    SIGNALS = (signal.SIGTERM, signal.SIGINT)
+
+    def __init__(self):
+        self.raised = False
+        self._old = {s: signal.signal(s, self._raise) for s in self.SIGNALS}
+
+    def _raise(self, signum, frame):
+        self.raised = True
+
+    def restore(self):
+        for s, h in self._old.items():
+            signal.signal(s, h)
+
+    def agreed(self, device, world):
+        """Has any rank been signalled?  A signal can reach the ranks at different updates, so they agree through a
+        one-element all-reduce (MAX) after every update."""
+        if world == 1:
+            return self.raised
+        f = torch.tensor([int(self.raised)], dtype=torch.int32, device=device)
+        torch.distributed.all_reduce(f, op=torch.distributed.ReduceOp.MAX)
+        return bool(f.item())
 
 
 def main(argv=None):
@@ -263,6 +367,12 @@ def main(argv=None):
     parser = build_parser()
     init_args_for_env(parser, ['x'] + list(argv))
     args = derive_args(parser.parse_args(argv))
+    if args.resume and args.load:
+        parser.error("--resume continues a run from its checkpoint and run state; it takes no --load")
+    if args.resumable and not args.save:
+        parser.error("--resumable writes the run state beside the --save checkpoint; give --save")
+    run = read_run_file(args.resume) if args.resume else None
+    args.resumable = args.resumable or bool(args.resume and args.save)
 
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
@@ -272,6 +382,8 @@ def main(argv=None):
     dev = torch.device("cuda", local)
     if world > 1:
         torch.distributed.init_process_group("nccl", device_id=dev)
+    if run is not None and args.seed == -1:          # a resumed run plays on the streams of the run it continues
+        args.seed = int(run['state']['fingerprint']['seed'])
     if args.seed == -1:                              # main.py:157-158; ONE draw for the whole job: rank 0's
         seed = torch.tensor([int(np.random.randint(0, 10000))], dtype=torch.int64, device=dev)
         if world > 1:
@@ -306,17 +418,45 @@ def main(argv=None):
     evals = []
     if args.load:
         evals = load_checkpoint(args.load, policy_net, log, trainer)
+    start_ep, start_update, partial = 0, 0, None
+    if run is not None:
+        evals = resume_checkpoint(args.resume, run, policy_net, log, trainer)
+        start_ep, start_update, partial = run['ep'], run['update'], run['stat']
     eval_slots = world * (args.eval_nenvs or args.nenvs)
+    stop = StopOnSignal() if args.resumable else None
+    try:
+        _train(args, trainer, policy_net, env, log, evals, eval_slots, rank, world, dev, stop, start_ep, start_update,
+               partial)
+    finally:
+        if stop is not None:
+            stop.restore()
+    if world > 1:
+        torch.distributed.destroy_process_group()
+    return 0
 
-    for ep in range(args.num_epochs):
+
+def _train(args, trainer, policy_net, env, log, evals, eval_slots, rank, world, dev, stop, start_ep, start_update,
+           partial):
+    """The epoch loop of main.py:207-258 from epoch start_ep, update start_update, with the merged stat partial of the
+    updates of that epoch already done (a resumed run)."""
+    for ep in range(start_ep, args.num_epochs):
         epoch_begin = time.time()
-        stat = dict()
-        for n in range(args.epoch_size):
+        first = ep == start_ep
+        stat = dict(partial) if first and partial else dict()
+        for n in range(start_update if first else 0, args.epoch_size):
             if args.rollout_only:
                 batch, s = trainer.run_batch(ep)
             else:
                 s = trainer.train_batch(ep)              # main.py:213: the 0-based epoch drives the TJ curriculum
             merge_stat(s, stat)
+            if stop is not None and stop.agreed(dev, world):
+                state = trainer.run_state()              # gathered from every rank
+                if rank == 0:
+                    save_checkpoint(args.save, policy_net, log, trainer, evals if (evals or args.eval_every) else None,
+                                    dict(ep=ep, update=n + 1, stat=stat, state=state))
+                    print('Stopped in epoch {} after update {} of {}; continue with --resume {}'.format(
+                        ep + 1, n + 1, args.epoch_size, args.save), flush=True)
+                return
         epoch_time = time.time() - epoch_begin
         nsteps = stat.get('num_steps', 0)
         epoch = update_log(log, stat)
@@ -338,13 +478,11 @@ def main(argv=None):
             if rank == 0:
                 print(eval_line(es, args.eval_greedy, args.eval_episodes, eval_slots))
         ck = evals if (evals or args.eval_every) else None     # without evaluation the checkpoint stays as it was
+        run = dict(ep=ep + 1, update=0, stat=None, state=trainer.run_state()) if args.resumable else None
         if args.save_every and ep and args.save != '' and ep % args.save_every == 0 and rank == 0:
-            save_checkpoint(args.save + '_' + str(ep), policy_net, log, trainer, ck)
+            save_checkpoint(args.save + '_' + str(ep), policy_net, log, trainer, ck, run)
         if args.save != '' and rank == 0:                # main.py:257-258: every epoch
-            save_checkpoint(args.save, policy_net, log, trainer, ck)
-    if world > 1:
-        torch.distributed.destroy_process_group()
-    return 0
+            save_checkpoint(args.save, policy_net, log, trainer, ck, run)
 
 
 if __name__ == '__main__':

@@ -24,6 +24,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from .trainer import check_fingerprint
 from .utils import merge_stat
 
 
@@ -230,3 +231,20 @@ class MultiGPUTrainer(object):
     def load_state_dict(self, state):
         self.trainer.load_state_dict(state)
         self.sync_parameters()
+
+    def run_state(self):
+        """Trainer.run_state over every rank: each rank's state is gathered to rank 0, which returns
+        {'fingerprint', 'ranks': [rank 0's, rank 1's, ...]}; the other ranks return None.  Every rank must call it."""
+        tr = self.trainer
+        if not _dist_on():
+            return tr.run_state()
+        mine = tr.rank_state()
+        got = [None] * self.world if self.rank == 0 else None
+        dist.gather_object(mine, got, dst=0)
+        return dict(fingerprint=tr.run_fingerprint(), ranks=got) if self.rank == 0 else None
+
+    def load_run_state(self, state):
+        """Every rank loads the same state (written by rank 0) and takes its own slice; the fingerprint, world size
+        included, must match."""
+        check_fingerprint(state['fingerprint'], self.trainer.run_fingerprint())
+        self.trainer.load_rank_state(state['ranks'][self.rank])

@@ -157,6 +157,7 @@ class Trainer(object):
         self._buf = None
         self._record_mode = None             # 'full' | 'window' per allocation (record_mode)
         self._ff_K = None                    # graph_update: kernels_ff chunk length frozen into the captured update
+        self.ff_chunk_pin = None             # kernels_ff chunk length of a resumed run's last update (load_rank_state)
         self._graphs = {}                    # 'rollout' | 'evaluate' | 'update' -> (key, graphs, result) (_replay)
         self._side = None                    # stream of the dense observation writer (_overlap_obs)
         # graph_update: train_batch replays the whole update from CUDA graphs (update)
@@ -1094,7 +1095,9 @@ class Trainer(object):
     def _ff_chunk_steps(self, T, cfg):
         """Lock-steps per chunk K of ic3_ff_grad_chunk for a T-step rollout: what the workspace of K steps needs must fit
         in the device's free memory plus the allocator's unused reserve, minus RECORD_MARGIN_BYTES; K * B * N is at most
-        FF_CHUNK_ROWS (at least one step)."""
+        FF_CHUNK_ROWS (at least one step).  A resumed run keeps the K its last update used (ff_chunk_pin)."""
+        if self.ff_chunk_pin is not None:
+            return int(self.ff_chunk_pin)
         e = self.env.env
         lib = _lib.load()
         rows = e.nenvs * self.args.nagents
@@ -1284,3 +1287,84 @@ class Trainer(object):
 
     def load_state_dict(self, state):
         self.optimizer.load_state_dict(state)
+
+    # ------------------------------------------------------------------ run state (resuming a run)
+    # What crosses an update boundary besides the parameters and the RMSprop state of state_dict: the env's device state
+    # (its tick / episode counters key the Philox streams), the traffic-junction curriculum, the evaluation env once it
+    # exists, and the kernels_ff chunk length K (gradients for different K differ in the last bits).  Graph caches are
+    # not state: the first update after a load captures anew.
+
+    def run_fingerprint(self):
+        """What shapes the run, as plain values: load_run_state refuses a state taken under other values."""
+        a, e = self.args, self.env.env
+        dist = torch.distributed
+        fp = {k: getattr(a, k, None) for k in RUN_FINGERPRINT_ARGS}
+        fp.update(world=dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1,
+                  nenvs=e.nenvs, eval_nenvs=int(getattr(a, 'eval_nenvs', None) or e.nenvs), seed=int(getattr(a, 'seed', 0)),
+                  grad_impl=self.grad_impl, policy_impl=getattr(self.policy_net, 'policy_impl', None),
+                  use_graph=self.use_graph, graph_update=self.graph_update)
+        return fp
+
+    def run_state(self):
+        """{'fingerprint': run_fingerprint(), 'ranks': [this process's state]} on the host; load_run_state takes it."""
+        return dict(fingerprint=self.run_fingerprint(), ranks=[self.rank_state()])
+
+    def load_run_state(self, state):
+        """Continue the run that run_state() was taken from (the parameters and the optimizer come from state_dict).
+        Refuses, before touching the device, a state whose fingerprint differs from this trainer's."""
+        check_fingerprint(state['fingerprint'], self.run_fingerprint())
+        if len(state['ranks']) != 1:
+            raise ValueError("the run state holds %d ranks; MultiGPUTrainer.load_run_state takes it" % len(state['ranks']))
+        self.load_rank_state(state['ranks'][0])
+
+    def rank_state(self):
+        """This process's part of the run state: its training env, its evaluation env (None before the first
+        evaluation) and the kernels_ff chunk length of the last update (None for other gradients)."""
+        ev = getattr(self, '_eval', None)
+        return dict(env=self._env_state(self.env.env), eval=None if ev is None else self._env_state(ev['env']),
+                    ff_chunk_steps=getattr(self, 'ff_chunk_steps', None) if self.grad_ff else None)
+
+    def load_rank_state(self, d):
+        self._load_env_state(self.env.env, d['env'])
+        if d['eval'] is not None:
+            self._load_env_state(self._eval_state()['env'], d['eval'])
+        self.ff_chunk_pin = d['ff_chunk_steps']
+
+    def _env_state(self, e):
+        d = dict(device={k: v.cpu() for k, v in zip(e._STATE, e.snapshot())})
+        if self.is_tj:
+            d.update(exact_rate=e.exact_rate, add_rate=e.add_rate, epoch_last_update=e.epoch_last_update)
+        return d
+
+    def _load_env_state(self, e, d):
+        snap = []
+        for k in e._STATE:
+            live, v = getattr(e, k), d['device'][k]
+            if v.shape != live.shape or v.dtype != live.dtype:
+                raise ValueError("run state field %s is %s %s, the env holds %s %s" % (k, v.dtype, tuple(v.shape),
+                                                                                       live.dtype, tuple(live.shape)))
+            snap.append(v.to(live.device))
+        e.restore(snap)
+        if self.is_tj:
+            e.exact_rate, e.add_rate, e.epoch_last_update = d['exact_rate'], d['add_rate'], d['epoch_last_update']
+            e.cfg.spawn_thr = e._spawn_thr()
+
+
+# The arguments of a run's fingerprint besides those Trainer.run_fingerprint resolves: env and geometry, policy, loss
+# and optimizer, and the loop (a missing one reads None)
+RUN_FINGERPRINT_ARGS = (
+    'env_name', 'nagents', 'dim', 'vision', 'mode', 'nenemies', 'enemy_comm', 'no_stay', 'moving_prey', 'difficulty',
+    'vocab_type', 'add_rate_min', 'add_rate_max', 'curr_start', 'curr_end',
+    'commnet', 'random', 'recurrent', 'rnn_type', 'hid_size', 'hard_attn', 'comm_mode', 'comm_passes', 'comm_mask_zero',
+    'comm_action_one', 'share_weights', 'mean_ratio', 'detach_gap', 'obs_mode', 'forward_grad',
+    'gamma', 'lrate', 'entr', 'value_coeff', 'normalize_rewards', 'grad_window',
+    'batch_size', 'max_steps', 'batch_boundary', 'epoch_size', 'rollout_only')
+
+
+def check_fingerprint(stored, current):
+    """Raise ValueError naming every field whose stored value differs from the current one."""
+    diff = ['%s (stored %r, now %r)' % (k, stored.get(k), current.get(k))
+            for k in sorted(set(stored) | set(current)) if stored.get(k) != current.get(k)]
+    if diff:
+        raise ValueError("the run state belongs to another configuration: " + ', '.join(diff) +
+                         "; a run resumes only under the configuration it started with")
