@@ -161,6 +161,11 @@ class EvalTrace(C.Structure):
                 ("valid", _p), ("comm_prob", _p), ("route_id", _p)]
 
 
+class EvalCommIO(C.Structure):
+    _fields_ = [("h", _p), ("comm", _p), ("alive", _p), ("fresh", _p), ("H", C.c_int32), ("comm_avg", C.c_int32),
+                ("hard", C.c_int32)]
+
+
 # every symbol include/ic3net_b200.h declares: name -> (restype, argtypes)
 _PTR = C.c_void_p
 SYMBOLS = {
@@ -201,6 +206,9 @@ SYMBOLS = {
     "ic3_random_policy_step": (C.c_int, [C.POINTER(PolicyCfg), C.POINTER(PolicyIO), _PTR, _PTR]),
     "ic3_trace_step": (C.c_int, [C.POINTER(EvalStepIO), C.POINTER(EvalTrace), C.c_int32, _PTR]),
     "ic3_comm_map_step": (C.c_int, [C.POINTER(EvalStepIO), _PTR, _PTR]),
+    "ic3_trace_comm_step": (C.c_int, [C.POINTER(EvalStepIO), C.POINTER(EvalCommIO), C.POINTER(EvalTrace), _PTR, _PTR,
+                                      _PTR, C.c_int32, _PTR]),
+    "ic3_message_map_step": (C.c_int, [C.POINTER(EvalStepIO), C.POINTER(EvalCommIO), _PTR, _PTR]),
     "ic3_returns_scan": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, _PTR, _PTR, _PTR, _PTR,
                                    _PTR]),
     "ic3_bptt_workspace_bytes": (C.c_uint64, [C.POINTER(BpttPlan)]),

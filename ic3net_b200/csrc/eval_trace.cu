@@ -147,6 +147,177 @@ __global__ void __launch_bounds__(256) comm_map_kernel(EvalArgs a, unsigned long
 constexpr int kMapCtas = 264;                        // 2 per SM of an H100 SXM: few global flushes, every SM busy
 constexpr size_t kMapSmemMax = 96 * 1024;
 
+// ---- messages (ic3_trace_comm_step / ic3_message_map_step) -------------------------------------------------------
+
+struct CommArgs {
+  EvalEnv env;
+  ic3_eval_step_io io;
+  ic3_eval_comm_io cm;
+};
+
+int comm_check(const ic3_eval_step_io* io, const ic3_eval_comm_io* cm, CommArgs* a) {
+  int rc = eval_check(io, &a->env);
+  if (rc) return rc;
+  if (!cm || !cm->h || !cm->alive || !cm->fresh || (cm->hard && !cm->comm)) return IC3_E_NULL;
+  if (cm->H < 16 || cm->H > 1024 || cm->H % 16) return IC3_E_RANGE;
+  if (cm->comm_avg < 0 || cm->comm_avg > 1 || cm->hard < 0 || cm->hard > 1) return IC3_E_RANGE;
+  a->io = *io;
+  a->cm = *cm;
+  return IC3_OK;
+}
+
+// The gates of one slot, computed by a whole warp (lane j reads row j): bit j of g = g_j, of live = the row's message
+// is its h (alive and not fresh); den = S's divisor.
+struct SlotGates {
+  uint32_t g, live;
+  double den;
+};
+
+__device__ __forceinline__ SlotGates slot_gates(const ic3_eval_comm_io& cm, int e, int NA, int lane) {
+  const bool fr = cm.fresh[e] != 0;
+  bool al = false, cmj = false;
+  if (lane < NA) {
+    al = fr || cm.alive[(size_t)e * NA + lane] != 0;
+    cmj = cm.hard ? (!fr && cm.comm[(size_t)e * NA + lane] != 0) : true;
+  }
+  const uint32_t alive = __ballot_sync(0xffffffffu, al), g = __ballot_sync(0xffffffffu, al && cmj);
+  const int n_alive = __popc(alive);
+  return SlotGates{g, fr ? 0u : alive, (cm.comm_avg && n_alive > 1) ? (double)(n_alive - 1) : 1.0};
+}
+
+// The messages of one column: m[j] = h_j for a live row, else 0 (all loads issued together); returns
+// sum_j g_j m_j in float64, in agent order.
+__device__ __forceinline__ double load_messages(const ic3_eval_comm_io& cm, const SlotGates& s, int e, int NA, int col,
+                                                float (&m)[IC3_MAX_AGENTS]) {
+#pragma unroll
+  for (int j = 0; j < IC3_MAX_AGENTS; ++j)
+    m[j] = (j < NA && (s.live >> j & 1u)) ? cm.h[((size_t)e * NA + j) * cm.H + col] : 0.f;
+  double tot = 0.0;
+#pragma unroll
+  for (int j = 0; j < IC3_MAX_AGENTS; ++j)
+    if (j < NA && (s.g >> j & 1u)) tot += (double)m[j];
+  return tot;
+}
+
+// S_k of one column from the column's gated sum
+__device__ __forceinline__ float received(const SlotGates& s, int k, double tot, float mk) {
+  return (s.g >> k & 1u) ? (float)((tot - (double)mk) / s.den) : 0.f;
+}
+
+// One CTA of 128 threads per recorded slot, thread = column.
+__global__ void __launch_bounds__(128) trace_comm_kernel(CommArgs a, ic3_eval_trace tr, float* __restrict__ msg_h,
+                                                         uint8_t* __restrict__ msg_gate, float* __restrict__ msg_in,
+                                                         int t) {
+  const EvalEnv& v = a.env;
+  const ic3_eval_comm_io& cm = a.cm;
+  const int k = blockIdx.x, NA = v.NA, H = cm.H, lane = threadIdx.x & 31;
+  const int e = tr.slots[k];
+  if (e < 0 || e >= v.B) {
+    if (threadIdx.x == 0) atomicOr(a.io.err, IC3_ERR_TRACE_SLOT);
+    return;
+  }
+  const size_t row = ((size_t)t * tr.K + k) * NA;
+  const bool ok = a.io.halted[e] == 0;
+  const SlotGates s = ok ? slot_gates(cm, e, NA, lane) : SlotGates{0u, 0u, 1.0};
+  for (int j = threadIdx.x; j < NA; j += blockDim.x) msg_gate[row + j] = (uint8_t)(s.g >> j & 1u);
+  for (int col = threadIdx.x; col < H; col += blockDim.x) {
+    float m[IC3_MAX_AGENTS];
+    const double tot = load_messages(cm, s, e, NA, col, m);
+#pragma unroll
+    for (int j = 0; j < IC3_MAX_AGENTS; ++j) {
+      if (j >= NA) break;
+      msg_h[(row + j) * H + col] = m[j];
+      msg_in[(row + j) * H + col] = received(s, j, tot, m[j]);
+    }
+  }
+}
+
+__device__ __forceinline__ long long fixed32(float v) { return llrintf(v * 4294967296.f); }
+
+// Warp per slot, CTA y owns columns [16y, 16y + 16): lanes 0-15 add the sent messages of those columns, lanes 16-31
+// the received ones, so each h element is loaded by one warp once; lane i first reads row i's keys, which the row loop
+// takes by shuffle.  PRIV: the CTA's [R][32] slice (and, for y == 0, the senders counts) is summed in shared memory and
+// flushed once with global atomics; otherwise global atomics.
+template <bool PRIV>
+__global__ void __launch_bounds__(1024) message_map_kernel(CommArgs a, unsigned long long* __restrict__ sums, int R) {
+  extern __shared__ unsigned long long s_sum[];      // [R][32], then senders [R]
+  const EvalEnv& v = a.env;
+  const ic3_eval_step_io& io = a.io;
+  const ic3_eval_comm_io& cm = a.cm;
+  const int H = cm.H, NA = v.NA, S = io.max_steps, P = v.npos;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
+  const int role = lane >> 4, col = blockIdx.y * 16 + (lane & 15);
+  const bool counts = blockIdx.y == 0 && lane == 0;
+  const int nsh = R * 32 + (blockIdx.y == 0 ? R : 0);
+  unsigned long long* g_blk = sums + (size_t)role * R * H + col;     // [R, H] block of this lane, at its column
+  unsigned long long* g_cnt = sums + (size_t)2 * R * H;
+  if (PRIV) {
+    for (int i = threadIdx.x; i < nsh; i += blockDim.x) s_sum[i] = 0ull;
+    __syncthreads();
+  }
+  auto add = [&](int key, long long val) {
+    if (!val) return;
+    if (PRIV) atomicAdd(&s_sum[key * 32 + lane], (unsigned long long)val);
+    else atomicAdd(&g_blk[(size_t)key * H], (unsigned long long)val);
+  };
+  auto count = [&](int key) {
+    if (PRIV) atomicAdd(&s_sum[R * 32 + key], 1ull);
+    else atomicAdd(&g_cnt[key], 1ull);
+  };
+  const int nf = v.pp ? v.N : NA;
+  for (int e = blockIdx.x * nwarp + warp; e < v.B; e += gridDim.x * nwarp) {
+    if (io.halted[e]) continue;                      // warp-uniform
+    const SlotGates s = slot_gates(cm, e, NA, lane);
+    float m[IC3_MAX_AGENTS];
+    const double tot = load_messages(cm, s, e, NA, col, m);
+    // row `lane`'s keys: cell (or -1), prey flag (or -1); -2 = not counted
+    int my_cell = -2, my_on = -1;
+    if (lane < nf && (!v.alive || v.alive[(size_t)e * v.N + lane])) {
+      const int32_t* l = v.loc + ((size_t)e * v.rows + lane) * 2;
+      const int c = l[0] * v.width + l[1];
+      my_cell = (c >= 0 && c < P) ? c : -1;
+      if (v.pp) {
+        const int32_t* q = v.loc + ((size_t)e * v.rows + v.N) * 2;
+        my_on = (l[0] == q[0] && l[1] == q[1]) ? 1 : 0;
+      }
+    }
+    const int te = io.t_ep[e];
+    const bool in_t = te >= 0 && te < S;
+#pragma unroll
+    for (int i = 0; i < IC3_MAX_AGENTS; ++i) {
+      if (i >= nf) break;
+      const int cell = __shfl_sync(0xffffffffu, my_cell, i), on = __shfl_sync(0xffffffffu, my_on, i);
+      if (cell == -2) continue;
+      const bool open = s.g >> i & 1u;
+      if (role == 0 && !open) continue;
+      const long long val = fixed32(role == 0 ? m[i] : received(s, i, tot, m[i]));
+      if (cell >= 0) add(cell, val);
+      if (in_t) add(P + te, val);
+      if (on >= 0) add(P + S + on, val);
+      if (counts && open) {
+        if (cell >= 0) count(cell);
+        if (in_t) count(P + te);
+        if (on >= 0) count(P + S + on);
+      }
+    }
+  }
+  if (PRIV) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < R * 32; i += blockDim.x) {
+      const unsigned long long val = s_sum[i];
+      const int l = i & 31;
+      if (val) atomicAdd(&sums[(size_t)(l >> 4) * R * H + (size_t)(i >> 5) * H + blockIdx.y * 16 + (l & 15)], val);
+    }
+    if (blockIdx.y == 0)
+      for (int i = threadIdx.x; i < R; i += blockDim.x)
+        if (s_sum[R * 32 + i]) atomicAdd(&g_cnt[i], s_sum[R * 32 + i]);
+  }
+}
+
+constexpr int kMsgCtas = 132;                        // one 1024-thread CTA per SM of an H100 SXM
+constexpr int kMsgThreads = 1024;
+constexpr size_t kMsgSmemMax = 200 * 1024;
+
 }  // namespace
 
 extern "C" int ic3_trace_step(const ic3_eval_step_io* io, const ic3_eval_trace* tr, int32_t t, void* stream) {
@@ -190,6 +361,45 @@ extern "C" int ic3_comm_map_step(const ic3_eval_step_io* io, uint64_t* counts, v
     comm_map_kernel<true><<<grid, 256, smem, s>>>(a, c, ncount);
   } else {
     comm_map_kernel<false><<<grid, 256, 0, s>>>(a, c, ncount);
+  }
+  IC3_LAUNCH_CHECK();
+  return IC3_OK;
+}
+
+extern "C" int ic3_trace_comm_step(const ic3_eval_step_io* io, const ic3_eval_comm_io* cm, const ic3_eval_trace* tr,
+                                   float* msg_h, uint8_t* msg_gate, float* msg_in, int32_t t, void* stream) {
+  CommArgs a;
+  int rc = comm_check(io, cm, &a);
+  if (rc) return rc;
+  if (!tr || !tr->slots || !io->err || !msg_h || !msg_gate || !msg_in) return IC3_E_NULL;
+  if (tr->T < 1 || tr->K < 1 || t < 0 || t >= tr->T) return IC3_E_RANGE;
+  trace_comm_kernel<<<tr->K, 128, 0, (cudaStream_t)stream>>>(a, *tr, msg_h, msg_gate, msg_in, t);
+  IC3_LAUNCH_CHECK();
+  return IC3_OK;
+}
+
+extern "C" int ic3_message_map_step(const ic3_eval_step_io* io, const ic3_eval_comm_io* cm, int64_t* sums,
+                                    void* stream) {
+  CommArgs a;
+  int rc = comm_check(io, cm, &a);
+  if (rc) return rc;
+  if (!sums) return IC3_E_NULL;
+  const int R = a.env.npos + io->max_steps + (a.env.pp ? 2 : 0);
+  const int ny = cm->H / 16;
+  const int nx = (int)std::max<long long>(1, std::min<long long>((a.env.B + 31) / 32, std::max(1, kMsgCtas / ny)));
+  const dim3 grid(nx, ny);
+  const size_t smem = (size_t)R * 33 * sizeof(unsigned long long);
+  unsigned long long* s_ = reinterpret_cast<unsigned long long*>(sums);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (smem <= kMsgSmemMax) {
+    if (smem > 48 * 1024) {
+      const cudaError_t e = cudaFuncSetAttribute(message_map_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 (int)kMsgSmemMax);
+      if (e != cudaSuccess) return (int)e;
+    }
+    message_map_kernel<true><<<grid, kMsgThreads, smem, s>>>(a, s_, R);
+  } else {
+    message_map_kernel<false><<<grid, kMsgThreads, 0, s>>>(a, s_, R);
   }
   IC3_LAUNCH_CHECK();
   return IC3_OK;

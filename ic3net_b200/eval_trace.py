@@ -1,6 +1,7 @@
 """Evaluation recorder behind ``Trainer.evaluate_trace``: per-step trajectories of chosen evaluation slots and a map of
 where agents open their communication gate, kept on the device while the evaluation plays (csrc/eval_trace.cu,
-ic3_trace_step / ic3_comm_map_step) and copied to the host once at the end.
+ic3_trace_step / ic3_comm_map_step) and copied to the host once at the end.  With ``messages`` it also keeps what the
+agents send and receive (ic3_trace_comm_step / ic3_message_map_step), read before each policy step overwrites h.
 
 Every array lives in one device byte arena, each behind a 16-byte guard band that no kernel writes, so the whole
 recording comes back in one device->host copy."""
@@ -39,9 +40,11 @@ class EvalTraceResult(object):
     loc_next [T, K, rows, 2] int16 (entering step t; after its move, before the auto-reset), alive [T, K, NA] uint8,
     action [T, K, NA, nheads] int8, value and reward [T, K, NA] float32, t_ep [T, K] int16, done, success and valid
     [T, K] uint8, comm_prob [T, K, NA] float32 (with --hard_attn, else None), route_id [T, K, N] int16 (traffic junction,
-    else None) and env_id [K] (global env ids)."""
+    else None) and env_id [K] (global env ids).  With messages: msg_h and msg_in [T, K, NA, H] float32 (the hidden
+    state each agent sends entering step t, and the communication vector S it receives) and msg_gate [T, K, NA] uint8
+    (its gate g); else None."""
     FIELDS = ('loc', 'loc_next', 'alive', 'action', 'value', 'reward', 't_ep', 'done', 'success', 'valid', 'comm_prob',
-              'route_id', 'env_id')
+              'route_id', 'env_id', 'msg_h', 'msg_gate', 'msg_in')
 
     def __init__(self, **arrays):
         for k in self.FIELDS:
@@ -53,11 +56,13 @@ class EvalTraceResult(object):
 
 
 class Recorder(object):
-    """The device buffers of one evaluate_trace configuration and the launches that fill them.  step(t) runs between
-    policy step t and env step t, finish(T) after the last env step; rollout_fields() are the ic3_rollout_io hooks the
-    env step fills for it."""
+    """The device buffers of one evaluate_trace configuration and the launches that fill them.  pre_step(t) runs before
+    policy step t, step(t) between policy step t and env step t, finish(T) after the last env step; rollout_fields()
+    are the ic3_rollout_io hooks the env step fills for it."""
 
-    def __init__(self, trainer, e, b, T, slots, comm_map):
+    MSG_SCALE = 2.0 ** -32            # a message map sum times this is the sum of the float messages
+
+    def __init__(self, trainer, e, b, T, slots, comm_map, messages=False):
         args = trainer.args
         dev = e.device
         self.e, self.b, self.T, self.K = e, b, int(T), len(slots)
@@ -79,10 +84,19 @@ class Recorder(object):
             spec.append(('comm_prob', (T, K, NA), torch.float32))
         if self.is_tj:
             spec.append(('route_id', (T, K, NA), i16))
+        self.messages = bool(messages)
+        self.H = int(args.hid_size)
+        if self.messages:
+            spec += [('msg_h', (T, K, NA, self.H), torch.float32), ('msg_gate', (T, K, NA), u8),
+                     ('msg_in', (T, K, NA, self.H), torch.float32)]
         self.map_keys = self._map_keys() if comm_map else []
         nmap = sum(n for _, n in self.map_keys)
         if nmap:
             spec.append(('counts', (nmap,), torch.int64))
+        # message map (ic3_message_map_step): sent [R, H], recv [R, H], senders [R] over R key rows
+        self.msg_rows = self.npos + self.max_steps + (0 if self.is_tj else 2)
+        if self.messages and comm_map:
+            spec.append(('msg_sums', ((2 * self.H + 1) * self.msg_rows,), torch.int64))
         spec += [('slots', (K,), torch.int32), ('out_loc', (e.nenvs, rows, 2), torch.int32),
                  ('out_success', (e.nenvs,), u8)]
         # arena: [guard][array][pad to 16][guard][array]...[guard]
@@ -97,6 +111,7 @@ class Recorder(object):
         self.t['out_loc'].zero_()
         self.t['out_success'].zero_()
         self.counts = self.t.get('counts')
+        self.msg_sums = self.t.get('msg_sums')
         self.host_names = [n for n, _, _ in spec if n not in ('slots', 'out_loc', 'out_success')]
         pp = not self.is_tj
         self.io = _lib.EvalStepIO(
@@ -112,6 +127,11 @@ class Recorder(object):
                                  action=p('action'), value=p('value'), reward=p('reward'), t_ep=p('t_ep'),
                                  done=p('done'), success=p('success'), valid=p('valid'), comm_prob=p('comm_prob'),
                                  route_id=p('route_id'))
+        if self.messages:
+            self.comm_io = _lib.EvalCommIO(h=b['h'].data_ptr(), comm=b['comm'].data_ptr() if self.hard else None,
+                                           alive=b['alive'].data_ptr(), fresh=b['fresh'].data_ptr(), H=self.H,
+                                           comm_avg=int(getattr(args, 'comm_mode', 'avg') == 'avg'),
+                                           hard=int(self.hard))
 
     def _map_keys(self):
         """(key, length) of the comm-map blocks in ic3_comm_map_step's layout."""
@@ -128,6 +148,19 @@ class Recorder(object):
     def begin(self):
         if self.counts is not None:
             self.counts.zero_()
+        if self.msg_sums is not None:
+            self.msg_sums.zero_()
+
+    def pre_step(self, t, s):
+        """Before policy step t: the messages of step t, read from h before the step overwrites it."""
+        if not self.messages:
+            return
+        lib = _lib.load()
+        _lib.check(lib.ic3_trace_comm_step(C.byref(self.io), C.byref(self.comm_io), C.byref(self.tr),
+                                           self.t['msg_h'].data_ptr(), self.t['msg_gate'].data_ptr(),
+                                           self.t['msg_in'].data_ptr(), t, s))
+        if self.msg_sums is not None:
+            _lib.check(lib.ic3_message_map_step(C.byref(self.io), C.byref(self.comm_io), self.msg_sums.data_ptr(), s))
 
     def step(self, t, s):
         lib = _lib.load()
@@ -153,7 +186,7 @@ class Recorder(object):
                 torch.int64: np.int64, torch.int32: np.int32}
         get = lambda name: host[self.layout[name][0]:self.layout[name][0] + self.layout[name][1]].view(
             npdt[self.layout[name][3]]).reshape(self.layout[name][2]).copy()
-        arrays = {n: get(n) for n in self.host_names if n != 'counts'}
+        arrays = {n: get(n) for n in self.host_names if n not in ('counts', 'msg_sums')}
         arrays['env_id'] = int(self.e.cfg.env_id0) + np.asarray(self.slots, dtype=np.int64)
         cmap = None
         if self.counts is not None:
@@ -162,4 +195,30 @@ class Recorder(object):
             for key, n in self.map_keys:
                 cmap[key] = c[o:o + n].copy()
                 o += n
+        if self.msg_sums is not None:
+            cmap.update(self._message_map(get('msg_sums'), cmap))
         return EvalTraceResult(**arrays), cmap
+
+    def _message_map(self, sums, cmap):
+        """The message map's blocks under msg_* keys: int64 sums of sent and received messages (scale msg_scale) by
+        cell, by episode step and, predator-prey, on / off the prey; the open senders' counts; and float64 means
+        where a count exists (NaN elsewhere): sent over the open senders, received over every counted agent (the comm
+        map's visits)."""
+        R, H, P, S = self.msg_rows, self.H, self.npos, self.max_steps
+        sent, recv, senders = sums[:R * H].reshape(R, H), sums[R * H:2 * R * H].reshape(R, H), sums[2 * R * H:]
+        parts = [('', slice(0, P), 'visits'), ('_t', slice(P, P + S), 'visits_t')]
+        if not self.is_tj:
+            parts.append(('_reached', slice(P + S, R), 'visits_reached'))
+        out = dict(msg_scale=np.float64(self.MSG_SCALE))
+
+        def mean(total, n):
+            n = n.astype(np.float64)[:, None]
+            with np.errstate(invalid='ignore', divide='ignore'):
+                return np.where(n > 0, total.astype(np.float64) * self.MSG_SCALE / n, np.nan)
+        for suffix, rows, visits in parts:
+            out['msg_sent' + suffix] = sent[rows].copy()
+            out['msg_recv' + suffix] = recv[rows].copy()
+            out['msg_senders' + suffix] = senders[rows].copy()
+            out['msg_sent_mean' + suffix] = mean(sent[rows], senders[rows])
+            out['msg_recv_mean' + suffix] = mean(recv[rows], cmap[visits])
+        return out

@@ -112,6 +112,10 @@ def build_parser():
                         help='with --eval_every: record every evaluation and write PREFIX_epoch<E>.npz (rank 0\'s slots: '
                              'per-step trajectories and the map of where agents open their gate)')
     parser.add_argument('--eval_trace_slots', type=int, default=8, help='evaluation slots recorded by --eval_trace')
+    parser.add_argument('--eval_trace_messages', action='store_true', default=False,
+                        help='with --eval_trace: also record what the agents communicate (recurrent CommNet / IC3Net, '
+                             'one comm pass): the hidden state each sends, its gate and the vector it receives, and '
+                             'their sums by cell and episode step (msg_* and map_msg_* arrays)')
     parser.add_argument('--resumable', action='store_true', default=False,
                         help='with --save: every checkpoint write also writes the run state to <checkpoint>.run, and '
                              'SIGTERM / SIGINT save both and exit after the update in flight, so --resume can continue '
@@ -294,7 +298,8 @@ def read_run_file(path):
 
 
 def save_eval_trace(prefix, epoch, args, grid_shape, trace, cmap):
-    """PREFIX_epoch<E>.npz: the trace's arrays, the comm map's under 'map_<key>', and what it takes to read them."""
+    """PREFIX_epoch<E>.npz: the trace's arrays, the comm map's (and the message map's) under 'map_<key>', and what it
+    takes to read them (with messages also hid_size)."""
     d = dict(trace.arrays())
     for k, v in (cmap or {}).items():
         d['map_' + k] = v
@@ -305,6 +310,8 @@ def save_eval_trace(prefix, epoch, args, grid_shape, trace, cmap):
              naction_heads=np.asarray(args.naction_heads, dtype=np.int64), max_steps=np.int64(args.max_steps),
              episodes=np.int64(args.eval_episodes), greedy=np.int64(bool(args.eval_greedy)),
              hard_attn=np.int64(bool(args.hard_attn and args.commnet)))
+    if trace.msg_h is not None:
+        d['hid_size'] = np.int64(args.hid_size)
     np.savez(prefix + '_epoch%d.npz' % epoch, **d)
 
 
@@ -371,6 +378,8 @@ def main(argv=None):
         parser.error("--resume continues a run from its checkpoint and run state; it takes no --load")
     if args.resumable and not args.save:
         parser.error("--resumable writes the run state beside the --save checkpoint; give --save")
+    if args.eval_trace_messages and not args.eval_trace:
+        parser.error("--eval_trace_messages adds to the recording of --eval_trace; give --eval_trace")
     run = read_run_file(args.resume) if args.resume else None
     args.resumable = args.resumable or bool(args.resume and args.save)
 
@@ -468,7 +477,8 @@ def _train(args, trainer, policy_net, env, log, evals, eval_slots, rank, world, 
             if args.eval_trace:
                 cfg, tj = env.env.cfg, args.env_name == 'traffic_junction'
                 es, trace, cmap = trainer.evaluate_trace(args.eval_episodes, args.eval_greedy,
-                                                         slots=min(args.eval_trace_slots, args.eval_nenvs or args.nenvs))
+                                                         slots=min(args.eval_trace_slots, args.eval_nenvs or args.nenvs),
+                                                         messages=args.eval_trace_messages)
                 if rank == 0:
                     save_eval_trace(args.eval_trace, epoch, args, (cfg.h, cfg.w) if tj else (cfg.dim, cfg.dim),
                                     trace, cmap)

@@ -212,15 +212,18 @@ class MultiGPUTrainer(object):
             dist.all_reduce(vec, op=dist.ReduceOp.SUM)
         return tr.stat_from_vector(vec.cpu().numpy(), e)
 
-    def evaluate_trace(self, episodes=1, greedy=False, epoch=None, slots=8, comm_map=True):
-        """Trainer.evaluate_trace on every rank's evaluation slots: the statistics vector and the comm map are summed
-        over ranks (one all-reduce each), the trace is of this rank's slots (its env_id holds their global ids)."""
+    def evaluate_trace(self, episodes=1, greedy=False, epoch=None, slots=8, comm_map=True, messages=False):
+        """Trainer.evaluate_trace on every rank's evaluation slots: the statistics vector, the comm map and the message
+        map's integer sums are summed over ranks (one all-reduce each, exact), the trace is of this rank's slots (its
+        env_id holds their global ids)."""
         tr = self.trainer
-        vec, e, rec = tr.evaluate_trace_vector(episodes, greedy, epoch, slots, comm_map)
+        vec, e, rec = tr.evaluate_trace_vector(episodes, greedy, epoch, slots, comm_map, messages)
         if _dist_on():
             dist.all_reduce(vec, op=dist.ReduceOp.SUM)
             if rec.counts is not None:
                 dist.all_reduce(rec.counts, op=dist.ReduceOp.SUM)
+            if rec.msg_sums is not None:
+                dist.all_reduce(rec.msg_sums, op=dist.ReduceOp.SUM)
         stat = tr.stat_from_vector(vec.cpu().numpy(), e)
         trace, cmap = rec.to_host()
         return stat, trace, cmap

@@ -399,7 +399,8 @@ class Trainer(object):
         rollout's; evaluate passes its own, which hold no records and one lock-step of action / log-prob / value
         scratch, and no observation block: x comes from the env state); episodes > 0: episode quota
         (ic3_rollout_io.episodes); greedy: argmax actions (ic3_policy_cfg.greedy); recorder: an eval_trace.Recorder
-        that keeps every lock-step between its policy step and its env step (evaluate_trace)."""
+        that keeps every lock-step before its policy step and between its policy step and its env step
+        (evaluate_trace)."""
         b = self._buf if b is None else b
         e = self.env.env if e is None else e
         if self.random_policy:
@@ -477,6 +478,8 @@ class Trainer(object):
                                h_out=hout.data_ptr(), c_out=cout.data_ptr(), value=b['value'][r].data_ptr(),
                                logp=b['logp'][r].data_ptr(), action=b['action'][r].data_ptr(),
                                workspace=_lib.ptr(ws), err=b['err'].data_ptr(), **src)
+            if recorder is not None:
+                recorder.pre_step(t, s)
             _lib.check(lib.ic3_policy_step(C.byref(cfg), C.byref(w), C.byref(io), s))
             if window and hc:
                 # max |c'| of this step: the backward's operand scale needs the bound over every step's c before it
@@ -773,18 +776,36 @@ class Trainer(object):
         vec, e = self.evaluate_vector(episodes, greedy, epoch)
         return self.stat_from_vector(vec.cpu().numpy(), e)
 
-    def evaluate_trace_vector(self, episodes=1, greedy=False, epoch=None, slots=8, comm_map=True):
+    def _check_messages(self):
+        """Raise NotImplementedError unless the policy is the recurrent (LSTM) CommNet / IC3Net with one comm pass,
+        whose messages evaluate_trace(messages=True) records."""
+        net, args = self.policy_net, self.args
+        if self.random_policy:
+            raise NotImplementedError("evaluate_trace(messages=True): models.Random does not communicate")
+        if bool(getattr(net, 'args', args).comm_mask_zero):
+            raise NotImplementedError("evaluate_trace(messages=True): the policy does not communicate (models.MLP, "
+                                      "models.RNN or --comm_mask_zero)")
+        if not net.recurrent:
+            raise NotImplementedError("evaluate_trace(messages=True) records the recurrent CommNet / IC3Net (LSTM "
+                                      "cell); the non-recurrent policy is outside its scope")
+        if int(args.comm_passes) != 1:
+            raise NotImplementedError("evaluate_trace(messages=True) records one comm pass, not comm_passes %d"
+                                      % int(args.comm_passes))
+
+    def evaluate_trace_vector(self, episodes=1, greedy=False, epoch=None, slots=8, comm_map=True, messages=False):
         """evaluate_trace without the host read: (device statistics vector, evaluation env, eval_trace.Recorder holding
         the trajectories and the comm map on the device)."""
+        if messages:
+            self._check_messages()
         e, b, T = self._eval_prepare(episodes, greedy, epoch)
         episodes = int(episodes)
         slots = eval_trace.parse_slots(slots, e.nenvs)
-        key = (T, slots, bool(comm_map))
+        key = (T, slots, bool(comm_map), bool(messages))
         rec = self._eval.get('trace')
         if rec is None or rec.key != key:
             self._graphs.pop('evaluate_trace', None)       # its graph writes into the recorder it replaces
             self._eval['trace'] = None
-            rec = self._eval['trace'] = eval_trace.Recorder(self, e, b, T, slots, bool(comm_map))
+            rec = self._eval['trace'] = eval_trace.Recorder(self, e, b, T, slots, bool(comm_map), bool(messages))
             rec.key = key
         self._begin(T, None, b, e)
 
@@ -797,14 +818,17 @@ class Trainer(object):
             run()
         return self.stat_vector(b, e), e, rec
 
-    def evaluate_trace(self, episodes=1, greedy=False, epoch=None, slots=8, comm_map=True):
+    def evaluate_trace(self, episodes=1, greedy=False, epoch=None, slots=8, comm_map=True, messages=False):
         """evaluate, recording what the agents do: returns (stat, trace, cmap).  stat is what evaluate returns for the
         same call (the same loop, env, buffers and random streams).  trace (eval_trace.EvalTraceResult) holds every
         lock-step of the recorded slots -- ``slots``: the first K evaluation slots, or a sequence of distinct local slot
         numbers -- as [T, K, ...] numpy arrays, T = episodes * max_steps.  cmap (comm_map; else None): integer counts
         over every slot of visits to each cell and each episode step and, with --hard_attn, of gate openings there
-        (ic3_comm_map_step).  The trace and the map come back in one device->host copy."""
-        vec, e, rec = self.evaluate_trace_vector(episodes, greedy, epoch, slots, comm_map)
+        (ic3_comm_map_step).  messages (recurrent CommNet / IC3Net with one comm pass; NotImplementedError otherwise):
+        the trace also holds the hidden state each agent sends, its gate and the vector S it receives (msg_h, msg_gate,
+        msg_in), and cmap the message map (msg_* keys, eval_trace.Recorder._message_map).  The trace and the map come
+        back in one device->host copy."""
+        vec, e, rec = self.evaluate_trace_vector(episodes, greedy, epoch, slots, comm_map, messages)
         stat = self.stat_from_vector(vec.cpu().numpy(), e)
         trace, cmap = rec.to_host()
         return stat, trace, cmap

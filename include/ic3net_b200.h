@@ -57,7 +57,8 @@ enum {
                                fp32 SIMT kernels (policy_impl = 'simt') for such a model */
   IC3_ERR_GRAD_DIV = 0x400, /* ic3_rmsprop_step_dev: the step count it divides by was not a positive finite number; the
                                parameters, gradients and second moments were left unchanged */
-  IC3_ERR_TRACE_SLOT = 0x800 /* ic3_trace_step: a recorded slot index lies outside [0, B); nothing was written for it */
+  IC3_ERR_TRACE_SLOT = 0x800 /* ic3_trace_step, ic3_trace_comm_step: a recorded slot index lies outside [0, B); nothing
+                                was written for it */
 };
 
 enum { IC3_PP_MIXED = 0, IC3_PP_COOPERATIVE = 1, IC3_PP_COMPETITIVE = 2 };
@@ -508,6 +509,39 @@ int ic3_trace_step(const ic3_eval_step_io* io, const ic3_eval_trace* tr, int32_t
  *   visits_reached[2], open_reached[2] (index 1: the predator stands on the prey);
  * without a gate (comm_col < 0) the open* blocks are absent.  Integer sums: the counts do not depend on the order. */
 int ic3_comm_map_step(const ic3_eval_step_io* io, uint64_t* counts, void* stream);
+
+/* What the agents communicate (Trainer.evaluate_trace(messages=True)), recurrent CommNet / IC3Net with one comm pass
+ * (comm.py:134-244).  At lock-step t agent j sends m_j = h_j, its hidden state entering the step (0 when the slot is
+ * fresh), gated by g_j = alive_j * comm_j with hard attention, alive_j without (fresh: comm = 0, alive = 1).  Agent k
+ * receives S_k = g_k * sum_{j != k} g_j h_j, divided by (n_alive - 1) with comm_avg and n_alive > 1 (n_alive counted
+ * before gating, every row when fresh).  The sum over j runs in float64 in agent order and S_k is rounded to float32
+ * once, so every call computes the same S_k.  Both calls run BEFORE policy step t (the step overwrites h in place). */
+typedef struct {
+  const float* h;          /* [B, NA, H] the policy's hidden state entering step t (ic3_policy_io.h) */
+  const uint8_t* comm;     /* [B, NA] ic3_policy_io.comm_action (required with hard) */
+  const uint8_t* alive;    /* [B, NA] ic3_policy_io.alive */
+  const uint8_t* fresh;    /* [B] ic3_policy_io.fresh */
+  int32_t H;               /* hid_size: a multiple of 16, 16 .. 1024 */
+  int32_t comm_avg;        /* args.comm_mode == 'avg' */
+  int32_t hard;            /* args.hard_attn && args.commnet */
+} ic3_eval_comm_io;
+
+/* Row t (0 <= t < T) of the K slots of tr (T, K and slots are read; the other fields of tr are not):
+ *   msg_h [T, K, NA, H]: h entering step t; 0 when fresh, for a row that is not alive and for padding rows;
+ *   msg_gate [T, K, NA]: g (0 for padding rows);  msg_in [T, K, NA, H]: S.
+ * A slot index outside [0, B) raises IC3_ERR_TRACE_SLOT. */
+int ic3_trace_comm_step(const ic3_eval_step_io* io, const ic3_eval_comm_io* cm, const ic3_eval_trace* tr,
+                        float* msg_h, uint8_t* msg_gate, float* msg_in, int32_t t, void* stream);
+
+/* Adds this lock-step's messages into sums (device int64), over the rows ic3_comm_map_step counts (slots still
+ * playing, friendly, alive), keyed by the same state entering step t.  Each float v is added as llrint(v * 2^32), so
+ * the sums are exact and do not depend on the order.  R = npos + max_steps (+ 2 for predator_prey) key rows: the
+ * cell (cell = row * width + col), then npos + t_ep, then (predator_prey) npos + max_steps + (the predator stands on
+ * the prey).  Layout:
+ *   sent[R, H]    sum of h over open senders (g = 1),
+ *   recv[R, H]    sum of S over every counted row (its count is ic3_comm_map_step's visits block),
+ *   senders[R]    number of open senders. */
+int ic3_message_map_step(const ic3_eval_step_io* io, const ic3_eval_comm_io* cm, int64_t* sums, void* stream);
 
 /* ------------------------------------------------------------------------
  * REINFORCE returns  (trainer.py:160-173), the first step of Trainer.compute_grad
